@@ -1,12 +1,12 @@
 #!/usr/bin/env python3
-"""bench.py -- MobileNet-v2-int8 hot-path throughput on B200 (driver contract in the task statement).
+"""bench.py -- MobileNet-v2-int8 hot-path throughput on one H100 per replica.
 
   python bench.py --gpus N --steps K --warmup W          # our arm (CUDA, through the C ABI)
   python bench.py --impl reference --gpus N ...           # the reference's own CPU implementation of the same path
 
 A "step" = one pass of the hot path over one batch of synthetic input.  Workload at N=1 = BASELINE.json
 configs[1]: MobileNet-v2 int8 .mnn, batch 32, the 36 dense int8 convolutions (ConvInt8 path only), every layer
-on its own resident NHWC16 activation (240 MB of distinct traffic per step > 126 MB L2, so consecutive steps
+on its own resident NHWC16 activation (240 MB of distinct traffic per step > 50 MB L2, so consecutive steps
 cannot be served from L2).  N>1: one replica per GPU, batch 32 each (weak scaling), the model bytes broadcast once
 from rank 0 over NCCL at session build, no steady-state communication.
 """
@@ -77,7 +77,7 @@ def measured_peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return float(d["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 class ClockSampler(threading.Thread):
@@ -247,6 +247,24 @@ def run_reference(args, rank):
     print(json.dumps(line), flush=True)
 
 
+DUMP_SAMPLE = 1 << 18      # 36 layers x 2^18 float32 values = 37.7 MB at most
+
+
+def dump_outputs(sess, out_dir):
+    """The int8 output of every conv of the session (what the step computed last), as float32 <layer>.npy in the NHWC16 layout
+    the layers write; layers larger than DUMP_SAMPLE values are sampled at fixed positions (seeded by the layer size), so two
+    builds run with the same arguments can be compared value for value."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    sess.stream.synchronize()
+    for i, (node, _, _, y) in enumerate(sess.layers):
+        v = y.data.cpu().numpy().reshape(-1)
+        if v.size > DUMP_SAMPLE:
+            v = v[np.sort(np.random.default_rng(v.size).choice(v.size, DUMP_SAMPLE, replace=False))]
+        name = "".join(ch if ch.isalnum() or ch in "-_." else "_" for ch in f"{i:02d}_{node.name}")
+        np.save(os.path.join(out_dir, name + ".npy"), v.astype(np.float32))
+
+
 def _max_over_ranks(torch, dist, world, ms):
     t = torch.tensor([ms], device="cuda")
     if world > 1:
@@ -267,6 +285,9 @@ def main():
                     help="mbv2 = the driver's line (BASELINE configs[1]); resnet_wino / qwen = configs[2] / configs[3] alone")
     ap.add_argument("--wino-unit", type=int, default=6, choices=[2, 4, 6])
     ap.add_argument("--qwen-layers", type=int, default=24)
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write every conv output of the last step to DIR/<layer>.npy (float32; a fixed "
+                         "seeded sample of at most %d values per layer)" % DUMP_SAMPLE)
     args = ap.parse_args()
     rank = int(os.environ.get("RANK", "0"))
     world = int(os.environ.get("WORLD_SIZE", "1"))
@@ -326,6 +347,8 @@ def main():
     barrier()
     my_ms = ev0.elapsed_time(ev1)
     ms_total = _max_over_ranks(torch, dist, world, my_ms)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(sess, args.dump_outputs)
     # a longer look at the same loop (several K-step windows, >= 0.25 s): the median window guards the short K-step region
     # against one straggling host-side graph launch (round-1 SCALE N=4 dip)
     win = []
@@ -475,14 +498,6 @@ def main():
     if rank == 0:
         peak, peak_src = measured_peaks()
         achieved = sess.bytes / (ms_per_step / 1e3) / 1e9
-        traffic = None
-        # dram__bytes_read.sum + dram__bytes_write.sum over the kernels of one step, from the committed ncu capture of this
-        # command (tools/prof_traffic.sh); written bytes largely stay in the 126 MB L2 under ncu's per-kernel replay
-        for name in ("r02_traffic_mbv2_convpath.json", "r01_traffic_mbv2_convpath.json"):
-            tp = os.path.join(ROOT, "profiles", name)
-            if os.path.exists(tp):
-                traffic = json.load(open(tp)).get("traffic_bytes_per_step")
-                break
         use_plugin = bool(plug and plug.get("value"))
         e2e = {"value": plug["value"] if use_plugin else e2e_pipe, "unit": "img/s",
                "h2d_bytes_per_step": (plug.get("h2d_bytes_per_step") if use_plugin else h2d),
@@ -501,12 +516,12 @@ def main():
             "value": value, "unit": "img/s", "n_gpus": world, "steps": K, "warmup": W, "ms_per_step": ms_per_step,
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "s8", "data": "synthetic",
             "config": {"workload": WORKLOAD, "batch_per_gpu": BATCH_PER_GPU,
-                       "implementation": "sm_100a CUDA through the C ABI: conv-group persistent tcgen05 kernel + stem kernel, CUDA-graph replay",
+                       "implementation": "sm_90a CUDA through the C ABI: conv-group persistent wgmma kernel + stem kernel, CUDA-graph replay",
                        "parallelism": f"dp{world} replicas, NCCL model broadcast at build",
                        "l2": "inputs larger than L2 (240 MB distinct bytes per step)",
                        "graph": not args.no_graph, "numa_node": numa_node},
             "roofline": {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                         "traffic": traffic, "peak_source": peak_src, "kernel": "conv_group_tcgen05_kernel" if sess.group is not None else "gemm_i8_tcgen05_kernel",
+                         "traffic": None, "peak_source": peak_src, "kernel": "conv_group_wgmma_kernel" if sess.group is not None else "gemm_i8_wgmma_kernel",
                          "algorithmic_bytes_per_step": sess.bytes, "macs_per_step": sess.macs},
             "timing": {"ms_per_step_median_window": ms_median / K, "windows": len(win), "per_rank_ms_per_step": per_rank_ms},
             "e2e": e2e,

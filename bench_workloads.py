@@ -17,18 +17,14 @@ import time
 import numpy as np
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
-INT8_DENSE_PEAK_TOPS = 4500.0   # nominal dense int8 tcgen05 peak of one B200 (MEASURED_PEAKS.json has bf16 only)
-# int8 tensor peak: kind::i8 M128 x N256 x K32 issues every 128 clk per SM = 8190 MAC/clk/SM x 148 SMs x 1.965 GHz (max clock)
-# = 4.43 POP/s, measured by tools/microbench/umma_rate.cu on this pool's B200 (profiles/r01_umma_rate_microbench.jsonl);
-# MEASURED_PEAKS.json holds bf16 only.  The nominal dense figure is 4.5 POP/s.
-INT8_MEASURED_PEAK_TOPS = 4431.0
+INT8_DENSE_PEAK_TOPS = 1979.0   # H100 SXM data sheet, dense int8 (a card at a lower power limit reaches less)
 
 
 def _peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
-    return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+    return 3350.0, "H100 SXM data sheet (3.35 TB/s HBM3)"
 
 
 def _timeit(torch, stream, fn, K, W):
@@ -154,7 +150,7 @@ def run_resnet_wino(args, sampler_cls, rank=0, world=1, local_rank=0):
                      "phases_ms": {"input_transform": ms[1], "position_gemms_unfused": ms[2], "output_transform_unfused": ms[4],
                                    "gemms_plus_output_as_executed": ms[6], "all": ms[7],
                                    "note": "F(2,3) executes the position GEMMs and the output transform as ONE kernel (accumulators of all "
-                                           "16 positions resident in TMEM); the unfused kernels are timed for comparison"},
+                                           "16 positions resident in registers); the unfused kernels are timed for comparison"},
                      "gemm": {"bound": "tensor", "achieved": gemm_ops / (ms[2] / 1e3) / 1e12, "peak": INT8_DENSE_PEAK_TOPS,
                               "unit": "TOP/s", "frac": gemm_ops / (ms[2] / 1e3) / 1e12 / INT8_DENSE_PEAK_TOPS,
                               "peak_source": "nominal dense int8 (4.5 POPS)"},
@@ -167,7 +163,7 @@ def run_resnet_wino(args, sampler_cls, rank=0, world=1, local_rank=0):
 
 def run_resnet_direct(args, sampler_cls, rank=0, world=1, local_rank=0):
     """The same 13 ResNet-50 3x3/s1 layers at batch 64 WITHOUT a winogradAttr (what a Revert-quantised r50 .mnn carries): the direct
-    int8 convolution.  Three device-timed variants: the round-1 mma.sync implicit GEMM (variant 1), the tcgen05 implicit GEMM one
+    int8 convolution.  Three device-timed variants: the round-1 mma.sync implicit GEMM (variant 1), the wgmma implicit GEMM one
     launch per layer (variant 2), and all 13 layers in one conv-group launch.  Tensor-bound: 192.4 GOP per batch (SURVEY 8d C3)."""
     import torch
     from mnn_b200 import _capi
@@ -220,7 +216,7 @@ def run_resnet_direct(args, sampler_cls, rank=0, world=1, local_rank=0):
     ms = {}
     sampler = sampler_cls(local_rank)
     sampler.start()
-    for name, fn in (("mma_sync_per_layer", per_layer(1)), ("tcgen05_per_layer", per_layer(2)), ("tcgen05_conv_group", lambda: grp.onExecute())):
+    for name, fn in (("mma_sync_per_layer", per_layer(1)), ("wgmma_per_layer", per_layer(2)), ("wgmma_conv_group", lambda: grp.onExecute())):
         gr = graph_of(fn)
 
         def replay(gr=gr):
@@ -238,9 +234,9 @@ def run_resnet_direct(args, sampler_cls, rank=0, world=1, local_rank=0):
         "config": {"workload": "ResNet-50 int8 3x3/s1 layer set, batch 64, direct convolution (no winogradAttr)", "batch_per_gpu": B,
                    "best_variant": best},
         "variants_ms": ms,
-        "roofline": {"bound": "tensor", "kernel": "conv_group_tcgen05_kernel (implicit GEMM, kind::i8)", "achieved": tops,
-                     "peak": INT8_MEASURED_PEAK_TOPS, "unit": "TOP/s", "frac": tops / INT8_MEASURED_PEAK_TOPS, "traffic": None,
-                     "peak_source": "measured tcgen05 kind::i8 issue rate (tools/microbench/umma_rate.cu)",
+        "roofline": {"bound": "tensor", "kernel": "conv_group_wgmma_kernel (implicit GEMM, wgmma s8)", "achieved": tops,
+                     "peak": INT8_DENSE_PEAK_TOPS, "unit": "TOP/s", "frac": tops / INT8_DENSE_PEAK_TOPS, "traffic": None,
+                     "peak_source": "H100 SXM data sheet, dense int8",
                      "gop_per_batch": 2 * macs / 1e9, "algorithmic_mb": bytes_alg / 1e6},
         "gpu_launches": K, "clocks": sampler.result(),
     }
@@ -404,11 +400,9 @@ def run_qwen(args, sampler_cls, rank=0, world=1, local_rank=0, decode=False):
                    "parallelism": f"dp{world} replicas (sequences sharded), one NCCL broadcast of the int8 weight arena at build",
                    "build_seconds": build_s,
                    "l2": f"distinct int8 weights per layer ({wbytes / 1e6:.0f} MB + 311 MB lm_head) exceed L2"},
-        "roofline": {"bound": "tensor", "kernel": "gemm_i8_2cta_kernel", "achieved": achieved, "peak": INT8_MEASURED_PEAK_TOPS,
-                     "unit": "TOP/s", "frac": achieved / INT8_MEASURED_PEAK_TOPS, "traffic": None,
-                     "peak_source": "measured: tcgen05 kind::i8 issue-rate microbenchmark (tools/microbench/umma_rate.cu, 4431 TOP/s at "
-                                    "1965 MHz); nominal dense int8 is 4500",
-                     "frac_of_nominal": achieved / INT8_DENSE_PEAK_TOPS, "ops_per_step_per_gpu": ops},
+        "roofline": {"bound": "tensor", "kernel": "gemm_i8_wgmma_kernel (2-CTA cluster)", "achieved": achieved, "peak": INT8_DENSE_PEAK_TOPS,
+                     "unit": "TOP/s", "frac": achieved / INT8_DENSE_PEAK_TOPS, "traffic": None,
+                     "peak_source": "H100 SXM data sheet, dense int8", "ops_per_step_per_gpu": ops},
         "e2e": {"value": world * 1e3 / (e2e_ms * (scale_layers if nl != 24 else 1.0)), "unit": "fwd/s",
                 "h2d_bytes_per_step": int(hx.numel() * 4), "d2h_bytes_per_step": int(hy.numel() * 4)},
         "gpu_launches": 2 * (len(execs) + 1) * K, "clocks": sampler.result(),

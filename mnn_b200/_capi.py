@@ -1,7 +1,7 @@
 """ctypes binding of include/mnn_b200.h -- the same C ABI the MNN plugin binds (see INTEGRATION.md).
 
 The product path is CUDA only: importing this module builds nothing and falls back to nothing.  If
-libmnn_b200.so is missing or no sm_100 device is present every entry point raises.
+libmnn_b200.so is missing or no sm_90 device is present every entry point raises.
 """
 import ctypes as C
 import os

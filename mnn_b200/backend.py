@@ -68,7 +68,7 @@ class Runtime:
 
     def __init__(self, device_id: int = 0, adopt_torch_stream: bool = True):
         if not torch.cuda.is_available():
-            raise MnnB200Error("mnn_b200 needs a CUDA device (sm_100a); there is no CPU fallback")
+            raise MnnB200Error("mnn_b200 needs a CUDA device (sm_90a); there is no CPU fallback")
         torch.cuda.set_device(device_id)
         self.device = torch.device("cuda", device_id)
         self._h = C.c_void_p()

@@ -1,4 +1,4 @@
-"""Builds libmnn_b200.so (CUDA kernels + C ABI) in-tree for sm_100a with nvcc.  No torch involvement."""
+"""Builds libmnn_b200.so (CUDA kernels + C ABI) in-tree for sm_90a (H100) with nvcc.  No torch involvement."""
 import os
 import subprocess
 import sys
@@ -6,29 +6,12 @@ import sys
 HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmnn_b200.so")
-SOURCES = ["capi.cu", "conv_int8_mma.cu", "elementwise.cu", "gemm_i8_tcgen05.cu", "winograd_int8.cu", "gemm_f16_tcgen05.cu", "gemm_i8_tcgen05_2cta.cu", "conv_int8_stem.cu", "conv_group_tcgen05.cu", "linear_w8_gemv.cu"]
-NVCC_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+SOURCES = ["capi.cu", "conv_int8_mma.cu", "elementwise.cu", "gemm_i8_wgmma.cu", "winograd_int8.cu", "gemm_f16_wgmma.cu", "conv_int8_stem.cu", "conv_group_wgmma.cu", "linear_w8_gemv.cu"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
+NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-ffp-contract=off,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 # every float operation in that file is an explicit intrinsic / PTX instruction: no implicit contraction wanted anywhere in it
-PER_FILE_FLAGS = {"conv_group_tcgen05.cu": ["--fmad=false"]}
-
-
-def build_variant(name, defines):
-    """An A/B measurement build of the same sources with extra -D flags -> mnn_b200/libmnn_b200_<name>.so (select it with
-    MNNB200_LIB=<path>); objects go to a scratch directory so the product objects are untouched."""
-    import tempfile
-    nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    out = os.path.join(HERE, f"libmnn_b200_{name}.so")
-    with tempfile.TemporaryDirectory() as d:
-        objs, procs = [], []
-        for s in SOURCES:
-            o = os.path.join(d, s[:-3] + ".o")
-            objs.append(o)
-            procs.append(subprocess.Popen([nvcc, "-c", os.path.join(CSRC, s), "-o", o] + NVCC_FLAGS + PER_FILE_FLAGS.get(s, []) + defines))
-        if any(p.wait() for p in procs):
-            raise RuntimeError("nvcc failed")
-        subprocess.check_call([nvcc, "-shared", "-o", out] + objs + ["-gencode", "arch=compute_100a,code=sm_100a", "-lcudart"])
-    return out
+PER_FILE_FLAGS = {"conv_group_wgmma.cu": ["--fmad=false"]}
 
 
 def build(force=False, verbose=False):
@@ -54,19 +37,9 @@ def build(force=False, verbose=False):
             failed = True
     if failed:
         raise RuntimeError("nvcc failed")
-    subprocess.check_call([nvcc, "-shared", "-o", LIB] + objs + ["-gencode", "arch=compute_100a,code=sm_100a",
-                                                                   "-lcudart"])
+    subprocess.check_call([nvcc, "-shared", "-o", LIB] + objs + ARCH + ["-lcudart"])
     return LIB
 
 
 if __name__ == "__main__":
-    if "--variant-nopark" in sys.argv:
-        print(build_variant("nopark", ["-DMNNB200_PARK_NS=0"]))
-    elif "--variant-scalar" in sys.argv:
-        print(build_variant("scalar", ["-DMNNB200_EPI_SCALAR"]))
-    elif "--variant-nowatchdog" in sys.argv:
-        print(build_variant("nowatchdog", ["-DMNNB200_NO_WATCHDOG", "-DMNNB200_PARK_NS=0"]))
-    elif "--variant-pipelined" in sys.argv:
-        print(build_variant("pipelined", ["-DMNNB200_EPI_PIPELINED"]))
-    else:
-        print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))
+    print(build(force="--force" in sys.argv, verbose="-v" in sys.argv))

@@ -1,4 +1,4 @@
-// capi.cu -- host side of the B200 backend: runtime (device/stream/memory), the Execution objects
+// capi.cu -- host side of the H100 backend: runtime (device/stream/memory), the Execution objects
 // (create = Resource upload, resize = quant-info fold + launch plan, execute = enqueue) and the C ABI
 // declared in include/mnn_b200.h.  Mirrors the roles of CUDARuntime / CUDABackend / ConvInt8CutlassExecution
 // in the reference (source/backend/cuda/core/runtime/CUDARuntime.cpp, core/CUDABackend.cpp,
@@ -58,7 +58,7 @@ struct mnnb200_graph {
 struct mnnb200_exec {
     mnnb200_runtime* rt = nullptr;
     int kind = 0;  // 1 conv, 2 depthwise, 3 linear
-    int variant = 0;  // 0 auto, 1 mma.sync implicit GEMM, 2 tcgen05 GEMM
+    int variant = 0;  // 0 auto, 1 mma.sync implicit GEMM, 2 wgmma GEMM
     double cost_bytes = 0, cost_macs = 0;
     std::vector<void*> dev_bufs;  // everything freed at destroy
     virtual ~mnnb200_exec() {
@@ -139,7 +139,7 @@ static mnnb200_status make_tmap_u8(CUtensorMap* m, const void* ptr, int rank, co
     if (r != CUDA_SUCCESS) return fail(MNNB200_CUDA_ERROR, "cuTensorMapEncodeTiled (rank " + std::to_string(rank) + ") failed: " + std::to_string((int)r));
     return MNNB200_OK;
 }
-// columns per tcgen05 work item: split N into equal chunks of at most 256 columns (multiple of 16)
+// columns per wgmma work item: split N into equal chunks of at most 256 columns (multiple of 16)
 // When the M tiles alone cannot fill the GPU (the 7x7 / 14x14 feature maps of MobileNet: 13 / 49 tiles), N is split
 // further (down to 32 columns) so that m_tiles * n_chunks approaches the SM count: a lone CTA streaming a whole K x (A + B)
 // panel through one SM's L2 port is what bounds those layers, not the math.
@@ -168,7 +168,7 @@ struct ConvInt8Exec : mnnb200_exec {
     std::vector<int32_t> h_isum;           // sum_k w[oc][k]
     std::vector<int32_t> h_tapsum;         // [OCp][taps] sum_c w[oc][tap][c]: padding correction of the implicit-GEMM kernel
     int zin = 0;                           // input zero point of the last resize
-    struct GroupState* solo = nullptr;     // this layer alone on the conv-group kernel (implicit GEMM on tcgen05)
+    struct GroupState* solo = nullptr;     // this layer alone on the conv-group kernel (implicit GEMM on wgmma)
     const void* solo_x = nullptr;
     const void* solo_y = nullptr;
     ~ConvInt8Exec() override;
@@ -178,7 +178,7 @@ struct ConvInt8Exec : mnnb200_exec {
     ConvParams p;
     int tile = TILE_128x64;
     bool resized = false;
-    // tcgen05 path (1x1, stride 1, no pad): A = activation [M][Cp], B = weights [OCp][Cp]
+    // wgmma path (1x1, stride 1, no pad): A = activation [M][Cp], B = weights [OCp][Cp]
     bool gemm_ok = false;
     int bn = 0;
     CUtensorMap tmap_b;
@@ -186,9 +186,9 @@ struct ConvInt8Exec : mnnb200_exec {
     const void* tmap_a_ptr = nullptr;
 };
 
-static bool tcgen05_default() {
+static bool tensor_core_default() {
     static int v = -1;
-    if (v < 0) { const char* e = getenv("MNNB200_TCGEN05"); v = e ? atoi(e) : 1; }
+    if (v < 0) { const char* e = getenv("MNNB200_WGMMA"); v = e ? atoi(e) : 1; }
     return v != 0;
 }
 
@@ -231,7 +231,7 @@ static mnnb200_status conv_create_common(mnnb200_runtime* rt, const mnnb200_conv
     return MNNB200_OK;
 }
 
-// ---- conv group: one persistent launch over a list of convolutions (conv_group_tcgen05.cu) ----------------------------
+// ---- conv group: one persistent launch over a list of convolutions (conv_group_wgmma.cu) ----------------------------
 struct GroupState {
     mnnb200_runtime* rt = nullptr;
     GroupMapsParam* h_maps = nullptr;       // host: passed by value as the kernel's __grid_constant__ parameter
@@ -273,7 +273,7 @@ static int conv_group_mode(const ConvInt8Exec* e) {
 static mnnb200_status group_setup_layer(GroupState& gs, ConvInt8Exec* e, const int8_t* x, int8_t* y, int bn_override,
                                         GroupLayerMaps& mp, GroupLayerParams& q, GroupConvGeom& g, double* load_bytes, double* mma_ns) {
     const int mode = conv_group_mode(e);
-    if (mode < 0) return fail(MNNB200_NOT_SUPPORT, "conv group: a member is not a resized conv the tcgen05 group kernel takes");
+    if (mode < 0) return fail(MNNB200_NOT_SUPPORT, "conv group: a member is not a resized conv the wgmma group kernel takes");
     const ConvParams& p = e->p;
     int chunks = (e->OCp + kGroupMaxBN - 1) / kGroupMaxBN;
     int bn = ((e->OCp + chunks - 1) / chunks + 15) & ~15;
@@ -521,9 +521,9 @@ mnnb200_status mnnb200_runtime_create(int device_id, void* stream, mnnb200_runti
     auto* rt = new mnnb200_runtime;
     rt->device = device_id;
     CK(cudaGetDeviceProperties(&rt->prop, device_id));
-    if (rt->prop.major < 10) {
+    if (rt->prop.major != 9) {
         delete rt;
-        return fail(MNNB200_NOT_SUPPORT, "mnn_b200 is built for sm_100a only");
+        return fail(MNNB200_NOT_SUPPORT, "mnn_b200 is built for sm_90a (H100) only");
     }
     if (stream) {
         rt->stream = (cudaStream_t)stream;
@@ -916,8 +916,8 @@ mnnb200_status mnnb200_conv_int8_execute(mnnb200_exec* ex, const int8_t* x, int8
     ConvParams p = e->p;
     p.x = x;
     p.y = y;
-    if (e->variant == 2 && !e->gemm_ok && conv_group_mode(e) != 1) return fail(MNNB200_NOT_SUPPORT, "tcgen05 variant: this conv shape is not taken by the implicit-GEMM kernel (stride_w > 2?)");
-    const bool use_gemm = e->gemm_ok && (e->variant == 2 || (e->variant == 0 && tcgen05_default()));
+    if (e->variant == 2 && !e->gemm_ok && conv_group_mode(e) != 1) return fail(MNNB200_NOT_SUPPORT, "wgmma variant: this conv shape is not taken by the implicit-GEMM kernel (stride_w > 2?)");
+    const bool use_gemm = e->gemm_ok && (e->variant == 2 || (e->variant == 0 && tensor_core_default()));
     if (use_gemm) {
         if (e->tmap_a_ptr != (const void*)x) {
             mnnb200_status st = make_tmap_i8(&e->tmap_a, x, p.M, e->Cp, 128);
@@ -929,7 +929,7 @@ mnnb200_status mnnb200_conv_int8_execute(mnnb200_exec* ex, const int8_t* x, int8
         g.a = x; g.b = e->d_w; g.M = p.M; g.N = e->OCp; g.K = e->Cp;
         g.y_i8 = y; g.ldy = e->OCp; g.wscale = e->d_wscale; g.bias = e->d_bias; g.wsum128 = e->d_wsum128;
         g.scale_x = p.scale_x; g.minv = p.minv; g.maxv = p.maxv; g.OC = e->d.oc;
-        CK(launch_gemm_i8_tcgen05(g, &e->tmap_a, &e->tmap_b, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
+        CK(launch_gemm_i8_wgmma(g, &e->tmap_a, &e->tmap_b, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
         return MNNB200_OK;
     }
     static const int stem_default = [] { const char* v = getenv("MNNB200_STEM"); return v ? atoi(v) : 1; }();
@@ -938,10 +938,10 @@ mnnb200_status mnnb200_conv_int8_execute(mnnb200_exec* ex, const int8_t* x, int8
         CK(launch_conv_int8_stem(p, e->rt->stream));
         return MNNB200_OK;
     }
-    // k > 1 / strided / dilated convs: implicit GEMM on tcgen05 (this layer alone on the conv-group kernel).  variant 0 = auto,
+    // k > 1 / strided / dilated convs: implicit GEMM on wgmma (this layer alone on the conv-group kernel).  variant 0 = auto,
     // 2 = forced; variant 1 keeps the mma.sync kernel.  MNNB200_IGEMM=0 turns the auto selection off.
     static const int igemm_default = [] { const char* v = getenv("MNNB200_IGEMM"); return v ? atoi(v) : 1; }();
-    if (!e->gemm_ok && (e->variant == 2 || (e->variant == 0 && igemm_default && tcgen05_default())) && conv_group_mode(e) == 1) {
+    if (!e->gemm_ok && (e->variant == 2 || (e->variant == 0 && igemm_default && tensor_core_default())) && conv_group_mode(e) == 1) {
         if (!e->solo || e->solo_x != (const void*)x || e->solo_y != (const void*)y) {
             if (!e->solo) { e->solo = new GroupState; e->solo->rt = e->rt; }
             else CK(cudaStreamSynchronize(e->rt->stream));
@@ -1189,7 +1189,7 @@ mnnb200_status mnnb200_linear_w8_resize(mnnb200_exec* ex, int tokens) {
     mnnb200_status st;
     if ((st = make_tmap_i8(&e->tmap_a, e->d_xq, tokens, e->icp, 128))) return st;
     if ((st = make_tmap_i8(&e->tmap_b, e->d_w, e->ocp, e->icp, e->bn))) return st;
-    // tensor-bound shapes run on CTA pairs (UMMA M = 256): needs >= 256 rows and a B tile that splits into two halves
+    // tensor-bound shapes run on CTA pairs (2-CTA cluster, 256 rows): needs >= 256 rows and a B tile that splits into two halves
     e->bn2 = 0;
     if (tokens >= 256 && e->ocp >= 64) {
         int chunks = (e->ocp + 255) / 256;
@@ -1224,7 +1224,7 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
     }
     CK(launch_dynamic_quant(x, e->tokens, e->ic, e->icp, e->d_xq, e->d_dq, e->d_srcsum, e->rt->stream));
     if (e->variant == 3 && !e->bn2) return fail(MNNB200_NOT_SUPPORT, "the CTA-pair variant needs >= 256 tokens and >= 64 output channels");
-    if (e->variant == 2 || e->variant == 3 || (e->variant == 0 && tcgen05_default())) {
+    if (e->variant == 2 || e->variant == 3 || (e->variant == 0 && tensor_core_default())) {
         GemmI8Params g;
         memset(&g, 0, sizeof(g));
         g.a = e->d_xq; g.b = e->d_w; g.M = e->tokens; g.N = e->ocp; g.K = e->icp;
@@ -1236,7 +1236,7 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
             CK(launch_gemm_i8_2cta(g, &e->tmap_a, &e->tmap_b_half, e->bn2, e->rt->stream, e->rt->prop.multiProcessorCount));
             return MNNB200_OK;
         }
-        CK(launch_gemm_i8_tcgen05(g, &e->tmap_a, &e->tmap_b, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
+        CK(launch_gemm_i8_wgmma(g, &e->tmap_a, &e->tmap_b, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
         return MNNB200_OK;
     }
     CK(launch_conv_int8_igemm(p, e->tile, e->rt->stream));
@@ -1248,7 +1248,7 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
 // Int8 Winograd conv (SURVEY a5/a6): host side = ConvInt8Winograd::makeWinoResource + onResize
 // (source/backend/cpu/compute/ConvInt8Winograd.cpp:25-126, 183-241) -- float weight transform G (w_q * wscale) G^T,
 // per-(position, oc) requantisation, scale/offset tables -- then three enqueues per execute:
-// input transform -> alpha^2 batched tcgen05 int8 GEMMs -> output transform + requantise.
+// input transform -> alpha^2 batched wgmma int8 GEMMs -> output transform + requantise.
 // =================================================================================================
 struct WinoConvInt8Exec : mnnb200_exec {
     mnnb200_conv_desc d;
@@ -1262,7 +1262,7 @@ struct WinoConvInt8Exec : mnnb200_exec {
     float* d_m = nullptr;
     size_t v_bytes = 0, m_bytes = 0;
     WinoParams p;
-    CUtensorMap tmap_a, tmap_b, tmap_b32;   // tmap_b32: 32-row boxes of U for the fused F(2,3) kernel
+    CUtensorMap tmap_a, tmap_b, tmap_u_fused;   // tmap_u_fused: kWinoFusedBN-row boxes of U for the fused F(2,3) kernel
     bool resized = false;
 };
 
@@ -1420,7 +1420,7 @@ mnnb200_status mnnb200_conv_int8_wino_resize(mnnb200_exec* ex, int n, int ih, in
     p.v = e->d_v; p.m = e->d_m;
     if ((st = make_tmap_i8(&e->tmap_a, e->d_v, e->alpha2 * p.Mpad, e->Cp, 128))) return st;
     if ((st = make_tmap_i8(&e->tmap_b, e->d_u, e->alpha2 * e->OCb, e->Cp, e->bn))) return st;
-    if (e->unit == 2 && (st = make_tmap_i8(&e->tmap_b32, e->d_u, e->alpha2 * e->OCb, e->Cp, 32))) return st;
+    if (e->unit == 2 && (st = make_tmap_i8(&e->tmap_u_fused, e->d_u, e->alpha2 * e->OCb, e->Cp, kWinoFusedBN))) return st;
     // algorithmic bytes / MACs in direct-conv terms (SURVEY 8d C3): int8 in + out + weights once; MACs of the direct form
     e->cost_bytes = (double)n * ih * iw * d.ic + (double)n * OH * OW * d.oc + (double)d.oc * d.ic * 9;
     e->cost_macs = (double)n * OH * OW * d.oc * d.ic * 9;
@@ -1448,16 +1448,16 @@ mnnb200_status mnnb200_conv_int8_wino_execute_phases(mnnb200_exec* ex, const int
     WinoParams p = e->p;
     p.x = x; p.y = y;
     if (phases & 1) CK(launch_wino_input(p, e->rt->stream));
-    // F(2,3): position GEMMs + output transform fused (16 accumulators resident in TMEM, no fp32 M round trip); the three-
+    // F(2,3): position GEMMs + output transform fused (16 accumulators resident in registers, no fp32 M round trip); the three-
     // kernel form stays selectable (MNNB200_WINO_FUSED=0, or a single phase bit for per-kernel timing)
     static const int fused_default = [] { const char* v = getenv("MNNB200_WINO_FUSED"); return v ? atoi(v) : 1; }();
     if (e->unit == 2 && fused_default && (phases & 6) == 6) {
         WinoFusedParams f;
         f.y = y; f.scale = e->d_scale; f.offset = e->d_offset; f.fused_bias = e->d_fused; f.wsum128 = e->d_wsum128;
         f.K = e->Cp; f.Mpad = p.Mpad; f.OCb = e->OCb; f.OCp = e->OCp; f.OC = e->d.oc;
-        f.m_tiles = p.Mpad / 128; f.oc_chunks = (e->OCp + 31) / 32; f.OH = p.OH; f.OW = p.OW; f.hU = p.hU; f.wU = p.wU; f.T = p.T;
+        f.m_tiles = p.Mpad / 128; f.oc_chunks = (e->OCp + kWinoFusedBN - 1) / kWinoFusedBN; f.OH = p.OH; f.OW = p.OW; f.hU = p.hU; f.wU = p.wU; f.T = p.T;
         f.out_inv = p.out_inv; f.minv = p.minv; f.maxv = p.maxv;
-        CK(launch_wino_f23_fused(f, &e->tmap_a, &e->tmap_b32, e->rt->stream, e->rt->prop.multiProcessorCount));
+        CK(launch_wino_f23_fused(f, &e->tmap_a, &e->tmap_u_fused, e->rt->stream, e->rt->prop.multiProcessorCount));
         return MNNB200_OK;
     }
     if (!(phases & 2)) {
@@ -1469,7 +1469,7 @@ mnnb200_status mnnb200_conv_int8_wino_execute_phases(mnnb200_exec* ex, const int
     g.a = e->d_v; g.b = e->d_u; g.M = (int)p.T; g.N = e->OCp; g.K = e->Cp;
     g.y_f32 = e->d_m; g.ldy = e->OCp; g.wscale = e->d_scale; g.bias = e->d_offset; g.wsum128 = e->d_wsum128; g.OC = e->d.oc;
     g.batch = e->alpha2; g.a_batch_rows = p.Mpad; g.b_batch_rows = e->OCb; g.c_batch_stride = e->OCp; g.wino = 1;
-    CK(launch_gemm_i8_tcgen05(g, &e->tmap_a, &e->tmap_b, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
+    CK(launch_gemm_i8_wgmma(g, &e->tmap_a, &e->tmap_b, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
     if (phases & 4) CK(launch_wino_output(p, e->rt->stream));
     return MNNB200_OK;
 }
@@ -1481,7 +1481,7 @@ mnnb200_status mnnb200_conv_int8_wino_execute_phases(mnnb200_exec* ex, const int
 // =================================================================================================
 struct MatMulExec : mnnb200_exec {
     int batch = 0, e = 0, l = 0, h = 0, lp = 0, ta = 0, tb = 0, in_f16 = 0, bn = 0;
-    int tf32 = 0, esize = 2;               // tf32: fp32 operands consumed by kind::tf32 (no conversion pass); else fp16 operands
+    int tf32 = 0, esize = 2;               // tf32: fp32 operands consumed as tf32 (no conversion pass); else fp16 operands
     void *d_a = nullptr, *d_b = nullptr;   // K-major scratch operands [batch][e][lp], [batch][h][lp] (only when a pack is needed)
     CUtensorMap tmap_a, tmap_b;
     const void *tmap_a_ptr = nullptr, *tmap_b_ptr = nullptr;
@@ -1494,8 +1494,8 @@ mnnb200_status mnnb200_matmul_create(mnnb200_runtime* rt, int batch, int e, int 
     auto* m = new MatMulExec;
     m->rt = rt; m->kind = 5; m->batch = batch; m->e = e; m->l = l; m->h = h; m->ta = transpose_a; m->tb = transpose_b;
     m->in_f16 = inputs_are_f16;
-    // fp32 operands: kind::tf32 reads them in place (K-major operands need no pass at all); MNNB200_MATMUL_TF32=0 forces the
-    // convert-to-fp16 path (kind::f16, twice the MMA rate, one extra pass over both operands)
+    // fp32 operands: tf32 wgmma reads them in place (K-major operands need no pass at all); MNNB200_MATMUL_TF32=0 forces the
+    // convert-to-fp16 path (f16 wgmma, twice the MMA rate, one extra pass over both operands)
     static const int tf32_default = [] { const char* v = getenv("MNNB200_MATMUL_TF32"); return v ? atoi(v) : 1; }();
     m->tf32 = (!inputs_are_f16 && tf32_default) ? 1 : 0;
     m->esize = m->tf32 ? 4 : 2;
@@ -1547,7 +1547,7 @@ mnnb200_status mnnb200_matmul_execute(mnnb200_exec* ex, const void* a, const voi
         if ((st = make_tmap_i8(&m->tmap_b, pb, m->batch * m->h + (b_direct ? 0 : 256), (int)row_bytes, m->bn))) return st;
         m->tmap_b_ptr = pb;
     }
-    CK(launch_gemm_f16_tcgen05(&m->tmap_a, &m->tmap_b, m->batch, m->e, m->h, (int)row_bytes, m->tf32, m->e, m->h, m->bn, c, bias,
+    CK(launch_gemm_f16_wgmma(&m->tmap_a, &m->tmap_b, m->batch, m->e, m->h, (int)row_bytes, m->tf32, m->e, m->h, m->bn, c, bias,
                                m->rt->stream, m->rt->prop.multiProcessorCount));
     return MNNB200_OK;
 }
@@ -1555,7 +1555,7 @@ mnnb200_status mnnb200_matmul_execute(mnnb200_exec* ex, const void* a, const voi
 
 // =================================================================================================
 // Whole-net program: a chain of DEPENDENT int8 ops (convs of both modes, depthwise convs, eltwise adds) in ONE cooperative launch
-// of the conv-group kernel's program mode (conv_group_tcgen05.cu, kernels.h ProgItem).  Replaces the structure of
+// of the conv-group kernel's program mode (conv_group_wgmma.cu, kernels.h ProgItem).  Replaces the structure of
 // Pipeline::execute's op-by-op walk (source/core/Pipeline.cpp:1167-1211) for such a run of commands; each op's arithmetic is its
 // own execution's (nothing changes numerically).  Dependencies are derived from the tensors' device addresses:
 //   RAW  per item: the producer tiles that cover the item's input pixel range (per-tile progress flags);
@@ -1609,7 +1609,7 @@ mnnb200_status mnnb200_net_program_add_conv(mnnb200_exec* prog, mnnb200_exec* co
     NetProgramExec::OpRec r;
     if (conv->kind == 1) {
         auto* e = static_cast<ConvInt8Exec*>(conv);
-        if (conv_group_mode(e) < 0) return fail(MNNB200_NOT_SUPPORT, "net_program_add_conv: conv not taken by the tcgen05 kernels");
+        if (conv_group_mode(e) < 0) return fail(MNNB200_NOT_SUPPORT, "net_program_add_conv: conv not taken by the wgmma kernels");
         r.type = 0; r.conv = e;
         r.in0_bytes = (size_t)e->p.N * e->p.IH * e->p.IW * e->Cp;
         r.out_bytes = (size_t)e->p.M * e->OCp;

@@ -1,4 +1,4 @@
-// common.cuh -- small device helpers shared by the sm_100a kernels.
+// common.cuh -- small device helpers shared by the sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

@@ -1,0 +1,544 @@
+// conv_group_wgmma.cu -- ONE persistent launch for a whole LIST of int8 convolutions.
+//
+// One launch per 1x1 convolution pays the launch -> barrier init -> cold TMA -> epilogue -> teardown chain for a few MB of
+// traffic per layer.  Here the per-layer state (TMA descriptors + epilogue constants) lives in a device-side layer table
+// and the tiles of ALL layers form one host-built schedule dealt round-robin to the CTAs (every CTA, one per SM, gets the
+// same mix of layers), so barriers are set up once per step, the TMA producer runs ahead across layer boundaries (the next
+// layer's operands are already in flight while the current tile's epilogue drains) and there is no per-layer tail.
+//
+// Replaces (structure) the per-op Execution::onExecute walk of Pipeline::execute (source/core/Pipeline.cpp:1069-1140)
+// over ConvInt8CutlassExecution::onExecute (source/backend/cuda/execution/int8/ConvInt8CutlassExecution.cu:381-445)
+// for runs of int8 convolutions; arithmetic = the CPU backend's (see gemm_i8_wgmma.cu / common.cuh).
+//
+// Layer modes (kernels.h): 0 = GEMM-shaped 1x1 conv (A is the activation itself); 1 = implicit GEMM for any kernel size /
+// stride <= 2 / dilation / padding: the A tile of a K block (tap, channel chunk) is gathered by R TMA boxes of BH output rows x
+// TWp pixels from a 4D {C, W, H, N} view of the input -- no im2col buffer (the reference writes and re-reads one:
+// Im2Col_packC_16, ConvInt8CutlassExecution.cu:16-68), out-of-image taps are zero-filled by the TMA unit and, when the input
+// zero point is not 0, put back in the epilogue as z_in * sum_{OOB taps} w from a small per-border-class table.
+//
+// Weight tiles are CACHED in shared memory across work items (4 slots tagged (layer, n chunk, K block) + a 36 KB resident set
+// for layers whose K blocks all fit): with round-robin scheduling all CTAs work on the same layer at the same time, and
+// re-fetching the same few weight lines for every item from every SM serialises in L2.
+//
+//   warp 8:    TMA producer (cp.async.bulk.tensor.2d/4d, 128B / 64B swizzle or 16-byte interleaved chunks, 6-stage ring of
+//              16 KB activation tiles)
+//   warps 0-7: two consumer warpgroups, 64 rows of the 128-row tile each: wgmma.mma_async m64nNk32 s8 (N = bn <= 128,
+//              accumulators in registers) -> CPU-exact requant -> stores straight to the NHWC16 output rows; per-column
+//              constants staged in shared memory per (layer, n chunk)
+// PROG = true adds dependency flags between tiles and SIMT ops on the consumer warps (whole-net program, opt-in).
+#include <cuda.h>
+#include <cstdlib>
+#include "common.cuh"
+#include "hopper_common.cuh"
+#include "host_util.h"
+#include "kernels.h"
+#include "simt_ops.cuh"
+
+namespace mnnb200 {
+
+namespace {
+using namespace hop;
+
+constexpr int kBM = 128;
+constexpr int kBK = 128;                          // bytes of K per stage (one 128B swizzle row)
+constexpr int kStages = 6;                        // activation-tile ring
+constexpr int kMaxBN = kGroupMaxBN;               // 128
+constexpr int kStageA = kBM * kBK;                // 16 KB
+constexpr int kStageB = kMaxBN * kBK;             // 16 KB
+constexpr int kStageBytes = kStageA;               // the stage ring holds ACTIVATION tiles only
+constexpr int kBSlots = 4;                        // weight-tile cache: (layer, n chunk, K block) -> slot
+constexpr int kOffB = kStages * kStageA;
+constexpr int kConstBytes = 3 * kMaxBN * 4;       // wscale, bias, wsum128 per column
+
+constexpr int kOffResident = kOffB + kBSlots * kStageB;  // the RESIDENT weight set
+constexpr int kResidentBytes = 36 * 1024;
+static_assert(kOffResident % 1024 == 0, "resident weight tiles need 1 KB alignment");
+constexpr int kOffConsts = kOffResident + kResidentBytes;
+constexpr int kOffLayers = kOffConsts + kConstBytes;
+constexpr int kOffRbTab = kOffLayers + kGroupMaxLayers * (int)sizeof(GroupLayerParams);   // producer: [3][16] row-box coordinates
+constexpr int kOffBSlot = kOffRbTab + 3 * 16 * 4;                                          // [kStages] weight slot of the block in each stage
+constexpr int kOffBars = kOffBSlot + 32;                                                   // (kStages ints, padded)
+constexpr int kSmemTotal = kOffBars + 256;
+static_assert(kSmemTotal + 1024 <= 227 * 1024, "conv group kernel: shared memory plan does not fit");
+static_assert(sizeof(GroupLayerParams) % 16 == 0, "layer params are copied with 16-byte loads");
+
+// requant_cpu_exact (common.cuh) with the +-0.5 select done as copysign(0.5, f): one LOP3, identical result
+__device__ __forceinline__ int requant_fast(int acc_u, float wscale, float scale_x, float bias_float, float minv, float maxv) {
+    float f = __fmul_rn(__int2float_rn(acc_u), wscale);
+    f = __fmul_rn(f, scale_x);
+    f = __fadd_rn(f, bias_float);
+    f = fminf(f, maxv);
+    f = fmaxf(f, minv);
+    float h = __int_as_float((__float_as_int(f) & 0x80000000) | 0x3f000000);
+    return __float2int_rz(__fadd_rn(f, h));
+}
+// the same sequence for accumulators with |acc_u| < 2^22: float(acc_u) = as_float(0x4B400000 + acc_u) - 1.5 * 2^23 is exact (the
+// integer lands in the mantissa of a float in [2^23, 2^24)): one IADD + one FADD instead of an I2F on the conversion unit
+__device__ __forceinline__ int requant_fast_small(int acc_u, float wscale, float scale_x, float bias_float, float minv, float maxv) {
+    float f = __fmul_rn(__fsub_rn(__int_as_float(0x4B400000 + acc_u), 12582912.0f), wscale);
+    f = __fmul_rn(f, scale_x);
+    f = __fadd_rn(f, bias_float);
+    f = fminf(f, maxv);
+    f = fmaxf(f, minv);
+    float h = __int_as_float((__float_as_int(f) & 0x80000000) | 0x3f000000);
+    return __float2int_rz(__fadd_rn(f, h));
+}
+
+// ---- program mode: progress flags in global memory (acquire loads / release adds at gpu scope)
+__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
+    int v;
+    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
+    return v;
+}
+__device__ __forceinline__ void red_release_gpu(int* p, int v) {
+    asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
+}
+// bounded like the mbarrier waits: a dependency that never arrives traps the kernel instead of wedging the GPU
+__device__ __forceinline__ void wait_flag_ge(const int* p, int target) {
+    long long t0 = 0;
+    uint32_t spins = 0;
+    while (ld_acquire_gpu(p) < target) {
+        __nanosleep(64);
+        if ((++spins & 0x3fffu) == 0) {
+            const long long now = clock64();
+            if (t0 == 0) t0 = now;
+            else if (now - t0 > 8000000000ll) __trap();
+        }
+    }
+}
+
+// work item = `cnt` consecutive M tiles of one (layer, n chunk): layer << 26 | n chunk << 20 | (cnt - 1) << 14 | first m tile.
+// The producer pays its per-item bookkeeping (schedule word, layer parameters, descriptors, dependency waits) once per item.
+__device__ __forceinline__ void decode_item(uint32_t w, int& layer, int& nc, int& mt, int& cnt) {
+    layer = (int)(w >> 26);
+    nc = (int)((w >> 20) & 0x3fu);
+    cnt = (int)((w >> 14) & 0x3fu) + 1;
+    mt = (int)(w & 0x3fffu);
+}
+
+// PROG = false: conv group (independent layers, items = 32-bit words of `sched`).
+// PROG = true : whole-net program (items = ProgItem records with dependencies; SIMT ops on the consumer warps).
+template <bool PROG>
+__global__ void __launch_bounds__(kThreads, 1)
+conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLayerParams* __restrict__ params,
+                        const GroupConvGeom* __restrict__ geom, int n_layers, const uint32_t* __restrict__ sched, int sched_stride,
+                        const ProgItem* __restrict__ items, const ProgOpWar* __restrict__ war, const ProgSimtOp* __restrict__ simt,
+                        int* __restrict__ flags, int* __restrict__ opdone) {
+    extern __shared__ __align__(1024) uint8_t smem_raw[];
+    const uint32_t raw = smem_u32(smem_raw);
+    const uint32_t base = (raw + 1023u) & ~1023u;
+    uint8_t* smem = smem_raw + (base - raw);
+
+    const uint32_t bar0 = base + kOffBars;
+    auto full_bar = [&](int s) { return bar0 + 8u * s; };
+    auto empty_bar = [&](int s) { return bar0 + 8u * (kStages + s); };
+    const GroupLayerParams* sl = reinterpret_cast<const GroupLayerParams*>(smem + kOffLayers);
+    const uint32_t* my = PROG ? nullptr : sched + (size_t)blockIdx.x * sched_stride;
+    const ProgItem* myp = PROG ? items + (size_t)blockIdx.x * sched_stride : nullptr;
+    auto item_word = [&](int i) -> uint32_t { return PROG ? myp[i].w0 : my[i]; };
+
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+
+    // layer table -> smem (read by every role for every item)
+    {
+        const int4* src = reinterpret_cast<const int4*>(params);
+        int4* dst = reinterpret_cast<int4*>(smem + kOffLayers);
+        const int n16 = n_layers * (int)(sizeof(GroupLayerParams) / 16);
+        for (int i = threadIdx.x; i < n16; i += kThreads) dst[i] = src[i];
+    }
+    if (warp == 8 && lane == 0) {
+        for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }
+        asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
+    }
+    __syncthreads();
+
+    if (warp == 8) {
+        // ================= TMA producer =================
+        if (lane == 0) {
+            int stage = 0, phase = 0;
+            // weight-tile cache, all bookkeeping in registers (this thread's instruction count per K block is what bounds the kernel
+            // on short K loops; a shared-memory tag table measured 8-30 % slower):
+            //  * 4 slots of 16 KB tagged (layer, n chunk, K block), FIFO replacement: layers with <= 4 K blocks keep their weights
+            //    across the M tiles a CTA computes;
+            //  * one RESIDENT set in the 36 KB behind them for a layer whose K blocks ALL fit there although there are more than
+            //    four (3x3 x 64 channels: 9 tiles of 4 KB): tile kb lives at kb * tile bytes, loaded during the first M tile only --
+            //    without it such a layer reloads 4 KB per 7 KB activation block and runs 4 blocks deep instead of 6.
+            uint32_t btag0 = 0xffffffffu, btag1 = 0xffffffffu, btag2 = 0xffffffffu, btag3 = 0xffffffffu;
+            int buse0 = -1, buse1 = -1, buse2 = -1, buse3 = -1, bvictim = 0, blk = 0;
+            uint32_t res_key = 0xffffffffu;      // (layer, n chunk) owning the resident set
+            int res_loaded = 0, res_use = -1;    // K blocks of it already loaded; last block that read the set
+            volatile int* stage_bslot = reinterpret_cast<volatile int*>(smem + kOffBSlot);
+            // returns the byte offset (from kOffB) of the slot holding tile `key`; *miss = the tile has to be loaded into it
+            auto b_lookup = [&](uint32_t key, bool* miss) -> int {
+                *miss = false;
+                int slot;
+                if (key == btag0) slot = 0;
+                else if (key == btag1) slot = 1;
+                else if (key == btag2) slot = 2;
+                else if (key == btag3) slot = 3;
+                else {
+                    *miss = true;
+                    slot = bvictim;
+                    bvictim = (bvictim + 1) & 3;
+                    const int u = slot == 0 ? buse0 : (slot == 1 ? buse1 : (slot == 2 ? buse2 : buse3));
+                    // the MMAs of block u read the old tile: wait until that block's stage was released (blocks <= blk - kStages
+                    // are known to be: this thread waited on their empty barriers when it reused their stages)
+                    if (u >= 0 && u > blk - kStages) mbar_wait(empty_bar(u % kStages), (uint32_t)((u / kStages) & 1));
+                    if (slot == 0) btag0 = key; else if (slot == 1) btag1 = key; else if (slot == 2) btag2 = key; else btag3 = key;
+                }
+                if (slot == 0) buse0 = blk; else if (slot == 1) buse1 = blk; else if (slot == 2) buse2 = blk; else buse3 = blk;
+                return slot * kStageB;
+            };
+            // the resident set: (layer, n chunk) `key`, K block kb, tile_bytes per K block
+            auto b_resident = [&](uint32_t key, int kb, int tile_bytes, bool* miss) -> int {
+                if (key != res_key) {
+                    if (res_use >= 0 && res_use > blk - kStages) mbar_wait(empty_bar(res_use % kStages), (uint32_t)((res_use / kStages) & 1));
+                    res_key = key;
+                    res_loaded = 0;
+                }
+                *miss = kb >= res_loaded;
+                if (*miss) res_loaded = kb + 1;
+                res_use = blk;
+                return kBSlots * kStageB + kb * tile_bytes;
+            };
+            for (int i = 0;; ++i) {
+                const uint32_t w = item_word(i);
+                if (w == kGroupSchedEnd) break;
+                int L, nc, mt0, cnt;
+                decode_item(w, L, nc, mt0, cnt);
+                const GroupLayerParams& lp = sl[L];
+                if (PROG) {
+                    if (lp.mode >= 2) continue;                      // SIMT op: the epilogue warps run it
+                    const ProgItem& it = myp[i];                    // RAW: the producer tiles covering this item's input
+                    for (int j = 0; j < it.dep0_count; ++j) wait_flag_ge(flags + it.dep0_first + j, it.dep0_need);
+                    asm volatile("fence.proxy.async;\n" ::: "memory");   // generic-proxy writes of other SMs -> this SM's TMA reads
+                }
+                const void* ta = &mp.a[L];
+                const void* tb = &mp.b[L];
+                if (lp.mode == 0) {
+                    const int num_kb = lp.num_kb, bn = lp.bn;
+                    const uint32_t key0 = ((uint32_t)L << 16) | ((uint32_t)nc << 8);
+                    for (int t = 0; t < cnt; ++t) {
+                        const int row0 = (mt0 + t) * kBM;
+                        for (int kb = 0; kb < num_kb; ++kb) {
+                            mbar_wait(empty_bar(stage), phase ^ 1);
+                            bool miss;
+                            const int bs = b_lookup(key0 | (uint32_t)kb, &miss);
+                            stage_bslot[stage] = bs;
+                            mbar_expect_tx(full_bar(stage), (uint32_t)(kStageA + (miss ? bn * kBK : 0)));
+                            const uint32_t a_dst = base + stage * kStageBytes;
+                            tma_load_2d(a_dst, ta, full_bar(stage), kb * kBK, row0);
+                            if (miss) tma_load_2d(base + kOffB + bs, tb, full_bar(stage), kb * kBK, nc * bn);
+                            if (++stage == kStages) { stage = 0; phase ^= 1; }
+                            ++blk;
+                        }
+                    }
+                    continue;
+                }
+                // ---- implicit GEMM: the tile's R output rows -> (image, first input row, first input column)
+                const GroupConvGeom& g = geom[L];
+                const int R = lp.R, TWp = lp.TWp, cb = lp.cb;
+                const int KW = g.KW, sw = g.sw, dh = g.dh, dw = g.dw, cpt = g.cpt, Cp = g.Cp;
+                const void* ta1 = &mp.a1[L];
+                int* rb_n = reinterpret_cast<int*>(smem + kOffRbTab);
+                int* rb_ih0 = rb_n + 16;
+                int* rb_iw0 = rb_n + 32;
+                for (int t = 0; t < cnt; ++t) {
+                const int mt = mt0 + t;
+                const int BH = g.BH, box_rows = BH * TWp;    // a box = BH output rows x TWp pixels
+                for (int j = 0; j < R; ++j) {
+                    const int rb = mt * R + j;
+                    int n = g.NB, oh = 0, seg = 0;          // n = NB: every coordinate of the box is out of bounds -> zeros
+                    if (rb < g.rowboxes) { seg = rb % g.SEG; const int t = rb / g.SEG; oh = (t % g.OHB) * BH; n = t / g.OHB; }
+                    rb_n[j] = n; rb_ih0[j] = oh * g.sh - g.ph; rb_iw0[j] = seg * TWp * sw - g.pw;
+                }
+                const int rows_bytes = R * box_rows;        // x cb = A bytes per chunk
+                if (cb >= 64) {
+                    // this loop runs on ONE thread, once per K block: everything that can be hoisted is (tap -> (kh, kw) by
+                    // counters, stride 1 / 2 parity by mask and shift, the first two boxes' coordinates in registers)
+                    int cc = 0, kh = 0, kw = 0, bk = 0;
+                    const int swm = sw - 1;                          // sw is 1 or 2 (conv_group_mode)
+                    const int n0 = rb_n[0], ih00 = rb_ih0[0], iw00 = rb_iw0[0];
+                    const int n1 = rb_n[1], ih01 = rb_ih0[1], iw01 = rb_iw0[1];
+                    const uint32_t key0 = ((uint32_t)L << 16) | ((uint32_t)nc << 8);
+                    const bool untagged = lp.num_kb > 256;           // such a layer gets tags no other block has: always a miss
+                    const uint32_t a_bytes = (uint32_t)(rows_bytes * cb), b_bytes = (uint32_t)(lp.bn * cb);
+                    const int brow = nc * lp.bn;
+                    // more than 4 K blocks, but all of them fit the resident set (tiles at 1 KB multiples: swizzle atoms stay aligned)
+                    const bool resident = lp.num_kb > kBSlots && (b_bytes & 1023u) == 0 && lp.num_kb * (int)b_bytes <= kResidentBytes;
+                    for (int kb = 0; kb < lp.num_kb; ++kb) {
+                        mbar_wait(empty_bar(stage), phase ^ 1);
+                        bool miss;
+                        const int bs = resident ? b_resident(key0, kb, (int)b_bytes, &miss)
+                                                : b_lookup(untagged ? (0x80000000u | (uint32_t)blk) : (key0 | (uint32_t)kb), &miss);
+                        stage_bslot[stage] = bs;
+                        mbar_expect_tx(full_bar(stage), a_bytes + (miss ? b_bytes : 0u));
+                        const uint32_t a_dst = base + stage * kStageBytes;
+                        const int dcol = kw * dw, drow = kh * dh, ccb = cc * cb;
+                        {
+                            const int iw = iw00 + dcol, par = iw & swm;
+                            tma_load_4d(a_dst, par ? ta1 : ta, full_bar(stage), ccb, (iw - par) >> swm, ih00 + drow, n0);
+                        }
+                        if (R > 1) {
+                            const int iw = iw01 + dcol, par = iw & swm;
+                            tma_load_4d(a_dst + box_rows * cb, par ? ta1 : ta, full_bar(stage), ccb, (iw - par) >> swm, ih01 + drow, n1);
+                        }
+                        for (int j = 2; j < R; ++j) {
+                            const int iw = rb_iw0[j] + dcol, par = iw & swm;
+                            tma_load_4d(a_dst + j * box_rows * cb, par ? ta1 : ta, full_bar(stage), ccb, (iw - par) >> swm,
+                                        rb_ih0[j] + drow, rb_n[j]);
+                        }
+                        if (miss) tma_load_2d(base + kOffB + bs, tb, full_bar(stage), bk, brow);
+                        bk += cb;
+                        if (++cc == cpt) { cc = 0; bk += Cp - cpt * cb; if (++kw == KW) { kw = 0; ++kh; } }
+                        if (++stage == kStages) { stage = 0; phase ^= 1; }
+                        ++blk;
+                    }
+                } else {
+                    // 16-byte chunks (Cp not a multiple of 64): up to 8 chunks (128 bytes of K) per stage, no swizzle
+                    const int taps = g.KH * KW;
+                    for (int kb = 0; kb < lp.num_kb; ++kb) {
+                        const int q0 = kb * 8;
+                        const int nq = (g.chunks - q0) < 8 ? (g.chunks - q0) : 8;
+                        mbar_wait(empty_bar(stage), phase ^ 1);
+                        bool miss;
+                        const int bs = b_lookup(lp.num_kb > 256 ? (0x80000000u | (uint32_t)blk)
+                                                                : (((uint32_t)L << 16) | ((uint32_t)nc << 8) | (uint32_t)kb), &miss);
+                        stage_bslot[stage] = bs;
+                        mbar_expect_tx(full_bar(stage), (uint32_t)(nq * (rows_bytes * 16 + (miss ? lp.bn * 16 : 0))));
+                        const uint32_t a_dst = base + stage * kStageBytes;
+                        for (int ql = 0; ql < nq; ++ql) {
+                            const int q = q0 + ql;
+                            const int tap = q / cpt, cc = q - tap * cpt;
+                            const bool dummy = tap >= taps;          // the padding chunk of an odd chunk count: zeros
+                            const int kh = tap / KW, kw = tap - kh * KW;
+                            for (int j = 0; j < R; ++j) {
+                                const int iw = rb_iw0[j] + kw * dw;
+                                int par = iw % sw; par = par < 0 ? par + sw : par;
+                                tma_load_4d(a_dst + ql * (kBM * 16) + j * box_rows * 16, par ? ta1 : ta, full_bar(stage), cc * 16,
+                                            (iw - par) / sw, rb_ih0[j] + kh * dh, dummy ? g.NB : rb_n[j]);
+                            }
+                            if (miss) tma_load_2d(base + kOffB + bs + ql * (lp.bn * 16), tb, full_bar(stage), q * 16, nc * lp.bn);
+                        }
+                        if (++stage == kStages) { stage = 0; phase ^= 1; }
+                        ++blk;
+                    }
+                }
+                }   // tiles of the item
+            }
+        }
+    } else {
+        // ================= two consumer warpgroups: wgmma main loop + epilogue =================
+        const int ct = threadIdx.x;                  // 0..255
+        const int wg = ct >> 7;                      // rows [64 wg, 64 wg + 64) of the tile
+        const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int q4 = lane & 3;
+        float* cst = reinterpret_cast<float*>(smem + kOffConsts);
+        const int* wsum = reinterpret_cast<const int*>(cst) + 2 * kMaxBN;
+        uint32_t cached = 0xffffffffu;            // (layer, n chunk) whose constants are in cst
+        int stage = 0, phase = 0;
+        int acc[kMaxBN / 2];
+#pragma unroll
+        for (int i = 0; i < kMaxBN / 2; ++i) acc[i] = 0;
+
+        for (int i = 0;; ++i) {
+            const uint32_t w = item_word(i);
+            if (w == kGroupSchedEnd) break;
+            int L, nc, mt0, cnt;
+            decode_item(w, L, nc, mt0, cnt);
+            const GroupLayerParams& lp = sl[L];
+            if (PROG && lp.mode >= 2) {
+                // ---- SIMT work item on the 256 consumer threads: wait for the inputs (RAW) and for the readers of a reused output
+                //      buffer (WAR), run the op's work indices, publish
+                const int mt = mt0;
+                const ProgItem& it = myp[i];
+                const ProgOpWar& wr = war[L];
+                if (ct == 0) {
+                    for (int j = 0; j < it.dep0_count; ++j) wait_flag_ge(flags + it.dep0_first + j, it.dep0_need);
+                    for (int j = 0; j < it.dep1_count; ++j) wait_flag_ge(flags + it.dep1_first + j, it.dep1_need);
+                    for (int j = 0; j < wr.n_war; ++j) wait_flag_ge(opdone + wr.war_op[j], wr.war_target[j]);
+                }
+                named_sync(2, kConsumerThreads);
+                const ProgSimtOp& so = simt[L];
+                if (lp.mode == 2) {
+                    const DwParams& dp = so.dw;
+                    const size_t wpr = dw_work_per_row(dp);
+                    const int r0 = mt * wr.rows_per_item;
+                    const int r1 = (r0 + wr.rows_per_item) < wr.total_rows ? (r0 + wr.rows_per_item) : wr.total_rows;
+                    const size_t i1 = (size_t)r1 * wpr;
+                    if (dw_is_3x3_fast(dp)) {
+                        if (dp.sh == 1) { for (size_t k = (size_t)r0 * wpr + ct; k < i1; k += kConsumerThreads) dwconv3x3_work<1, true>(dp, k); }
+                        else { for (size_t k = (size_t)r0 * wpr + ct; k < i1; k += kConsumerThreads) dwconv3x3_work<2, true>(dp, k); }
+                    } else {
+                        for (size_t k = (size_t)r0 * wpr + ct; k < i1; k += kConsumerThreads) dwconv_generic_work<true>(dp, k);
+                    }
+                } else {
+                    const AddParams& ap = so.add;
+                    const size_t c0 = (size_t)mt * wr.rows_per_item;
+                    const size_t c1 = (c0 + wr.rows_per_item) < ap.chunks ? (c0 + wr.rows_per_item) : ap.chunks;
+                    for (size_t k = c0 + ct; k < c1; k += kConsumerThreads) binary_add_work<true>(ap, k);
+                }
+                __threadfence();
+                named_sync(2, kConsumerThreads);
+                if (ct == 0) { red_release_gpu(flags + it.sig, 1); red_release_gpu(opdone + L, 1); }
+                continue;
+            }
+            const int bn = lp.bn, n0 = nc * bn, cb = lp.cb;
+            const int ncols = (lp.N - n0) < bn ? (lp.N - n0) : bn;      // valid (16-padded) columns of this chunk
+            const int nblk = ncols >> 3;
+            if ((w >> 20) != cached) {
+                // reload the per-column constants once every consumer is done READING the previous item's, then publish
+                named_sync(1, kConsumerThreads);
+                for (int j = ct; j < ncols; j += kConsumerThreads) {
+                    const int n = n0 + j;
+                    const bool v = n < lp.OC;
+                    cst[j] = v ? lp.wscale[n] : 0.f;
+                    cst[kMaxBN + j] = v ? lp.bias[n] : 0.f;
+                    reinterpret_cast<int*>(cst)[2 * kMaxBN + j] = v ? lp.wsum128[n] : 0;
+                }
+                named_sync(1, kConsumerThreads);
+                cached = w >> 20;
+            }
+            const float scale_x = lp.scale_x, minv = lp.minv, maxv = lp.maxv;
+            const bool small_acc = lp.K <= 128;    // |sum (x + 128) w| <= 128 * 255 * 128 < 2^22
+            for (int t = 0; t < cnt; ++t) {
+                const int mt = mt0 + t;
+                int prev = -1;
+                for (int kb = 0; kb < lp.num_kb; ++kb) {
+                    mbar_wait(full_bar(stage), phase);
+                    const uint32_t a_addr = base + stage * kStageBytes;
+                    const uint32_t b_addr = base + kOffB + (uint32_t)(*reinterpret_cast<volatile int*>(smem + kOffBSlot + 4 * stage));
+                    fence_acc(acc);
+                    wgmma_fence();
+                    if (cb == 128) {
+                        const int kleft = lp.K - kb * kBK;
+                        const int nmma = (lp.mode != 0 || kleft >= kBK) ? 4 : (kleft + 31) / 32;
+                        for (int k = 0; k < nmma; ++k)
+                            wgmma_bn<Kind::S8, kMaxBN>(acc, bn, gdesc_sw128(a_addr + wg * 64 * 128 + k * 32), gdesc_sw128(b_addr + k * 32), 128,
+                                                       (kb | k) != 0);
+                    } else if (cb == 64) {
+                        for (int k = 0; k < 2; ++k)
+                            wgmma_bn<Kind::S8, kMaxBN>(acc, bn, gdesc(a_addr + wg * 64 * 64 + k * 32, kSw64, 16, 512),
+                                                       gdesc(b_addr + k * 32, kSw64, 16, 512), 64, (kb | k) != 0);
+                    } else {
+                        const int nq = (lp.K / 16 - kb * 8) < 8 ? (lp.K / 16 - kb * 8) : 8;     // K = 16 * chunks (even)
+                        for (int u = 0; u < (nq >> 1); ++u)
+                            wgmma_bn<Kind::S8, kMaxBN>(acc, bn, gdesc(a_addr + 2 * u * (kBM * 16) + wg * 64 * 16, kSwNone, kBM * 16, 128),
+                                                       gdesc(b_addr + 2 * u * (bn * 16), kSwNone, bn * 16, 128), 16, (kb | u) != 0);
+                    }
+                    wgmma_commit();
+                    wgmma_wait<1>();                 // the previous stage's MMAs are done: hand its slot back
+                    fence_acc(acc);
+                    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(prev)); }
+                    prev = stage;
+                    if (++stage == kStages) { stage = 0; phase ^= 1; }
+                }
+                wgmma_wait<0>();
+                fence_acc(acc);
+                __syncwarp();
+                if (lane == 0) mbar_arrive(empty_bar(prev));
+
+                if (PROG) {      // WAR before this warp's stores: readers (or the previous writer) of a reused buffer are done
+                    if (lane == 0) {
+                        const ProgOpWar& wr = war[L];
+                        for (int j = 0; j < wr.n_war; ++j) wait_flag_ge(opdone + wr.war_op[j], wr.war_target[j]);
+                    }
+                    __syncwarp();
+                }
+                // ---- epilogue from the accumulator fragments: register i = row r_base + 8 * ((i >> 1) & 1),
+                //      column 8 * (i >> 2) + 2 * q4 + (i & 1); two output bytes per store
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {
+                    const int r = r_base + 8 * h;
+                    int8_t* yrow = nullptr;
+                    const int32_t* corrp = nullptr;    // border pixel of a padded conv with z_in != 0: + z_in * sum_{OOB taps} w
+                    if (lp.mode == 0) {
+                        if (mt * kBM + r < lp.M) yrow = lp.y + (size_t)(mt * kBM + r) * lp.ldy + n0;
+                    } else {
+                        // implicit-GEMM layers: which output pixel accumulator row r is, and its border class
+                        const GroupConvGeom& g = geom[L];
+                        const int box_rows = g.BH * lp.TWp;
+                        const int j = r / box_rows, rem = r - j * box_rows;
+                        const int brow = rem / lp.TWp, pcol = rem - brow * lp.TWp;
+                        const int rb = mt * lp.R + j;
+                        if (j < lp.R && rb < g.rowboxes) {
+                            const int seg = rb % g.SEG, tt = rb / g.SEG;
+                            const int oh = (tt % g.OHB) * g.BH + brow, n = tt / g.OHB;
+                            const int ow = seg * lp.TWp + pcol;
+                            if (ow < g.OW) {
+                                yrow = lp.y + (size_t)((n * g.OH + oh) * g.OW + ow) * lp.ldy + n0;
+                                if (g.corr != nullptr) {
+                                    const int cls = (int)g.hcls[oh] * g.wc_count + (int)g.wcls[ow];
+                                    if (cls != g.interior_cls) corrp = g.corr + (size_t)cls * lp.N + n0;
+                                }
+                            }
+                        }
+                    }
+                    if (yrow == nullptr) continue;
+#pragma unroll
+                    for (int j = 0; j < kMaxBN / 8; ++j) {
+                        if (j < nblk) {
+                            const int c = j * 8 + 2 * q4;
+                            int k0 = wsum[c], k1 = wsum[c + 1];
+                            if (corrp != nullptr) { k0 += __ldg(corrp + c); k1 += __ldg(corrp + c + 1); }
+                            const int a0 = acc[j * 4 + 2 * h] + k0, a1 = acc[j * 4 + 2 * h + 1] + k1;
+                            int q0, q1;
+                            if (small_acc) {      // |acc_u| < 2^22: int -> float on the FP32 pipe (exact), not on the conversion unit
+                                q0 = requant_fast_small(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
+                                q1 = requant_fast_small(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                            } else {
+                                q0 = requant_fast(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
+                                q1 = requant_fast(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                            }
+                            if (n0 + c >= lp.OC) q0 = 0;         // NHWC16 channel padding stays zero
+                            if (n0 + c + 1 >= lp.OC) q1 = 0;
+                            *reinterpret_cast<uint16_t*>(yrow + c) = (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8));
+                        }
+                    }
+                }
+                if (PROG) {
+                    __threadfence();   // this thread's output stores are visible gpu-wide before the flag below
+                    named_sync(2, kConsumerThreads);
+                    if (ct == 0) { red_release_gpu(flags + myp[i].sig + t, 1); red_release_gpu(opdone + L, 1); }
+                }
+            }   // tiles of the item
+        }
+    }
+}
+
+}  // namespace
+
+cudaError_t launch_conv_group(const GroupMapsParam* maps_host, const GroupLayerParams* params, const GroupConvGeom* geom, int n_layers,
+                              const uint32_t* sched, int sched_stride, int grid, cudaStream_t stream) {
+    cudaError_t e = ensure_max_dynamic_smem((const void*)conv_group_wgmma_kernel<false>, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    ++g_launch_count;
+    conv_group_wgmma_kernel<false><<<grid, kThreads, kSmemTotal + 1024, stream>>>(*maps_host, params, geom, n_layers, sched, sched_stride,
+                                                                                  nullptr, nullptr, nullptr, nullptr, nullptr);
+    return cudaGetLastError();
+}
+
+// The program kernel's CTAs wait on each other's progress flags: every CTA of the grid must be resident at once, which a
+// cooperative launch guarantees (it fails instead of deadlocking if the grid does not fit).
+cudaError_t launch_net_program(const GroupMapsParam* maps_host, const GroupLayerParams* params, const GroupConvGeom* geom, int n_ops,
+                               const ProgItem* items, int item_stride, const ProgOpWar* war, const ProgSimtOp* simt, int* flags,
+                               int* opdone, int grid, cudaStream_t stream) {
+    cudaError_t e = ensure_max_dynamic_smem((const void*)conv_group_wgmma_kernel<true>, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    ++g_launch_count;
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(kThreads);
+    cfg.dynamicSmemBytes = kSmemTotal + 1024;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeCooperative;
+    attr[0].val.cooperative = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = 1;
+    const uint32_t* no_sched = nullptr;
+    return cudaLaunchKernelEx(&cfg, conv_group_wgmma_kernel<true>, *maps_host, params, geom, n_ops, no_sched, item_stride, items, war, simt,
+                              flags, opdone);
+}
+
+}  // namespace mnnb200

@@ -1,4 +1,4 @@
-// kernels.h -- host-callable launchers of the sm_100a kernels (all enqueue-only on the given stream).
+// kernels.h -- host-callable launchers of the sm_90a kernels (all enqueue-only on the given stream).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -42,7 +42,7 @@ cudaError_t launch_conv_int8_igemm(const ConvParams& p, int tile, cudaStream_t s
 bool conv_int8_stem_supported(const ConvParams& p, int ic);
 cudaError_t launch_conv_int8_stem(const ConvParams& p, cudaStream_t stream);
 
-// tcgen05 (UMMA kind::i8, TMEM accumulators, TMA operand loads) GEMM for 1x1/stride-1 convs and linear layers
+// wgmma (s8 x s8 -> s32, register accumulators, TMA operand loads) GEMM for 1x1/stride-1 convs and linear layers
 struct GemmI8Params {
     const int8_t* a;  // [M][K]  row-major, K % 16 == 0
     const int8_t* b;  // [Nw][K] row-major ("column-major" B), zero padded rows
@@ -67,17 +67,16 @@ struct GemmI8Params {
     //   y = float(acc + wsum128[a][n]) * wscale[a][n] + bias[a][n]        (wino = 1)
     int batch, a_batch_rows, b_batch_rows, c_batch_stride, wino;
 };
-cudaError_t launch_gemm_i8_tcgen05(const GemmI8Params& p, const void* tmap_a, const void* tmap_b, int bn,
-                                   cudaStream_t stream, int sm_count);
-int gemm_i8_tcgen05_smem_bytes(int bn);
-// ---- one persistent launch over a LIST of int8 convolutions (conv_group_tcgen05.cu).  Two layer modes:
+cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& p, const void* tmap_a, const void* tmap_b, int bn, cudaStream_t stream,
+                                 int sm_count);
+// ---- one persistent launch over a LIST of int8 convolutions (conv_group_wgmma.cu).  Two layer modes:
 //   mode 0  GEMM-shaped (1x1, stride 1, no pad): A = the NHWC16 activation as a 2D matrix, one TMA box per K block
 //   mode 1  implicit GEMM (any kernel / stride <= 2 / dilation / padding): an M tile = R whole output rows of TWp pixels each; the
 //           A operand of K block (tap, channel chunk) is gathered by R TMA boxes from a 4D {C, W, H, N} view of the input
 //           (one view per column parity for stride 2); out-of-image taps are zero-filled by TMA and, for a non-zero input zero
 //           point, corrected in the epilogue with a per-(border class, oc) table  z_in * sum_{OOB taps} w
 constexpr int kGroupMaxLayers = 64;
-constexpr int kGroupMaxBN = 128;     // 4 accumulator stages x 128 TMEM columns
+constexpr int kGroupMaxBN = 128;     // 64 accumulator registers per consumer thread
 constexpr uint32_t kGroupSchedEnd = 0xffffffffu;
 struct alignas(64) GroupLayerMaps { CUtensorMap_st_opaque a, b, a1, pad_; };   // a1: odd-column view (stride 2, mode 1)
 // The TMA descriptors of ALL layers travel as ONE __grid_constant__ kernel parameter (24 KB of the 32 KB parameter space): a
@@ -130,19 +129,20 @@ cudaError_t launch_net_program(const GroupMapsParam* maps_host, const GroupLayer
                                const ProgItem* items, int item_stride, const ProgOpWar* war, const ProgSimtOp* simt, int* flags,
                                int* opdone, int grid, cudaStream_t stream);
 
-// CTA-pair variant (cta_group::2, UMMA M = 256) for the tensor-bound linear layers; fp32 dynamic-quant epilogue only.
-// tmap_b must have a box of bn/2 rows (each CTA of the pair loads half of the B tile); bn % 32 == 0.
+// CTA-pair variant (2-CTA cluster, 256 x bn per pair, B halves multicast to both CTAs) for the tensor-bound linear layers;
+// fp32 dynamic-quant epilogue only.  tmap_b must have a box of bn/2 rows (each CTA of the pair loads half of the B tile);
+// bn % 32 == 0.
 cudaError_t launch_gemm_i8_2cta(const GemmI8Params& p, const void* tmap_a, const void* tmap_b_half, int bn, cudaStream_t stream,
                                 int sm_count);
 
-// float (batched) MatMul on tcgen05 kind::f16 (gemm_f16_tcgen05.cu): operands packed to K-major fp16 first
+// float (batched) MatMul on wgmma f16 / tf32 (gemm_f16_wgmma.cu): operands packed to K-major fp16 first
 cudaError_t launch_pack_kmajor_f16(const void* src, int src_is_f16, void* dst, int batch, int rows, int k, int kp, int trans,
                                    cudaStream_t s);
 cudaError_t launch_pack_kmajor_f32(const float* src, float* dst, int batch, int rows, int k, int kp, int trans, cudaStream_t s);
-// k_bytes = bytes of one K-major operand row; tf32 = 1: operands are fp32 consumed as tf32 (kind::tf32), else fp16 (kind::f16)
-cudaError_t launch_gemm_f16_tcgen05(const void* tmap_a, const void* tmap_b, int batch, int M, int N, int k_bytes, int tf32,
-                                    int a_batch_rows, int b_batch_rows, int bn, float* c, const float* bias, cudaStream_t stream,
-                                    int sm_count);
+// k_bytes = bytes of one K-major operand row; tf32 = 1: operands are fp32 consumed as tf32, else fp16
+cudaError_t launch_gemm_f16_wgmma(const void* tmap_a, const void* tmap_b, int batch, int M, int N, int k_bytes, int tf32,
+                                  int a_batch_rows, int b_batch_rows, int bn, float* c, const float* bias, cudaStream_t stream,
+                                  int sm_count);
 
 // elementwise / data movement
 cudaError_t launch_float_to_int8(const float* x, int n, int c, int h, int w, float inv_scale, float zero, float minv,
@@ -186,7 +186,7 @@ cudaError_t launch_softmax_int8(const int8_t* x, int rows, int c, int cp, float 
                                 float minv, float maxv, int8_t* y, cudaStream_t s);
 
 // int8 Winograd F(m x m, 3 x 3) transform kernels (winograd_int8.cu); the alpha^2 position GEMMs run on the batched
-// tcgen05 GEMM above.  Scratch: v = [alpha^2][Mpad][Cp] int8, m = [alpha^2][Mpad][OCp] fp32, Mpad = T rounded up to 128.
+// wgmma GEMM above.  Scratch: v = [alpha^2][Mpad][Cp] int8, m = [alpha^2][Mpad][OCp] fp32, Mpad = T rounded up to 128.
 struct WinoParams {
     const int8_t* x;   // [N][IH][IW][Cp]
     int8_t* v;
@@ -202,7 +202,9 @@ struct WinoParams {
     float in_zero[64]; // inputZeroPoint[a]
 };
 cudaError_t launch_wino_input(const WinoParams& p, cudaStream_t s);
-// F(2,3): the 16 position GEMMs + output transform + requantise fused (all 16 accumulators resident in TMEM, no fp32 M tensor)
+// F(2,3): the 16 position GEMMs + output transform + requantise fused (all 16 accumulators in registers, no fp32 M tensor);
+// tmap_u has boxes of kWinoFusedBN rows
+constexpr int kWinoFusedBN = 8;
 struct WinoFusedParams {
     int8_t* y;
     const float *scale, *offset, *fused_bias;   // [16][OCp], [16][OCp], [OCp]

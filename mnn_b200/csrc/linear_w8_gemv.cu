@@ -6,7 +6,7 @@
 //     operation for operation; 8-22 KB of fp32 per token out of L2) into shared memory -- no separate quantise launch, no
 //     int8 activation round trip;
 //   * every warp streams R weight rows with 16-byte non-allocating loads (each weight byte is read exactly once: HBM-bound),
-//     dp4a into int32, butterfly reduce, then the SAME fp32 epilogue as gemm_i8_tcgen05's EPI 1 -- int32 sums are
+//     dp4a into int32, butterfly reduce, then the SAME fp32 epilogue as gemm_i8_wgmma's EPI 1 -- int32 sums are
 //     order-independent, so the result is bit-identical to the tensor-core path;
 //   * programmatic dependent launch: the first weight chunk is requested before griddepcontrol.wait, so the next layer's blocks
 //     are resident and loading while this layer drains (a decode step is ~120 dependent launches of 2-10 us each).
@@ -272,7 +272,7 @@ __global__ void __launch_bounds__(256) linear_w8_gemv_kernel(GemvW8Params p) {
                 int a = acc[t][r];
 #pragma unroll
                 for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-                // lane (t * R + r) finishes output (token t, row n0 + r): gemm_i8_tcgen05.cu EPI 1, operation for operation
+                // lane (t * R + r) finishes output (token t, row n0 + r): gemm_i8_wgmma.cu EPI 1, operation for operation
                 if (lane == t * R + r) {
                     const int n = n0 + r, m = t;
                     if (n < p.oc && m < p.tokens) {

@@ -1,6 +1,6 @@
 // simt_ops.cuh -- the per-work-index bodies of the HBM-bound int8 neighbours of the conv path (depthwise conv, eltwise add) as
 // device functions, shared by the stand-alone kernels (elementwise.cu) and by the whole-net program kernel
-// (conv_group_tcgen05.cu), where the epilogue warps execute them between GEMM tiles.
+// (conv_group_wgmma.cu), where the consumer warps execute them between GEMM tiles.
 //
 // COH = false: activations through the read-only path (ld.global.nc): the producer kernel has finished.
 // COH = true : activations written earlier in the SAME launch by other SMs: L2-coherent loads (ld.global.cg), never the

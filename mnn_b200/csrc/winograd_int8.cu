@@ -3,7 +3,7 @@
 // Arithmetic = the reference CPU backend's ConvInt8Winograd (source/backend/cpu/compute/ConvInt8Winograd.cpp:306-356,
 // 396-651) on the x86 AVX2 build, bit for bit: int8 -> float, B^T d B in fp32 with the exact operation order of
 // x86_x64/avx/WinogradFunctions.cpp:358-553, per-position requantisation to int8, [alpha^2 batched int8 GEMMs on
-// tcgen05 -- gemm_i8_tcgen05.cu, EPI 2], A^T M A in fp32 (:555-579, 661-712, 981-1051), FloatToInt8.
+// wgmma -- gemm_i8_wgmma.cu, EPI 2], A^T M A in fp32 (:555-579, 661-712, 981-1051), FloatToInt8.
 // Replaces the structure of the reference CUDA backend's float-only WinoInputTrans / WinoTrans2Output
 // (source/backend/cuda/execution/WinogradTrans.cuh:7-595): there one thread walks one (tile, channel) with 16 strided
 // scalar loads; here a thread owns CPT adjacent channels of one tile, so a warp reads/writes whole 32..128-byte
@@ -15,7 +15,7 @@
 #include "common.cuh"
 #include "host_util.h"
 #include "kernels.h"
-#include "tcgen05_common.cuh"
+#include "hopper_common.cuh"
 
 namespace mnnb200 {
 
@@ -249,69 +249,41 @@ __global__ void __launch_bounds__(256) wino_output_kernel(const WinoParams p) {
 
 // =====================================================================================================================
 // F(2x2, 3x3) with the 16 position GEMMs and the output transform in ONE kernel: all 16 accumulators of a (128-tile,
-// 32-channel) block live in TMEM at once (16 x 32 = 512 columns -- the whole tensor memory of the SM), so the fp32 M tensor
+// 8-channel) block live in registers at once (16 positions x 4 per thread of each consumer warpgroup), so the fp32 M tensor
 // (16 bytes per output byte, written and read back through HBM by the three-kernel form) never exists.
-//   warp 0: TMA producer (V[a] tile 128 x K, U[a] chunk 32 x K per stage), warp 1: tcgen05.mma kind::i8 M128 x N32 x K32 into
-//   columns [32a, 32a+32), warp 2: TMEM alloc, warps 4..11: epilogue -- lane = Winograd tile, per 4 channels: 16 x
-//   tcgen05.ld (one per position) -> acc*scale[a][oc] + offset[a][oc] -> A^T M A in the reference's exact fp32 order ->
-//   FloatToInt8 -> one 16-byte store per output pixel (16 channels of this warp's slice).
-// Arithmetic identical to gemm_i8_tcgen05_kernel<2> + wino_output_kernel<4,4>, bit for bit.
+//   warp 8: TMA producer (V[a] tile 128 x K, U[a] chunk 8 x K per stage); warps 0-7: two consumer warpgroups, 64 Winograd
+//   tiles each: wgmma m64n8k32 s8 per position into acc[a] -> acc*scale[a][oc] + offset[a][oc] -> A^T M A in the
+//   reference's exact fp32 order -> FloatToInt8 -> stores per output pixel.  A thread holds every position of its
+//   (tile, channel) pairs, so the output transform needs no data exchange.
+// Arithmetic identical to gemm_i8_wgmma_kernel<2> + wino_output_kernel<4,4>, bit for bit.
 // =====================================================================================================================
-using namespace t5;
-constexpr int kFStages = 6, kFBN = 32, kFStageBytes = 128 * 128 + kFBN * 128, kFEpiWarps = 8;
-constexpr int kFThreads = 128 + kFEpiWarps * 32;
+using namespace hop;
+constexpr int kFStages = 6, kFBN = kWinoFusedBN, kFStageBytes = 128 * 128 + kFBN * 128;
 
-__device__ __forceinline__ uint32_t f_idesc_i8(int n) {
-    return (2u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)(128 >> 4) << 24);
-}
-__device__ __forceinline__ void f_umma_i8(uint32_t d_tmem, uint64_t a_desc, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n"
-        ".reg .pred p;\n"
-        "setp.ne.b32 p, %4, 0;\n"
-        "tcgen05.mma.cta_group::1.kind::i8 [%0], %1, %2, %3, p;\n"
-        "}\n" ::"r"(d_tmem),
-        "l"(a_desc), "l"(b_desc), "r"(idesc), "r"(accumulate)
-        : "memory");
-}
-__device__ __forceinline__ void tmem_ld4(uint32_t taddr, int (&v)[4]) {
-    asm volatile("tcgen05.ld.sync.aligned.32x32b.x4.b32 {%0,%1,%2,%3}, [%4];\n" : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]) : "r"(taddr) : "memory");
-}
-
-__global__ void __launch_bounds__(kFThreads, 1)
+__global__ void __launch_bounds__(kThreads, 1)
 wino_f23_fused_kernel(const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_u, const WinoFusedParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
     uint8_t* smem = smem_raw + (base - raw);
-    const int off_consts = kFStages * kFStageBytes;                 // [3][16][32] floats/ints
+    const int off_consts = kFStages * kFStageBytes;                 // [3][16][8] floats/ints
     const int off_bars = off_consts + 3 * 16 * kFBN * 4;
     const uint32_t bar0 = base + off_bars;
     auto full_bar = [&](int s) { return bar0 + 8u * s; };
     auto empty_bar = [&](int s) { return bar0 + 8u * (kFStages + s); };
-    const uint32_t tfull_bar = bar0 + 8u * (2 * kFStages), tempty_bar = bar0 + 8u * (2 * kFStages + 1);
-    volatile uint32_t* tmem_slot = reinterpret_cast<volatile uint32_t*>(smem + off_bars + 8 * (2 * kFStages + 2));
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int num_kb = (p.K + 127) / 128;
     const int work_total = p.m_tiles * p.oc_chunks;
 
-    if (warp == 0 && lane == 0) {
-        asm volatile("prefetch.tensormap [%0];\n" ::"l"(&tmap_v));
-        asm volatile("prefetch.tensormap [%0];\n" ::"l"(&tmap_u));
-    }
-    if (warp == 1 && lane == 0) {
-        for (int s = 0; s < kFStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 1); }
-        mbar_init(tfull_bar, 1);
-        mbar_init(tempty_bar, kFEpiWarps);
+    if (warp == 8 && lane == 0) {
+        prefetch_tmap(&tmap_v);
+        prefetch_tmap(&tmap_u);
+        for (int s = 0; s < kFStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }
         asm volatile("fence.mbarrier_init.release.cluster;\n" ::: "memory");
     }
-    if (warp == 2) tmem_alloc(smem_u32((const void*)tmem_slot), 512);
-    fence_before();
     __syncthreads();
-    fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0) {
+    if (warp == 8) {
         if (lane == 0) {
             int stage = 0, phase = 0;
             for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
@@ -327,111 +299,95 @@ wino_f23_fused_kernel(const __grid_constant__ CUtensorMap tmap_v, const __grid_c
                     }
             }
         }
-    } else if (warp == 1) {
-        if (lane == 0) {
-            const uint32_t idesc = f_idesc_i8(kFBN);
-            int stage = 0, phase = 0, tphase = 0;
-            for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
-                mbar_wait(tempty_bar, tphase ^ 1);                         // the epilogue has drained all 512 columns
-                fence_after();
-                for (int a = 0; a < 16; ++a)
-                    for (int kb = 0; kb < num_kb; ++kb) {
-                        mbar_wait(full_bar(stage), phase);
-                        fence_after();
-                        const uint32_t a_addr = base + stage * kFStageBytes, b_addr = a_addr + 128 * 128;
-                        const int kleft = p.K - kb * 128;
-                        const int nmma = kleft >= 128 ? 4 : (kleft + 31) / 32;
-                        for (int k = 0; k < nmma; ++k)
-                            f_umma_i8(tmem_base + (uint32_t)(a * kFBN), umma_desc(a_addr + k * 32), umma_desc(b_addr + k * 32), idesc, (kb | k) != 0);
-                        umma_commit(empty_bar(stage));
-                        if (++stage == kFStages) { stage = 0; phase ^= 1; }
-                    }
-                umma_commit(tfull_bar);
-                tphase ^= 1;
-            }
-        }
-    } else if (warp >= 4) {
-        const int ew = warp - 4, q = ew & 3, slice = ew >> 2;             // slice: which 16 of the 32 channels
-        const int et = threadIdx.x - 128, r = q * 32 + lane;
+    } else {
+        const int ct = threadIdx.x, wg = ct >> 7;
+        const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+        const int q4 = lane & 3;
         float* c_scale = reinterpret_cast<float*>(smem + off_consts);
         float* c_off = c_scale + 16 * kFBN;
         int* c_wsum = reinterpret_cast<int*>(c_off + 16 * kFBN);
-        int tphase = 0;
+        int stage = 0, phase = 0;
+        int acc[16][4];
+#pragma unroll
+        for (int a = 0; a < 16; ++a)
+#pragma unroll
+            for (int i = 0; i < 4; ++i) acc[a][i] = 0;
         for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
             const int ch = w % p.oc_chunks, mt = w / p.oc_chunks;
             const int oc0 = ch * kFBN;
-            asm volatile("bar.sync 1, %0;\n" ::"n"(kFEpiWarps * 32) : "memory");          // previous item's readers are done
-            for (int i = et; i < 16 * kFBN; i += kFEpiWarps * 32) {
+            named_sync(1, kConsumerThreads);                              // previous item's readers are done
+            for (int i = ct; i < 16 * kFBN; i += kConsumerThreads) {
                 const int a = i / kFBN, j = i - a * kFBN, oc = oc0 + j;
                 const bool v = oc < p.OC;
                 c_scale[i] = v ? p.scale[a * p.OCp + oc] : 0.f;
                 c_off[i] = v ? p.offset[a * p.OCp + oc] : 0.f;
                 c_wsum[i] = v ? p.wsum128[a * p.OCp + oc] : 0;
             }
-            asm volatile("bar.sync 1, %0;\n" ::"n"(kFEpiWarps * 32) : "memory");
-            mbar_wait_warp(tfull_bar, tphase, lane);
-            fence_after();
-            const long long t = (long long)mt * 128 + r;
-            const bool tile_ok = t < p.T;
-            const int wx = (int)(t % p.wU), hy = (int)((t / p.wU) % p.hU), b = (int)(t / ((long long)p.wU * p.hU));
-            const uint32_t trow = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(slice * 16);
-            uint32_t outw[4][4];                                          // [pixel j*2+i][4-channel group] packed bytes
+            named_sync(1, kConsumerThreads);
+            int prev = -1;
 #pragma unroll
-            for (int g = 0; g < 4; ++g) {
-                float s[4][16];                                           // [channel][position]
-                int v[16][4];
+            for (int a = 0; a < 16; ++a) {
+                for (int kb = 0; kb < num_kb; ++kb) {
+                    mbar_wait(full_bar(stage), phase);
+                    const uint32_t a_addr = base + stage * kFStageBytes + wg * 64 * 128, b_addr = base + stage * kFStageBytes + 128 * 128;
+                    const int kleft = p.K - kb * 128;
+                    const int nmma = kleft >= 128 ? 4 : (kleft + 31) / 32;
+                    fence_acc(acc[a]);
+                    wgmma_fence();
+                    for (int k = 0; k < nmma; ++k)
+                        wgmma<Kind::S8, kFBN>(acc[a], gdesc_sw128(a_addr + k * 32), gdesc_sw128(b_addr + k * 32), (kb | k) != 0);
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    fence_acc(acc[a]);
+                    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(prev)); }
+                    prev = stage;
+                    if (++stage == kFStages) { stage = 0; phase ^= 1; }
+                }
+            }
+            wgmma_wait<0>();
 #pragma unroll
-                for (int a = 0; a < 16; ++a) tmem_ld4(trow + (uint32_t)(a * kFBN + g * 4), v[a]);   // 16 loads in flight, one wait
-                asm volatile("tcgen05.wait::ld.sync.aligned;\n" ::: "memory");
+            for (int a = 0; a < 16; ++a) fence_acc(acc[a]);
+            __syncwarp();
+            if (lane == 0) mbar_arrive(empty_bar(prev));
+            // register i of acc[a] = tile r_base + 8 * (i >> 1), channel 2 * q4 + (i & 1)
 #pragma unroll
-                for (int a = 0; a < 16; ++a) {
+            for (int h = 0; h < 2; ++h) {
+                const long long t = (long long)mt * 128 + r_base + 8 * h;
+                const bool tile_ok = t < p.T;
+                const int wx = (int)(t % p.wU), hy = (int)((t / p.wU) % p.hU), b = (int)(t / ((long long)p.wU * p.hU));
+                uint32_t outw[4] = {0, 0, 0, 0};                          // [pixel j*2+i] two packed bytes
 #pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        const int j = a * kFBN + slice * 16 + g * 4 + c;
+                for (int e = 0; e < 2; ++e) {
+                    const int cc = 2 * q4 + e, oc = oc0 + cc;
+                    float s[16];                                          // [position]
+#pragma unroll
+                    for (int a = 0; a < 16; ++a) {
+                        const int j = a * kFBN + cc;
                         // position GEMM output (avx/GemmInt8.cpp:672-772 float branch): float(acc) * scale[a][oc] + offset[a][oc]
-                        s[c][a] = __fadd_rn(__fmul_rn(__int2float_rn(v[a][c] + c_wsum[j]), c_scale[j]), c_off[j]);
+                        s[a] = __fadd_rn(__fmul_rn(__int2float_rn(acc[a][2 * h + e] + c_wsum[j]), c_scale[j]), c_off[j]);
                     }
-                }
-                if (g == 3) {                                             // last TMEM read of this item by this warp
-                    fence_before();
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive(tempty_bar);
-                }
 #pragma unroll
-                for (int c = 0; c < 4; ++c) {
+                    for (int k = 0; k < 4; ++k) wino_dst<4, 4>(&s[k]);           // dstTransYFunc: along y, per column
 #pragma unroll
-                    for (int k = 0; k < 4; ++k) wino_dst<4, 4>(&s[c][k]);           // dstTransYFunc: along y, per column
+                    for (int j = 0; j < 2; ++j) wino_dst<4, 1>(&s[j * 4]);       // dstTransXFunc: along x, per output row
 #pragma unroll
-                    for (int j = 0; j < 2; ++j) wino_dst<4, 1>(&s[c][j * 4]);       // dstTransXFunc: along x, per output row
-                }
-#pragma unroll
-                for (int px = 0; px < 4; ++px) {
-                    uint32_t packed = 0;
-#pragma unroll
-                    for (int c = 0; c < 4; ++c) {
-                        const int oc = oc0 + slice * 16 + g * 4 + c;
+                    for (int px = 0; px < 4; ++px) {
                         int qv = 0;
-                        if (oc < p.OC) qv = quant_cpu_exact(s[c][(px >> 1) * 4 + (px & 1)], p.out_inv, p.fused_bias[oc], p.minv, p.maxv);
-                        packed |= (uint32_t)(qv & 0xff) << (8 * c);
+                        if (oc < p.OC) qv = quant_cpu_exact(s[(px >> 1) * 4 + (px & 1)], p.out_inv, p.fused_bias[oc], p.minv, p.maxv);
+                        outw[px] |= (uint32_t)(qv & 0xff) << (8 * e);
                     }
-                    outw[px][g] = packed;
                 }
-            }
-            if (tile_ok && oc0 + slice * 16 < p.OCp) {
+                if (tile_ok) {
 #pragma unroll
-                for (int px = 0; px < 4; ++px) {
-                    const int oy = hy * 2 + (px >> 1), ox = wx * 2 + (px & 1);
-                    if (oy < p.OH && ox < p.OW)
-                        *reinterpret_cast<uint4*>(p.y + (((size_t)b * p.OH + oy) * p.OW + ox) * p.OCp + oc0 + slice * 16) =
-                            make_uint4(outw[px][0], outw[px][1], outw[px][2], outw[px][3]);
+                    for (int px = 0; px < 4; ++px) {
+                        const int oy = hy * 2 + (px >> 1), ox = wx * 2 + (px & 1);
+                        if (oy < p.OH && ox < p.OW)
+                            *reinterpret_cast<uint16_t*>(p.y + (((size_t)b * p.OH + oy) * p.OW + ox) * p.OCp + oc0 + 2 * q4) = (uint16_t)outw[px];
+                    }
                 }
             }
-            tphase ^= 1;
         }
     }
-    fence_before();
-    __syncthreads();
-    if (warp == 2) tmem_dealloc(tmem_base, 512);
 }
 
 }  // namespace
@@ -467,7 +423,7 @@ cudaError_t launch_wino_f23_fused(const WinoFusedParams& p, const void* tmap_v, 
     const int work = p.m_tiles * p.oc_chunks;
     const int grid = work < sm_count ? work : sm_count;
     ++g_launch_count;
-    wino_f23_fused_kernel<<<grid, kFThreads, smem, s>>>(*reinterpret_cast<const CUtensorMap*>(tmap_v), *reinterpret_cast<const CUtensorMap*>(tmap_u), p);
+    wino_f23_fused_kernel<<<grid, kThreads, smem, s>>>(*reinterpret_cast<const CUtensorMap*>(tmap_v), *reinterpret_cast<const CUtensorMap*>(tmap_u), p);
     return cudaGetLastError();
 }
 

@@ -276,6 +276,17 @@ def ref_run_model(model, batch, seed, outdir, threads=1):
     return recs
 
 
+def refdump_input(seed, shape):
+    """the input `refdump run` feeds the model (fillInput, oracle/refdump.cpp): std::mt19937(seed) through libstdc++'s
+    uniform_real_distribution<float>(-1, 1) -- float(word) / 2^32, scaled and shifted in fp32 -- so that stored reference outputs
+    can be checked without the reference."""
+    n = int(np.prod(shape))
+    u = np.random.RandomState(seed).randint(0, 2 ** 32, size=n, dtype=np.uint32)
+    r = u.astype(np.float32) / np.float32(4294967296.0)
+    r = np.where(r >= np.float32(1), np.nextafter(np.float32(1), np.float32(0)), r).astype(np.float32)
+    return (r * np.float32(2.0) + np.float32(-1.0)).astype(np.float32).reshape(shape)
+
+
 def ref_bench(model, batch, threads, warmup, iters):
     import json
     r = _run_refdump(["bench", model, batch, threads, warmup, iters], timeout=3600)

@@ -1,5 +1,6 @@
-"""Parity AT THE BENCH CONFIGS THEMSELVES (-m gpu; round-1 VERDICT weak #1): the sizes BASELINE.json's configs name, checked
-against the LIVE reference built under oracle/_ref (which travels to the GPU box) -- not smaller stand-ins.
+"""Parity AT THE BENCH CONFIGS THEMSELVES (-m gpu): the sizes BASELINE.json's configs name -- not smaller stand-ins -- checked
+against the reference's outputs recorded by tests/golden/make_config_golden.py (hashes of the bit-exact outputs, sampled rows of
+the fp32 ones); the plugin legs need the reference core itself (oracle/_ref) and run only where it was built.
 
   C2  MobileNet-v2 int8 .mnn, batch 32: every command's int8 output, plugin vs MNN_FORWARD_CPU and WholeNetSession vs
       MNN_FORWARD_CPU (position-weighted 64-bit sums of the dequantised tensors: REFDUMP_HASH=1, oracle/refdump.cpp)
@@ -7,6 +8,7 @@ against the LIVE reference built under oracle/_ref (which travels to the GPU box
   C4  Qwen-1.8B linear shapes at 4096 tokens: 2048->6144 (+bias, asymmetric) and 5504->2048 vs `refdump linear`
   +   a .mnn whose Convolution carries a winogradAttr through the PLUGIN (reference AVX2 core + libmnn_b200_plugin.so)
 """
+import hashlib
 import json
 import os
 import subprocess
@@ -16,14 +18,14 @@ import numpy as np
 import pytest
 
 from oracle import oracle as O
-from tests.cases import random_wino_case, wino_oracle
+from tests.golden.make_config_golden import C4_CASES, c3_case, c4_inputs
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 PLUGIN = os.path.join(ROOT, "mnn_b200", "libmnn_b200_plugin.so")
 MODEL = os.path.join(ROOT, "tests", "golden", "mbv2_int8.mnn")
+GOLDEN = os.path.join(ROOT, "tests", "golden", "config_golden.npz")
 FP_INTERNAL = ("MobilenetV2/Predictions/Softmax",)      # expf vs the reference's polynomial: +-1 LSB (documented in DESIGN.md)
-needs_ref = pytest.mark.skipif(not O.have_reference(), reason="oracle/_ref not on this box")
 needs_ref2 = pytest.mark.skipif(not O.have_reference_avx2(), reason="oracle/_ref/refdump_avx2 not on this box")
 
 
@@ -75,85 +77,82 @@ def _diagnose(d, batch, threads, ncmd):
             f"{signed_zero} equal values with different zero sign")
 
 
-@needs_ref
 def test_c2_mbv2_batch32_every_op_plugin_and_session_vs_cpu_backend():
-    """BASELINE configs[1] at its own batch: the unmodified reference pipeline on the plugin, and the WholeNetSession host, both
-    against MNN_FORWARD_CPU on the same 32 x 3 x 224 x 224 input; every int8 tensor bit-exact (softmax +-1 LSB excluded)."""
-    assert os.path.exists(PLUGIN), "mnn_b200/libmnn_b200_plugin.so is missing although the reference core is present"
+    """BASELINE configs[1] at its own batch: the WholeNetSession host against MNN_FORWARD_CPU on refdump's 32 x 3 x 224 x 224
+    seed-5 input (the recorded position-weighted 64-bit sums of the dequantised tensors, REFDUMP_HASH=1), every int8 tensor
+    bit-exact (softmax +-1 LSB excluded); where the reference core is built, also the unmodified reference pipeline on the plugin
+    against MNN_FORWARD_CPU in the same run."""
     from mnn_b200.session import WholeNetSession
     batch = 32
-    threads = min(os.cpu_count() or 1, 32)
-    with tempfile.TemporaryDirectory() as d:
-        cpu, _ = _refdump_run(O.REFDUMP, O.REF_DIR, MODEL, batch, 5, os.path.join(d, "cpu"), threads, False)
-        gpu, stats = _refdump_run(O.REFDUMP, O.REF_DIR, MODEL, batch, 5, os.path.join(d, "gpu"), 4, True)
-        assert stats is not None and stats["plugin_declined"] == 0, stats
-        assert [(r["name"], r["type"]) for r in cpu] == [(r["name"], r["type"]) for r in gpu]
-        n_int8 = 0
-        for idx, (a, b) in enumerate(zip(cpu, gpu)):
-            if a["apply_quant"] and a["name"] not in FP_INTERNAL:
-                if a["file"] != b["file"]:
-                    raise AssertionError(f"plugin vs CPU backend differ at batch 32: {a['name']} ({a['type']}): " +
-                                         _diagnose(d, batch, threads, idx + 1))
-                n_int8 += 1
-        assert n_int8 >= 60, n_int8
-        # the C-ABI host on the same input
-        x = np.fromfile(os.path.join(d, "cpu", "input.f32"), np.float32).reshape(batch, 3, 224, 224)
-        sess = WholeNetSession(MODEL, batch)
-        sess.capture()
-        sess.set_input(x)
-        sess.run()
-        checked = 0
-        for r in cpu:
-            if r["name"] not in sess.checkpoints or r["scale"] <= 0 or not r["apply_quant"] or r["name"] in FP_INTERNAL:
-                continue
-            q = sess.read_int8(r["name"]).reshape(r["dims"])
-            f = (q.astype(np.float32) - np.float32(r["zero"])) * np.float32(r["scale"])       # MNNInt8ScaleToFloat
-            assert r["file"] == "hash:%016x" % wsum64(f), f"WholeNetSession vs CPU backend differ at batch 32: {r['name']}"
-            checked += 1
-        assert checked >= 60, checked
-        # ... and the same forward with the conv / depthwise / add chain fused into ONE cooperative launch (net program)
-        prog = WholeNetSession(MODEL, batch, program=True)
-        assert prog.programs and prog.launches_per_step <= 12
-        prog.capture()
-        prog.set_input(x)
-        prog.run()
-        for name in sess.checkpoints:
-            a, b = sess.read_int8(name), prog.read_int8(name)
-            assert np.array_equal(a, b), f"net program vs per-op kernels differ at batch 32: {name}: {np.count_nonzero(a != b)} values"
+    g = np.load(GOLDEN)
+    cpu = [dict(name=str(n), file=str(h), scale=float(sc), zero=float(z), dims=[int(v) for v in str(dm).split(",")])
+           for n, h, sc, z, dm in zip(g["b32_names"], g["b32_hash"], g["b32_scale"], g["b32_zero"], g["b32_dims"])]
+    if O.have_reference():
+        assert os.path.exists(PLUGIN), "mnn_b200/libmnn_b200_plugin.so is missing although the reference core is present"
+        threads = min(os.cpu_count() or 1, 32)
+        with tempfile.TemporaryDirectory() as d:
+            live, _ = _refdump_run(O.REFDUMP, O.REF_DIR, MODEL, batch, 5, os.path.join(d, "cpu"), threads, False)
+            gpu, stats = _refdump_run(O.REFDUMP, O.REF_DIR, MODEL, batch, 5, os.path.join(d, "gpu"), 4, True)
+            assert stats is not None and stats["plugin_declined"] == 0, stats
+            assert [(r["name"], r["type"]) for r in live] == [(r["name"], r["type"]) for r in gpu]
+            n_int8 = 0
+            for idx, (a, b) in enumerate(zip(live, gpu)):
+                if a["apply_quant"] and a["name"] not in FP_INTERNAL:
+                    if a["file"] != b["file"]:
+                        raise AssertionError(f"plugin vs CPU backend differ at batch 32: {a['name']} ({a['type']}): " +
+                                             _diagnose(d, batch, threads, idx + 1))
+                    n_int8 += 1
+            assert n_int8 >= 60, n_int8
+    # the C-ABI host on the same input
+    x = O.refdump_input(5, (batch, 3, 224, 224))
+    sess = WholeNetSession(MODEL, batch)
+    sess.capture()
+    sess.set_input(x)
+    sess.run()
+    checked = 0
+    for r in cpu:
+        if r["name"] not in sess.checkpoints or r["name"] in FP_INTERNAL:
+            continue
+        q = sess.read_int8(r["name"]).reshape(r["dims"])
+        f = (q.astype(np.float32) - np.float32(r["zero"])) * np.float32(r["scale"])       # MNNInt8ScaleToFloat
+        assert r["file"] == "hash:%016x" % wsum64(f), f"WholeNetSession vs CPU backend differ at batch 32: {r['name']}"
+        checked += 1
+    assert checked >= 60, checked
+    # ... and the same forward with the conv / depthwise / add chain fused into ONE cooperative launch (net program)
+    prog = WholeNetSession(MODEL, batch, program=True)
+    assert prog.programs and prog.launches_per_step <= 12
+    prog.capture()
+    prog.set_input(x)
+    prog.run()
+    for name in sess.checkpoints:
+        a, b = sess.read_int8(name), prog.read_int8(name)
+        assert np.array_equal(a, b), f"net program vs per-op kernels differ at batch 32: {name}: {np.count_nonzero(a != b)} values"
 
 
-@needs_ref2
 @pytest.mark.parametrize("C_,HW", [(64, 56), (512, 7)])
 def test_c3_resnet_f63_batch64_vs_live_reference(backend, C_, HW):
     """BASELINE configs[2]: ResNet-50 3x3/s1, batch 64, int8 Winograd F(6,3) -- the first and the last layer class, full size,
-    bit-exact against the reference's AVX2 build (ConvInt8Winograd)."""
+    bit-exact against the reference's AVX2 build (ConvInt8Winograd; its output's sha256 is recorded)."""
     from tests.test_winograd import run_wino
-    rng = np.random.default_rng(C_ + HW)
-    c = random_wino_case(rng, 6, 64, C_, C_, HW, HW, 1, True)
-    y, ex = run_wino(backend, c, 6)
-    ref = wino_oracle(O, c, 6, O.ref_wino)
-    assert y.shape == ref.shape
-    assert np.array_equal(y, ref), f"{np.count_nonzero(y != ref)} of {y.size} differ, max {np.abs(y.astype(int) - ref.astype(int)).max()}"
-    assert (np.abs(ref.astype(int)) == 127).mean() < 0.5
+    y, ex = run_wino(backend, c3_case(C_, HW), 6)
+    assert y.shape == (64, C_, HW, HW)
+    assert hashlib.sha256(np.ascontiguousarray(y).tobytes()).hexdigest() == str(np.load(GOLDEN)[f"c3_{C_}_{HW}"]), \
+        "F(6,3) output differs from the reference's"
+    assert (np.abs(y.astype(int)) == 127).mean() < 0.5
     assert ex.cost()[1] == 64.0 * HW * HW * C_ * C_ * 9
 
 
-@needs_ref
-@pytest.mark.parametrize("ic,oc,asym,has_bias", [(2048, 6144, True, True), (5504, 2048, True, False)])
+@pytest.mark.parametrize("ic,oc,asym,has_bias", C4_CASES)
 def test_c4_qwen_linear_4096_tokens_vs_live_reference(backend, ic, oc, asym, has_bias):
     """BASELINE configs[3]: the two extreme Qwen-1.8B linear shapes at the full 4096 tokens against the reference CPU backend's
-    dynamic-quant W8A8 (`refdump linear`, Memory_Low), 1e-3 relative (north_star); both product kernels (single CTA / CTA pair)."""
+    dynamic-quant W8A8 (`refdump linear`, Memory_Low; sampled rows and max|y| recorded), 1e-3 relative (north_star); both
+    product kernels (single CTA / CTA pair)."""
     from mnn_b200.backend import Op, Tensor
     import torch
-    rng = np.random.default_rng(ic + oc)
     T = 4096
-    x = rng.uniform(-1, 1, (T, ic)).astype(np.float32)
-    wq = rng.integers(-128, 128, (oc, ic), dtype=np.int8)
-    alpha = rng.uniform(0.001, 0.01, oc).astype(np.float32)
-    wmin = (alpha * rng.uniform(-8, 8, oc)).astype(np.float32) if asym else None
-    bias = rng.uniform(-1, 1, oc).astype(np.float32) if has_bias else None
-    al = np.stack([wmin, alpha], 1).astype(np.float32).ravel() if asym else alpha
-    ref = O.ref_linear(x, wq, al, asym=asym, bias=bias, threads=min(os.cpu_count() or 1, 32))
+    x, wq, alpha, wmin, bias = c4_inputs(ic, oc, asym, has_bias)
+    g = np.load(os.path.join(ROOT, "tests", "golden", f"config_c4_{ic}_{oc}.npz"))
+    rows, ref, absmax = g["rows"], g["y"], float(g["absmax"])
     # refdump is fed the wire form {min, scale}; the C ABI takes the offset of SIGNED int8 weights (see _signed_offset)
     from mnn_b200 import _capi
     for variant in (2, 3):
@@ -167,7 +166,9 @@ def test_c4_qwen_linear_4096_tokens_vs_live_reference(backend, ic, oc, asym, has
         assert ex.onExecute([xt], [yt]) == 0
         backend.onSync()
         y = yt.data.cpu().numpy()
-        err = np.abs(y - ref).max() / np.abs(ref).max()
+        assert np.isfinite(y).all(), f"variant {variant}: unwritten outputs"
+        assert abs(np.abs(y).max() - absmax) <= 1e-3 * absmax, f"variant {variant}: max|y| {np.abs(y).max()} vs {absmax}"
+        err = np.abs(y[rows] - ref).max() / absmax
         assert err <= 1e-3, f"variant {variant}: rel err {err}"
 
 

@@ -75,7 +75,7 @@ SHAPES = [  # ic, oc, kh, kw, n, ih, iw, stride, pad, relu, dilate  -- MobileNet
     (37, 53, 3, 2, 2, 13, 9, (1, 2), (2, 1), 1, (2, 1)),
     (5, 7, 1, 1, 1, 1, 1, (1, 1), (0, 0), 0, (1, 1)),       # single pixel, tiny channels
     (200, 130, 1, 1, 1, 5, 3, (1, 1), (0, 0), 1, (1, 1)),
-    (96, 24, 1, 1, 4, 56, 56, (1, 1), (0, 0), 0, (1, 1)),     # many M tiles: persistent loop, TMEM double buffering
+    (96, 24, 1, 1, 4, 56, 56, (1, 1), (0, 0), 0, (1, 1)),     # many M tiles: persistent loop, stage ring reuse
     (576, 160, 1, 1, 4, 7, 7, (1, 1), (0, 0), 0, (1, 1)),     # 5 K blocks
     (960, 320, 1, 1, 8, 7, 7, (1, 1), (0, 0), 0, (1, 1)),     # 8 K blocks (ring wraps), 2 N chunks
     # narrow-K 1x1 convs on big maps: pixel-packed GEMM rows (P = 128 / p16(ic) pixels per row, block-diagonal weights)
@@ -85,7 +85,7 @@ SHAPES = [  # ic, oc, kh, kw, n, ih, iw, stride, pad, relu, dilate  -- MobileNet
     (64, 40, 1, 1, 1, 40, 40, (1, 1), (0, 0), 1, (1, 1)),     # P = 2, oc 40 -> 48: zero padding INSIDE every pixel block
     (10, 20, 1, 1, 3, 32, 32, (1, 1), (0, 0), 1, (1, 1)),     # P = 8, ragged ic and oc
     (130, 530, 1, 1, 2, 9, 9, (1, 1), (0, 0), 1, (1, 1)),     # ragged K and N, 3 N chunks
-    # implicit GEMM on tcgen05 (variant 2 / auto): 128-byte, 64-byte and 16-byte K chunks, stride 2, dilation, ragged tiles
+    # implicit GEMM on wgmma (variant 2 / auto): 128-byte, 64-byte and 16-byte K chunks, stride 2, dilation, ragged tiles
     (128, 128, 3, 3, 2, 14, 14, (1, 1), (1, 1), 1, (1, 1)),   # ResNet 3x3 class, cb = 128, 9 K blocks
     (256, 200, 3, 3, 1, 7, 7, (1, 1), (1, 1), 0, (1, 1)),     # cb = 128 x 2 chunks per tap, 18 K blocks, 2 N chunks, R = 16
     (64, 64, 3, 3, 3, 28, 28, (1, 1), (1, 1), 1, (1, 1)),     # cb = 64 (SWIZZLE_64B), TWp = 32, R = 4
@@ -103,7 +103,7 @@ SHAPES = [  # ic, oc, kh, kw, n, ih, iw, stride, pad, relu, dilate  -- MobileNet
 def test_modern_conv_vs_oracle(backend, shape, variant):
     ic, oc, kh, kw, n, ih, iw, st, pad, relu, dl = shape
     if variant == 2 and st[1] > 2:
-        pytest.skip("the tcgen05 implicit-GEMM kernel takes stride_w <= 2 (two column-parity TMA views)")
+        pytest.skip("the wgmma implicit-GEMM kernel takes stride_w <= 2 (two column-parity TMA views)")
     rng = np.random.default_rng(ic * 1000 + oc)
     c = random_modern_case(rng, ic, oc, kh, kw, n, ih, iw, st, pad, relu, dl)
     bf, sx = O.fold_modern(c["w"], c["ws"], c["bias"], c["s_in"], c["z_in"], c["s_out"], c["z_out"])
@@ -283,7 +283,7 @@ def test_linear_w8_decode_gemv_bit_exact(backend, tokens, ic, oc, asym, has_bias
 @pytest.mark.parametrize("tokens,ic,oc,asym,has_bias", [(512, 2048, 1024, True, False), (256, 128, 64, False, True),
                                                         (700, 520, 300, True, True), (1024, 5504, 2048, False, False)])
 def test_linear_w8_cta_pair_variant_bit_exact(backend, tokens, ic, oc, asym, has_bias):
-    """The cta_group::2 (UMMA M = 256) kernel must produce exactly what the single-CTA kernel and the oracle produce:
+    """The CTA-pair (2-CTA cluster, 256 rows, multicast weights) kernel must produce exactly what the single-CTA kernel and the oracle produce:
     ragged M (700 = 2 full pair tiles + 188 rows), ragged N (300 -> two 160-column chunks), K tail (520), deep K (5504)."""
     import torch
     from mnn_b200 import _capi
@@ -303,7 +303,7 @@ def test_linear_w8_cta_pair_variant_bit_exact(backend, tokens, ic, oc, asym, has
         _capi.check(_capi.lib().mnnb200_conv_int8_set_variant(ex._h, variant))
         assert ex.onResize([xin], [yout]) == 0
         yout.data = torch.full((tokens, oc), float("nan"), device="cuda")
-        for _ in range(2):      # twice: barrier phases / TMEM reuse across launches
+        for _ in range(2):      # twice: barrier phases across launches
             assert ex.onExecute([xin], [yout]) == 0
         backend.onSync()
         outs[variant] = yout.data.cpu().numpy()
@@ -314,7 +314,7 @@ def test_linear_w8_cta_pair_variant_bit_exact(backend, tokens, ic, oc, asym, has
 
 
 def test_lite_two_ctas_per_sm_configuration_bit_exact():
-    """The opt-in `MNNB200_LITE=1` configuration of the tcgen05 GEMM (384-thread CTAs, two per SM, TMEM sized to the tile)
+    """The opt-in `MNNB200_LITE=1` configuration of the wgmma GEMM (two CTAs per SM, tiles <= 128 columns, smaller shared-memory plan)
     is selected through an environment variable read once per process: re-run the 1x1 parity cases in a child process."""
     import subprocess
     import sys
@@ -369,7 +369,7 @@ GROUP_SHAPES = [  # ic, oc, n, ih, iw, relu  -- every MobileNet-v2 1x1 class + r
 
 
 def test_conv_group_vs_oracle_and_single(backend):
-    """All members in ONE launch: every output equals the oracle and the per-layer tcgen05 kernel bit for bit."""
+    """All members in ONE launch: every output equals the oracle and the per-layer wgmma kernel bit for bit."""
     from mnn_b200.backend import ConvGroupExecution, Op, QuantAttr, Tensor
     layers = []
     for (ic, oc, n, ih, iw, relu) in GROUP_SHAPES:
@@ -395,7 +395,7 @@ def test_conv_group_vs_oracle_and_single(backend):
         yout.data.fill_(77)            # poison again: the group must overwrite every valid byte
     grp = ConvGroupExecution(backend, [l[2] for l in layers])
     assert grp.bind([l[3] for l in layers], [l[4] for l in layers]) == 0
-    for rep in range(2):                # second pass: barriers / TMEM of a fresh launch, same answer
+    for rep in range(2):                # second pass: barriers of a fresh launch, same answer
         assert grp.onExecute() == 0
         backend.onSync()
         for (c, relu, ex, xin, yout), single in zip(layers, singles):
@@ -448,7 +448,7 @@ def test_conv_group_mixed_gemm_and_implicit_members(backend):
 def test_conv_group_rejects_unsupported_member(backend):
     from mnn_b200.backend import ConvGroupExecution, Op, QuantAttr, Tensor
     rng = np.random.default_rng(3)
-    c = random_modern_case(rng, 16, 16, 3, 3, 1, 9, 9, (1, 3), (1, 1), 0)       # stride_w = 3: not on the tcgen05 kernels
+    c = random_modern_case(rng, 16, 16, 3, 3, 1, 9, 9, (1, 3), (1, 1), 0)       # stride_w = 3: not on the wgmma kernels
     op = Op(type="ConvInt8", conv=dict(ic=16, oc=16, kernel=(3, 3), stride=(1, 3), pad=(1, 1), dilate=(1, 1), group=1, relu=False),
             weight=c["w"], wscale=c["ws"], bias=c["bias"])
     xin = backend.onAcquire(Tensor((1, 16, 9, 9), "int8", QuantAttr(c["s_in"], c["z_in"], -128, 127)))

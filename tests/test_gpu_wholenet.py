@@ -1,7 +1,7 @@
-"""GPU: the whole MobileNet-v2 int8 .mnn on the CUDA path (no CPU fallback) against the REAL reference CPU backend:
-committed checkpoints always, every op live when oracle/_ref is present on the box."""
+"""GPU: the whole MobileNet-v2 int8 .mnn on the CUDA path (no CPU fallback) against the outputs of the REAL reference CPU
+backend, recorded under tests/golden (committed checkpoints at batch 1, every op at batch 2)."""
+import hashlib
 import os
-import tempfile
 
 import numpy as np
 import pytest
@@ -33,53 +33,46 @@ def test_wholenet_checkpoints_vs_reference_golden():
     assert np.abs(out - ref).max() <= 1e-3 * max(np.abs(ref).max(), 1e-6) + 0.05   # one softmax LSB = scale ~0.03
 
 
-@pytest.mark.skipif(not O.have_reference(), reason="oracle/_ref not on this box")
+def check_vs_reference_b2(sess, tag=""):
+    """every int8 checkpoint of a batch-2 forward on refdump's seed-11 input against the reference CPU backend's output, recorded
+    by tests/golden/make_config_golden.py (sha256 of each tensor; the softmax output in full, +-1 LSB)"""
+    g = np.load(os.path.join(GOLD, "config_golden.npz"))
+    full = {n: g[f"b2_full{i}"] for i, n in enumerate(FP_INTERNAL)}
+    checked = 0
+    for name, h in zip((str(n) for n in g["b2_names"]), (str(h) for h in g["b2_sha256"])):
+        if name not in sess.checkpoints:
+            continue
+        got = sess.read_int8(name)
+        if name in full:
+            dmax = np.abs(got.astype(int) - full[name].reshape(got.shape).astype(int)).max()
+            assert dmax <= 1, f"{tag}{name}: max |diff| = {dmax}"
+        else:
+            assert hashlib.sha256(np.ascontiguousarray(got).tobytes()).hexdigest() == h, f"{tag}{name} differs from the reference"
+        checked += 1
+    assert checked >= 60, checked       # 36 conv + 17 depthwise + 10 add + pool + softmax
+
+
 @pytest.mark.parametrize("batch", [2])
 def test_wholenet_every_op_vs_live_reference(batch):
     from mnn_b200.session import WholeNetSession
-    with tempfile.TemporaryDirectory() as d:
-        recs = O.ref_run_model(MODEL, batch, 11, d, 8)
-        x = np.fromfile(os.path.join(d, "input.f32"), np.float32).reshape(batch, 3, 224, 224)
-        sess = WholeNetSession(MODEL, batch)
-        sess.capture()                      # CUDA-graph replay is the product path
-        sess.set_input(x)
-        sess.run()
-        checked = 0
-        for r in recs:
-            if r["name"] not in sess.checkpoints or r["scale"] <= 0 or not r["apply_quant"]:
-                continue
-            f = np.fromfile(os.path.join(d, r["file"]), np.float32).reshape(r["dims"])
-            q = np.rint(f / np.float32(r["scale"]) + np.float32(r["zero"])).astype(np.int8)
-            got = sess.read_int8(r["name"])
-            dmax = np.abs(got.astype(int) - q.reshape(got.shape).astype(int)).max()
-            assert dmax <= (1 if r["name"] in FP_INTERNAL else 0), f"{r['name']}: max |diff| = {dmax}"
-            checked += 1
-        assert checked >= 60, checked       # 36 conv + 17 depthwise + 10 add + pool + softmax
+    x = O.refdump_input(11, (batch, 3, 224, 224))
+    sess = WholeNetSession(MODEL, batch)
+    sess.capture()                      # CUDA-graph replay is the product path
+    sess.set_input(x)
+    sess.run()
+    check_vs_reference_b2(sess)
 
 
-@pytest.mark.skipif(not O.have_reference(), reason="oracle/_ref not on this box")
 def test_wholenet_program_mode_every_op_vs_live_reference():
     """The same .mnn with its conv / depthwise / add chain fused into ONE cooperative launch (net program: dependency flags between
-    tiles of consecutive layers): every checkpoint still equals the live reference, twice in a row (flags are re-armed per launch)."""
+    tiles of consecutive layers): every checkpoint still equals the reference, twice in a row (flags are re-armed per launch)."""
     from mnn_b200.session import WholeNetSession
     batch = 2
-    with tempfile.TemporaryDirectory() as d:
-        recs = O.ref_run_model(MODEL, batch, 11, d, 8)
-        x = np.fromfile(os.path.join(d, "input.f32"), np.float32).reshape(batch, 3, 224, 224)
-        sess = WholeNetSession(MODEL, batch, program=True)
-        assert sess.programs and sess.launches_per_step <= 12, [s[0] for s in sess.steps]
-        sess.capture()
-        for rep in range(2):
-            sess.set_input(x)
-            sess.run()
-            checked = 0
-            for r in recs:
-                if r["name"] not in sess.checkpoints or r["scale"] <= 0 or not r["apply_quant"]:
-                    continue
-                f = np.fromfile(os.path.join(d, r["file"]), np.float32).reshape(r["dims"])
-                q = np.rint(f / np.float32(r["scale"]) + np.float32(r["zero"])).astype(np.int8)
-                got = sess.read_int8(r["name"])
-                dmax = np.abs(got.astype(int) - q.reshape(got.shape).astype(int)).max()
-                assert dmax <= (1 if r["name"] in FP_INTERNAL else 0), f"rep {rep} {r['name']}: max |diff| = {dmax}"
-                checked += 1
-            assert checked >= 60, checked
+    x = O.refdump_input(11, (batch, 3, 224, 224))
+    sess = WholeNetSession(MODEL, batch, program=True)
+    assert sess.programs and sess.launches_per_step <= 12, [s[0] for s in sess.steps]
+    sess.capture()
+    for rep in range(2):
+        sess.set_input(x)
+        sess.run()
+        check_vs_reference_b2(sess, f"rep {rep} ")

@@ -1,5 +1,5 @@
 """Float MatMul / BatchMatMul (SURVEY a9): oracle pinned on the reference CPU backend and on a committed fixture; the
-tcgen05 kind::f16 path (-m gpu) within BASELINE's 1e-3 (max|d| / max|ref|)."""
+wgmma f16 / tf32 path (-m gpu) within BASELINE's 1e-3 (max|d| / max|ref|)."""
 import os
 
 import numpy as np

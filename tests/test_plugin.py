@@ -1,6 +1,6 @@
 """The drop-in boundary, end to end (-m gpu): the UNMODIFIED reference core (oracle/_ref/libMNN.so: Interpreter, Session,
 Pipeline, geometry, quant-cast insertion) schedules tests/golden/mbv2_int8.mnn on MNN_FORWARD_CUDA, where the only registered
-RuntimeCreator is mnn_b200/libmnn_b200_plugin.so (mnn_b200/csrc/plugin/b200_plugin.cpp -> C ABI -> sm_100a kernels).  Every
+RuntimeCreator is mnn_b200/libmnn_b200_plugin.so (mnn_b200/csrc/plugin/b200_plugin.cpp -> C ABI -> sm_90a kernels).  Every
 command's output tensor, read back through the plugin's onCopyBuffer, must equal what the same process produces on
 MNN_FORWARD_CPU -- bit for bit for int8 tensors (compared at the dequantised boundary, SURVEY F6), and the plugin must have
 created EVERY command (nothing handed back to the CPU backup backend)."""
