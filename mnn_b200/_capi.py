@@ -66,13 +66,6 @@ SIGNATURES = {
     "mnnb200_conv_group_bind": (C.c_int, [P, C.POINTER(P), C.POINTER(P)]),
     "mnnb200_conv_group_execute": (C.c_int, [P]),
     "mnnb200_conv_int8_groupable": (C.c_int, [P]),
-    "mnnb200_net_program_create": (C.c_int, [P, C.POINTER(P)]),
-    "mnnb200_net_program_add_conv": (C.c_int, [P, P, P, P]),
-    "mnnb200_net_program_add_binary_add": (C.c_int, [P, P, C.c_float, C.c_int, P, C.c_float, C.c_int, P, C.c_float, C.c_int, C.c_int,
-                                           C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
-    "mnnb200_net_program_finalize": (C.c_int, [P]),
-    "mnnb200_net_program_execute": (C.c_int, [P]),
-    "mnnb200_net_program_op_count": (C.c_int, [P]),
     "mnnb200_conv_int8_wino_create": (C.c_int, [P, C.POINTER(ConvDesc), P, P, P, P, C.c_int, C.POINTER(P)]),
     "mnnb200_conv_int8_wino_resize": (C.c_int, _RESIZE),
     "mnnb200_conv_int8_wino_execute": (C.c_int, [P, P, P]),

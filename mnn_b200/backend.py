@@ -210,41 +210,6 @@ class ConvGroupExecution(Execution):
         return _capi.lib().mnnb200_conv_group_execute(self._h)
 
 
-class NetProgramExecution(Execution):
-    """ONE cooperative launch for a chain of dependent int8 ops (convs, depthwise convs, eltwise adds): mnnb200_net_program_*.
-    steps = [(execution, inputs, outputs)] in execution order; dependencies are derived from the tensors' device addresses."""
-
-    def __init__(self, backend, steps):
-        super().__init__(backend)
-        L = _capi.lib()
-        check(L.mnnb200_net_program_create(backend.runtime._h, C.byref(self._h)), "net_program_create")
-        self.members = [s[0] for s in steps]        # keep the member executions alive
-        for ex, ins, outs in steps:
-            if isinstance(ex, ConvInt8Execution):
-                check(L.mnnb200_net_program_add_conv(self._h, ex._h, ins[0].ptr(), outs[0].ptr()), "net_program_add_conv")
-            elif isinstance(ex, BinaryAddInt8Execution):
-                a, b_, y = ins[0], ins[1], outs[0]
-                n, c, h, w = y.shape
-                qa, qb, qy = a.quant, b_.quant, y.quant
-                check(L.mnnb200_net_program_add_binary_add(self._h, a.ptr(), qa.scale, int(qa.zero), b_.ptr(), qb.scale, int(qb.zero),
-                                                           y.ptr(), qy.scale, int(qy.zero), int(qy.min), int(qy.max), n, c, h, w),
-                      "net_program_add_binary_add")
-            else:
-                raise MnnB200Error(f"{type(ex).__name__} cannot join a net program")
-        check(L.mnnb200_net_program_finalize(self._h), "net_program_finalize")
-
-    @staticmethod
-    def joinable(ex) -> bool:
-        if isinstance(ex, BinaryAddInt8Execution):
-            return True
-        if isinstance(ex, ConvInt8Execution):
-            return ex.depthwise or bool(_capi.lib().mnnb200_conv_int8_groupable(ex._h))
-        return False
-
-    def onExecute(self, inputs=None, outputs=None):
-        return _capi.lib().mnnb200_net_program_execute(self._h)
-
-
 def encode_winograd_attr(units):
     """WinogradInt8Attr::encode (source/core/WinogradInt8Attr.hpp:45-63): units = [(kyStart, kxStart, kernelY, kernelX,
     unitY, unitX, inputScales[a2], inputZeroPoints[a2], weightScales[a2*oc])] -> the int32 blob stored in

@@ -85,6 +85,5 @@ __device__ __forceinline__ int4 ld_nc_16(const void* p) {
 }
 
 extern std::atomic<unsigned long long> g_launch_count;  // host-side counter (capi.cu); any thread may launch
-extern int g_use_pdl;                      // programmatic dependent launch on/off (env MNNB200_PDL, default on)
 
 }  // namespace mnnb200

@@ -25,14 +25,12 @@
 //   warps 0-7: two consumer warpgroups, 64 rows of the 128-row tile each: wgmma.mma_async m64nNk32 s8 (N = bn <= 128,
 //              accumulators in registers) -> CPU-exact requant -> stores straight to the NHWC16 output rows; per-column
 //              constants staged in shared memory per (layer, n chunk)
-// PROG = true adds dependency flags between tiles and SIMT ops on the consumer warps (whole-net program, opt-in).
 #include <cuda.h>
 #include <cstdlib>
 #include "common.cuh"
 #include "hopper_common.cuh"
 #include "host_util.h"
 #include "kernels.h"
-#include "simt_ops.cuh"
 
 namespace mnnb200 {
 
@@ -84,31 +82,8 @@ __device__ __forceinline__ int requant_fast_small(int acc_u, float wscale, float
     return __float2int_rz(__fadd_rn(f, h));
 }
 
-// ---- program mode: progress flags in global memory (acquire loads / release adds at gpu scope)
-__device__ __forceinline__ int ld_acquire_gpu(const int* p) {
-    int v;
-    asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(p) : "memory");
-    return v;
-}
-__device__ __forceinline__ void red_release_gpu(int* p, int v) {
-    asm volatile("red.release.gpu.global.add.s32 [%0], %1;" ::"l"(p), "r"(v) : "memory");
-}
-// bounded like the mbarrier waits: a dependency that never arrives traps the kernel instead of wedging the GPU
-__device__ __forceinline__ void wait_flag_ge(const int* p, int target) {
-    long long t0 = 0;
-    uint32_t spins = 0;
-    while (ld_acquire_gpu(p) < target) {
-        __nanosleep(64);
-        if ((++spins & 0x3fffu) == 0) {
-            const long long now = clock64();
-            if (t0 == 0) t0 = now;
-            else if (now - t0 > 8000000000ll) __trap();
-        }
-    }
-}
-
 // work item = `cnt` consecutive M tiles of one (layer, n chunk): layer << 26 | n chunk << 20 | (cnt - 1) << 14 | first m tile.
-// The producer pays its per-item bookkeeping (schedule word, layer parameters, descriptors, dependency waits) once per item.
+// The producer pays its per-item bookkeeping (schedule word, layer parameters, descriptors) once per item.
 __device__ __forceinline__ void decode_item(uint32_t w, int& layer, int& nc, int& mt, int& cnt) {
     layer = (int)(w >> 26);
     nc = (int)((w >> 20) & 0x3fu);
@@ -116,14 +91,9 @@ __device__ __forceinline__ void decode_item(uint32_t w, int& layer, int& nc, int
     mt = (int)(w & 0x3fffu);
 }
 
-// PROG = false: conv group (independent layers, items = 32-bit words of `sched`).
-// PROG = true : whole-net program (items = ProgItem records with dependencies; SIMT ops on the consumer warps).
-template <bool PROG>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLayerParams* __restrict__ params,
-                        const GroupConvGeom* __restrict__ geom, int n_layers, const uint32_t* __restrict__ sched, int sched_stride,
-                        const ProgItem* __restrict__ items, const ProgOpWar* __restrict__ war, const ProgSimtOp* __restrict__ simt,
-                        int* __restrict__ flags, int* __restrict__ opdone) {
+                        const GroupConvGeom* __restrict__ geom, int n_layers, const uint32_t* __restrict__ sched, int sched_stride) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     const uint32_t raw = smem_u32(smem_raw);
     const uint32_t base = (raw + 1023u) & ~1023u;
@@ -133,9 +103,7 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
     auto full_bar = [&](int s) { return bar0 + 8u * s; };
     auto empty_bar = [&](int s) { return bar0 + 8u * (kStages + s); };
     const GroupLayerParams* sl = reinterpret_cast<const GroupLayerParams*>(smem + kOffLayers);
-    const uint32_t* my = PROG ? nullptr : sched + (size_t)blockIdx.x * sched_stride;
-    const ProgItem* myp = PROG ? items + (size_t)blockIdx.x * sched_stride : nullptr;
-    auto item_word = [&](int i) -> uint32_t { return PROG ? myp[i].w0 : my[i]; };
+    const uint32_t* my = sched + (size_t)blockIdx.x * sched_stride;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -202,17 +170,11 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                 return kBSlots * kStageB + kb * tile_bytes;
             };
             for (int i = 0;; ++i) {
-                const uint32_t w = item_word(i);
+                const uint32_t w = my[i];
                 if (w == kGroupSchedEnd) break;
                 int L, nc, mt0, cnt;
                 decode_item(w, L, nc, mt0, cnt);
                 const GroupLayerParams& lp = sl[L];
-                if (PROG) {
-                    if (lp.mode >= 2) continue;                      // SIMT op: the epilogue warps run it
-                    const ProgItem& it = myp[i];                    // RAW: the producer tiles covering this item's input
-                    for (int j = 0; j < it.dep0_count; ++j) wait_flag_ge(flags + it.dep0_first + j, it.dep0_need);
-                    asm volatile("fence.proxy.async;\n" ::: "memory");   // generic-proxy writes of other SMs -> this SM's TMA reads
-                }
                 const void* ta = &mp.a[L];
                 const void* tb = &mp.b[L];
                 if (lp.mode == 0) {
@@ -342,47 +304,11 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
         for (int i = 0; i < kMaxBN / 2; ++i) acc[i] = 0;
 
         for (int i = 0;; ++i) {
-            const uint32_t w = item_word(i);
+            const uint32_t w = my[i];
             if (w == kGroupSchedEnd) break;
             int L, nc, mt0, cnt;
             decode_item(w, L, nc, mt0, cnt);
             const GroupLayerParams& lp = sl[L];
-            if (PROG && lp.mode >= 2) {
-                // ---- SIMT work item on the 256 consumer threads: wait for the inputs (RAW) and for the readers of a reused output
-                //      buffer (WAR), run the op's work indices, publish
-                const int mt = mt0;
-                const ProgItem& it = myp[i];
-                const ProgOpWar& wr = war[L];
-                if (ct == 0) {
-                    for (int j = 0; j < it.dep0_count; ++j) wait_flag_ge(flags + it.dep0_first + j, it.dep0_need);
-                    for (int j = 0; j < it.dep1_count; ++j) wait_flag_ge(flags + it.dep1_first + j, it.dep1_need);
-                    for (int j = 0; j < wr.n_war; ++j) wait_flag_ge(opdone + wr.war_op[j], wr.war_target[j]);
-                }
-                named_sync(2, kConsumerThreads);
-                const ProgSimtOp& so = simt[L];
-                if (lp.mode == 2) {
-                    const DwParams& dp = so.dw;
-                    const size_t wpr = dw_work_per_row(dp);
-                    const int r0 = mt * wr.rows_per_item;
-                    const int r1 = (r0 + wr.rows_per_item) < wr.total_rows ? (r0 + wr.rows_per_item) : wr.total_rows;
-                    const size_t i1 = (size_t)r1 * wpr;
-                    if (dw_is_3x3_fast(dp)) {
-                        if (dp.sh == 1) { for (size_t k = (size_t)r0 * wpr + ct; k < i1; k += kConsumerThreads) dwconv3x3_work<1, true>(dp, k); }
-                        else { for (size_t k = (size_t)r0 * wpr + ct; k < i1; k += kConsumerThreads) dwconv3x3_work<2, true>(dp, k); }
-                    } else {
-                        for (size_t k = (size_t)r0 * wpr + ct; k < i1; k += kConsumerThreads) dwconv_generic_work<true>(dp, k);
-                    }
-                } else {
-                    const AddParams& ap = so.add;
-                    const size_t c0 = (size_t)mt * wr.rows_per_item;
-                    const size_t c1 = (c0 + wr.rows_per_item) < ap.chunks ? (c0 + wr.rows_per_item) : ap.chunks;
-                    for (size_t k = c0 + ct; k < c1; k += kConsumerThreads) binary_add_work<true>(ap, k);
-                }
-                __threadfence();
-                named_sync(2, kConsumerThreads);
-                if (ct == 0) { red_release_gpu(flags + it.sig, 1); red_release_gpu(opdone + L, 1); }
-                continue;
-            }
             const int bn = lp.bn, n0 = nc * bn, cb = lp.cb;
             const int ncols = (lp.N - n0) < bn ? (lp.N - n0) : bn;      // valid (16-padded) columns of this chunk
             const int nblk = ncols >> 3;
@@ -438,13 +364,6 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                 __syncwarp();
                 if (lane == 0) mbar_arrive(empty_bar(prev));
 
-                if (PROG) {      // WAR before this warp's stores: readers (or the previous writer) of a reused buffer are done
-                    if (lane == 0) {
-                        const ProgOpWar& wr = war[L];
-                        for (int j = 0; j < wr.n_war; ++j) wait_flag_ge(opdone + wr.war_op[j], wr.war_target[j]);
-                    }
-                    __syncwarp();
-                }
                 // ---- epilogue from the accumulator fragments: register i = row r_base + 8 * ((i >> 1) & 1),
                 //      column 8 * (i >> 2) + 2 * q4 + (i & 1); two output bytes per store
 #pragma unroll
@@ -496,11 +415,6 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                         }
                     }
                 }
-                if (PROG) {
-                    __threadfence();   // this thread's output stores are visible gpu-wide before the flag below
-                    named_sync(2, kConsumerThreads);
-                    if (ct == 0) { red_release_gpu(flags + myp[i].sig + t, 1); red_release_gpu(opdone + L, 1); }
-                }
             }   // tiles of the item
         }
     }
@@ -510,35 +424,11 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
 
 cudaError_t launch_conv_group(const GroupMapsParam* maps_host, const GroupLayerParams* params, const GroupConvGeom* geom, int n_layers,
                               const uint32_t* sched, int sched_stride, int grid, cudaStream_t stream) {
-    cudaError_t e = ensure_max_dynamic_smem((const void*)conv_group_wgmma_kernel<false>, 227 * 1024);
+    cudaError_t e = ensure_max_dynamic_smem((const void*)conv_group_wgmma_kernel, 227 * 1024);
     if (e != cudaSuccess) return e;
     ++g_launch_count;
-    conv_group_wgmma_kernel<false><<<grid, kThreads, kSmemTotal + 1024, stream>>>(*maps_host, params, geom, n_layers, sched, sched_stride,
-                                                                                  nullptr, nullptr, nullptr, nullptr, nullptr);
+    conv_group_wgmma_kernel<<<grid, kThreads, kSmemTotal + 1024, stream>>>(*maps_host, params, geom, n_layers, sched, sched_stride);
     return cudaGetLastError();
-}
-
-// The program kernel's CTAs wait on each other's progress flags: every CTA of the grid must be resident at once, which a
-// cooperative launch guarantees (it fails instead of deadlocking if the grid does not fit).
-cudaError_t launch_net_program(const GroupMapsParam* maps_host, const GroupLayerParams* params, const GroupConvGeom* geom, int n_ops,
-                               const ProgItem* items, int item_stride, const ProgOpWar* war, const ProgSimtOp* simt, int* flags,
-                               int* opdone, int grid, cudaStream_t stream) {
-    cudaError_t e = ensure_max_dynamic_smem((const void*)conv_group_wgmma_kernel<true>, 227 * 1024);
-    if (e != cudaSuccess) return e;
-    ++g_launch_count;
-    cudaLaunchConfig_t cfg = {};
-    cfg.gridDim = dim3(grid);
-    cfg.blockDim = dim3(kThreads);
-    cfg.dynamicSmemBytes = kSmemTotal + 1024;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeCooperative;
-    attr[0].val.cooperative = 1;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    const uint32_t* no_sched = nullptr;
-    return cudaLaunchKernelEx(&cfg, conv_group_wgmma_kernel<true>, *maps_host, params, geom, n_ops, no_sched, item_stride, items, war, simt,
-                              flags, opdone);
 }
 
 }  // namespace mnnb200

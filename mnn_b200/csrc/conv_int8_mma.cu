@@ -19,7 +19,7 @@ namespace mnnb200 {
 constexpr int BK = 64;      // bytes of K per pipeline stage (= 4 x 16-byte chunks)
 constexpr int STAGES = 4;   // cp.async ring depth
 
-template <int BM, int BN, int WM, int WN, int EPI>
+template <int BM, int BN, int WM, int WN>
 __global__ void __launch_bounds__(WM * WN * 32) conv_int8_igemm_kernel(const ConvParams p) {
     constexpr int THREADS = WM * WN * 32;
     constexpr int WTM = BM / WM, WTN = BN / WN;  // warp tile
@@ -160,45 +160,6 @@ __global__ void __launch_bounds__(WM * WN * 32) conv_int8_igemm_kernel(const Con
     __syncthreads();
 
     const int g = lane >> 2, t4 = lane & 3;
-    if (EPI == 1) {
-        // ---- fp32 epilogue (dynamic-quant linear): unfused mul/add sequence of the CPU float-output GEMM tail
-#pragma unroll
-        for (int ni = 0; ni < NI; ++ni) {
-            int n = n0 + wn0 + ni * 8 + t4 * 2;
-            float al[2] = {0.f, 0.f}, ws[2] = {0.f, 0.f}, wz[2] = {0.f, 0.f}, bs[2] = {0.f, 0.f};
-            int k128[2] = {0, 0};
-#pragma unroll
-            for (int j = 0; j < 2; ++j)
-                if (n + j < p.OC) {
-                    al[j] = p.wscale[n + j]; ws[j] = p.wsumf[n + j]; k128[j] = p.wsum128[n + j];
-                    wz[j] = p.wzero ? p.wzero[n + j] : 0.f; bs[j] = p.bias ? p.bias[n + j] : 0.f;
-                }
-#pragma unroll
-            for (int mi = 0; mi < MI; ++mi)
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    int m = m0 + wm0 + mi * 16 + g + h * 8;
-                    if (m >= p.M) continue;
-                    float dqm = p.dq[m], ss = p.srcsum[m];
-                    float corr = __fmul_rn(dqm, -128.f);
-                    float o[2];
-#pragma unroll
-                    for (int j = 0; j < 2; ++j) {
-                        float f = __fmul_rn(__int2float_rn(acc[mi][ni][h * 2 + j] + k128[j]), al[j]);
-                        f = __fmul_rn(f, dqm);
-                        f = __fadd_rn(f, __fmul_rn(corr, ws[j]));
-                        f = __fadd_rn(__fmul_rn(ss, wz[j]), f);
-                        if (p.bias) f = __fadd_rn(f, bs[j]);
-                        if (p.relu || p.relu6) { f = fminf(f, p.relu6 ? 6.0f : 3.4028234663852886e38f); f = fmaxf(f, 0.f); }
-                        o[j] = f;
-                    }
-                    float* dst = p.y_f32 + (size_t)m * p.ldy + n;
-                    if (n + 1 < p.OC && ((p.ldy & 1) == 0)) *reinterpret_cast<float2*>(dst) = make_float2(o[0], o[1]);
-                    else { if (n < p.OC) dst[0] = o[0]; if (n + 1 < p.OC) dst[1] = o[1]; }
-                }
-        }
-        return;
-    }
     // ---- epilogue: CPU-exact requantisation, staged through smem for 16-byte NHWC16 stores
     uint8_t* sC = smem;  // [BM][CPITCH]
 #pragma unroll
@@ -234,13 +195,13 @@ __global__ void __launch_bounds__(WM * WN * 32) conv_int8_igemm_kernel(const Con
     }
 }
 
-template <int BM, int BN, int WM, int WN, int EPI>
-static cudaError_t launch_cfg2(const ConvParams& p, cudaStream_t stream) {
+template <int BM, int BN, int WM, int WN>
+static cudaError_t launch_cfg(const ConvParams& p, cudaStream_t stream) {
     constexpr int THREADS = WM * WN * 32;
     const int smem_pipe = STAGES * (BM + BN) * BK;
     const int smem_epi = BM * (BN + 16);
     const int smem = smem_pipe > smem_epi ? smem_pipe : smem_epi;
-    auto kern = conv_int8_igemm_kernel<BM, BN, WM, WN, EPI>;
+    auto kern = conv_int8_igemm_kernel<BM, BN, WM, WN>;
     {
         cudaError_t e = ensure_max_dynamic_smem((const void*)kern, smem);
         if (e != cudaSuccess) return e;
@@ -254,14 +215,9 @@ static cudaError_t launch_cfg2(const ConvParams& p, cudaStream_t stream) {
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
     attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
-    cfg.numAttrs = g_use_pdl ? 1 : 0;
+    cfg.numAttrs = 1;
     ++g_launch_count;
     return cudaLaunchKernelEx(&cfg, kern, p);
-}
-
-template <int BM, int BN, int WM, int WN>
-static cudaError_t launch_cfg(const ConvParams& p, cudaStream_t stream) {
-    return p.epi == 1 ? launch_cfg2<BM, BN, WM, WN, 1>(p, stream) : launch_cfg2<BM, BN, WM, WN, 0>(p, stream);
 }
 
 void conv_tile_shape(int tile, int* bm, int* bn) {

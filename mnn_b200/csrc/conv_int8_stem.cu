@@ -71,7 +71,7 @@ __global__ void __launch_bounds__(128) conv_int8_stem_kernel(const ConvParams p)
 }  // namespace
 
 bool conv_int8_stem_supported(const ConvParams& p, int ic) {
-    return ic <= 4 && p.Cp == 16 && (p.OCp == 16 || p.OCp == 32 || p.OCp == 64) && p.epi == 0;
+    return ic <= 4 && p.Cp == 16 && (p.OCp == 16 || p.OCp == 32 || p.OCp == 64);
 }
 
 cudaError_t launch_conv_int8_stem(const ConvParams& p, cudaStream_t stream) {

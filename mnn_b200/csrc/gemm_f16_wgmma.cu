@@ -3,8 +3,8 @@
 // SURVEY a9: the attention QK^T / PV matmuls MNN-LLM leaves outside its fused attention op, and every other MatMul /
 // BatchMatMul the geometry stage emits.  Replaces MatMulExecution's 18 CUTLASS mma.sync variants
 // (source/backend/cuda/execution/MatMulExecution.cu:306-1050) with one persistent TMA + wgmma kernel:
-//   1. pack kernels bring both operands to K-major fp16 ([b][e][lp], [b][h][lp], lp = l padded to 8; fp32 -> fp16
-//      round-to-nearest, the transposes that transposeA / !transposeB imply are done in the same pass through smem);
+//   1. pack kernels bring an operand that is not K-major already to K-major form in its own type ([b][e][lp], [b][h][lp],
+//      lp = l padded to 16 bytes; the transposes that transposeA / !transposeB imply are done in the same pass through smem);
 //   2. gemm_f16_wgmma_kernel: warp 8 = TMA producer (128B-swizzled stages), warps 0-7 = two consumer warpgroups
 //      (wgmma.mma_async m64nNk16 f16 or m64nNk8 tf32, fp32 accumulators in registers, 64 rows of the 128-row tile each)
 //      whose epilogue adds the bias and stores fp32 straight from the accumulator fragments.
@@ -136,7 +136,7 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
     }
 }
 
-// ---- operand pack: src fp32 or fp16, logical [b][rows][k] (trans = 0: memory is [rows][k]; trans = 1: memory is [k][rows])
+// ---- operand pack: src fp16, logical [b][rows][k] (trans = 0: memory is [rows][k]; trans = 1: memory is [k][rows])
 //      -> dst fp16 [b][rows][kp], zero padded along k.  32x32 smem tile transpose when trans = 1.
 template <typename T>
 __global__ void pack_kmajor_f16_kernel(const T* __restrict__ src, __half* __restrict__ dst, int rows, int k, int kp, int trans) {
@@ -199,11 +199,9 @@ cudaError_t launch_pack_kmajor_f32(const float* src, float* dst, int batch, int 
     return cudaGetLastError();
 }
 
-cudaError_t launch_pack_kmajor_f16(const void* src, int src_is_f16, void* dst, int batch, int rows, int k, int kp, int trans,
-                                   cudaStream_t s) {
+cudaError_t launch_pack_kmajor_f16(const void* src, void* dst, int batch, int rows, int k, int kp, int trans, cudaStream_t s) {
     dim3 grid((kp + 31) / 32, (rows + 31) / 32, batch), block(32, 8);
-    if (src_is_f16) pack_kmajor_f16_kernel<__half><<<grid, block, 0, s>>>((const __half*)src, (__half*)dst, rows, k, kp, trans);
-    else pack_kmajor_f16_kernel<float><<<grid, block, 0, s>>>((const float*)src, (__half*)dst, rows, k, kp, trans);
+    pack_kmajor_f16_kernel<__half><<<grid, block, 0, s>>>((const __half*)src, (__half*)dst, rows, k, kp, trans);
     ++g_launch_count;
     return cudaGetLastError();
 }

@@ -14,7 +14,6 @@
 //   * pair mode (launch_gemm_i8_2cta): a 2-CTA cluster computes 256 x bn; each CTA loads its own 128 rows of A and HALF of
 //     the B tile, multicast into both CTAs' shared memory, so each SM ingests 3/4 of the operand bytes of a lone CTA
 #include <cuda.h>
-#include <cstdlib>
 #include "common.cuh"
 #include "hopper_common.cuh"
 #include "host_util.h"
@@ -32,19 +31,18 @@ constexpr int kMaxBN = 256;
 constexpr int kStageBytesA = kBM * kBK;          // 16 KB
 constexpr int kConstBytes = kMaxBN * 4 * 5;      // per-column epilogue constants
 constexpr int kSmemBudget = 227 * 1024 - 1024;   // minus the 1024B alignment slack
-constexpr int kLiteBudget = 110 * 1024;
 
 struct SmemPlan {
     int stages, stage_bytes, resident_b;   // resident_b: B (weights) loaded once per CTA
     int off_resb, off_consts, off_bars, total;
 };
-__host__ __device__ inline SmemPlan make_plan(int bn, int n_chunks, int num_kb, int budget, bool pair) {
+__host__ __device__ inline SmemPlan make_plan(int bn, int n_chunks, int num_kb, bool pair) {
     SmemPlan pl;
     const int resb_bytes = bn * kBK * num_kb;
-    pl.resident_b = (!pair && n_chunks == 1 && resb_bytes <= (budget >= kSmemBudget ? 72 * 1024 : 24 * 1024)) ? 1 : 0;
+    pl.resident_b = (!pair && n_chunks == 1 && resb_bytes <= 72 * 1024) ? 1 : 0;
     pl.stage_bytes = kStageBytesA + (pl.resident_b ? 0 : bn * kBK);
     const int fixed = (pl.resident_b ? resb_bytes : 0) + kConstBytes + 256;
-    const int st = (budget - fixed) / pl.stage_bytes;
+    const int st = (kSmemBudget - fixed) / pl.stage_bytes;
     pl.stages = st > kMaxStages ? kMaxStages : (st < 2 ? 2 : st);
     pl.off_resb = pl.stages * pl.stage_bytes;
     pl.off_consts = pl.off_resb + (pl.resident_b ? resb_bytes : 0);
@@ -73,7 +71,6 @@ struct KParams {
     int relu, relu6, has_bias;
     // batched mode (Winograd: one GEMM per transform position): work item = (batch, m_tile, n_chunk)
     int batch, a_batch_rows, b_batch_rows, c_batch_stride;
-    int smem_budget;
     int one_tile;   // grid == number of work items: every CTA owns exactly one (batch, m tile, n chunk)
 };
 
@@ -90,9 +87,9 @@ __device__ __forceinline__ int requant_fast(int acc_u, float wscale, float scale
 }
 
 // EPI 0: int8 requant (conv), 1: fp32 dynamic-quant linear, 2: fp32 Winograd position GEMM.  PAIR: 2-CTA cluster (EPI 1).
-// MAXBN bounds the tile width (and the accumulator registers); MINB = 2 is the opt-in "lite" configuration (two CTAs per SM).
-template <int EPI, bool PAIR, int MAXBN, int MINB>
-__global__ void __launch_bounds__(kThreads, MINB)
+// MAXBN bounds the tile width (and the accumulator registers).
+template <int EPI, bool PAIR, int MAXBN>
+__global__ void __launch_bounds__(kThreads, 1)
 gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_constant__ CUtensorMap tmap_b, const KParams p) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
     // dynamic smem base is only guaranteed 16B aligned: round up to 1024 (SWIZZLE_128B requirement)
@@ -103,7 +100,7 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
     // "fixed tile": the CTA's n chunk (and batch) never changes, so its weights can stay resident and its per-column
     // constants are loaded once -- and, since neither depends on the previous layer, BEFORE griddepcontrol.wait.
     const bool fixed_tile = !PAIR && (p.one_tile || p.n_chunks * p.batch == 1);
-    const SmemPlan pl = make_plan(p.bn, fixed_tile ? 1 : p.n_chunks * p.batch, num_kb, p.smem_budget, PAIR);
+    const SmemPlan pl = make_plan(p.bn, fixed_tile ? 1 : p.n_chunks * p.batch, num_kb, PAIR);
     int nc0 = 0, bt0 = 0;
     if (p.one_tile) { nc0 = blockIdx.x % p.n_chunks; bt0 = (blockIdx.x / p.n_chunks) / p.m_tiles; }
     const int S = pl.stages;
@@ -315,7 +312,7 @@ cudaError_t launch(Kern kern, const CUtensorMap* ta, const CUtensorMap* tb, cons
         attr[0].val.programmaticStreamSerializationAllowed = 1;
     }
     cfg.attrs = attr;
-    cfg.numAttrs = (pair || g_use_pdl) ? 1 : 0;
+    cfg.numAttrs = 1;
     ++g_launch_count;
     return cudaLaunchKernelEx(&cfg, kern, *ta, *tb, p);
 }
@@ -331,7 +328,6 @@ KParams make_params(const GemmI8Params& g, int bn) {
     p.relu = g.relu; p.relu6 = g.relu6; p.has_bias = g.bias != nullptr;
     p.batch = g.batch > 0 ? g.batch : 1;
     p.a_batch_rows = g.a_batch_rows; p.b_batch_rows = g.b_batch_rows; p.c_batch_stride = g.c_batch_stride;
-    p.smem_budget = kSmemBudget;
     p.one_tile = 0;
     return p;
 }
@@ -344,27 +340,16 @@ cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& g, const void* tmap_a, cons
     KParams p = make_params(g, bn);
     const int epi = g.y_f32 == nullptr ? 0 : (g.wino ? 2 : 1);
     const int num_kb = (g.K + kBK - 1) / kBK;
-    // lite configuration: int8 epilogue, tile <= 128 columns, and a smem plan of >= min(3, num_kb) stages inside 110 KB, so
-    // that two CTAs share an SM; opt-in (MNNB200_LITE=1)
-    static const int lite_default = [] { const char* v = getenv("MNNB200_LITE"); return v ? atoi(v) : 0; }();
-    bool lite = false;
-    if (epi == 0 && bn <= 128 && lite_default) {
-        const SmemPlan lp = make_plan(bn, p.n_chunks * p.batch, num_kb, kLiteBudget, false);
-        lite = lp.total <= kLiteBudget && lp.stages >= (num_kb < 3 ? num_kb : 3);
-    }
-    p.smem_budget = lite ? kLiteBudget : kSmemBudget;
     const int work = p.batch * p.m_tiles * p.n_chunks;
-    const int slots = lite ? 2 * sm_count : sm_count;
-    const int grid = work < slots ? work : slots;
+    const int grid = work < sm_count ? work : sm_count;
     p.one_tile = grid == work ? 1 : 0;
     const bool fixed_tile = p.one_tile || p.n_chunks * p.batch == 1;
-    const int smem = make_plan(bn, fixed_tile ? 1 : p.n_chunks * p.batch, num_kb, p.smem_budget, false).total + 1024;
+    const int smem = make_plan(bn, fixed_tile ? 1 : p.n_chunks * p.batch, num_kb, false).total + 1024;
     const CUtensorMap* ta = reinterpret_cast<const CUtensorMap*>(tmap_a);
     const CUtensorMap* tb = reinterpret_cast<const CUtensorMap*>(tmap_b);
-    if (lite) return launch(gemm_i8_wgmma_kernel<0, false, 128, 2>, ta, tb, p, grid, smem, kLiteBudget + 2048, false, stream);
-    if (epi == 0) return launch(gemm_i8_wgmma_kernel<0, false, 256, 1>, ta, tb, p, grid, smem, 227 * 1024, false, stream);
-    if (epi == 1) return launch(gemm_i8_wgmma_kernel<1, false, 256, 1>, ta, tb, p, grid, smem, 227 * 1024, false, stream);
-    return launch(gemm_i8_wgmma_kernel<2, false, 256, 1>, ta, tb, p, grid, smem, 227 * 1024, false, stream);
+    if (epi == 0) return launch(gemm_i8_wgmma_kernel<0, false, 256>, ta, tb, p, grid, smem, 227 * 1024, false, stream);
+    if (epi == 1) return launch(gemm_i8_wgmma_kernel<1, false, 256>, ta, tb, p, grid, smem, 227 * 1024, false, stream);
+    return launch(gemm_i8_wgmma_kernel<2, false, 256>, ta, tb, p, grid, smem, 227 * 1024, false, stream);
 }
 
 cudaError_t launch_gemm_i8_2cta(const GemmI8Params& g, const void* tmap_a, const void* tmap_b_half, int bn, cudaStream_t stream,
@@ -374,11 +359,11 @@ cudaError_t launch_gemm_i8_2cta(const GemmI8Params& g, const void* tmap_a, const
     p.batch = 1;
     p.m_tiles = (g.M + 2 * kBM - 1) / (2 * kBM);
     const int num_kb = (g.K + kBK - 1) / kBK;
-    const int smem = make_plan(bn, p.n_chunks, num_kb, kSmemBudget, true).total + 1024;
+    const int smem = make_plan(bn, p.n_chunks, num_kb, true).total + 1024;
     const int work = p.m_tiles * p.n_chunks;
     int pairs = sm_count / 2;
     if (work < pairs) pairs = work;
-    return launch(gemm_i8_wgmma_kernel<1, true, 256, 1>, reinterpret_cast<const CUtensorMap*>(tmap_a),
+    return launch(gemm_i8_wgmma_kernel<1, true, 256>, reinterpret_cast<const CUtensorMap*>(tmap_a),
                   reinterpret_cast<const CUtensorMap*>(tmap_b_half), p, 2 * pairs, smem, 227 * 1024, true, stream);
 }
 

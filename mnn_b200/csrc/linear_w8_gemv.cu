@@ -311,7 +311,7 @@ cudaError_t launch_t(const GemvW8Params& p, cudaStream_t stream, int sms) {
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-    attr[0].val.programmaticStreamSerializationAllowed = g_use_pdl ? 1 : 0;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
     cfg.attrs = attr;
     cfg.numAttrs = 1;
     return cudaLaunchKernelEx(&cfg, linear_w8_gemv_kernel<T, R, U>, p);

@@ -96,7 +96,6 @@ public:
         : Backend(MNN_FORWARD_CUDA), mRuntime(rt), mH(h), mMemoryLow(memoryLow) {
         if (const char* v = getenv("MNNB200_PLUGIN_GRAPH")) mGraphEnabled = atoi(v) != 0;
         if (const char* v = getenv("MNNB200_PLUGIN_HOSTREG")) mHostRegEnabled = atoi(v) != 0;
-        if (const char* v = getenv("MNNB200_PLUGIN_PROGRAM")) mProgramEnabled = atoi(v) != 0;
     }
     bool memoryLow() const { return mMemoryLow; }
     ~B200Backend() override {
@@ -119,9 +118,7 @@ public:
     // ---- one forward = onExecuteBegin, Execution::onExecute x N, onExecuteEnd (Pipeline::execute, source/core/Pipeline.cpp:1167-1230).
     //      Run 1 after a resize executes eagerly (module load, descriptor creation).  From run 2 on the executions only LOG
     //      their call (DEFER); onExecuteEnd then
-    //        - first time: turns the logged forward into a PLAN -- runs of convolutions / depthwise convolutions / eltwise adds
-    //          become whole-net programs (one cooperative launch each, mnnb200_net_program_*), everything else keeps its own
-    //          launch -- and captures that plan into a CUDA graph;
+    //        - first time: captures the logged calls, each with its own kernel launches, into a CUDA graph;
     //        - afterwards: checks that the logged forward is the captured one and launches the graph (one host call per forward).
     //      Anything that needs the device mid-run (Tensor::copyToHostTensor from a callback, a command on the CPU backup backend
     //      reading a device tensor) calls interrupt(): the deferred calls are flushed eagerly and the run goes on eagerly.
@@ -140,8 +137,6 @@ public:
     bool buildAndCapture() const;
     void dropGraph() const {
         if (mGraph) { mnnb200_runtime_sync(mH); mnnb200_graph_destroy(mGraph); mGraph = nullptr; }
-        for (auto p : mPrograms) mnnb200_exec_destroy(p);
-        mPrograms.clear();
         mRuns = 0; mGraphBroken = false; mTrace.clear(); mPending.clear();
     }
 
@@ -277,16 +272,12 @@ private:
     bool mMemoryLow;
     std::shared_ptr<PoolState> mPool{new PoolState};
     bool mGraphEnabled = true, mHostRegEnabled = false;   // MNNB200_PLUGIN_HOSTREG=1: pin user tensors in place (see pinned())
-    bool mProgramEnabled = false;           // MNNB200_PLUGIN_PROGRAM=1: runs of conv / depthwise / add become whole-net programs (one
-                                            // cooperative launch each); bit-exact, but not faster than the captured per-op kernels yet
     mutable bool mInRun = false, mGraphBroken = false;
     mutable Mode mMode = EAGER;
     mutable int mRuns = 0;
     mutable mnnb200_graph* mGraph = nullptr;
     mutable std::vector<Call> mPending;
     mutable std::vector<uint64_t> mTrace;   // signature of the captured forward
-    mutable std::vector<mnnb200_exec*> mPrograms;
-    mutable int mPlanLaunches = 0;
     mutable void* mStageDev = nullptr;
     mutable size_t mStageDevBytes = 0;
     mutable void* mStageHost = nullptr;
@@ -304,8 +295,6 @@ public:
         return launch(inputs, outputs);
     }
     virtual ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) = 0;
-    // appends this call to a whole-net program (mnnb200_net_program_add_*); false = this op keeps its own launch
-    virtual bool addToProgram(mnnb200_exec*, const std::vector<Tensor*>&, const std::vector<Tensor*>&) { return false; }
 };
 
 void B200Backend::onExecuteBegin() const {
@@ -321,41 +310,17 @@ void B200Backend::interrupt() const {
     for (auto& c : mPending) c.exec->launch(*c.in, *c.out);
     mPending.clear();
 }
-// Plan + capture the logged forward.  Programs are built BEFORE the capture starts (their setup allocates and copies).
+// Capture the logged forward: every pending call launches its own kernels into one CUDA graph.
 bool B200Backend::buildAndCapture() const {
-    struct Step { mnnb200_exec* prog; const Call* call; };
-    std::vector<Step> plan;
-    size_t i = 0;
-    const size_t n = mPending.size();
-    while (i < n) {
-        mnnb200_exec* prog = nullptr;
-        size_t j = i;
-        if (mProgramEnabled && mnnb200_net_program_create(mH, &prog) == MNNB200_OK) {
-            while (j < n && j - i < 64 && mPending[j].exec->addToProgram(prog, *mPending[j].in, *mPending[j].out)) ++j;
-            if (j - i >= 2 && mnnb200_net_program_finalize(prog) == MNNB200_OK) {
-                mPrograms.push_back(prog);
-                plan.push_back({prog, nullptr});
-                i = j;
-                continue;
-            }
-            mnnb200_exec_destroy(prog);     // a single op, or a chain the program kernel does not take: plain launches
-        }
-        plan.push_back({nullptr, &mPending[i]});
-        ++i;
-    }
     if (mnnb200_graph_begin_capture(mH) != MNNB200_OK) return false;
     bool ok = true;
-    for (auto& st : plan) {
-        if (st.prog) ok = ok && mnnb200_net_program_execute(st.prog) == MNNB200_OK;
-        else ok = ok && st.call->exec->launch(*st.call->in, *st.call->out) == NO_ERROR;
-    }
+    for (auto& c : mPending) ok = ok && c.exec->launch(*c.in, *c.out) == NO_ERROR;
     mnnb200_graph* g = nullptr;
     if (mnnb200_graph_end_capture(mH, &g) != MNNB200_OK || !ok) {
         if (g) mnnb200_graph_destroy(g);
         return false;
     }
     mGraph = g;
-    mPlanLaunches = (int)plan.size();
     mTrace.clear();
     for (auto& c : mPending) mTrace.push_back(c.sig);
     return true;
@@ -597,10 +562,6 @@ public:
                                   : (mDepthwise ? mnnb200_dwconv_int8_execute(mRes->h, x, y) : mnnb200_conv_int8_execute(mRes->h, x, y));
         return toErr(st, "conv execute");
     }
-    bool addToProgram(mnnb200_exec* prog, const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        if (mWino) return false;
-        return mnnb200_net_program_add_conv(prog, mRes->h, (const int8_t*)dev(inputs[0]), (int8_t*)dev(outputs[0])) == MNNB200_OK;
-    }
     // Execution::onClone (source/core/Execution.hpp:63): a clone owns its own resize state; the packed weights are re-created
     // from the op (the C ABI keeps epilogue constants per execution), dst == nullptr is the capability query
     bool onClone(Backend* bn, const Op* op, Execution** dst) override {
@@ -742,13 +703,6 @@ public:
 class BinaryAddInt8Exec : public B200Exec {
 public:
     BinaryAddInt8Exec(Backend* bn) : B200Exec(bn) {}
-    bool addToProgram(mnnb200_exec* prog, const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        auto d = dims4(outputs[0]);
-        auto q0 = TensorUtils::getQuantInfo(inputs[0]), q1 = TensorUtils::getQuantInfo(inputs[1]), qo = TensorUtils::getQuantInfo(outputs[0]);
-        return mnnb200_net_program_add_binary_add(prog, (const int8_t*)dev(inputs[0]), q0[0], (int)q0[1], (const int8_t*)dev(inputs[1]), q1[0],
-                                                  (int)q1[1], (int8_t*)dev(outputs[0]), qo[0], (int)qo[1], (int)qo[2], (int)qo[3], d.n, d.c,
-                                                  d.h, d.w) == MNNB200_OK;
-    }
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto d = dims4(outputs[0]);
         auto q0 = TensorUtils::getQuantInfo(inputs[0]), q1 = TensorUtils::getQuantInfo(inputs[1]), qo = TensorUtils::getQuantInfo(outputs[0]);

@@ -11,7 +11,6 @@
 //
 // Every float step is an explicitly rounded intrinsic: ptxas must not contract mul+add (the CPU code is unfused).
 #include <cuda.h>
-#include <cstdlib>
 #include "common.cuh"
 #include "host_util.h"
 #include "kernels.h"
@@ -104,7 +103,6 @@ __global__ void __launch_bounds__(256) wino_input_kernel(const WinoParams p) {
             if (in) {
                 const int8_t* src = p.x + (((size_t)b * p.IH + iy) * p.IW + ix) * p.Cp + cg * CPT;
                 if (CPT == 4) *reinterpret_cast<int*>(q) = *reinterpret_cast<const int*>(src);
-                else if (CPT == 2) *reinterpret_cast<short*>(q) = *reinterpret_cast<const short*>(src);
                 else q[0] = src[0];
             }
 #pragma unroll
@@ -128,12 +126,11 @@ __global__ void __launch_bounds__(256) wino_input_kernel(const WinoParams p) {
         for (int c = 0; c < CPT; ++c)   // MNNFloat2Int8(scale = 1/inputScale[a], zero = inputZero[a], -127, 127)
             q[c] = (int8_t)quant_cpu_exact(d[c][a], p.in_inv[a], p.in_zero[a], -127.f, 127.f);
         if (CPT == 4) *reinterpret_cast<int*>(dst + a * a_stride) = *reinterpret_cast<int*>(q);
-        else if (CPT == 2) *reinterpret_cast<short*>(dst + a * a_stride) = *reinterpret_cast<short*>(q);
         else dst[a * a_stride] = q[0];
     }
 }
 
-// Word-wide variant for the larger tiles (alpha = 6, 8): the thread still owns 4 adjacent channels, i.e. one 32-bit word per
+// Word-wide variant for F(6,3) (alpha = 6): the thread still owns 4 adjacent channels, i.e. one 32-bit word per
 // pixel on both sides, but the four channels are transformed ONE AFTER THE OTHER so that only alpha^2 floats are live
 // (plus the packed input and output words) instead of 4 * alpha^2.  Same arithmetic per channel as wino_input_kernel.
 template <int ALPHA>
@@ -395,21 +392,17 @@ wino_f23_fused_kernel(const __grid_constant__ CUtensorMap tmap_v, const __grid_c
 cudaError_t launch_wino_input(const WinoParams& p, cudaStream_t s) {
     ++g_launch_count;
     const int alpha = p.unit + 2;
-    static const int seq4 = [] { const char* v = getenv("MNNB200_WINO_SEQ4"); return v ? atoi(v) : 1; }();
-    // measured (r01): alpha = 6: 0.259 -> 0.239 ms on the ResNet set; alpha = 8: no gain (255 registers, 8 warps per SM), so
-    // F(6,3) keeps the one-channel-per-thread kernel unless MNNB200_WINO_SEQ4=2
-    if ((seq4 && alpha == 6) || (seq4 == 2 && alpha == 8)) {
+    // measured (r01): alpha = 6: 0.259 -> 0.239 ms on the ResNet set with the word-wide kernel; alpha = 8: no gain there (255
+    // registers, 8 warps per SM), so F(6,3) keeps the one-channel-per-thread kernel
+    if (alpha == 6) {
         const long long threads = (long long)p.T * (p.Cp / 4);
-        const unsigned grid = (unsigned)((threads + 127) / 128);
-        if (alpha == 6) wino_input_seq4_kernel<6><<<grid, 128, 0, s>>>(p);
-        else wino_input_seq4_kernel<8><<<grid, 128, 0, s>>>(p);
+        wino_input_seq4_kernel<6><<<(unsigned)((threads + 127) / 128), 128, 0, s>>>(p);
         return cudaGetLastError();
     }
-    const int cpt = alpha == 4 ? 4 : (alpha == 6 ? 2 : 1);
+    const int cpt = alpha == 4 ? 4 : 1;
     const long long threads = (long long)p.T * (p.Cp / cpt);
     const unsigned grid = (unsigned)((threads + 255) / 256);
     if (alpha == 4) wino_input_kernel<4, 4><<<grid, 256, 0, s>>>(p);
-    else if (alpha == 6) wino_input_kernel<6, 2><<<grid, 256, 0, s>>>(p);
     else if (alpha == 8) wino_input_kernel<8, 1><<<grid, 256, 0, s>>>(p);
     else return cudaErrorInvalidValue;
     return cudaGetLastError();

@@ -5,14 +5,13 @@ ConvPathSession runs ONLY the dense int8 convolutions of a model, each on its ow
 (BASELINE.json configs[1]: "ConvInt8 im2col+IMMA path only").  WholeNetSession (added later) chains every op.
 """
 import ctypes as C
-import os
 from typing import List, Optional
 
 import numpy as np
 import torch
 
 from . import _capi, graph, mnn_file
-from .backend import Backend, ConvGroupExecution, NetProgramExecution, Op, QuantAttr, Runtime, Tensor, up16
+from .backend import Backend, ConvGroupExecution, Op, QuantAttr, Runtime, Tensor, up16
 
 
 def _qattr(q: Optional[mnn_file.QuantInfo]) -> QuantAttr:
@@ -44,7 +43,7 @@ def conv_op_from_node(node: mnn_file.OpNode) -> Op:
 
 
 class ConvPathSession:
-    def __init__(self, model, batch: int, device_id: int = 0, input_hw=(224, 224), seed: int = 0, group: Optional[bool] = None):
+    def __init__(self, model, batch: int, device_id: int = 0, input_hw=(224, 224), seed: int = 0):
         self.stream = torch.cuda.Stream(device=device_id)
         with torch.cuda.stream(self.stream):
             self.runtime = Runtime(device_id)            # adopts self.stream
@@ -80,19 +79,14 @@ class ConvPathSession:
             # persistent launch (conv group); the rest (3x3 stem, strided convs) keep their own kernels
             self.group = None
             self.singles = list(self.layers)
-            if group is None:
-                group = os.environ.get("MNNB200_GROUP", "1") != "0"
-            if group:
-                members = [l for l in self.layers if ConvGroupExecution.groupable(l[1])]
-                if os.environ.get("MNNB200_GROUP_NO_IMPLICIT", "0") != "0":     # measurement: keep k > 1 convs out of the group
-                    members = [l for l in members if tuple(l[0].conv.kernel) == (1, 1) and tuple(l[0].conv.stride) == (1, 1)]
-                if len(members) >= 2:
-                    self.group = ConvGroupExecution(self.backend, [l[1] for l in members])
-                    st = self.group.bind([l[2] for l in members], [l[3] for l in members])
-                    if st != 0:
-                        raise RuntimeError(f"conv_group_bind -> {st}: {_capi.lib().mnnb200_last_error().decode()}")
-                    ids = {id(l[1]) for l in members}
-                    self.singles = [l for l in self.layers if id(l[1]) not in ids]
+            members = [l for l in self.layers if ConvGroupExecution.groupable(l[1])]
+            if len(members) >= 2:
+                self.group = ConvGroupExecution(self.backend, [l[1] for l in members])
+                st = self.group.bind([l[2] for l in members], [l[3] for l in members])
+                if st != 0:
+                    raise RuntimeError(f"conv_group_bind -> {st}: {_capi.lib().mnnb200_last_error().decode()}")
+                ids = {id(l[1]) for l in members}
+                self.singles = [l for l in self.layers if id(l[1]) not in ids]
         self.stream.synchronize()
         self.graph: Optional[torch.cuda.CUDAGraph] = None
         self.launches_per_step = len(self.singles) + (1 if self.group is not None else 0)
@@ -205,16 +199,13 @@ class WholeNetSession:
       casts (FloatToInt8 / Int8ToFloat) are inserted where producer and consumer disagree.
     The network input is fp32 NCHW (FloatToInt8 inside the copy), the output fp32 (dequantised)."""
 
-    def __init__(self, model, batch: int, device_id: int = 0, input_hw=(224, 224), program: Optional[bool] = None):
+    def __init__(self, model, batch: int, device_id: int = 0, input_hw=(224, 224)):
         self.stream = torch.cuda.Stream(device=device_id)
         with torch.cuda.stream(self.stream):
             self.runtime = Runtime(device_id)
         self.backend: Backend = self.runtime.onCreate()
         self.net = model if isinstance(model, mnn_file.Net) else mnn_file.load(model)
         net = self.net
-        if program is None:
-            program = os.environ.get("MNNB200_PROGRAM", "0") != "0"
-        self.use_program = program
         self.batch = batch
         in_node = next(op for op in net.ops if op.type == "Input")
         ic0 = in_node.attrs["dims"][1]
@@ -226,35 +217,9 @@ class WholeNetSession:
         dev = self.runtime.device
         with torch.cuda.stream(self.stream):
             self._build(net, in_node, dev)
-            if self.use_program:
-                self._fuse_programs()
         self.stream.synchronize()
         self.graph = None
         self.launches_per_step = len(self.steps)
-
-    def _fuse_programs(self):
-        """Maximal runs of consecutive convs / depthwise convs / eltwise adds become ONE cooperative launch each (net program)."""
-        fused, run = [], []
-
-        def flush():
-            if len(run) >= 2:
-                prog = NetProgramExecution(self.backend, [(ex, ins, outs) for _, ex, ins, outs in run])
-                fused.append(("program[%d ops: %s .. %s]" % (len(run), run[0][0], run[-1][0]), prog, [], []))
-            else:
-                fused.extend(run)
-            run.clear()
-        for step in self.steps:
-            if NetProgramExecution.joinable(step[1]) and len(run) < 64:
-                run.append(step)
-            else:
-                flush()
-                if NetProgramExecution.joinable(step[1]):
-                    run.append(step)
-                else:
-                    fused.append(step)
-        flush()
-        self.programs = [s[1] for s in fused if isinstance(s[1], NetProgramExecution)]
-        self.steps = fused
 
     # -- helpers
     def _q(self, idx):

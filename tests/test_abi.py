@@ -16,7 +16,7 @@ def test_header_symbols_exported():
     L = ctypes.CDLL(_capi.LIB_PATH)
     for name in declared:
         assert hasattr(L, name), f"{name} not exported"
-    assert _capi.lib().mnnb200_abi_version() == 1
+    assert _capi.lib().mnnb200_abi_version() == 2
 
 
 def test_no_cpu_fallback_without_gpu():

@@ -118,15 +118,6 @@ def test_c2_mbv2_batch32_every_op_plugin_and_session_vs_cpu_backend():
         assert r["file"] == "hash:%016x" % wsum64(f), f"WholeNetSession vs CPU backend differ at batch 32: {r['name']}"
         checked += 1
     assert checked >= 60, checked
-    # ... and the same forward with the conv / depthwise / add chain fused into ONE cooperative launch (net program)
-    prog = WholeNetSession(MODEL, batch, program=True)
-    assert prog.programs and prog.launches_per_step <= 12
-    prog.capture()
-    prog.set_input(x)
-    prog.run()
-    for name in sess.checkpoints:
-        a, b = sess.read_int8(name), prog.read_int8(name)
-        assert np.array_equal(a, b), f"net program vs per-op kernels differ at batch 32: {name}: {np.count_nonzero(a != b)} values"
 
 
 @pytest.mark.parametrize("C_,HW", [(64, 56), (512, 7)])

@@ -157,7 +157,7 @@ def test_depthwise_vs_oracle(backend):
         assert np.array_equal(y, ref)
 
 
-@pytest.mark.parametrize("variant", [1, 2])
+@pytest.mark.parametrize("variant", [2])
 def test_linear_w8_dynamic_vs_oracle(backend, variant):
     """fp32 output: tolerance 1e-3 relative to max|ref| (BASELINE.json north_star)."""
     import torch
@@ -313,19 +313,6 @@ def test_linear_w8_cta_pair_variant_bit_exact(backend, tokens, ic, oc, asym, has
         assert np.array_equal(outs[3], O.linear_w8_dynamic(x, wq, alpha, wzero, bias))
 
 
-def test_lite_two_ctas_per_sm_configuration_bit_exact():
-    """The opt-in `MNNB200_LITE=1` configuration of the wgmma GEMM (two CTAs per SM, tiles <= 128 columns, smaller shared-memory plan)
-    is selected through an environment variable read once per process: re-run the 1x1 parity cases in a child process."""
-    import subprocess
-    import sys
-    env = dict(os.environ, MNNB200_LITE="1")
-    root = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-    r = subprocess.run([sys.executable, "-m", "pytest", os.path.join(root, "tests", "test_gpu_parity.py"), "-m", "gpu", "-q", "-x",
-                        "-k", "test_modern_conv_vs_oracle and 2-"], env=env, cwd=root, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0, r.stdout[-1500:]
-    assert " passed" in r.stdout
-
-
 def test_error_behaviour_mirrors_mnn_error_codes(backend):
     """Status codes are numerically MNN::ErrorCode (include/MNN/ErrorCode.hpp): COMPUTE_SIZE_ERROR = 3 for an empty shape,
     NO_EXECUTION = 4 for execute before resize, NOT_SUPPORT = 2 / INVALID_VALUE = 5 for what the path does not take."""
@@ -345,6 +332,10 @@ def test_error_behaviour_mirrors_mnn_error_codes(backend):
     oh, ow = C.c_int(0), C.c_int(0)
     assert L.mnnb200_conv_int8_resize(h, 1, 1, 1, 0.1, 0, 0.1, 0, -127, 127, C.byref(oh), C.byref(ow)) == 0 and (oh.value, ow.value) == (1, 1)
     assert L.mnnb200_dwconv_int8_resize(h, 1, 4, 4, 0.1, 0, 0.1, 0, -127, 127, C.byref(oh), C.byref(ow)) == 5    # wrong execution kind
+    L.mnnb200_exec_destroy(h)
+    wl = np.ones((8, 8), np.int8)
+    assert L.mnnb200_linear_w8_create(rt, 8, 8, wl.ctypes.data_as(C.c_void_p), ws.ctypes.data_as(C.c_void_p), None, None, 0, 0, C.byref(h)) == 0
+    assert L.mnnb200_conv_int8_set_variant(h, 1) == 5                                 # mma.sync variant: convolutions only
     L.mnnb200_exec_destroy(h)
     dg = ConvDesc(8, 8, 3, 3, 1, 1, 1, 1, 1, 1, 2, 0)
     assert L.mnnb200_conv_int8_create(rt, C.byref(dg), w.ctypes.data_as(C.c_void_p), ws.ctypes.data_as(C.c_void_p), None, C.byref(h)) == 2   # grouped conv

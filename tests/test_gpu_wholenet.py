@@ -62,17 +62,3 @@ def test_wholenet_every_op_vs_live_reference(batch):
     sess.run()
     check_vs_reference_b2(sess)
 
-
-def test_wholenet_program_mode_every_op_vs_live_reference():
-    """The same .mnn with its conv / depthwise / add chain fused into ONE cooperative launch (net program: dependency flags between
-    tiles of consecutive layers): every checkpoint still equals the reference, twice in a row (flags are re-armed per launch)."""
-    from mnn_b200.session import WholeNetSession
-    batch = 2
-    x = O.refdump_input(11, (batch, 3, 224, 224))
-    sess = WholeNetSession(MODEL, batch, program=True)
-    assert sess.programs and sess.launches_per_step <= 12, [s[0] for s in sess.steps]
-    sess.capture()
-    for rep in range(2):
-        sess.set_input(x)
-        sess.run()
-        check_vs_reference_b2(sess, f"rep {rep} ")
