@@ -149,7 +149,8 @@ MNNB200_API mnnb200_status mnnb200_scale_int8_execute(mnnb200_exec* e, const int
 MNNB200_API mnnb200_status mnnb200_pool_int8(mnnb200_runtime* rt, const int8_t* x_nhwc16, int n, int c, int ih, int iw, int kh,
                                              int kw, int stride_h, int stride_w, int pad_h, int pad_w, int is_avg,
                                              int8_t* y_nhwc16, int oh, int ow);
-/* float ReLU (CPURelu.cpp, MNNReluWithSlope): y = x < 0 ? x * slope : x over `count` contiguous floats */
+/* float ReLU (CPURelu.cpp, MNNReluWithSlope): y = x < 0 ? x * slope : x over `count` contiguous floats.
+ * x and y must be 16-byte aligned (the kernel moves float4 words): INVALID_VALUE otherwise, before anything is enqueued. */
 MNNB200_API mnnb200_status mnnb200_relu_f32(mnnb200_runtime* rt, const float* x, size_t count, float slope, float* y);
 /* float Reduction over the middle axis of [outside][axis][inside] (CPUReduction.cpp): op 0 SUM, 1 MEAN, 2 MAX, 3 MIN, 4 PROD */
 MNNB200_API mnnb200_status mnnb200_reduce_f32(mnnb200_runtime* rt, const float* x, int outside, int axis, int inside, int op,

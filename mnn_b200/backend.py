@@ -292,18 +292,9 @@ class AvgPoolInt8Execution(Execution):
         self.a = op.extra
 
     def onResize(self, inputs, outputs):
+        from .graph import float_pool_params      # ShapePool + CPUPool resolution (ceilModel, pads, SAME/VALID, global)
         n, c, h, w = inputs[0].shape
-        a = self.a
-        if a.get("is_global"):
-            self.k, self.s, self.p, self.pt = (h, w), (1, 1), (0, 0), 1
-        else:
-            self.k, self.s, self.p, self.pt = a["kernel"], a["stride"], a.get("pad", (0, 0)), a.get("pad_type", 0)
-        if a.get("is_global"):
-            oh, ow = 1, 1
-        else:
-            from .graph import pool_out_and_pad      # ShapePool + CPUPool pad resolution (ceilModel, pads, SAME/VALID)
-            oh, ow, ph, pw = pool_out_and_pad(h, w, a)
-            self.p = (ph, pw)
+        oh, ow, self.k, self.s, self.p, self.pt = float_pool_params(h, w, self.a)
         outputs[0].shape = (n, c, oh, ow)
         return NO_ERROR
 

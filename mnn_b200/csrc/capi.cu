@@ -745,6 +745,8 @@ mnnb200_status mnnb200_pool_int8(mnnb200_runtime* rt, const int8_t* x, int n, in
 }
 mnnb200_status mnnb200_relu_f32(mnnb200_runtime* rt, const float* x, size_t count, float slope, float* y) {
     if (!rt || !x || !y) return fail(MNNB200_INVALID_VALUE, "relu_f32: NULL argument");
+    // the kernel moves float4 words: both buffers must be 16-byte aligned (every device allocation is)
+    if (((uintptr_t)x & 15) || ((uintptr_t)y & 15)) return fail(MNNB200_INVALID_VALUE, "relu_f32: x / y not 16-byte aligned");
     if (count == 0) return MNNB200_OK;
     CK(launch_relu_f32(x, y, count, slope, rt->stream));
     return MNNB200_OK;

@@ -461,9 +461,13 @@ __global__ void pool_f32_kernel(const PoolParams p, const float* __restrict__ x,
                 }
             r = interior ? sum : __fmul_rn(sum, div);
         } else {
-            r = -3.4028234663852886e38f;
-            for (int ky = khs; ky < khe; ++ky)
-                for (int kx = kws; kx < kwe; ++kx) r = fmaxf(r, xp[(size_t)(iy0 + ky) * p.IW + ix0 + kx]);
+            // pooling_max_pad (CPUPool.hpp:19-51) reads the edge row / column for a tap in the padding, so a window wholly in
+            // the padding (large pads, ceil mode) takes its edge's maximum; the reduction starts at VEC(-16777216)
+            const int ys = min(max(iy0, 0), p.IH - 1), ye = min(max(iy0 + p.KH - 1, 0), p.IH - 1);
+            const int xs = min(max(ix0, 0), p.IW - 1), xe = min(max(ix0 + p.KW - 1, 0), p.IW - 1);
+            r = -16777216.f;
+            for (int yy = ys; yy <= ye; ++yy)
+                for (int xx = xs; xx <= xe; ++xx) r = fmaxf(r, xp[(size_t)yy * p.IW + xx]);
         }
         y[i] = r;
     }

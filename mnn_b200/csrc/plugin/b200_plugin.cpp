@@ -725,9 +725,9 @@ public:
         } else if (mP->padType() == PoolPadType_VALID) {
             pw = ph = 0;
         }
-        if (!mP->isGlobal() && mP->pads() != nullptr && mP->padType() == PoolPadType_CAFFE && mP->pads()->size() == 4) {
-            ph = mP->pads()->data()[0]; pw = mP->pads()->data()[1];
-            padType = (int)PoolPadType_VALID;
+        if (!mP->isGlobal() && mP->pads() != nullptr && mP->padType() == PoolPadType_CAFFE) {   // CPUPool.cpp:67-73
+            if (mP->pads()->size() == 4) { ph = mP->pads()->data()[0]; pw = mP->pads()->data()[1]; }
+            padType = (int)PoolPadType_VALID;   // any pads vector: DEFAULT counting then excludes the padding
         }
         return toErr(mnnb200_pool_f32(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(in), in->batch(), in->channel(),
                                       in->height(), in->width(), kh, kw, sh, sw, ph, pw, padType, (int)mP->countType(),

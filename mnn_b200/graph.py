@@ -50,6 +50,23 @@ def pool_out_and_pad(h, w, a):
     return oh, ow, ph, pw
 
 
+def float_pool_params(h, w, a):
+    """What CPUPool::onResize (CPUPool.cpp:25-75) hands to the float pooling functions:
+    -> (oh, ow, kernel, stride, begin pads, pad type).  Unlike CPUPoolInt8 it keeps the op's kernel unclamped, also in the
+    SAME pad; and a CAFFE pool that carries a `pads` vector, of any length, runs as VALID, so that DEFAULT counting
+    excludes the padding."""
+    pt = a.get("pad_type", 0)
+    if a.get("is_global"):
+        return 1, 1, (h, w), (h, w), (0, 0), pt
+    oh, ow, ph, pw = pool_out_and_pad(h, w, a)
+    (kh, kw), (sh, sw) = a["kernel"], a["stride"]
+    if pt == 2:
+        ph, pw = max(0, (oh - 1) * sh + kh - h) // 2, max(0, (ow - 1) * sw + kw - w) // 2
+    if pt == 0 and a.get("pads") is not None:
+        pt = 1
+    return oh, ow, (kh, kw), (sh, sw), (ph, pw), pt
+
+
 def infer_shapes(net: Net, input_shape) -> Dict[int, tuple]:
     shapes: Dict[int, tuple] = {}
     for op in net.ops:

@@ -186,11 +186,14 @@ def binary_add_int8(x0, q0, x1, q1, qo):
     return y
 
 
-def avgpool_int8_via_float(x, kernel, stride, pad, qi, qo, pad_type=1, count_type=0):
+def avgpool_int8_via_float(x, kernel, stride, pad, qi, qo, pad_type=1, count_type=0, out=None):
+    """out = (oh, ow) when the output size comes from pool_resolve (pads, ceil mode, kernels larger than the input)"""
     x = np.ascontiguousarray(x, np.int8)
     n, c, ih, iw = x.shape
     kh, kw = kernel
-    if pad_type == 2:
+    if out is not None:
+        oh, ow = out
+    elif pad_type == 2:
         oh, ow = -(-ih // stride[0]), -(-iw // stride[1])
     elif pad_type == 1:
         oh, ow = (ih - kh) // stride[0] + 1, (iw - kw) // stride[1] + 1
@@ -409,6 +412,125 @@ def ref_matmul(a, b, transpose_a=False, transpose_b=False):
         open(req, "wb").write(hdr + a3.tobytes() + b3.tobytes())
         _run_refdump(["matmul", req, out])
         return np.fromfile(out, np.float32).reshape(a.shape[:-2] + (e, h))
+
+
+# --------------------------------------------------------------------------------------------
+# float Pooling: output size of ShapePool (source/shape/ShapePool.cpp:38-77), the kernel / stride / pad / pad type that
+# CPUPool::onResize hands to the pooling function (source/backend/cpu/CPUPool.cpp:25-75), and poolingAvg / poolingMax
+# (CPUPool.hpp:19-394) in their fp32 operation order.  Restated in numpy; pinned on the reference by tests/test_pool.py.
+# --------------------------------------------------------------------------------------------
+POOL_CAFFE, POOL_VALID, POOL_SAME = 0, 1, 2
+
+
+def pool_resolve(ih, iw, kernel, stride, pad=(0, 0), pads=None, pad_type=POOL_CAFFE, ceil_model=True, is_global=False):
+    """-> (oh, ow, (kh, kw), (sh, sw), (ph, pw), pad_type): pad = (padY, padX) of the op; pads = Pool.pads or None.
+    A CAFFE pool that carries a `pads` vector of any length runs as VALID (so DEFAULT counting excludes the padding);
+    only a 4-value `pads` replaces the begin pads."""
+    (kh, kw), (sh, sw), (ph, pw) = kernel, stride, pad
+    if is_global:
+        return 1, 1, (ih, iw), (ih, iw), (0, 0), pad_type
+    h, w = ih, iw
+    if pads is not None:
+        if len(pads) == 2:
+            h += pads[0] + pads[1]
+        elif len(pads) == 4:
+            h += pads[0] + pads[2]
+            w += pads[1] + pads[3]
+    else:
+        h += 2 * ph
+        w += 2 * pw
+    ckh, ckw = min(kh, h), min(kw, w)             # ShapePool clamps the kernel for the output size only
+    if pad_type == POOL_SAME:
+        oh, ow = -(-h // sh), -(-w // sw)
+    elif pad_type == POOL_VALID:
+        oh, ow = -(-(h - ckh + 1) // sh), -(-(w - ckw + 1) // sw)
+    elif ceil_model:
+        oh, ow = -(-(h - ckh) // sh) + 1, -(-(w - ckw) // sw) + 1
+    else:
+        oh, ow = (h - ckh) // sh + 1, (w - ckw) // sw + 1
+    if pad_type == POOL_SAME:
+        ph, pw = max(0, (oh - 1) * sh + kh - ih) // 2, max(0, (ow - 1) * sw + kw - iw) // 2
+    elif pad_type == POOL_VALID:
+        ph, pw = 0, 0
+    if pads is not None and pad_type == POOL_CAFFE:
+        if len(pads) == 4:
+            ph, pw = pads[0], pads[1]
+        pad_type = POOL_VALID
+    return oh, ow, (kh, kw), (sh, sw), (ph, pw), pad_type
+
+
+def pool_f32(x, is_avg, kernel, stride, pad=(0, 0), pads=None, pad_type=POOL_CAFFE, count_type=0, ceil_model=True,
+             is_global=False):
+    """x fp32 [n][c][ih][iw] -> the reference CPU backend's float Pooling output, bit for bit.
+    count_type: 0 DEFAULT (INCLUDE_PADDING for a CAFFE pad type after resolution, else EXCLUDE), 1 INCLUDE, 2 EXCLUDE."""
+    x = np.ascontiguousarray(x, np.float32)
+    n, c, ih, iw = x.shape
+    oh, ow, (kh, kw), (sh, sw), (ph, pw), pt = pool_resolve(ih, iw, kernel, stride, pad, pads, pad_type, ceil_model, is_global)
+    if count_type == 0:
+        count_type = 1 if pt == POOL_CAFFE else 2
+    f32 = np.float32
+    y = np.empty((n, c, oh, ow), np.float32)
+    # the "mid rect" of poolingAvg / poolingMax: windows that lie wholly inside the input
+    l, t, r, b = 0, 0, ow, oh
+    while l * sw - pw < 0 and l < ow:
+        l += 1
+    while t * sh - ph < 0 and t < oh:
+        t += 1
+    while (r - 1) * sw - pw + (kw - 1) >= iw and r > l:
+        r -= 1
+    while (b - 1) * sh - ph + (kh - 1) >= ih and b > t:
+        b -= 1
+    for oy in range(oh):
+        for ox in range(ow):
+            iy0, ix0 = oy * sh - ph, ox * sw - pw
+            inner = t <= oy < b and l <= ox < r
+            if not is_avg:
+                # pooling_max_pad reads the edge row / column for a tap in the padding; VEC(MAXVALUE) = -2^24 starts the max
+                m = np.full((n, c), f32(-16777216.0))
+                for ky in range(kh):
+                    yy = min(max(iy0 + ky, 0), ih - 1)
+                    for kx in range(kw):
+                        m = np.maximum(m, x[:, :, yy, min(max(ix0 + kx, 0), iw - 1)])
+                y[:, :, oy, ox] = m
+                continue
+            s = np.zeros((n, c), np.float32)
+            if inner:
+                div = f32(1.0) / f32(kh * kw)
+                for ky in range(kh):
+                    for kx in range(kw):
+                        s = (s + x[:, :, iy0 + ky, ix0 + kx] * div).astype(np.float32)
+                y[:, :, oy, ox] = s
+                continue
+            khs, khe = max(0, -iy0), min(kh, ih - iy0)
+            kws, kwe = max(0, -ix0), min(kw, iw - ix0)
+            if count_type == 1:
+                count = (min(iy0 + kh, ih + ph) - iy0) * (min(ix0 + kw, iw + pw) - ix0)
+            else:
+                count = (khe - khs) * (kwe - kws)
+            for ky in range(khs, khe):
+                for kx in range(kws, kwe):
+                    s = (s + x[:, :, iy0 + ky, ix0 + kx]).astype(np.float32)
+            y[:, :, oy, ox] = s * (f32(1.0) / f32(count)) if count > 0 else f32(0)
+    return y
+
+
+def ref_pool_f32(x, is_avg, kernel, stride, pad=(0, 0), pads=None, pad_type=POOL_CAFFE, count_type=0, ceil_model=True,
+                 is_global=False):
+    """ONE float Pooling op through the reference CPU backend (refdump poolf)."""
+    x = np.ascontiguousarray(x, np.float32)
+    n, c, ih, iw = x.shape
+    pv = [] if pads is None else list(pads)
+    hdr = struct.pack("<16i", n, c, ih, iw, kernel[0], kernel[1], stride[0], stride[1], pad[0], pad[1], int(is_avg),
+                      int(pad_type), int(count_type), int(ceil_model), int(is_global), -1 if pads is None else len(pv))
+    hdr += struct.pack(f"<{len(pv)}i", *pv)
+    with tempfile.TemporaryDirectory() as d:
+        req, out = os.path.join(d, "req.bin"), os.path.join(d, "out.bin")
+        with open(req, "wb") as f:
+            f.write(hdr + x.tobytes())
+        _run_refdump(["poolf", req, out])
+        raw = open(out, "rb").read()
+    dims = struct.unpack("<4i", raw[:16])
+    return np.frombuffer(raw[16:], np.float32).reshape(dims).copy()
 
 
 # --------------------------------------------------------------------------------------------

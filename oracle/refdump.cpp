@@ -357,6 +357,62 @@ static int cmdPool(const char* reqPath, const char* outPath) {
     return 0;
 }
 
+struct PoolFReq { int32_t n, c, ih, iw, kh, kw, sh, sw, ph, pw, isAvg, padType, countType, ceilModel, isGlobal, npads; };
+// poolf <req.bin> <out.bin>: {Input, Pooling} on float tensors (no quant info: CPUPool with the core's MNNPoolingAvg /
+// MNNPoolingMax).  npads = -1: no Pool.pads vector, else npads int32 values follow the header, then x [n][c][ih][iw] fp32.
+// Writes int32 dims[4] + y fp32 NCHW.
+static int cmdPoolF(const char* reqPath, const char* outPath) {
+    auto buf = readFile(reqPath);
+    PoolFReq r; memcpy(&r, buf.data(), sizeof(r));
+    const char* p = buf.data() + sizeof(r);
+    std::vector<int32_t> pads(r.npads > 0 ? r.npads : 0);
+    if (!pads.empty()) { memcpy(pads.data(), p, pads.size() * 4); p += pads.size() * 4; }
+    const float* x = (const float*)p;
+    std::unique_ptr<NetT> net(new NetT);
+    net->tensorName = {"x", "y"}; net->outputName = {"y"}; net->sourceType = NetSource_CAFFE;
+    {
+        std::unique_ptr<OpT> in(new OpT);
+        in->type = OpType_Input; in->name = "x"; in->outputIndexes = {0};
+        in->main.type = OpParameter_Input; in->main.value = new InputT;
+        auto ip = in->main.AsInput();
+        ip->dims = {r.n, r.c, r.ih, r.iw}; ip->dtype = DataType_DT_FLOAT; ip->dformat = MNN_DATA_FORMAT_NC4HW4;
+        net->oplists.emplace_back(std::move(in));
+    }
+    {
+        std::unique_ptr<OpT> op(new OpT);
+        op->type = OpType_Pooling; op->name = "y"; op->inputIndexes = {0}; op->outputIndexes = {1};
+        op->main.type = OpParameter_Pool; op->main.value = new PoolT;
+        auto pl = op->main.AsPool();
+        pl->kernelX = r.kw; pl->kernelY = r.kh; pl->strideX = r.sw; pl->strideY = r.sh; pl->padX = r.pw; pl->padY = r.ph;
+        pl->type = r.isAvg ? PoolType_AVEPOOL : PoolType_MAXPOOL; pl->padType = (PoolPadType)r.padType;
+        pl->countType = (AvgPoolCountType)r.countType; pl->ceilModel = r.ceilModel != 0; pl->isGlobal = r.isGlobal != 0;
+        if (r.npads >= 0) pl->pads = pads;
+        net->oplists.emplace_back(std::move(op));
+    }
+    flatbuffers::FlatBufferBuilder fb(1024);
+    fb.Finish(Net::Pack(fb, net.get()));
+    std::shared_ptr<Interpreter> itp(Interpreter::createFromBuffer(fb.GetBufferPointer(), fb.GetSize()), Interpreter::destroy);
+    ScheduleConfig c; c.type = MNN_FORWARD_CPU; c.numThread = 1;
+    BackendConfig bc; bc.precision = BackendConfig::Precision_High; c.backendConfig = &bc;
+    auto s = itp->createSession(c);
+    if (!s) return 2;
+    auto input = itp->getSessionInput(s, nullptr);
+    {
+        Tensor host(input, Tensor::CAFFE);
+        memcpy(host.host<float>(), x, (size_t)host.elementSize() * 4);
+        input->copyFromHostTensor(&host);
+    }
+    if (itp->runSession(s) != NO_ERROR) return 2;
+    auto output = itp->getSessionOutput(s, nullptr);
+    Tensor hostOut(output, Tensor::CAFFE);
+    output->copyToHostTensor(&hostOut);
+    int32_t hdr[4] = {hostOut.length(0), hostOut.length(1), hostOut.length(2), hostOut.length(3)};
+    std::ofstream o(outPath, std::ios::binary);
+    o.write((const char*)hdr, sizeof(hdr));
+    o.write((const char*)hostOut.host<float>(), (size_t)hostOut.elementSize() * 4);
+    return 0;
+}
+
 struct LinReq { int32_t tokens, ic, oc, asym, relu, relu6, hasBias, pad; };   // pad = number of K blocks of the weight scales (0 / 1: per channel)
 // linear <req.bin> <out.bin>: weight-quantised Conv1x1 (what MNN-LLM lowers nn.Linear to,
 // transformers/llm/export/utils/mnn_converter.py:767-787) run with Memory_Low => W8A8 dynamic quant.
@@ -686,6 +742,7 @@ int main(int argc, char** argv) {
     std::string cmd = argv[1];
     if (cmd == "conv" && argc >= 4) return cmdConv(argv[2], argv[3]);
     if (cmd == "pool" && argc >= 4) return cmdPool(argv[2], argv[3]);
+    if (cmd == "poolf" && argc >= 4) return cmdPoolF(argv[2], argv[3]);
     if (cmd == "matmul" && argc >= 4) return cmdMatMul(argv[2], argv[3]);
     if (cmd == "wino" && argc >= 4) return cmdWino(argv[2], argv[3]);
     if (cmd == "linear" && argc >= 4) return cmdLinear(argv[2], argv[3], argc > 4 ? atoi(argv[4]) : 1);

@@ -198,10 +198,27 @@ def matmul_golden():
     print("matmul_golden.npz:", len(CASES), "cases")
 
 
+def pool_golden():
+    """float Pooling outputs of the real reference CPU backend (refdump poolf): AVE on every config of tests/test_pool.py, MAX
+    on the ones whose windows start past the input or lie wholly in the padding."""
+    from tests.test_pool import POOL_CONFIGS, pool_input, pool_kwargs
+    rng = np.random.default_rng(909)
+    out = {}
+    cases = [(ci, True) for ci in range(len(POOL_CONFIGS))] + [(3, False), (14, False), (18, False)]
+    for i, (ci, is_avg) in enumerate(cases):
+        x = pool_input(rng, 2, 3, POOL_CONFIGS[ci])
+        out.update({f"p{i}_cfg": ci, f"p{i}_avg": int(is_avg), f"p{i}_x": x,
+                    f"p{i}_y": O.ref_pool_f32(x, is_avg, **pool_kwargs(POOL_CONFIGS[ci]))})
+    out["ncase"] = len(cases)
+    np.savez_compressed(os.path.join(HERE, "pool_golden.npz"), **out)
+    print("pool_golden.npz:", len(cases), "cases")
+
+
 if __name__ == "__main__":
-    # python tests/golden/make_golden.py [conv] [dw_linear] [block_linear] [hashes] [checkpoints] [wino] [matmul]   (default: all)
+    # python tests/golden/make_golden.py [conv] [dw_linear] [block_linear] [hashes] [checkpoints] [wino] [matmul] [pool]
+    # (default: all)
     assert O.have_reference(), "build oracle/_ref first: python oracle/build_ref.py"
-    which = set(sys.argv[1:]) or {"conv", "dw_linear", "block_linear", "hashes", "checkpoints", "wino", "matmul"}
+    which = set(sys.argv[1:]) or {"conv", "dw_linear", "block_linear", "hashes", "checkpoints", "wino", "matmul", "pool"}
     if "conv" in which:
         conv_golden()
     if "dw_linear" in which:
@@ -216,3 +233,5 @@ if __name__ == "__main__":
         wino_golden()
     if "matmul" in which:
         matmul_golden()
+    if "pool" in which:
+        pool_golden()

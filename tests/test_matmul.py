@@ -41,6 +41,7 @@ def test_oracle_vs_live_reference():
 
 
 def run_matmul(backend, a, b, ta, tb, bias=None):
+    """a, b: fp32 or fp16 host arrays (fp16 operands select the f16 wgmma kernel)"""
     import torch
     from mnn_b200.backend import Op, Tensor
     dev = backend.runtime.device
@@ -79,3 +80,89 @@ def test_gpu_attention_shapes_vs_oracle(backend, bd, e, l, h, ta, tb):
     y = run_matmul(backend, a, b, ta, tb, bias)
     ref = O.matmul_f32(a, b, ta, tb, bias)
     assert np.abs(y - ref).max() <= 1e-3 * np.abs(ref).max(), np.abs(y - ref).max() / np.abs(ref).max()
+
+
+# ---- every element against float64 ------------------------------------------------------------------------------------
+# Worst-case model of the tensor-core accumulator: each wgmma k-step adds K products (K = 16 fp16 / 8 tf32) to the fp32
+# accumulator by aligning all K + 1 terms to the largest exponent and truncating, then truncating the normalised sum to
+# 24 bits.  Each step then errs by at most (K + 2) 2^-23 times the magnitude sum of its terms, which is at most
+# S = sum_k |a_ik| |b_kj|; over ceil(l / K) steps the accumulation error is <= (K + 2) ceil(l / K) 2^-23 S.
+# fp16 operands: products of 11-bit significands are exact in fp32, so that is all.  fp32 operands are read as tf32 (10-bit
+# mantissa, truncated): each operand errs by < 2^-10 relative, a product by < 2^-9 + 2^-20.  The epilogue's bias add
+# rounds once: <= 2^-24 |C + bias|, which 2^-23 (S + |bias|) covers.
+def tolerance(a64, b64, l, f16, bias):
+    s = np.matmul(np.abs(a64), np.abs(b64))
+    k = 16 if f16 else 8
+    tau = (k + 2) * -(-l // k) * 2.0 ** -23 + (0.0 if f16 else 2.0 ** -9 + 2.0 ** -20)
+    return tau * s + 2.0 ** -23 * (s + (0.0 if bias is None else np.abs(bias.astype(np.float64))))
+
+
+def check_vs_float64(y, a, b, ta, tb, bias):
+    f16 = a.dtype == np.float16
+    a64, b64 = a.astype(np.float64), b.astype(np.float64)
+    if ta:
+        a64 = np.swapaxes(a64, -1, -2)
+    if tb:
+        b64 = np.swapaxes(b64, -1, -2)
+    ref = np.matmul(a64, b64) + (0.0 if bias is None else bias.astype(np.float64))
+    assert y.shape == ref.shape and not np.isnan(y).any()
+    err, tol = np.abs(y - ref), tolerance(a64, b64, a64.shape[-1], f16, bias)
+    assert (err <= tol).all(), f"{np.count_nonzero(err > tol)} elements over; worst excess {(err - tol).max():.3g}"
+    # the ABI's accuracy contract against the CPU backend's fp32 matmul (O.matmul_f32 is pinned on it above)
+    c32 = O.matmul_f32(a.astype(np.float32), b.astype(np.float32), ta, tb, bias)
+    assert np.abs(y - c32).max() <= 1e-3 * np.abs(c32).max()
+
+
+# (batch dims, e, l, h, bias): l in {1, 3, 4, 8, 9, 65, 200}; batches with e % 128 != 0 (a 128-row tile spans two batches);
+# h > 256 (several N chunks); odd h with bias (the scalar store of the last column); e = 1
+MM_SHAPES = [((), 37, 1, 29, True), ((), 64, 3, 40, False), ((3,), 200, 4, 24, False), ((2,), 130, 8, 300, False),
+             ((), 1, 9, 17, True), ((2,), 150, 65, 33, True), ((), 129, 200, 513, True)]
+
+
+@pytest.mark.gpu
+@pytest.mark.parametrize("f16", [False, True], ids=["tf32", "f16"])
+@pytest.mark.parametrize("ta,tb", [(False, False), (False, True), (True, False), (True, True)])
+@pytest.mark.parametrize("si", range(len(MM_SHAPES)))
+def test_gpu_matmul_vs_float64(backend, si, ta, tb, f16):
+    bd, e, l, h, has_bias = MM_SHAPES[si]
+    rng = np.random.default_rng(si * 8 + ta * 4 + tb * 2 + f16)
+    a, b = make(rng, bd, e, l, h, ta, tb)
+    if f16:
+        a, b = a.astype(np.float16), b.astype(np.float16)
+    bias = rng.uniform(-1, 1, h).astype(np.float32) if has_bias else None
+    check_vs_float64(run_matmul(backend, a, b, ta, tb, bias), a, b, ta, tb, bias)
+
+
+@pytest.mark.gpu
+def test_gpu_matmul_rebinds_and_packs_misaligned(backend):
+    """One execution run three times: on aligned K-major operands (read in place), on other aligned buffers (the cached
+    tensor maps must follow the pointers), and on operands that start one float past a 16-byte boundary (must take the
+    pack path)."""
+    import torch
+    from mnn_b200.backend import Op, Tensor
+    bd, e, l, h = (2,), 150, 64, 72          # ta = 0, tb = 1, l % 4 == 0: both operands can be read in place
+    rng = np.random.default_rng(21)
+    bias = rng.uniform(-1, 1, h).astype(np.float32)
+
+    def dev(x, shift):
+        buf = torch.empty(x.size + shift, dtype=torch.float32, device=backend.runtime.device)
+        v = buf[shift:].view(x.shape)
+        v.copy_(torch.from_numpy(x))
+        assert (v.data_ptr() % 16 == 0) == (shift == 0)
+        return v
+
+    ex, y, seen = None, Tensor((1,), "float"), []
+    for shift in (0, 0, 1):
+        a, b = make(rng, bd, e, l, h, False, True)
+        ta_, tb_ = Tensor(a.shape, "float", None, dev(a, shift)), Tensor(b.shape, "float", None, dev(b, shift))
+        assert ta_.data.data_ptr() not in [t.data.data_ptr() for t in seen]
+        seen.append(ta_)
+        if ex is None:
+            ex = backend.onCreate([ta_, tb_], [y], Op(type="BatchMatMul", bias=bias, extra=dict(transpose_a=False,
+                                                                                                   transpose_b=True)))
+            assert ex is not None and ex.onResize([ta_, tb_], [y]) == 0
+            backend.onAcquire(y)
+        y.data.fill_(float("nan"))
+        assert ex.onExecute([ta_, tb_], [y]) == 0
+        backend.onSync()
+        check_vs_float64(y.data.cpu().numpy(), a, b, False, True, bias)
