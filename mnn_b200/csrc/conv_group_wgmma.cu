@@ -82,13 +82,13 @@ __device__ __forceinline__ int requant_fast_small(int acc_u, float wscale, float
     return __float2int_rz(__fadd_rn(f, h));
 }
 
-// work item = `cnt` consecutive M tiles of one (layer, n chunk): layer << 26 | n chunk << 20 | (cnt - 1) << 14 | first m tile.
+// work item = `cnt` consecutive M tiles of one (layer, n chunk), encoded as kernels.h describes.
 // The producer pays its per-item bookkeeping (schedule word, layer parameters, descriptors) once per item.
 __device__ __forceinline__ void decode_item(uint32_t w, int& layer, int& nc, int& mt, int& cnt) {
-    layer = (int)(w >> 26);
-    nc = (int)((w >> 20) & 0x3fu);
-    cnt = (int)((w >> 14) & 0x3fu) + 1;
-    mt = (int)(w & 0x3fffu);
+    layer = (int)(w >> kGroupItemLayerShift);
+    nc = (int)((w >> kGroupItemChunkShift) & kGroupItemChunkMask);
+    cnt = (int)((w >> kGroupItemCountShift) & kGroupItemCountMask) + 1;
+    mt = (int)(w & kGroupItemTileMask);
 }
 
 __global__ void __launch_bounds__(kThreads, 1)
@@ -219,7 +219,7 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                     // this loop runs on ONE thread, once per K block: everything that can be hoisted is (tap -> (kh, kw) by
                     // counters, stride 1 / 2 parity by mask and shift, the first two boxes' coordinates in registers)
                     int cc = 0, kh = 0, kw = 0, bk = 0;
-                    const int swm = sw - 1;                          // sw is 1 or 2 (conv_group_mode)
+                    const int swm = sw - 1;                          // sw is 1 or 2 (conv_plan)
                     const int n0 = rb_n[0], ih00 = rb_ih0[0], iw00 = rb_iw0[0];
                     const int n1 = rb_n[1], ih01 = rb_ih0[1], iw01 = rb_iw0[1];
                     const uint32_t key0 = ((uint32_t)L << 16) | ((uint32_t)nc << 8);
@@ -312,7 +312,7 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
             const int bn = lp.bn, n0 = nc * bn, cb = lp.cb;
             const int ncols = (lp.N - n0) < bn ? (lp.N - n0) : bn;      // valid (16-padded) columns of this chunk
             const int nblk = ncols >> 3;
-            if ((w >> 20) != cached) {
+            if ((w >> kGroupItemChunkShift) != cached) {
                 // reload the per-column constants once every consumer is done READING the previous item's, then publish
                 named_sync(1, kConsumerThreads);
                 for (int j = ct; j < ncols; j += kConsumerThreads) {
@@ -323,7 +323,7 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                     reinterpret_cast<int*>(cst)[2 * kMaxBN + j] = v ? lp.wsum128[n] : 0;
                 }
                 named_sync(1, kConsumerThreads);
-                cached = w >> 20;
+                cached = w >> kGroupItemChunkShift;
             }
             const float scale_x = lp.scale_x, minv = lp.minv, maxv = lp.maxv;
             const bool small_acc = lp.K <= 128;    // |sum (x + 128) w| <= 128 * 255 * 128 < 2^22

@@ -68,14 +68,13 @@ cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& p, const void* tmap_a, cons
 constexpr int kGroupMaxLayers = 64;
 constexpr int kGroupMaxBN = 128;     // 64 accumulator registers per consumer thread
 constexpr uint32_t kGroupSchedEnd = 0xffffffffu;
-struct alignas(64) GroupLayerMaps { CUtensorMap_st_opaque a, b, a1, pad_; };   // a1: odd-column view (stride 2, mode 1)
 // The TMA descriptors of ALL layers travel as ONE __grid_constant__ kernel parameter (24 KB of the 32 KB parameter space): a
 // descriptor that lives in global memory is re-fetched by the TMA unit for every cp.async.bulk.tensor (measured: ~1 us per
 // instruction, 2.8 us per work item with nothing else left in the kernel), one in the parameter bank is not.
 struct GroupMapsParam {
     CUtensorMap_st_opaque a[kGroupMaxLayers];
     CUtensorMap_st_opaque b[kGroupMaxLayers];
-    CUtensorMap_st_opaque a1[kGroupMaxLayers];
+    CUtensorMap_st_opaque a1[kGroupMaxLayers];   // odd-column view (stride 2, mode 1)
 };
 struct GroupLayerParams {            // copied to shared memory by every CTA
     int8_t* y;
@@ -99,7 +98,12 @@ struct GroupConvGeom {               // mode 1 only; stays in global memory (rea
     const int32_t* corr;             // [HC*WC][N] z_in * sum over the out-of-image taps of sum_c w[oc][tap][c]
     int wc_count, interior_cls;
 };
-// schedule: grid rows of sched_stride items, item = layer << 26 | n_chunk << 20 | (tiles - 1) << 14 | first m_tile, each row ends with kGroupSchedEnd
+// schedule: grid rows of sched_stride items, each row ends with kGroupSchedEnd.  item = layer << 26 | n chunk << 20 |
+// (tiles - 1) << 14 | first m tile; the host puts one M tile in every item (tile count field 0).  A layer whose n chunks or
+// M tiles these fields cannot hold is not taken by the conv-group kernel.
+constexpr int kGroupItemLayerShift = 26, kGroupItemChunkShift = 20, kGroupItemCountShift = 14;
+constexpr uint32_t kGroupItemChunkMask = 0x3fu, kGroupItemCountMask = 0x3fu, kGroupItemTileMask = 0x3fffu;
+constexpr int kGroupMaxNChunks = 63, kGroupMaxMTiles = 16383;
 cudaError_t launch_conv_group(const GroupMapsParam* maps_host, const GroupLayerParams* params, const GroupConvGeom* geom, int n_layers,
                               const uint32_t* sched, int sched_stride, int grid, cudaStream_t stream);
 

@@ -436,27 +436,40 @@ def test_conv_group_mixed_gemm_and_implicit_members(backend):
         assert np.array_equal(y, ref), (c["w"].shape, np.abs(y.astype(int) - ref.astype(int)).max())
 
 
-def test_conv_group_rejects_unsupported_member(backend):
+def _check_group_rejects(backend, ic, k, stride, pad, ih, iw):
+    """A conv the conv-group kernel cannot take: not groupable, bind refuses it, auto execute still runs it right."""
     from mnn_b200.backend import ConvGroupExecution, Op, QuantAttr, Tensor
     rng = np.random.default_rng(3)
-    c = random_modern_case(rng, 16, 16, 3, 3, 1, 9, 9, (1, 3), (1, 1), 0)       # stride_w = 3: not on the wgmma kernels
-    op = Op(type="ConvInt8", conv=dict(ic=16, oc=16, kernel=(3, 3), stride=(1, 3), pad=(1, 1), dilate=(1, 1), group=1, relu=False),
+    c = random_modern_case(rng, ic, ic, k, k, 1, ih, iw, stride, pad, 0)
+    op = Op(type="ConvInt8", conv=dict(ic=ic, oc=ic, kernel=(k, k), stride=stride, pad=pad, dilate=(1, 1), group=1, relu=False),
             weight=c["w"], wscale=c["ws"], bias=c["bias"])
-    xin = backend.onAcquire(Tensor((1, 16, 9, 9), "int8", QuantAttr(c["s_in"], c["z_in"], -128, 127)))
+    xin = backend.onAcquire(Tensor((1, ic, ih, iw), "int8", QuantAttr(c["s_in"], c["z_in"], -128, 127)))
     backend.onCopyBuffer(c["x"], xin)
-    yout = Tensor((1, 16, 1, 1), "int8", QuantAttr(c["s_out"], c["z_out"], -127, 127))
+    yout = Tensor((1, ic, 1, 1), "int8", QuantAttr(c["s_out"], c["z_out"], -127, 127))
     ex = backend.onCreate([xin], [yout], op)
     assert ex.onResize([xin], [yout]) == 0
     backend.onAcquire(yout)
     assert not ConvGroupExecution.groupable(ex)
     grp = ConvGroupExecution(backend, [ex])
     assert grp.bind([xin], [yout]) == 2      # NOT_SUPPORT, as Backend::onCreate returning nullptr would signal
-    # ... and the conv itself still runs (mma.sync implicit GEMM) and is right
+    # ... and the conv itself still runs in auto mode (wgmma GEMM or mma.sync implicit GEMM) and is right
     assert ex.onExecute([xin], [yout]) == 0
     backend.onSync()
     bf, sx = O.fold_modern(c["w"], c["ws"], c["bias"], c["s_in"], c["z_in"], c["s_out"], c["z_out"])
-    ref = O.conv_int8(c["x"], c["w"], c["ws"], sx, bf, stride=(1, 3), pad=(1, 1), z_in=c["z_in"], min_v=-127, max_v=127)
+    ref = O.conv_int8(c["x"], c["w"], c["ws"], sx, bf, stride=stride, pad=pad, z_in=c["z_in"], min_v=-127, max_v=127)
     assert np.array_equal(backend.onCopyBuffer(yout, "same"), ref)
+
+
+def test_conv_group_rejects_unsupported_member(backend):
+    _check_group_rejects(backend, 16, 3, (1, 3), (1, 1), 9, 9)        # stride_w = 3: not on the wgmma kernels
+
+
+@pytest.mark.parametrize("ic, k, stride, pad, ih, iw", [
+    (8, 3, (1, 1), (1, 1), 16400, 72),      # implicit GEMM with 16400 M tiles: more than the schedule word holds
+    (8, 1, (1, 1), (0, 0), 1449, 1449),     # 1x1 with 16404 M tiles of 128 rows: likewise
+])
+def test_conv_group_rejects_oversized_member(backend, ic, k, stride, pad, ih, iw):
+    _check_group_rejects(backend, ic, k, stride, pad, ih, iw)
 
 
 def test_scale_and_pool_int8_vs_oracle(backend):

@@ -1,7 +1,7 @@
 """Marginal cost of every layer INSIDE the persistent conv-group launch (MobileNet-v2 int8 conv path, batch 32): the step is
-timed with the full schedule and then with one layer's items left out (MNNB200_GROUP_SKIP); the difference is what that layer
-costs in situ (cache state, co-scheduling with the other layers), next to its algorithmic bytes and the HBM time those bytes
-would take.  Usage (on the GPU): python tools/group_layer_costs.py > layer_costs.json"""
+timed with the group of all layers and then with a group of every layer but one, bound to the same tensors; the difference is
+what that layer costs in situ (cache state, co-scheduling with the other layers), next to its algorithmic bytes and the HBM
+time those bytes would take.  Usage (on the GPU): python tools/group_layer_costs.py > layer_costs.json"""
 import json
 import os
 import sys
@@ -39,16 +39,13 @@ def time_steps(sess, steps=40, warm=5, reps=5):
 def main():
     sess = ConvPathSession(mnn_file.load(open(MODEL, "rb").read()), 32)
     members = [l for l in sess.layers if ConvGroupExecution.groupable(l[1])]
-    xs, ys = [l[2] for l in members], [l[3] for l in members]
 
     def rebuild(skip):
-        if skip is None:
-            os.environ.pop("MNNB200_GROUP_SKIP", None)
-        else:
-            os.environ["MNNB200_GROUP_SKIP"] = str(skip)
-        st = sess.group.bind(xs, ys)
-        assert st == 0, st
+        keep = [l for i, l in enumerate(members) if i != skip]
         sess.graph = None
+        sess.group = ConvGroupExecution(sess.backend, [l[1] for l in keep])
+        st = sess.group.bind([l[2] for l in keep], [l[3] for l in keep])
+        assert st == 0, st
         sess.capture()
 
     rebuild(None)
