@@ -424,7 +424,8 @@ static mnnb200_status group_build(GroupState& gs, const std::vector<ConvInt8Exec
     }
     // round-robin, item i -> CTA i mod grid: every CTA gets the same mix of layers, so the balance needs no cost model
     // (measured on MobileNet-v2 B=32: 0.28 ms against 0.81 ms for a contiguous cost-balanced partition).
-    // Two terminators per row: the epilogue groups walk items i = g, g + 2, ... and must each meet an end marker inside the row.
+    // Every role of a CTA walks its whole row up to the first terminator.  The row keeps a second one so that a walk over
+    // alternate items (i = g, g + 2, ..., one per consumer warpgroup) would also meet an end marker inside the row.
     const int grid = (int)std::min<size_t>(items.size(), (size_t)rt->prop.multiProcessorCount);
     const size_t stride = (items.size() + grid - 1) / grid + 2;
     std::vector<uint32_t> sched(stride * grid, kGroupSchedEnd);

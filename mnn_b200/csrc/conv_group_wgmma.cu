@@ -23,8 +23,8 @@
 //   warp 8:    TMA producer (cp.async.bulk.tensor.2d/4d, 128B / 64B swizzle or 16-byte interleaved chunks, 6-stage ring of
 //              16 KB activation tiles)
 //   warps 0-7: two consumer warpgroups, 64 rows of the 128-row tile each: wgmma.mma_async m64nNk32 s8 (N = bn <= 128,
-//              accumulators in registers) -> CPU-exact requant -> stores straight to the NHWC16 output rows; per-column
-//              constants staged in shared memory per (layer, n chunk)
+//              accumulators in registers; the per-item work is instantiated per bn, see consume_item) -> CPU-exact requant
+//              -> stores straight to the NHWC16 output rows; per-column constants staged in shared memory per (layer, n chunk)
 #include <cuda.h>
 #include <cstdlib>
 #include "common.cuh"
@@ -89,6 +89,122 @@ __device__ __forceinline__ void decode_item(uint32_t w, int& layer, int& nc, int
     nc = (int)((w >> kGroupItemChunkShift) & kGroupItemChunkMask);
     cnt = (int)((w >> kGroupItemCountShift) & kGroupItemCountMask) + 1;
     mt = (int)(w & kGroupItemTileMask);
+}
+
+// One work item on one consumer warpgroup: rows [64 wg, 64 wg + 64) of `cnt` M tiles x BN columns.  BN is a compile-time
+// constant so the accumulator array, the wgmma_span chain and the epilogue's column loop are fixed: a run-time switch on the
+// tile width between two wgmma instructions would make ptxas serialise every one of them.
+template <int BN>
+__device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const GroupConvGeom* __restrict__ gp, int n0, int nblk, int mt0,
+                                             int cnt, uint32_t base, const uint8_t* smem, const float* cst, int& stage, int& phase) {
+    const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+    const int wg = threadIdx.x >> 7;
+    const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
+    const int q4 = lane & 3;
+    // lp lives in shared memory, so ptxas cannot tell these are the same in every lane; the broadcast makes the branches
+    // around the wgmmas provably warp-uniform
+    const int cb = __shfl_sync(0xffffffffu, lp.cb, 0);
+    const int num_kb = __shfl_sync(0xffffffffu, lp.num_kb, 0);
+    const int* wsum = reinterpret_cast<const int*>(cst) + 2 * kMaxBN;
+    const uint32_t bar0 = base + kOffBars;
+    int acc[BN / 2];
+    // defined before the first fence: an undefined accumulator would be live from the kernel's entry, in every instantiation
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
+    const float scale_x = lp.scale_x, minv = lp.minv, maxv = lp.maxv;
+    const bool small_acc = lp.K <= 128;    // |sum (x + 128) w| <= 128 * 255 * 128 < 2^22
+    for (int t = 0; t < cnt; ++t) {
+        const int mt = mt0 + t;
+        int prev = -1;
+        for (int kb = 0; kb < num_kb; ++kb) {
+            mbar_wait(bar0 + 8u * stage, phase);
+            const uint32_t a_addr = base + stage * kStageBytes;
+            const uint32_t b_addr = base + kOffB + (uint32_t)(*reinterpret_cast<const volatile int*>(smem + kOffBSlot + 4 * stage));
+            fence_acc(acc);
+            wgmma_fence();
+            // every K block runs its full count of k-steps in one straight run: a condition per k-step would make ptxas
+            // serialise the wgmmas.  Past the end of a layer's K the weight tile holds zeros from the TMA unit (out-of-bounds
+            // fill), so those k-steps add nothing.
+            if (cb == 128) {
+#pragma unroll
+                for (int k = 0; k < 4; ++k)
+                    wgmma_span<Kind::S8, BN, 0>(acc, gdesc_sw128(a_addr + wg * 64 * 128 + k * 32), gdesc_sw128(b_addr + k * 32), 128,
+                                                (kb | k) != 0);
+            } else if (cb == 64) {
+#pragma unroll
+                for (int k = 0; k < 2; ++k)
+                    wgmma_span<Kind::S8, BN, 0>(acc, gdesc(a_addr + wg * 64 * 64 + k * 32, kSw64, 16, 512),
+                                                gdesc(b_addr + k * 32, kSw64, 16, 512), 64, (kb | k) != 0);
+            } else {
+#pragma unroll
+                for (int u = 0; u < 4; ++u)
+                    wgmma_span<Kind::S8, BN, 0>(acc, gdesc(a_addr + 2 * u * (kBM * 16) + wg * 64 * 16, kSwNone, kBM * 16, 128),
+                                                gdesc(b_addr + 2 * u * (BN * 16), kSwNone, BN * 16, 128), 16, (kb | u) != 0);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();                 // the previous stage's MMAs are done: hand its slot back
+            fence_acc(acc);
+            if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar0 + 8u * (kStages + prev)); }
+            prev = stage;
+            if (++stage == kStages) { stage = 0; phase ^= 1; }
+        }
+        wgmma_wait<0>();
+        fence_acc(acc);
+        __syncwarp();
+        if (lane == 0) mbar_arrive(bar0 + 8u * (kStages + prev));
+
+        // ---- epilogue from the accumulator fragments: register i = row r_base + 8 * ((i >> 1) & 1),
+        //      column 8 * (i >> 2) + 2 * q4 + (i & 1); two output bytes per store
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+            const int r = r_base + 8 * h;
+            int8_t* yrow = nullptr;
+            const int32_t* corrp = nullptr;    // border pixel of a padded conv with z_in != 0: + z_in * sum_{OOB taps} w
+            if (lp.mode == 0) {
+                if (mt * kBM + r < lp.M) yrow = lp.y + (size_t)(mt * kBM + r) * lp.ldy + n0;
+            } else {
+                // implicit-GEMM layers: which output pixel accumulator row r is, and its border class
+                const GroupConvGeom& g = *gp;
+                const int box_rows = g.BH * lp.TWp;
+                const int j = r / box_rows, rem = r - j * box_rows;
+                const int brow = rem / lp.TWp, pcol = rem - brow * lp.TWp;
+                const int rb = mt * lp.R + j;
+                if (j < lp.R && rb < g.rowboxes) {
+                    const int seg = rb % g.SEG, tt = rb / g.SEG;
+                    const int oh = (tt % g.OHB) * g.BH + brow, n = tt / g.OHB;
+                    const int ow = seg * lp.TWp + pcol;
+                    if (ow < g.OW) {
+                        yrow = lp.y + (size_t)((n * g.OH + oh) * g.OW + ow) * lp.ldy + n0;
+                        if (g.corr != nullptr) {
+                            const int cls = (int)g.hcls[oh] * g.wc_count + (int)g.wcls[ow];
+                            if (cls != g.interior_cls) corrp = g.corr + (size_t)cls * lp.N + n0;
+                        }
+                    }
+                }
+            }
+            if (yrow == nullptr) continue;
+#pragma unroll
+            for (int j = 0; j < BN / 8; ++j) {
+                if (j < nblk) {
+                    const int c = j * 8 + 2 * q4;
+                    int k0 = wsum[c], k1 = wsum[c + 1];
+                    if (corrp != nullptr) { k0 += __ldg(corrp + c); k1 += __ldg(corrp + c + 1); }
+                    const int a0 = acc[j * 4 + 2 * h] + k0, a1 = acc[j * 4 + 2 * h + 1] + k1;
+                    int q0, q1;
+                    if (small_acc) {      // |acc_u| < 2^22: int -> float on the FP32 pipe (exact), not on the conversion unit
+                        q0 = requant_fast_small(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
+                        q1 = requant_fast_small(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                    } else {
+                        q0 = requant_fast(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
+                        q1 = requant_fast(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                    }
+                    if (n0 + c >= lp.OC) q0 = 0;         // NHWC16 channel padding stays zero
+                    if (n0 + c + 1 >= lp.OC) q1 = 0;
+                    *reinterpret_cast<uint16_t*>(yrow + c) = (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8));
+                }
+            }
+        }
+    }
 }
 
 __global__ void __launch_bounds__(kThreads, 1)
@@ -257,7 +373,11 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                         ++blk;
                     }
                 } else {
-                    // 16-byte chunks (Cp not a multiple of 64): up to 8 chunks (128 bytes of K) per stage, no swizzle
+                    // 16-byte chunks (Cp not a multiple of 64): up to 8 chunks (128 bytes of K) per stage, no swizzle.  The consumer
+                    // runs all 8 chunks of every K block, so a weight tile always holds 8: past the last one they are all-zero boxes
+                    // (out of bounds), and whatever the activation stage holds there is multiplied by zero.  Only the weights get
+                    // the extra boxes, and only when a tile is loaded: the activation boxes are R per chunk and would be paid for in
+                    // every M tile by this thread.
                     const int taps = g.KH * KW;
                     for (int kb = 0; kb < lp.num_kb; ++kb) {
                         const int q0 = kb * 8;
@@ -267,7 +387,7 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                         const int bs = b_lookup(lp.num_kb > 256 ? (0x80000000u | (uint32_t)blk)
                                                                 : (((uint32_t)L << 16) | ((uint32_t)nc << 8) | (uint32_t)kb), &miss);
                         stage_bslot[stage] = bs;
-                        mbar_expect_tx(full_bar(stage), (uint32_t)(nq * (rows_bytes * 16 + (miss ? lp.bn * 16 : 0))));
+                        mbar_expect_tx(full_bar(stage), (uint32_t)(nq * rows_bytes * 16 + (miss ? 8 * lp.bn * 16 : 0)));
                         const uint32_t a_dst = base + stage * kStageBytes;
                         for (int ql = 0; ql < nq; ++ql) {
                             const int q = q0 + ql;
@@ -280,8 +400,10 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                                 tma_load_4d(a_dst + ql * (kBM * 16) + j * box_rows * 16, par ? ta1 : ta, full_bar(stage), cc * 16,
                                             (iw - par) / sw, rb_ih0[j] + kh * dh, dummy ? g.NB : rb_n[j]);
                             }
-                            if (miss) tma_load_2d(base + kOffB + bs + ql * (lp.bn * 16), tb, full_bar(stage), q * 16, nc * lp.bn);
                         }
+                        if (miss)
+                            for (int ql = 0; ql < 8; ++ql)
+                                tma_load_2d(base + kOffB + bs + ql * (lp.bn * 16), tb, full_bar(stage), (q0 + ql) * 16, nc * lp.bn);
                         if (++stage == kStages) { stage = 0; phase ^= 1; }
                         ++blk;
                     }
@@ -292,16 +414,9 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
     } else {
         // ================= two consumer warpgroups: wgmma main loop + epilogue =================
         const int ct = threadIdx.x;                  // 0..255
-        const int wg = ct >> 7;                      // rows [64 wg, 64 wg + 64) of the tile
-        const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
-        const int q4 = lane & 3;
         float* cst = reinterpret_cast<float*>(smem + kOffConsts);
-        const int* wsum = reinterpret_cast<const int*>(cst) + 2 * kMaxBN;
         uint32_t cached = 0xffffffffu;            // (layer, n chunk) whose constants are in cst
         int stage = 0, phase = 0;
-        int acc[kMaxBN / 2];
-#pragma unroll
-        for (int i = 0; i < kMaxBN / 2; ++i) acc[i] = 0;
 
         for (int i = 0;; ++i) {
             const uint32_t w = my[i];
@@ -309,7 +424,7 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
             int L, nc, mt0, cnt;
             decode_item(w, L, nc, mt0, cnt);
             const GroupLayerParams& lp = sl[L];
-            const int bn = lp.bn, n0 = nc * bn, cb = lp.cb;
+            const int bn = lp.bn, n0 = nc * bn;
             const int ncols = (lp.N - n0) < bn ? (lp.N - n0) : bn;      // valid (16-padded) columns of this chunk
             const int nblk = ncols >> 3;
             if ((w >> kGroupItemChunkShift) != cached) {
@@ -325,97 +440,17 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                 named_sync(1, kConsumerThreads);
                 cached = w >> kGroupItemChunkShift;
             }
-            const float scale_x = lp.scale_x, minv = lp.minv, maxv = lp.maxv;
-            const bool small_acc = lp.K <= 128;    // |sum (x + 128) w| <= 128 * 255 * 128 < 2^22
-            for (int t = 0; t < cnt; ++t) {
-                const int mt = mt0 + t;
-                int prev = -1;
-                for (int kb = 0; kb < lp.num_kb; ++kb) {
-                    mbar_wait(full_bar(stage), phase);
-                    const uint32_t a_addr = base + stage * kStageBytes;
-                    const uint32_t b_addr = base + kOffB + (uint32_t)(*reinterpret_cast<volatile int*>(smem + kOffBSlot + 4 * stage));
-                    fence_acc(acc);
-                    wgmma_fence();
-                    if (cb == 128) {
-                        const int kleft = lp.K - kb * kBK;
-                        const int nmma = (lp.mode != 0 || kleft >= kBK) ? 4 : (kleft + 31) / 32;
-                        for (int k = 0; k < nmma; ++k)
-                            wgmma_bn<Kind::S8, kMaxBN>(acc, bn, gdesc_sw128(a_addr + wg * 64 * 128 + k * 32), gdesc_sw128(b_addr + k * 32), 128,
-                                                       (kb | k) != 0);
-                    } else if (cb == 64) {
-                        for (int k = 0; k < 2; ++k)
-                            wgmma_bn<Kind::S8, kMaxBN>(acc, bn, gdesc(a_addr + wg * 64 * 64 + k * 32, kSw64, 16, 512),
-                                                       gdesc(b_addr + k * 32, kSw64, 16, 512), 64, (kb | k) != 0);
-                    } else {
-                        const int nq = (lp.K / 16 - kb * 8) < 8 ? (lp.K / 16 - kb * 8) : 8;     // K = 16 * chunks (even)
-                        for (int u = 0; u < (nq >> 1); ++u)
-                            wgmma_bn<Kind::S8, kMaxBN>(acc, bn, gdesc(a_addr + 2 * u * (kBM * 16) + wg * 64 * 16, kSwNone, kBM * 16, 128),
-                                                       gdesc(b_addr + 2 * u * (bn * 16), kSwNone, bn * 16, 128), 16, (kb | u) != 0);
-                    }
-                    wgmma_commit();
-                    wgmma_wait<1>();                 // the previous stage's MMAs are done: hand its slot back
-                    fence_acc(acc);
-                    if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(empty_bar(prev)); }
-                    prev = stage;
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                }
-                wgmma_wait<0>();
-                fence_acc(acc);
-                __syncwarp();
-                if (lane == 0) mbar_arrive(empty_bar(prev));
-
-                // ---- epilogue from the accumulator fragments: register i = row r_base + 8 * ((i >> 1) & 1),
-                //      column 8 * (i >> 2) + 2 * q4 + (i & 1); two output bytes per store
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    const int r = r_base + 8 * h;
-                    int8_t* yrow = nullptr;
-                    const int32_t* corrp = nullptr;    // border pixel of a padded conv with z_in != 0: + z_in * sum_{OOB taps} w
-                    if (lp.mode == 0) {
-                        if (mt * kBM + r < lp.M) yrow = lp.y + (size_t)(mt * kBM + r) * lp.ldy + n0;
-                    } else {
-                        // implicit-GEMM layers: which output pixel accumulator row r is, and its border class
-                        const GroupConvGeom& g = geom[L];
-                        const int box_rows = g.BH * lp.TWp;
-                        const int j = r / box_rows, rem = r - j * box_rows;
-                        const int brow = rem / lp.TWp, pcol = rem - brow * lp.TWp;
-                        const int rb = mt * lp.R + j;
-                        if (j < lp.R && rb < g.rowboxes) {
-                            const int seg = rb % g.SEG, tt = rb / g.SEG;
-                            const int oh = (tt % g.OHB) * g.BH + brow, n = tt / g.OHB;
-                            const int ow = seg * lp.TWp + pcol;
-                            if (ow < g.OW) {
-                                yrow = lp.y + (size_t)((n * g.OH + oh) * g.OW + ow) * lp.ldy + n0;
-                                if (g.corr != nullptr) {
-                                    const int cls = (int)g.hcls[oh] * g.wc_count + (int)g.wcls[ow];
-                                    if (cls != g.interior_cls) corrp = g.corr + (size_t)cls * lp.N + n0;
-                                }
-                            }
-                        }
-                    }
-                    if (yrow == nullptr) continue;
-#pragma unroll
-                    for (int j = 0; j < kMaxBN / 8; ++j) {
-                        if (j < nblk) {
-                            const int c = j * 8 + 2 * q4;
-                            int k0 = wsum[c], k1 = wsum[c + 1];
-                            if (corrp != nullptr) { k0 += __ldg(corrp + c); k1 += __ldg(corrp + c + 1); }
-                            const int a0 = acc[j * 4 + 2 * h] + k0, a1 = acc[j * 4 + 2 * h + 1] + k1;
-                            int q0, q1;
-                            if (small_acc) {      // |acc_u| < 2^22: int -> float on the FP32 pipe (exact), not on the conversion unit
-                                q0 = requant_fast_small(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
-                                q1 = requant_fast_small(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
-                            } else {
-                                q0 = requant_fast(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
-                                q1 = requant_fast(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
-                            }
-                            if (n0 + c >= lp.OC) q0 = 0;         // NHWC16 channel padding stays zero
-                            if (n0 + c + 1 >= lp.OC) q1 = 0;
-                            *reinterpret_cast<uint16_t*>(yrow + c) = (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8));
-                        }
-                    }
-                }
-            }   // tiles of the item
+            switch (lp.bn >> 4) {     // conv_plan: bn is a multiple of 16 <= kGroupMaxBN
+                case 1: consume_item<16>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 2: consume_item<32>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 3: consume_item<48>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 4: consume_item<64>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 5: consume_item<80>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 6: consume_item<96>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 7: consume_item<112>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 8: consume_item<128>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
+                default: __trap();
+            }
         }
     }
 }
