@@ -172,6 +172,11 @@ MNNB200_API mnnb200_status mnnb200_conv_group_bind(mnnb200_exec* group, const in
 MNNB200_API mnnb200_status mnnb200_conv_group_execute(mnnb200_exec* group);
 /* 1 if the (resized) conv execution can be a member of a conv group */
 MNNB200_API int mnnb200_conv_int8_groupable(mnnb200_exec* e);
+/* read-only view of the resized conv's layer on the conv-group kernel, as resize planned it: the first `count` (at most 10) of
+ * {mode (0 = 1x1 GEMM, 1 = implicit GEMM), cb (bytes of K per TMA chunk: 128 / 64 / 16), bn (tile width), n_chunks, m_tiles,
+ * num_kb (K blocks per tile), K, R (row boxes per M tile), TWp (pixels per row box), BH (output rows per box)} go to fields.
+ * NO_EXECUTION before resize, NOT_SUPPORT if the conv-group kernel does not take the conv.  Changes nothing. */
+MNNB200_API mnnb200_status mnnb200_conv_int8_group_plan(mnnb200_exec* e, int* fields, int count);
 
 /* ---- Int8 Winograd Conv2D F(m x m, 3 x 3), m = 2 / 4 / 6: the op carries a winogradAttr (per-position input scales /
  *      zero points and per-(position, oc) weight scales).  Replaces the structure of ConvWinogradExecution {Resource,

@@ -926,6 +926,16 @@ int mnnb200_conv_int8_groupable(mnnb200_exec* ex) {
     // down (measured on MobileNet-v2 B=32: 0.31 ms with the stem inside the group, 0.19 ms with it outside)
     return e->resized && e->plan.group && (e->plan.gemm || !e->plan.stem);
 }
+mnnb200_status mnnb200_conv_int8_group_plan(mnnb200_exec* ex, int* fields, int count) {
+    if (!ex || ex->kind != 1 || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_int8_group_plan: bad argument");
+    auto* e = static_cast<ConvInt8Exec*>(ex);
+    if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_int8_group_plan before resize");
+    if (!e->plan.group) return fail(MNNB200_NOT_SUPPORT, "conv_int8_group_plan: the conv-group kernel does not take this conv");
+    const GroupLayerParams& q = e->plan.q;
+    const int v[] = {q.mode, q.cb, q.bn, q.n_chunks, q.m_tiles, q.num_kb, q.K, q.R, q.TWp, e->plan.g.BH};
+    for (int i = 0; i < count && i < (int)(sizeof(v) / sizeof(v[0])); ++i) fields[i] = v[i];
+    return MNNB200_OK;
+}
 mnnb200_status mnnb200_conv_group_create(mnnb200_runtime* rt, mnnb200_exec* const* members, int count, mnnb200_exec** out) {
     if (!rt || !members || !out || count <= 0) return fail(MNNB200_INVALID_VALUE, "conv_group_create: bad argument");
     if (count > kGroupMaxLayers) return fail(MNNB200_NOT_SUPPORT, "conv_group_create: more than 64 members");
