@@ -273,6 +273,34 @@ MNNB200_API mnnb200_status mnnb200_matmul_create(mnnb200_runtime* rt, int batch,
                                                  int transpose_b, int inputs_are_f16, mnnb200_exec** out);
 MNNB200_API mnnb200_status mnnb200_matmul_execute(mnnb200_exec* e, const void* a, const void* b, const float* bias, float* c);
 
+/* ---- Float convolutions of fp32 models and their fp32 neighbours: the CPU backend's float path (CPUConvolution /
+ *      ConvolutionTiledExecutor, CPUConvolutionDepthwise, CPUBinary ADD, CPUScale, CPUSoftmax) on NCHW-linear device fp32 tensors.
+ *      Activation: desc->relu = ReLU, relu6 = ReLU6 (CPUConvolution.cpp:289-291), applied after the bias.
+ *      conv_f32: group == 1 (NOT_SUPPORT otherwise), any kernel / stride / dilation / padding.  create takes host weights
+ *                [oc][ic][kh][kw] and bias [oc] (may be NULL) and packs them once on the device as two TF32 halves w = w_hi + w_lo;
+ *                execute runs one split-TF32 wgmma implicit GEMM (a_hi*w_hi + a_hi*w_lo + a_lo*w_hi, fp32 accumulate: error near
+ *                fp32's).  resize plans the launch for the shape (*oh / *ow as in conv_int8_resize); set_pad sets the begin pads
+ *                (ConvolutionCommon::convolutionPad) of a conv_f32 or dwconv_f32 execution, before resize.
+ *      dwconv_f32: group == ic == oc, weights [c][kh][kw].
+ *      binary_add_f32: y = a + b over count elements (equal shapes, no broadcast).
+ *      scale_f32: y[n][c][h][w] = x * scale[c] + bias[c] (bias may be NULL).
+ *      softmax_f32: softmax over the middle axis of an [outside][axis][inside] view. */
+MNNB200_API mnnb200_status mnnb200_conv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight,
+                                                   const float* bias, int relu6, mnnb200_exec** out);
+MNNB200_API mnnb200_status mnnb200_conv_f32_set_pad(mnnb200_exec* e, int pad_h, int pad_w);
+MNNB200_API mnnb200_status mnnb200_conv_f32_resize(mnnb200_exec* e, int n, int ih, int iw, int* oh, int* ow);
+MNNB200_API mnnb200_status mnnb200_conv_f32_execute(mnnb200_exec* e, const float* x_nchw, float* y_nchw);
+MNNB200_API mnnb200_status mnnb200_dwconv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight,
+                                                     const float* bias, int relu6, mnnb200_exec** out);
+MNNB200_API mnnb200_status mnnb200_dwconv_f32_resize(mnnb200_exec* e, int n, int ih, int iw, int* oh, int* ow);
+MNNB200_API mnnb200_status mnnb200_dwconv_f32_execute(mnnb200_exec* e, const float* x_nchw, float* y_nchw);
+MNNB200_API mnnb200_status mnnb200_binary_add_f32(mnnb200_runtime* rt, const float* a, const float* b, float* y, size_t count);
+MNNB200_API mnnb200_status mnnb200_scale_f32_create(mnnb200_runtime* rt, int channels, const float* scale, const float* bias,
+                                                    mnnb200_exec** out);
+MNNB200_API mnnb200_status mnnb200_scale_f32_resize(mnnb200_exec* e, int n, int h, int w);
+MNNB200_API mnnb200_status mnnb200_scale_f32_execute(mnnb200_exec* e, const float* x_nchw, float* y_nchw);
+MNNB200_API mnnb200_status mnnb200_softmax_f32(mnnb200_runtime* rt, const float* x, int outside, int axis, int inside, float* y);
+
 MNNB200_API void mnnb200_exec_destroy(mnnb200_exec* e);
 
 #ifdef __cplusplus

@@ -94,6 +94,18 @@ SIGNATURES = {
     "mnnb200_linear_w8_execute": (C.c_int, [P, P, P]),
     "mnnb200_matmul_create": (C.c_int, [P] + [C.c_int] * 7 + [C.POINTER(P)]),
     "mnnb200_matmul_execute": (C.c_int, [P, P, P, P, P]),
+    "mnnb200_conv_f32_create": (C.c_int, [P, C.POINTER(ConvDesc), P, P, C.c_int, C.POINTER(P)]),
+    "mnnb200_conv_f32_set_pad": (C.c_int, [P, C.c_int, C.c_int]),
+    "mnnb200_conv_f32_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "mnnb200_conv_f32_execute": (C.c_int, [P, P, P]),
+    "mnnb200_dwconv_f32_create": (C.c_int, [P, C.POINTER(ConvDesc), P, P, C.c_int, C.POINTER(P)]),
+    "mnnb200_dwconv_f32_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "mnnb200_dwconv_f32_execute": (C.c_int, [P, P, P]),
+    "mnnb200_binary_add_f32": (C.c_int, [P, P, P, P, C.c_size_t]),
+    "mnnb200_scale_f32_create": (C.c_int, [P, C.c_int, P, P, C.POINTER(P)]),
+    "mnnb200_scale_f32_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int]),
+    "mnnb200_scale_f32_execute": (C.c_int, [P, P, P]),
+    "mnnb200_softmax_f32": (C.c_int, [P, P, C.c_int, C.c_int, C.c_int, P]),
     "mnnb200_exec_destroy": (None, [P]),
 }
 

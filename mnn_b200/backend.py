@@ -421,6 +421,34 @@ class MatMulExecution(Execution):
                                                   None if self.bias is None else C.c_void_p(self.bias.data_ptr()), outputs[0].ptr())
 
 
+class ConvF32Execution(Execution):
+    """Float Convolution (group 1, split-TF32 wgmma) or ConvolutionDepthwise on NCHW fp32 tensors: the CPU backend's float
+    convolutions.  op.weight fp32 [oc][ic/group][kh][kw], op.bias fp32 [oc] or None; op.conv['relu'] / op.relu6."""
+
+    def __init__(self, backend, op: Op, depthwise=False):
+        super().__init__(backend)
+        self.op, self.depthwise = op, depthwise
+        d = _desc(op.conv)
+        w = np.ascontiguousarray(op.weight, np.float32)
+        b = None if op.bias is None else np.ascontiguousarray(op.bias, np.float32)
+        f = _capi.lib().mnnb200_dwconv_f32_create if depthwise else _capi.lib().mnnb200_conv_f32_create
+        check(f(backend.runtime._h, C.byref(d), _np_ptr(w), _np_ptr(b), int(op.relu6), C.byref(self._h)),
+              "dwconv_f32_create" if depthwise else "conv_f32_create")
+
+    def onResize(self, inputs, outputs):
+        n, _, ih, iw = inputs[0].shape
+        oh, ow = C.c_int(0), C.c_int(0)
+        f = _capi.lib().mnnb200_dwconv_f32_resize if self.depthwise else _capi.lib().mnnb200_conv_f32_resize
+        st = f(self._h, n, ih, iw, C.byref(oh), C.byref(ow))
+        if st == 0:
+            outputs[0].shape = (n, self.op.conv["oc"], oh.value, ow.value)
+        return st
+
+    def onExecute(self, inputs, outputs):
+        f = _capi.lib().mnnb200_dwconv_f32_execute if self.depthwise else _capi.lib().mnnb200_conv_f32_execute
+        return f(self._h, inputs[0].ptr(), outputs[0].ptr())
+
+
 class Backend:
     """CUDABackend's role: creator map, buffer acquisition, host<->device copies with layout + quant casts."""
 
@@ -499,3 +527,13 @@ Backend.addCreator("SoftmaxInt8", lambda b, i, o, op: SoftmaxInt8Execution(b))
 Backend.addCreator("MatMul", lambda b, i, o, op: MatMulExecution(b, op))
 Backend.addCreator("BatchMatMul", lambda b, i, o, op: MatMulExecution(b, op))
 Backend.addCreator("LinearW8", lambda b, i, o, op: LinearW8Execution(b, op))
+
+
+def _create_conv_f32(b, i, o, op):
+    if op.conv.get("group", 1) != 1:      # grouped float convs are not taken (depthwise has its own op type)
+        return None
+    return ConvF32Execution(b, op)
+
+
+Backend.addCreator("Convolution", _create_conv_f32)
+Backend.addCreator("ConvolutionDepthwise", lambda b, i, o, op: ConvF32Execution(b, op, depthwise=True))

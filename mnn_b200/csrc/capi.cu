@@ -1493,3 +1493,218 @@ mnnb200_status mnnb200_matmul_execute(mnnb200_exec* ex, const void* a, const voi
     return MNNB200_OK;
 }
 }  // extern "C"
+
+// =================================================================================================
+// Float convolutions and their fp32 neighbours (device fp32 tensors are NCHW-linear): the CPU backend's float path
+// (CPUConvolution / ConvolutionTiledExecutor, CPUConvolutionDepthwise, CPUBinary ADD, CPUScale, CPUSoftmax) on the GPU.
+// =================================================================================================
+static int float_act(const mnnb200_conv_desc* d, int relu6) { return relu6 ? 2 : (d->relu ? 1 : 0); }
+
+struct ConvF32Exec : mnnb200_exec {
+    mnnb200_conv_desc d;
+    int act = 0, cp8 = 0, taps = 0, kp = 0, ocp = 0, bn = 0;
+    float *d_hi = nullptr, *d_lo = nullptr, *d_bias = nullptr;
+    CUtensorMap tmap_hi, tmap_lo;
+    ConvF32Params p;
+    bool resized = false;
+};
+struct DwConvF32Exec : mnnb200_exec {
+    mnnb200_conv_desc d;
+    int act = 0;
+    float *d_w = nullptr, *d_bias = nullptr;
+    DwF32Params p;
+    bool resized = false;
+};
+struct ScaleF32Exec : mnnb200_exec {
+    int c = 0, n = 0;
+    size_t plane = 0;
+    float *d_scale = nullptr, *d_bias = nullptr;
+    bool resized = false;
+};
+
+static bool conv_desc_valid(const mnnb200_conv_desc* d) {
+    return d->ic > 0 && d->oc > 0 && d->kh > 0 && d->kw > 0 && d->stride_h > 0 && d->stride_w > 0 && d->dilate_h > 0 &&
+           d->dilate_w > 0 && d->pad_h >= 0 && d->pad_w >= 0;
+}
+
+extern "C" {
+mnnb200_status mnnb200_conv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight, const float* bias,
+                                       int relu6, mnnb200_exec** out) {
+    if (!rt || !desc || !weight || !out) return fail(MNNB200_INVALID_VALUE, "conv_f32_create: NULL argument");
+    if (!conv_desc_valid(desc)) return fail(MNNB200_INVALID_VALUE, "conv_f32_create: bad descriptor");
+    if (desc->group != 1) return fail(MNNB200_NOT_SUPPORT, "conv_f32: group > 1 (depthwise has its own execution)");
+    auto* e = new ConvF32Exec;
+    e->rt = rt; e->kind = 8; e->d = *desc; e->act = float_act(desc, relu6);
+    e->taps = desc->kh * desc->kw;
+    e->cp8 = (desc->ic + 7) & ~7;
+    e->kp = (e->taps * e->cp8 + 31) & ~31;
+    e->ocp = (desc->oc + 127) & ~127;          // a whole number of tiles of every width: no weight tile reads past the array
+    const size_t wn = (size_t)desc->oc * desc->ic * e->taps, packed = (size_t)e->ocp * e->kp;
+    std::vector<float> hw(weight, weight + wn), hb(desc->oc, 0.f);
+    if (bias) hb.assign(bias, bias + desc->oc);
+    float* d_raw = nullptr;
+    mnnb200_status st;
+    if ((st = e->upload(hw, &d_raw)) || (st = e->upload(hb, &e->d_bias))) { delete e; return st; }
+    auto packed_buf = [&](float** p) -> mnnb200_status {
+        CK(cudaMalloc((void**)p, packed * sizeof(float)));
+        e->dev_bufs.push_back(*p);
+        return MNNB200_OK;
+    };
+    if ((st = packed_buf(&e->d_hi)) || (st = packed_buf(&e->d_lo))) { delete e; return st; }
+    cudaError_t ce = launch_pack_conv_w_f32(d_raw, desc->oc, desc->ic, e->taps, e->cp8, e->kp, e->ocp, e->d_hi, e->d_lo, rt->stream);
+    if (ce == cudaSuccess) ce = cudaStreamSynchronize(rt->stream);
+    for (auto& b : e->dev_bufs)                  // the unpacked weights are not needed after the split
+        if (b == d_raw) b = nullptr;
+    cudaFree(d_raw);
+    if (ce != cudaSuccess) { delete e; return fail(MNNB200_CUDA_ERROR, std::string("conv_f32_create: ") + cudaGetErrorString(ce)); }
+    *out = e;
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_conv_f32_set_pad(mnnb200_exec* ex, int pad_h, int pad_w) {
+    if (!ex || pad_h < 0 || pad_w < 0) return fail(MNNB200_INVALID_VALUE, "conv_f32_set_pad: bad argument");
+    if (ex->kind == 8) { auto* e = static_cast<ConvF32Exec*>(ex); e->d.pad_h = pad_h; e->d.pad_w = pad_w; }
+    else if (ex->kind == 9) { auto* e = static_cast<DwConvF32Exec*>(ex); e->d.pad_h = pad_h; e->d.pad_w = pad_w; }
+    else return fail(MNNB200_INVALID_VALUE, "conv_f32_set_pad: not a float convolution execution");
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_conv_f32_resize(mnnb200_exec* ex, int n, int ih, int iw, int* oh, int* ow) {
+    if (!ex || ex->kind != 8) return fail(MNNB200_INVALID_VALUE, "conv_f32_resize: not a float conv execution");
+    auto* e = static_cast<ConvF32Exec*>(ex);
+    const auto& d = e->d;
+    const int OH = (oh && *oh > 0) ? *oh : conv_out(ih, d.kh, d.stride_h, d.pad_h, d.dilate_h);
+    const int OW = (ow && *ow > 0) ? *ow : conv_out(iw, d.kw, d.stride_w, d.pad_w, d.dilate_w);
+    if (n <= 0 || ih <= 0 || iw <= 0 || OH <= 0 || OW <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "conv_f32_resize: empty output");
+    const long long M = (long long)n * OH * OW;
+    if (M > 0x7fffffffLL - 128 || (long long)n * d.ic * ih * iw > 0x7fffffffLL || (long long)n * d.oc * OH * OW > 0x7fffffffLL)
+        return fail(MNNB200_NOT_SUPPORT, "conv_f32_resize: tensor too large for 32-bit indexing");
+    // the plan, once per shape: tile width from the layer's shape (fill the SMs before widening the tile), then the weight maps
+    const int sm = e->rt->prop.multiProcessorCount;
+    const int m_tiles = (int)((M + 127) / 128);
+    int bn = d.oc <= 32 ? 32 : (d.oc <= 64 ? 64 : 128);
+    while (bn > 32 && (long long)m_tiles * ((d.oc + bn - 1) / bn) < sm) bn >>= 1;
+    mnnb200_status st;
+    if (bn != e->bn) {
+        if ((st = make_tmap_i8(&e->tmap_hi, e->d_hi, e->ocp, e->kp * 4, bn)) ||
+            (st = make_tmap_i8(&e->tmap_lo, e->d_lo, e->ocp, e->kp * 4, bn)))
+            return st;
+        e->bn = bn;
+    }
+    ConvF32Params& p = e->p;
+    memset(&p, 0, sizeof(p));
+    p.bias = e->d_bias;
+    p.N = n; p.IC = d.ic; p.IH = ih; p.IW = iw; p.OC = d.oc; p.OH = OH; p.OW = OW;
+    p.KH = d.kh; p.KW = d.kw; p.sh = d.stride_h; p.sw = d.stride_w; p.ph = d.pad_h; p.pw = d.pad_w; p.dh = d.dilate_h; p.dw = d.dilate_w;
+    p.Cp8 = e->cp8; p.taps = e->taps; p.M = (int)M; p.num_kb = e->kp / 32; p.m_tiles = m_tiles; p.n_chunks = (d.oc + bn - 1) / bn;
+    p.act = e->act;
+    e->cost_bytes = 4.0 * ((double)n * d.ic * ih * iw + (double)M * d.oc + (double)d.oc * d.ic * e->taps);
+    e->cost_macs = (double)M * d.oc * d.ic * e->taps;
+    e->resized = true;
+    if (oh) *oh = OH;
+    if (ow) *ow = OW;
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_conv_f32_execute(mnnb200_exec* ex, const float* x, float* y) {
+    if (!ex || ex->kind != 8) return fail(MNNB200_INVALID_VALUE, "conv_f32_execute: not a float conv execution");
+    auto* e = static_cast<ConvF32Exec*>(ex);
+    if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_f32_execute before resize");
+    if (!x || !y) return fail(MNNB200_INVALID_VALUE, "conv_f32_execute: NULL tensor");
+    ConvF32Params p = e->p;
+    p.x = x; p.y = y;
+    CK(launch_conv_f32_wgmma(p, &e->tmap_hi, &e->tmap_lo, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_dwconv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight, const float* bias,
+                                         int relu6, mnnb200_exec** out) {
+    if (!rt || !desc || !weight || !out) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_create: NULL argument");
+    if (!conv_desc_valid(desc)) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_create: bad descriptor");
+    if (desc->group != desc->ic || desc->ic != desc->oc) return fail(MNNB200_NOT_SUPPORT, "dwconv_f32: group == ic == oc required");
+    auto* e = new DwConvF32Exec;
+    e->rt = rt; e->kind = 9; e->d = *desc; e->act = float_act(desc, relu6);
+    std::vector<float> hw(weight, weight + (size_t)desc->oc * desc->kh * desc->kw), hb(desc->oc, 0.f);
+    if (bias) hb.assign(bias, bias + desc->oc);
+    mnnb200_status st;
+    if ((st = e->upload(hw, &e->d_w)) || (st = e->upload(hb, &e->d_bias))) { delete e; return st; }
+    *out = e;
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_dwconv_f32_resize(mnnb200_exec* ex, int n, int ih, int iw, int* oh, int* ow) {
+    if (!ex || ex->kind != 9) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_resize: not a float depthwise execution");
+    auto* e = static_cast<DwConvF32Exec*>(ex);
+    const auto& d = e->d;
+    const int OH = (oh && *oh > 0) ? *oh : conv_out(ih, d.kh, d.stride_h, d.pad_h, d.dilate_h);
+    const int OW = (ow && *ow > 0) ? *ow : conv_out(iw, d.kw, d.stride_w, d.pad_w, d.dilate_w);
+    if (n <= 0 || ih <= 0 || iw <= 0 || OH <= 0 || OW <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "dwconv_f32_resize: empty output");
+    DwF32Params& p = e->p;
+    memset(&p, 0, sizeof(p));
+    p.w = e->d_w; p.bias = e->d_bias;
+    p.N = n; p.C = d.oc; p.IH = ih; p.IW = iw; p.OH = OH; p.OW = OW; p.KH = d.kh; p.KW = d.kw;
+    p.sh = d.stride_h; p.sw = d.stride_w; p.ph = d.pad_h; p.pw = d.pad_w; p.dh = d.dilate_h; p.dw = d.dilate_w; p.act = e->act;
+    e->cost_bytes = 4.0 * ((double)n * d.oc * ih * iw + (double)n * d.oc * OH * OW + (double)d.oc * d.kh * d.kw);
+    e->cost_macs = (double)n * OH * OW * d.oc * d.kh * d.kw;
+    e->resized = true;
+    if (oh) *oh = OH;
+    if (ow) *ow = OW;
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_dwconv_f32_execute(mnnb200_exec* ex, const float* x, float* y) {
+    if (!ex || ex->kind != 9) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_execute: not a float depthwise execution");
+    auto* e = static_cast<DwConvF32Exec*>(ex);
+    if (!e->resized) return fail(MNNB200_NO_EXECUTION, "dwconv_f32_execute before resize");
+    if (!x || !y) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_execute: NULL tensor");
+    DwF32Params p = e->p;
+    p.x = x; p.y = y;
+    CK(launch_dwconv_f32(p, e->rt->stream));
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_binary_add_f32(mnnb200_runtime* rt, const float* a, const float* b, float* y, size_t count) {
+    if (!rt || !a || !b || !y) return fail(MNNB200_INVALID_VALUE, "binary_add_f32: NULL argument");
+    if (count == 0) return MNNB200_OK;
+    CK(launch_binary_add_f32(a, b, y, count, rt->stream));
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_scale_f32_create(mnnb200_runtime* rt, int channels, const float* scale, const float* bias, mnnb200_exec** out) {
+    if (!rt || !scale || !out || channels <= 0) return fail(MNNB200_INVALID_VALUE, "scale_f32_create: bad argument");
+    auto* e = new ScaleF32Exec;
+    e->rt = rt; e->kind = 10; e->c = channels;
+    std::vector<float> hs(scale, scale + channels), hb(channels, 0.f);
+    if (bias) hb.assign(bias, bias + channels);
+    mnnb200_status st;
+    if ((st = e->upload(hs, &e->d_scale)) || (st = e->upload(hb, &e->d_bias))) { delete e; return st; }
+    *out = e;
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_scale_f32_resize(mnnb200_exec* ex, int n, int h, int w) {
+    if (!ex || ex->kind != 10) return fail(MNNB200_INVALID_VALUE, "scale_f32_resize: not a float Scale execution");
+    auto* e = static_cast<ScaleF32Exec*>(ex);
+    if (n <= 0 || h <= 0 || w <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "scale_f32_resize: empty tensor");
+    e->n = n; e->plane = (size_t)h * w;
+    e->cost_bytes = 8.0 * n * e->c * (double)e->plane;
+    e->cost_macs = (double)n * e->c * (double)e->plane;
+    e->resized = true;
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_scale_f32_execute(mnnb200_exec* ex, const float* x, float* y) {
+    if (!ex || ex->kind != 10) return fail(MNNB200_INVALID_VALUE, "scale_f32_execute: not a float Scale execution");
+    auto* e = static_cast<ScaleF32Exec*>(ex);
+    if (!e->resized) return fail(MNNB200_NO_EXECUTION, "scale_f32_execute before resize");
+    if (!x || !y) return fail(MNNB200_INVALID_VALUE, "scale_f32_execute: NULL tensor");
+    CK(launch_scale_f32(x, e->d_scale, e->d_bias, y, e->n, e->c, e->plane, e->rt->stream));
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_softmax_f32(mnnb200_runtime* rt, const float* x, int outside, int axis, int inside, float* y) {
+    if (!rt || !x || !y || outside <= 0 || axis <= 0 || inside <= 0) return fail(MNNB200_INVALID_VALUE, "softmax_f32: bad argument");
+    CK(launch_softmax_f32(x, y, outside, axis, inside, rt->stream));
+    return MNNB200_OK;
+}
+}  // extern "C"

@@ -843,4 +843,101 @@ cudaError_t launch_reduce_f32(const float* x, float* y, int outside, int axis, i
     return cudaGetLastError();
 }
 
+// ---- fp32 depthwise conv (CPUConvolutionDepthwise): one thread per output element, NCHW (consecutive threads walk a row of the
+//      output plane, so reads along the input row coalesce for stride 1); bias, then ReLU / ReLU6 (CPUConvolution.cpp:289-291)
+__global__ void __launch_bounds__(256) dwconv_f32_kernel(const DwF32Params p) {
+    const size_t total = (size_t)p.N * p.C * p.OH * p.OW;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int ow = (int)(i % p.OW);
+        const size_t r = i / p.OW;
+        const int oh = (int)(r % p.OH);
+        const size_t nc = r / p.OH;
+        const int c = (int)(nc % p.C);
+        const float* xp = p.x + nc * p.IH * p.IW;
+        const float* wp = p.w + (size_t)c * p.KH * p.KW;
+        const int ih0 = oh * p.sh - p.ph, iw0 = ow * p.sw - p.pw;
+        float acc = 0.f;
+        for (int kh = 0; kh < p.KH; ++kh) {
+            const int ih = ih0 + kh * p.dh;
+            if ((unsigned)ih >= (unsigned)p.IH) continue;
+            for (int kw = 0; kw < p.KW; ++kw) {
+                const int iw = iw0 + kw * p.dw;
+                if ((unsigned)iw < (unsigned)p.IW) acc = fmaf(xp[(size_t)ih * p.IW + iw], wp[kh * p.KW + kw], acc);
+            }
+        }
+        float v = acc + p.bias[c];
+        if (p.act >= 1) v = fmaxf(v, 0.f);
+        if (p.act == 2) v = fminf(v, 6.f);
+        p.y[i] = v;
+    }
+}
+cudaError_t launch_dwconv_f32(const DwF32Params& p, cudaStream_t s) {
+    dwconv_f32_kernel<<<grid_for((size_t)p.N * p.C * p.OH * p.OW, 256), 256, 0, s>>>(p);
+    ++g_launch_count;
+    return cudaGetLastError();
+}
+
+// ---- fp32 BinaryOp ADD of two equally sized tensors (the residual add); float4 when both inputs and the output are 16-byte aligned
+__global__ void binary_add_f32_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ y, size_t n,
+                                      int vec) {
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    const size_t i0 = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    size_t done = 0;
+    if (vec) {
+        const size_t n4 = n >> 2;
+        for (size_t i = i0; i < n4; i += stride) {
+            const float4 u = reinterpret_cast<const float4*>(a)[i], v = reinterpret_cast<const float4*>(b)[i];
+            reinterpret_cast<float4*>(y)[i] = make_float4(u.x + v.x, u.y + v.y, u.z + v.z, u.w + v.w);
+        }
+        done = n4 << 2;
+    }
+    for (size_t i = done + i0; i < n; i += stride) y[i] = a[i] + b[i];
+}
+cudaError_t launch_binary_add_f32(const float* a, const float* b, float* y, size_t n, cudaStream_t s) {
+    const int vec = (((uintptr_t)a | (uintptr_t)b | (uintptr_t)y) & 15) == 0;
+    binary_add_f32_kernel<<<grid_for(vec ? (n >> 2) + 1 : n, 256), 256, 0, s>>>(a, b, y, n, vec);
+    ++g_launch_count;
+    return cudaGetLastError();
+}
+
+// ---- fp32 Scale (CPUScale, MNNScaleAndAddBias): y[n][c][i] = x[n][c][i] * scale[c] + bias[c]
+__global__ void scale_f32_kernel(const float* __restrict__ x, const float* __restrict__ scale, const float* __restrict__ bias,
+                                 float* __restrict__ y, int c, size_t plane, size_t total) {
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const int ch = (int)((i / plane) % c);
+        y[i] = fmaf(x[i], scale[ch], bias[ch]);
+    }
+}
+cudaError_t launch_scale_f32(const float* x, const float* scale, const float* bias, float* y, int n, int c, size_t plane,
+                             cudaStream_t s) {
+    const size_t total = (size_t)n * c * plane;
+    scale_f32_kernel<<<grid_for(total, 256), 256, 0, s>>>(x, scale, bias, y, c, plane, total);
+    ++g_launch_count;
+    return cudaGetLastError();
+}
+
+// ---- fp32 Softmax over the middle axis of [outside][axis][inside] (CPUSoftmax.cpp: max, sum of exp(x - max), divide).
+//      One warp per (outside, inside) column.
+__global__ void softmax_f32_kernel(const float* __restrict__ x, float* __restrict__ y, int outside, int axis, int inside) {
+    const size_t col = (blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5;
+    const int lane = threadIdx.x & 31;
+    if (col >= (size_t)outside * inside) return;
+    const size_t o = col / inside, in = col - o * inside;
+    const float* xp = x + o * axis * inside + in;
+    float* yp = y + o * axis * inside + in;
+    float mx = -3.402823466e38f;
+    for (int a = lane; a < axis; a += 32) mx = fmaxf(mx, xp[(size_t)a * inside]);
+    for (int s = 16; s > 0; s >>= 1) mx = fmaxf(mx, __shfl_xor_sync(0xffffffffu, mx, s));
+    float sum = 0.f;
+    for (int a = lane; a < axis; a += 32) sum += expf(xp[(size_t)a * inside] - mx);
+    for (int s = 16; s > 0; s >>= 1) sum += __shfl_xor_sync(0xffffffffu, sum, s);
+    const float inv = 1.f / sum;
+    for (int a = lane; a < axis; a += 32) yp[(size_t)a * inside] = expf(xp[(size_t)a * inside] - mx) * inv;
+}
+cudaError_t launch_softmax_f32(const float* x, float* y, int outside, int axis, int inside, cudaStream_t s) {
+    softmax_f32_kernel<<<grid_for((size_t)outside * inside * 32, 256), 256, 0, s>>>(x, y, outside, axis, inside);
+    ++g_launch_count;
+    return cudaGetLastError();
+}
+
 }  // namespace mnnb200

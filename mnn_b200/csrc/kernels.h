@@ -122,6 +122,39 @@ cudaError_t launch_gemm_f16_wgmma(const void* tmap_a, const void* tmap_b, int ba
                                   int a_batch_rows, int b_batch_rows, int bn, float* c, const float* bias, cudaStream_t stream,
                                   int sm_count);
 
+// fp32 Conv2D (group 1) on split-TF32 wgmma (conv_f32_wgmma.cu): NCHW-linear fp32 in and out.  Weights are packed once into two
+// K-major arrays hi / lo [ocp][kp] (k = tap * cp8 + c, cp8 = ic rounded up to 8, kp = taps * cp8 rounded up to 32), w = hi + lo.
+struct ConvF32Params {
+    const float* x;       // [N][IC][IH][IW]
+    float* y;             // [N][OC][OH][OW]
+    const float* bias;    // [OC]
+    int N, IC, IH, IW, OC, OH, OW;
+    int KH, KW, sh, sw, ph, pw, dh, dw;
+    int Cp8, taps;        // taps = KH * KW
+    int M, num_kb;        // M = N * OH * OW, num_kb = kp / 32
+    int m_tiles, n_chunks;
+    int act;              // 0 none, 1 ReLU, 2 ReLU6
+};
+cudaError_t launch_pack_conv_w_f32(const float* w, int oc, int ic, int taps, int cp8, int kp, int ocp, float* hi, float* lo,
+                                   cudaStream_t s);
+// tmap_hi / tmap_lo: 2D maps over the [ocp][kp * 4 bytes] weight arrays with {128 bytes, bn rows} boxes, 128B swizzle; bn 32 / 64 / 128
+cudaError_t launch_conv_f32_wgmma(const ConvF32Params& p, const void* tmap_hi, const void* tmap_lo, int bn, cudaStream_t s,
+                                  int sm_count);
+
+// fp32 neighbours of the float conv, all NCHW-linear.  dwconv: w [C][KH*KW]; act 0 none, 1 ReLU, 2 ReLU6
+struct DwF32Params {
+    const float* x;
+    const float* w;
+    const float* bias;
+    float* y;
+    int N, C, IH, IW, OH, OW, KH, KW, sh, sw, ph, pw, dh, dw, act;
+};
+cudaError_t launch_dwconv_f32(const DwF32Params& p, cudaStream_t s);
+cudaError_t launch_binary_add_f32(const float* a, const float* b, float* y, size_t n, cudaStream_t s);
+cudaError_t launch_scale_f32(const float* x, const float* scale, const float* bias, float* y, int n, int c, size_t plane,
+                             cudaStream_t s);
+cudaError_t launch_softmax_f32(const float* x, float* y, int outside, int axis, int inside, cudaStream_t s);
+
 // elementwise / data movement
 cudaError_t launch_float_to_int8(const float* x, int n, int c, int h, int w, float inv_scale, float zero, float minv,
                                  float maxv, int8_t* y, cudaStream_t s);

@@ -849,6 +849,130 @@ private:
     bool mZero = false;
 };
 
+// ---- fp32 models: the CPU backend's float path on NCHW-linear device tensors
+static bool isF32Nchw(const Tensor* t) {
+    return t->getType().code == halide_type_float && t->getType().bytes() == 4 && linearFormat(t) == MNN_DATA_FORMAT_NCHW;
+}
+// Convolution (group 1, split-TF32 wgmma) and ConvolutionDepthwise (also a Convolution whose group == ic == oc) on float tensors
+class ConvF32Exec : public B200Exec {
+public:
+    struct Resource { mnnb200_exec* h = nullptr; ~Resource() { if (h) mnnb200_exec_destroy(h); } };
+    ConvF32Exec(Backend* bn, const Op* op, std::shared_ptr<Resource> res, bool dw) : B200Exec(bn), mOp(op), mRes(res), mDepthwise(dw) {}
+    static Execution* create(B200Backend* bn, const Op* op) {
+        auto conv = op->main_as_Convolution2D();
+        if (!conv || !conv->common()) return nullptr;
+        auto cm = conv->common();
+        const int oc = cm->outputCount(), kh = cm->kernelY(), kw = cm->kernelX();
+        std::shared_ptr<ConvolutionCommon::Int8Common> quanCommon;
+        const float* w = nullptr;
+        int wsize = 0;
+        // plain float weights and IDST-coded ones, decoded as the CPU's float path does
+        ConvolutionCommon::getConvParameters(&quanCommon, bn, op, &w, &wsize);
+        if (!w || oc <= 0 || kh <= 0 || kw <= 0 || wsize <= 0) return nullptr;
+        const bool dw = op->type() == OpType_ConvolutionDepthwise || (cm->group() > 1 && cm->group() == oc && wsize == oc * kh * kw);
+        if (!dw && cm->group() != 1) return nullptr;          // grouped (1 < group < channels): not on this path
+        const int ic = dw ? oc : wsize / (oc * kh * kw);
+        if (ic <= 0 || (size_t)wsize != (size_t)oc * (dw ? 1 : ic) * kh * kw) return nullptr;
+        mnnb200_conv_desc d;
+        d.ic = ic; d.oc = oc; d.kh = kh; d.kw = kw; d.stride_h = cm->strideY(); d.stride_w = cm->strideX();
+        d.pad_h = 0; d.pad_w = 0; d.dilate_h = cm->dilateY(); d.dilate_w = cm->dilateX();   // pads: set at resize
+        d.group = dw ? oc : 1; d.relu = cm->relu() ? 1 : 0;
+        const float* bias = (conv->bias() && (int)conv->bias()->size() == oc) ? conv->bias()->data() : nullptr;
+        std::shared_ptr<Resource> res(new Resource);
+        mnnb200_status st = dw ? mnnb200_dwconv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &res->h)
+                               : mnnb200_conv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &res->h);
+        if (st != MNNB200_OK) {
+            if (st != MNNB200_NOT_SUPPORT) MNN_ERROR("mnn_b200 float conv create: %s\n", mnnb200_last_error());
+            return nullptr;
+        }
+        auto e = new ConvF32Exec(bn, op, res, dw);
+        e->mIc = ic;
+        return e;
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto in = inputs[0], out = outputs[0];
+        if (in->dimensions() != 4 || in->channel() != mIc) {   // the kernels index the input by the weights' channel count
+            MNN_ERROR("mnn_b200 float conv: input has %d channels, the weights %d\n", in->channel(), mIc);
+            return NOT_SUPPORT;
+        }
+        auto pad = ConvolutionCommon::convolutionPad(in, out, mOp->main_as_Convolution2D()->common());   // (padX, padY)
+        int oh = out->height(), ow = out->width();
+        mnnb200_status st = mnnb200_conv_f32_set_pad(mRes->h, pad.second, pad.first);
+        if (st == MNNB200_OK)
+            st = mDepthwise ? mnnb200_dwconv_f32_resize(mRes->h, in->batch(), in->height(), in->width(), &oh, &ow)
+                            : mnnb200_conv_f32_resize(mRes->h, in->batch(), in->height(), in->width(), &oh, &ow);
+        return toErr(st, "float conv resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto x = (const float*)dev(inputs[0]);
+        auto y = (float*)dev(outputs[0]);
+        return toErr(mDepthwise ? mnnb200_dwconv_f32_execute(mRes->h, x, y) : mnnb200_conv_f32_execute(mRes->h, x, y), "float conv");
+    }
+    // a clone owns its own resize state (the launch plan lives in the C execution), so the packed weights are made again from the op
+    bool onClone(Backend* bn, const Op* op, Execution** dst) override {
+        if (dst) {
+            *dst = create(static_cast<B200Backend*>(bn), op);
+            if (*dst == nullptr) return false;
+        }
+        return true;
+    }
+private:
+    const Op* mOp;
+    std::shared_ptr<Resource> mRes;
+    bool mDepthwise;
+    int mIc = 0;
+};
+class BinaryAddF32Exec : public B200Exec {
+public:
+    BinaryAddF32Exec(Backend* bn) : B200Exec(bn) {}
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        return toErr(mnnb200_binary_add_f32(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(inputs[0]),
+                                            (const float*)dev(inputs[1]), (float*)dev(outputs[0]), elemCount(outputs[0])), "BinaryOp add fp32");
+    }
+};
+class ScaleF32Exec : public B200Exec {
+public:
+    struct Resource { mnnb200_exec* h = nullptr; ~Resource() { if (h) mnnb200_exec_destroy(h); } };
+    ScaleF32Exec(Backend* bn, std::shared_ptr<Resource> r) : B200Exec(bn), mRes(r) {}
+    static Execution* create(B200Backend* bn, const Op* op) {
+        auto sc = op->main_as_Scale();
+        if (!sc || !sc->scaleData()) return nullptr;
+        const int c = (int)sc->scaleData()->size();
+        const float* bias = (sc->biasData() && (int)sc->biasData()->size() == c) ? sc->biasData()->data() : nullptr;
+        std::shared_ptr<Resource> res(new Resource);
+        if (mnnb200_scale_f32_create(bn->handle(), c, sc->scaleData()->data(), bias, &res->h) != MNNB200_OK) return nullptr;
+        return new ScaleF32Exec(bn, res);
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>&) override {
+        auto d = dims4(inputs[0]);
+        return toErr(mnnb200_scale_f32_resize(mRes->h, d.n, d.h, d.w), "Scale fp32 resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        return toErr(mnnb200_scale_f32_execute(mRes->h, (const float*)dev(inputs[0]), (float*)dev(outputs[0])), "Scale fp32");
+    }
+    bool onClone(Backend* bn, const Op* op, Execution** dst) override {
+        if (dst) *dst = create(static_cast<B200Backend*>(bn), op);
+        return true;
+    }
+private:
+    std::shared_ptr<Resource> mRes;
+};
+// Softmax over one axis of an [outside][axis][inside] view (CPUSoftmax.cpp)
+class SoftmaxF32Exec : public B200Exec {
+public:
+    SoftmaxF32Exec(Backend* bn, int axis) : B200Exec(bn), mAxis(axis) {}
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto in = inputs[0];
+        int outside = 1, inside = 1;
+        for (int i = 0; i < mAxis; ++i) outside *= in->length(i);
+        for (int i = mAxis + 1; i < in->dimensions(); ++i) inside *= in->length(i);
+        return toErr(mnnb200_softmax_f32(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(in), outside, in->length(mAxis),
+                                         inside, (float*)dev(outputs[0])), "Softmax fp32");
+    }
+private:
+    int mAxis;
+};
+
 Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs, const MNN::Op* op) {
     Execution* e = nullptr;
     const bool quantOut = !outputs.empty() && TensorUtils::getDescribe(outputs[0])->quantAttr.get() != nullptr &&
@@ -862,6 +986,11 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
                        inputs[0]->getType().code == halide_type_float && linearFormat(inputs[0]) == MNN_DATA_FORMAT_NCHW) {
                 e = LinearW8Exec::create(this, op);   // weight-quantised conv on float tensors: W8A8 only under Memory_Low, like the CPU
             }
+            // float conv; under Memory_Low the CPU runs an IDST-weight conv as W8A8 dynamic quantisation
+            // (ConvolutionFloatFactory.cpp:140-149), which only LinearW8Exec reproduces: such a conv is not taken in fp32
+            else if (!quantOut && op->type() == OpType_Convolution && inputs.size() == 1 && isF32Nchw(inputs[0]) &&
+                     !(mMemoryLow && op->main_as_Convolution2D() && op->main_as_Convolution2D()->quanParameter()))
+                e = ConvF32Exec::create(this, op);
             break;
         case OpType_MatMul:
             if (!quantOut && inputs.size() >= 2 && op->main_as_MatMul() && inputs[0]->getType().code == halide_type_float &&
@@ -871,6 +1000,7 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
         case OpType_ConvolutionDepthwise:
         case OpType_DepthwiseConvInt8:
             if (quantOut || op->type() == OpType_DepthwiseConvInt8) e = ConvInt8Exec::create(this, op, true);
+            else if (inputs.size() == 1 && isF32Nchw(inputs[0])) e = ConvF32Exec::create(this, op);
             break;
         case OpType_FloatToInt8:   // the cast kernels read/write NCHW-linear fp32 (NHWC-format tensors of <= 2 dims are the same bytes)
             // only the pipeline-inserted casts (quant info on the tensor, Pipeline.cpp:361-395); an op that carries its own
@@ -888,6 +1018,10 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
             if (quantOut && inputs.size() == 2 && op->main_as_BinaryOp() && op->main_as_BinaryOp()->opType() == BinaryOpOperation_ADD &&
                 op->main_as_BinaryOp()->activationType() == 0 && elemCount(inputs[0]) == elemCount(inputs[1]) && isInt8(inputs[0]) && isInt8(inputs[1]))
                 e = new BinaryAddInt8Exec(this);
+            else if (!quantOut && inputs.size() == 2 && op->main_as_BinaryOp() && op->main_as_BinaryOp()->opType() == BinaryOpOperation_ADD &&
+                     op->main_as_BinaryOp()->activationType() == 0 && elemCount(inputs[0]) == elemCount(outputs[0]) &&
+                     elemCount(inputs[1]) == elemCount(outputs[0]) && isF32Nchw(inputs[0]) && isF32Nchw(inputs[1]) && isF32Nchw(outputs[0]))
+                e = new BinaryAddF32Exec(this);   // equal sizes only (the residual add); broadcasts are declined
             break;
         case OpType_Pooling:
             if (!quantOut && op->main_as_Pool() && outputs.size() == 1 && inputs[0]->getType().code == halide_type_float &&
@@ -899,6 +1033,9 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
             break;
         case OpType_Scale:
             if (quantOut && inputs.size() == 1 && isInt8(inputs[0])) e = ScaleInt8Exec::create(this, op);
+            else if (!quantOut && inputs.size() == 1 && isF32Nchw(inputs[0]) && op->main_as_Scale() && op->main_as_Scale()->scaleData() &&
+                     (int)op->main_as_Scale()->scaleData()->size() == inputs[0]->channel())
+                e = ScaleF32Exec::create(this, op);
             break;
         case OpType_ReLU:
             if (!quantOut && inputs.size() == 1 && inputs[0]->getType().code == halide_type_float && inputs[0]->getType().bytes() == 4)
@@ -928,6 +1065,9 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
             bool inner1 = true;
             for (int i = axis + 1; i < inputs[0]->dimensions(); ++i) inner1 = inner1 && inputs[0]->length(i) == 1;
             if (quantOut && isInt8(inputs[0]) && axis == 1 && inner1) e = new SoftmaxInt8Exec(this);
+            else if (!quantOut && axis >= 0 && axis < inputs[0]->dimensions() && inputs[0]->getType().code == halide_type_float &&
+                     inputs[0]->getType().bytes() == 4 && (linearFormat(inputs[0]) == MNN_DATA_FORMAT_NCHW || inputs[0]->dimensions() <= 2))
+                e = new SoftmaxF32Exec(this, axis);   // <= 2 dims: NHWC-format tensors (TF models' logits) are the same bytes
             break;
         }
         case OpType_Raster: {
