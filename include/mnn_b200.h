@@ -301,6 +301,25 @@ MNNB200_API mnnb200_status mnnb200_scale_f32_resize(mnnb200_exec* e, int n, int 
 MNNB200_API mnnb200_status mnnb200_scale_f32_execute(mnnb200_exec* e, const float* x_nchw, float* y_nchw);
 MNNB200_API mnnb200_status mnnb200_softmax_f32(mnnb200_runtime* rt, const float* x, int outside, int axis, int inside, float* y);
 
+/* ---- Float BinaryOp / UnaryOp / ArgMax of fp32 models (CPUBinary, CPUEltwise, CPUUnary, CPUArgMax) on device fp32 tensors in
+ *      any one linear layout; all enqueue-only and capturable into a CUDA graph.
+ *      binary_f32: y[i] = a[i] op b[i] over count elements, then ReLU when relu != 0 (BinaryOp.activationType 1).  count_a and
+ *                  count_b are count or 1; a one-element side is broadcast and read on the device.  op = BinaryOpOperation:
+ *                  ADD 0, SUB 1, MUL 2, REALDIV 7, MINIMUM 8, MAXIMUM 9, SquaredDifference 14 ((a - b) * (a - b)); every op is one
+ *                  round-to-nearest fp32 operation, bit-identical to the CPU.  Any other op: NOT_SUPPORT.
+ *                  binary_add_f32 above is binary_f32 with ADD, equal counts and no ReLU.
+ *      unary_f32:  y[i] = op(x[i]), op = UnaryOpOperation: ABS 0, NEG 1, SQUARE 4, SQRT 5, RSQRT 6, EXP 7, LOG 8,
+ *                  RECIPROCAL 15, SIGMOID 29, TANH 30, HARDSWISH 31 ((x * min(max(x + 3, 0), 6)) / 6), GELU 32 (tanh form),
+ *                  GELU_STANDARD 33 (erf form), SILU 34.  ABS, NEG, SQUARE, SQRT, RSQRT, RECIPROCAL and HARDSWISH are exact
+ *                  round-to-nearest; the others within a few ulp.  Any other op: NOT_SUPPORT.
+ *      argmax_f32: y_int32[o][i] = the index along the middle axis of an [outside][axis][inside] view of the first maximum
+ *                  (is_min != 0: minimum), CPUArgMax with topK 1 and no max values. */
+MNNB200_API mnnb200_status mnnb200_binary_f32(mnnb200_runtime* rt, int op, const float* a, size_t count_a, const float* b,
+                                              size_t count_b, float* y, size_t count, int relu);
+MNNB200_API mnnb200_status mnnb200_unary_f32(mnnb200_runtime* rt, int op, const float* x, float* y, size_t count);
+MNNB200_API mnnb200_status mnnb200_argmax_f32(mnnb200_runtime* rt, const float* x, int outside, int axis, int inside, int is_min,
+                                              int32_t* y_int32);
+
 MNNB200_API void mnnb200_exec_destroy(mnnb200_exec* e);
 
 #ifdef __cplusplus

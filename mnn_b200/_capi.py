@@ -106,6 +106,9 @@ SIGNATURES = {
     "mnnb200_scale_f32_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int]),
     "mnnb200_scale_f32_execute": (C.c_int, [P, P, P]),
     "mnnb200_softmax_f32": (C.c_int, [P, P, C.c_int, C.c_int, C.c_int, P]),
+    "mnnb200_binary_f32": (C.c_int, [P, C.c_int, P, C.c_size_t, P, C.c_size_t, P, C.c_size_t, C.c_int]),
+    "mnnb200_unary_f32": (C.c_int, [P, C.c_int, P, P, C.c_size_t]),
+    "mnnb200_argmax_f32": (C.c_int, [P, P, C.c_int, C.c_int, C.c_int, C.c_int, P]),
     "mnnb200_exec_destroy": (None, [P]),
 }
 

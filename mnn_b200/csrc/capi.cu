@@ -1665,8 +1665,31 @@ mnnb200_status mnnb200_dwconv_f32_execute(mnnb200_exec* ex, const float* x, floa
 
 mnnb200_status mnnb200_binary_add_f32(mnnb200_runtime* rt, const float* a, const float* b, float* y, size_t count) {
     if (!rt || !a || !b || !y) return fail(MNNB200_INVALID_VALUE, "binary_add_f32: NULL argument");
+    return mnnb200_binary_f32(rt, kBinaryAdd, a, count, b, count, y, count, 0);
+}
+
+mnnb200_status mnnb200_binary_f32(mnnb200_runtime* rt, int op, const float* a, size_t count_a, const float* b, size_t count_b,
+                                  float* y, size_t count, int relu) {
+    if (!rt || !a || !b || !y) return fail(MNNB200_INVALID_VALUE, "binary_f32: NULL argument");
+    if (!binary_f32_supported(op)) return fail(MNNB200_NOT_SUPPORT, "binary_f32: op " + std::to_string(op) + " is not supported");
     if (count == 0) return MNNB200_OK;
-    CK(launch_binary_add_f32(a, b, y, count, rt->stream));
+    if ((count_a != count && count_a != 1) || (count_b != count && count_b != 1))
+        return fail(MNNB200_INVALID_VALUE, "binary_f32: each input must have count elements or one");
+    CK(launch_binary_f32(op, a, count_a != count, b, count_b != count, y, count, relu ? 1 : 0, rt->stream));
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_unary_f32(mnnb200_runtime* rt, int op, const float* x, float* y, size_t count) {
+    if (!rt || !x || !y) return fail(MNNB200_INVALID_VALUE, "unary_f32: NULL argument");
+    if (!unary_f32_supported(op)) return fail(MNNB200_NOT_SUPPORT, "unary_f32: op " + std::to_string(op) + " is not supported");
+    if (count == 0) return MNNB200_OK;
+    CK(launch_unary_f32(op, x, y, count, rt->stream));
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_argmax_f32(mnnb200_runtime* rt, const float* x, int outside, int axis, int inside, int is_min, int32_t* y) {
+    if (!rt || !x || !y || outside <= 0 || axis <= 0 || inside <= 0) return fail(MNNB200_INVALID_VALUE, "argmax_f32: bad argument");
+    CK(launch_argmax_f32(x, outside, axis, inside, is_min ? 1 : 0, y, rt->stream));
     return MNNB200_OK;
 }
 

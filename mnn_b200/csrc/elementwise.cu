@@ -877,25 +877,195 @@ cudaError_t launch_dwconv_f32(const DwF32Params& p, cudaStream_t s) {
     return cudaGetLastError();
 }
 
-// ---- fp32 BinaryOp ADD of two equally sized tensors (the residual add); float4 when both inputs and the output are 16-byte aligned
-__global__ void binary_add_f32_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ y, size_t n,
-                                      int vec) {
+// ---- fp32 BinaryOp (CPUBinary + MNNSelectBinaryFunctionForFloat): y = a op b, then ReLU when relu != 0 (activationType 1).
+//      a and b are either n elements or ONE element (read on the device: a runtime scalar may change between graph replays).
+//      Every op is a single IEEE operation in round-to-nearest (no FMA contraction): bit-identical to the CPU's float path.
+//      float4 when the full-size operands and the output are 16-byte aligned.  y may be a (Eltwise folds inputs into its output),
+//      so the pointers are not __restrict__.
+template <int OP>
+__device__ __forceinline__ float binary_f32_op(float a, float b) {
+    if (OP == kBinaryAdd) return __fadd_rn(a, b);
+    if (OP == kBinarySub) return __fsub_rn(a, b);
+    if (OP == kBinaryMul) return __fmul_rn(a, b);
+    if (OP == kBinaryRealDiv) return __fdiv_rn(a, b);
+    if (OP == kBinaryMinimum) return fminf(a, b);
+    if (OP == kBinaryMaximum) return fmaxf(a, b);
+    const float d = __fsub_rn(a, b);   // kBinarySquaredDifference
+    return __fmul_rn(d, d);
+}
+template <int OP>
+__device__ __forceinline__ float binary_f32_one(float a, float b, int relu) {
+    const float v = binary_f32_op<OP>(a, b);
+    return relu ? fmaxf(v, 0.f) : v;
+}
+template <int OP>
+__global__ void binary_f32_kernel(const float* a, const float* b, float* y, size_t n, int a_one, int b_one, int relu, int vec) {
+    const size_t stride = (size_t)gridDim.x * blockDim.x;
+    const size_t i0 = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
+    const float sa = a_one ? a[0] : 0.f, sb = b_one ? b[0] : 0.f;
+    size_t done = 0;
+    if (vec) {
+        const size_t n4 = n >> 2;
+        for (size_t i = i0; i < n4; i += stride) {
+            const float4 u = a_one ? make_float4(sa, sa, sa, sa) : reinterpret_cast<const float4*>(a)[i];
+            const float4 v = b_one ? make_float4(sb, sb, sb, sb) : reinterpret_cast<const float4*>(b)[i];
+            reinterpret_cast<float4*>(y)[i] = make_float4(binary_f32_one<OP>(u.x, v.x, relu), binary_f32_one<OP>(u.y, v.y, relu),
+                                                          binary_f32_one<OP>(u.z, v.z, relu), binary_f32_one<OP>(u.w, v.w, relu));
+        }
+        done = n4 << 2;
+    }
+    for (size_t i = done + i0; i < n; i += stride) y[i] = binary_f32_one<OP>(a_one ? sa : a[i], b_one ? sb : b[i], relu);
+}
+bool binary_f32_supported(int op) {
+    return op == kBinaryAdd || op == kBinarySub || op == kBinaryMul || op == kBinaryRealDiv || op == kBinaryMinimum ||
+           op == kBinaryMaximum || op == kBinarySquaredDifference;
+}
+cudaError_t launch_binary_f32(int op, const float* a, bool a_one, const float* b, bool b_one, float* y, size_t n, int relu,
+                              cudaStream_t s) {
+    const uintptr_t full = (a_one ? 0 : (uintptr_t)a) | (b_one ? 0 : (uintptr_t)b) | (uintptr_t)y;
+    const int vec = (full & 15) == 0;
+    const int grid = grid_for(vec ? (n >> 2) + 1 : n, 256);
+    switch (op) {
+        case kBinaryAdd: binary_f32_kernel<kBinaryAdd><<<grid, 256, 0, s>>>(a, b, y, n, a_one, b_one, relu, vec); break;
+        case kBinarySub: binary_f32_kernel<kBinarySub><<<grid, 256, 0, s>>>(a, b, y, n, a_one, b_one, relu, vec); break;
+        case kBinaryMul: binary_f32_kernel<kBinaryMul><<<grid, 256, 0, s>>>(a, b, y, n, a_one, b_one, relu, vec); break;
+        case kBinaryRealDiv: binary_f32_kernel<kBinaryRealDiv><<<grid, 256, 0, s>>>(a, b, y, n, a_one, b_one, relu, vec); break;
+        case kBinaryMinimum: binary_f32_kernel<kBinaryMinimum><<<grid, 256, 0, s>>>(a, b, y, n, a_one, b_one, relu, vec); break;
+        case kBinaryMaximum: binary_f32_kernel<kBinaryMaximum><<<grid, 256, 0, s>>>(a, b, y, n, a_one, b_one, relu, vec); break;
+        case kBinarySquaredDifference:
+            binary_f32_kernel<kBinarySquaredDifference><<<grid, 256, 0, s>>>(a, b, y, n, a_one, b_one, relu, vec);
+            break;
+        default: return cudaErrorInvalidValue;
+    }
+    ++g_launch_count;
+    return cudaGetLastError();
+}
+cudaError_t launch_binary_add_f32(const float* a, const float* b, float* y, size_t n, cudaStream_t s) {
+    return launch_binary_f32(kBinaryAdd, a, false, b, false, y, n, 0, s);
+}
+
+// ---- fp32 UnaryOp (CPUUnary::selectForFloat, CPUUnary.cpp:353-440).  HARDSWISH, ABS, NEG, SQUARE, SQRT, RSQRT and RECIPROCAL
+//      use the CPU's own formula in round-to-nearest steps; the transcendental ops (the CPU uses its own polynomials) are
+//      accurate to a few ulp: SIGMOID / SILU / GELU through expf in a cancellation-free form, GELU_STANDARD through erfcf.
+template <int OP>
+__device__ __forceinline__ float unary_f32_op(float x) {
+    if (OP == kUnaryAbs) return fabsf(x);
+    if (OP == kUnaryNeg) return -x;
+    if (OP == kUnarySquare) return __fmul_rn(x, x);
+    if (OP == kUnarySqrt) return __fsqrt_rn(x);
+    if (OP == kUnaryRsqrt) return __fdiv_rn(1.f, __fsqrt_rn(x));
+    if (OP == kUnaryReciprocal) return __fdiv_rn(1.f, x);
+    if (OP == kUnaryExp) return expf(x);
+    if (OP == kUnaryLog) return logf(x);
+    if (OP == kUnaryTanh) return tanhf(x);
+    if (OP == kUnarySigmoid) return __fdiv_rn(1.f, __fadd_rn(1.f, expf(-x)));
+    if (OP == kUnarySilu) return __fdiv_rn(x, __fadd_rn(1.f, expf(-x)));
+    if (OP == kUnaryHardSwish)   // x86_x64/sse/MathFunctions.cpp:251-259: (x * min(max(x + 3, 0), 6)) / 6
+        return __fdiv_rn(__fmul_rn(x, fminf(fmaxf(__fadd_rn(x, 3.f), 0.f), 6.f)), 6.f);
+    if (OP == kUnaryGelu) {      // 0.5 x (1 + tanh(z)) = x / (1 + exp(-2z)), z = 0.79788458 (x + 0.044715 x^3)
+        const float z = 0.79788458f * (x + 0.044715f * x * x * x);
+        return __fdiv_rn(x, __fadd_rn(1.f, expf(-2.f * z)));
+    }
+    return 0.5f * x * erfcf(-0.70710678f * x);   // kUnaryGeluStandard: 0.5 x (1 + erf(x / sqrt 2))
+}
+template <int OP>
+__global__ void unary_f32_kernel(const float* __restrict__ x, float* __restrict__ y, size_t n, int vec) {
     const size_t stride = (size_t)gridDim.x * blockDim.x;
     const size_t i0 = blockIdx.x * (size_t)blockDim.x + threadIdx.x;
     size_t done = 0;
     if (vec) {
         const size_t n4 = n >> 2;
         for (size_t i = i0; i < n4; i += stride) {
-            const float4 u = reinterpret_cast<const float4*>(a)[i], v = reinterpret_cast<const float4*>(b)[i];
-            reinterpret_cast<float4*>(y)[i] = make_float4(u.x + v.x, u.y + v.y, u.z + v.z, u.w + v.w);
+            const float4 u = reinterpret_cast<const float4*>(x)[i];
+            reinterpret_cast<float4*>(y)[i] = make_float4(unary_f32_op<OP>(u.x), unary_f32_op<OP>(u.y), unary_f32_op<OP>(u.z),
+                                                          unary_f32_op<OP>(u.w));
         }
         done = n4 << 2;
     }
-    for (size_t i = done + i0; i < n; i += stride) y[i] = a[i] + b[i];
+    for (size_t i = done + i0; i < n; i += stride) y[i] = unary_f32_op<OP>(x[i]);
 }
-cudaError_t launch_binary_add_f32(const float* a, const float* b, float* y, size_t n, cudaStream_t s) {
-    const int vec = (((uintptr_t)a | (uintptr_t)b | (uintptr_t)y) & 15) == 0;
-    binary_add_f32_kernel<<<grid_for(vec ? (n >> 2) + 1 : n, 256), 256, 0, s>>>(a, b, y, n, vec);
+template <int OP>
+static void launch_unary_op(const float* x, float* y, size_t n, int vec, int grid, cudaStream_t s) {
+    unary_f32_kernel<OP><<<grid, 256, 0, s>>>(x, y, n, vec);
+}
+bool unary_f32_supported(int op) {
+    switch (op) {
+        case kUnaryAbs: case kUnaryNeg: case kUnarySquare: case kUnarySqrt: case kUnaryRsqrt: case kUnaryReciprocal:
+        case kUnaryExp: case kUnaryLog: case kUnaryTanh: case kUnarySigmoid: case kUnarySilu: case kUnaryHardSwish:
+        case kUnaryGelu: case kUnaryGeluStandard:
+            return true;
+        default:
+            return false;
+    }
+}
+cudaError_t launch_unary_f32(int op, const float* x, float* y, size_t n, cudaStream_t s) {
+    const int vec = (((uintptr_t)x | (uintptr_t)y) & 15) == 0;
+    const int grid = grid_for(vec ? (n >> 2) + 1 : n, 256);
+    switch (op) {
+        case kUnaryAbs: launch_unary_op<kUnaryAbs>(x, y, n, vec, grid, s); break;
+        case kUnaryNeg: launch_unary_op<kUnaryNeg>(x, y, n, vec, grid, s); break;
+        case kUnarySquare: launch_unary_op<kUnarySquare>(x, y, n, vec, grid, s); break;
+        case kUnarySqrt: launch_unary_op<kUnarySqrt>(x, y, n, vec, grid, s); break;
+        case kUnaryRsqrt: launch_unary_op<kUnaryRsqrt>(x, y, n, vec, grid, s); break;
+        case kUnaryReciprocal: launch_unary_op<kUnaryReciprocal>(x, y, n, vec, grid, s); break;
+        case kUnaryExp: launch_unary_op<kUnaryExp>(x, y, n, vec, grid, s); break;
+        case kUnaryLog: launch_unary_op<kUnaryLog>(x, y, n, vec, grid, s); break;
+        case kUnaryTanh: launch_unary_op<kUnaryTanh>(x, y, n, vec, grid, s); break;
+        case kUnarySigmoid: launch_unary_op<kUnarySigmoid>(x, y, n, vec, grid, s); break;
+        case kUnarySilu: launch_unary_op<kUnarySilu>(x, y, n, vec, grid, s); break;
+        case kUnaryHardSwish: launch_unary_op<kUnaryHardSwish>(x, y, n, vec, grid, s); break;
+        case kUnaryGelu: launch_unary_op<kUnaryGelu>(x, y, n, vec, grid, s); break;
+        case kUnaryGeluStandard: launch_unary_op<kUnaryGeluStandard>(x, y, n, vec, grid, s); break;
+        default: return cudaErrorInvalidValue;
+    }
+    ++g_launch_count;
+    return cudaGetLastError();
+}
+
+// ---- ArgMax / ArgMin over the middle axis of [outside][axis][inside] -> int32 [outside][inside] (CPUArgMax.cpp:115-156, the
+//      non-NC4HW4 branch): the running best starts at -FLT_MAX (ArgMin: +FLT_MAX) with index 0 and is replaced only by a strictly
+//      better value, so the first extreme wins.  One warp per row when inside == 1 (lanes keep their own first best; the
+//      reduction prefers the better value, then the lower index), else one thread per (outside, inside) column.
+__device__ __forceinline__ bool argmax_better(float v, int i, float bv, int bi, int is_min) {
+    return (is_min ? v < bv : v > bv) || (v == bv && i < bi);
+}
+__global__ void argmax_f32_kernel(const float* __restrict__ x, int32_t* __restrict__ y, int outside, int axis, int inside,
+                                  int is_min) {
+    const float init = is_min ? 3.402823466e38f : -3.402823466e38f;
+    if (inside == 1) {
+        const int row = (int)((blockIdx.x * (size_t)blockDim.x + threadIdx.x) >> 5), lane = threadIdx.x & 31;
+        if (row >= outside) return;
+        const float* xp = x + (size_t)row * axis;
+        float best = init;
+        int idx = 0;
+        for (int a = lane; a < axis; a += 32) {
+            const float v = xp[a];
+            if (is_min ? v < best : v > best) { best = v; idx = a; }
+        }
+        for (int o = 16; o > 0; o >>= 1) {
+            const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+            const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+            if (argmax_better(ov, oi, best, idx, is_min)) { best = ov; idx = oi; }
+        }
+        if (lane == 0) y[row] = idx;
+        return;
+    }
+    const size_t total = (size_t)outside * inside;
+    for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
+        const size_t o = i / inside, in = i - o * inside;
+        const float* xp = x + o * axis * inside + in;
+        float best = init;
+        int idx = 0;
+        for (int a = 0; a < axis; ++a) {
+            const float v = xp[(size_t)a * inside];
+            if (is_min ? v < best : v > best) { best = v; idx = a; }
+        }
+        y[i] = idx;
+    }
+}
+cudaError_t launch_argmax_f32(const float* x, int outside, int axis, int inside, int is_min, int32_t* y, cudaStream_t s) {
+    if (inside == 1) argmax_f32_kernel<<<(unsigned)(((size_t)outside * 32 + 255) / 256), 256, 0, s>>>(x, y, outside, axis, inside, is_min);
+    else argmax_f32_kernel<<<grid_for((size_t)outside * inside, 256), 256, 0, s>>>(x, y, outside, axis, inside, is_min);
     ++g_launch_count;
     return cudaGetLastError();
 }

@@ -151,6 +151,24 @@ struct DwF32Params {
 };
 cudaError_t launch_dwconv_f32(const DwF32Params& p, cudaStream_t s);
 cudaError_t launch_binary_add_f32(const float* a, const float* b, float* y, size_t n, cudaStream_t s);
+// fp32 BinaryOp / UnaryOp codes: the reference's BinaryOpOperation / UnaryOpOperation values (schema TensorflowOp.fbs)
+enum {
+    kBinaryAdd = 0, kBinarySub = 1, kBinaryMul = 2, kBinaryRealDiv = 7, kBinaryMinimum = 8, kBinaryMaximum = 9,
+    kBinarySquaredDifference = 14,
+};
+enum {
+    kUnaryAbs = 0, kUnaryNeg = 1, kUnarySquare = 4, kUnarySqrt = 5, kUnaryRsqrt = 6, kUnaryExp = 7, kUnaryLog = 8,
+    kUnaryReciprocal = 15, kUnarySigmoid = 29, kUnaryTanh = 30, kUnaryHardSwish = 31, kUnaryGelu = 32, kUnaryGeluStandard = 33,
+    kUnarySilu = 34,
+};
+// y[i] = a op b (then ReLU when relu != 0); a_one / b_one: that side is one element, broadcast to all n
+bool binary_f32_supported(int op);
+cudaError_t launch_binary_f32(int op, const float* a, bool a_one, const float* b, bool b_one, float* y, size_t n, int relu,
+                              cudaStream_t s);
+bool unary_f32_supported(int op);
+cudaError_t launch_unary_f32(int op, const float* x, float* y, size_t n, cudaStream_t s);
+// index of the first maximum (is_min: minimum) along the middle axis of [outside][axis][inside] -> int32 [outside][inside]
+cudaError_t launch_argmax_f32(const float* x, int outside, int axis, int inside, int is_min, int32_t* y, cudaStream_t s);
 cudaError_t launch_scale_f32(const float* x, const float* scale, const float* bias, float* y, int n, int c, size_t plane,
                              cudaStream_t s);
 cudaError_t launch_softmax_f32(const float* x, float* y, int outside, int axis, int inside, cudaStream_t s);

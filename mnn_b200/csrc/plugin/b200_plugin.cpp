@@ -922,13 +922,106 @@ private:
     bool mDepthwise;
     int mIc = 0;
 };
-class BinaryAddF32Exec : public B200Exec {
+static bool isF32(const Tensor* t) { return t->getType().code == halide_type_float && t->getType().bytes() == 4; }
+// a full-size operand has the output's bytes: the same linear layout, or both of <= 2 dims (NCHW and NHWC are then the same)
+static bool sameLinear(const Tensor* t, const Tensor* out) {
+    return linearFormat(t) == linearFormat(out) || (t->dimensions() <= 2 && out->dimensions() <= 2);
+}
+// BinaryOp on float tensors (CPUBinary): with GEOMETRY_COMPUTE_MASK 0 every broadcast but a one-element side has been turned into
+// a Raster before the op (GeometryBinary.cpp), so each input is either the output's size or one element
+class BinaryF32Exec : public B200Exec {
 public:
-    BinaryAddF32Exec(Backend* bn) : B200Exec(bn) {}
-    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        return toErr(mnnb200_binary_add_f32(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(inputs[0]),
-                                            (const float*)dev(inputs[1]), (float*)dev(outputs[0]), elemCount(outputs[0])), "BinaryOp add fp32");
+    BinaryF32Exec(Backend* bn, int op, int relu) : B200Exec(bn), mOp(op), mRelu(relu) {}
+    static bool supports(int op) {
+        switch (op) {
+            case BinaryOpOperation_ADD: case BinaryOpOperation_SUB: case BinaryOpOperation_MUL: case BinaryOpOperation_REALDIV:
+            case BinaryOpOperation_MINIMUM: case BinaryOpOperation_MAXIMUM: case BinaryOpOperation_SquaredDifference:
+                return true;
+            default:
+                return false;
+        }
     }
+    static bool takes(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) {
+        if (inputs.size() != 2 || outputs.size() != 1 || !isF32(outputs[0])) return false;
+        const size_t n = elemCount(outputs[0]);
+        int full = 0;
+        for (auto t : inputs) {
+            if (!isF32(t)) return false;
+            const size_t c = elemCount(t);
+            if (c == n && sameLinear(t, outputs[0])) ++full;
+            else if (c != 1) return false;
+        }
+        return full >= 1 || n == 1;
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        return toErr(mnnb200_binary_f32(static_cast<B200Backend*>(backend())->handle(), mOp, (const float*)dev(inputs[0]), elemCount(inputs[0]),
+                                        (const float*)dev(inputs[1]), elemCount(inputs[1]), (float*)dev(outputs[0]), elemCount(outputs[0]),
+                                        mRelu), "BinaryOp fp32");
+    }
+private:
+    int mOp, mRelu;
+};
+// Eltwise SUM / PROD / MAXIMUM / SUB (CPUEltwise.cpp:46-85): inputs 0 and 1, then every further input folded into the output
+class EltwiseF32Exec : public B200Exec {
+public:
+    EltwiseF32Exec(Backend* bn, int op) : B200Exec(bn), mOp(op) {}
+    static int binaryOp(EltwiseType t) {
+        switch (t) {
+            case EltwiseType_PROD: return BinaryOpOperation_MUL;
+            case EltwiseType_SUM: return BinaryOpOperation_ADD;
+            case EltwiseType_MAXIMUM: return BinaryOpOperation_MAXIMUM;
+            case EltwiseType_SUB: return BinaryOpOperation_SUB;
+            default: return -1;
+        }
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto rt = static_cast<B200Backend*>(backend())->handle();
+        const size_t n = elemCount(outputs[0]);
+        auto y = (float*)dev(outputs[0]);
+        mnnb200_status st = mnnb200_binary_f32(rt, mOp, (const float*)dev(inputs[0]), n, (const float*)dev(inputs[1]), n, y, n, 0);
+        for (size_t i = 2; st == MNNB200_OK && i < inputs.size(); ++i)
+            st = mnnb200_binary_f32(rt, mOp, y, n, (const float*)dev(inputs[i]), n, y, n, 0);
+        return toErr(st, "Eltwise fp32");
+    }
+private:
+    int mOp;
+};
+class UnaryF32Exec : public B200Exec {
+public:
+    UnaryF32Exec(Backend* bn, int op) : B200Exec(bn), mOp(op) {}
+    static bool supports(int op) {
+        switch (op) {
+            case UnaryOpOperation_ABS: case UnaryOpOperation_NEG: case UnaryOpOperation_SQUARE: case UnaryOpOperation_SQRT:
+            case UnaryOpOperation_RSQRT: case UnaryOpOperation_EXP: case UnaryOpOperation_LOG: case UnaryOpOperation_RECIPROCAL:
+            case UnaryOpOperation_SIGMOID: case UnaryOpOperation_TANH: case UnaryOpOperation_HARDSWISH: case UnaryOpOperation_GELU:
+            case UnaryOpOperation_GELU_STANDARD: case UnaryOpOperation_SILU:
+                return true;
+            default:
+                return false;
+        }
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        return toErr(mnnb200_unary_f32(static_cast<B200Backend*>(backend())->handle(), mOp, (const float*)dev(inputs[0]),
+                                       (float*)dev(outputs[0]), elemCount(outputs[0])), "UnaryOp fp32");
+    }
+private:
+    int mOp;
+};
+// ArgMax / ArgMin with one index per position and no values (CPUArgMax's non-NC4HW4 branch): int32 output
+class ArgMaxExec : public B200Exec {
+public:
+    ArgMaxExec(Backend* bn, int axis, bool isMin) : B200Exec(bn), mAxis(axis), mIsMin(isMin) {}
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto in = inputs[0];
+        int outside = 1, inside = 1;
+        for (int i = 0; i < mAxis; ++i) outside *= in->length(i);
+        for (int i = mAxis + 1; i < in->dimensions(); ++i) inside *= in->length(i);
+        return toErr(mnnb200_argmax_f32(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(in), outside, in->length(mAxis),
+                                        inside, mIsMin ? 1 : 0, (int32_t*)dev(outputs[0])), "ArgMax");
+    }
+private:
+    int mAxis;
+    bool mIsMin;
 };
 class ScaleF32Exec : public B200Exec {
 public:
@@ -1018,11 +1111,40 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
             if (quantOut && inputs.size() == 2 && op->main_as_BinaryOp() && op->main_as_BinaryOp()->opType() == BinaryOpOperation_ADD &&
                 op->main_as_BinaryOp()->activationType() == 0 && elemCount(inputs[0]) == elemCount(inputs[1]) && isInt8(inputs[0]) && isInt8(inputs[1]))
                 e = new BinaryAddInt8Exec(this);
-            else if (!quantOut && inputs.size() == 2 && op->main_as_BinaryOp() && op->main_as_BinaryOp()->opType() == BinaryOpOperation_ADD &&
-                     op->main_as_BinaryOp()->activationType() == 0 && elemCount(inputs[0]) == elemCount(outputs[0]) &&
-                     elemCount(inputs[1]) == elemCount(outputs[0]) && isF32Nchw(inputs[0]) && isF32Nchw(inputs[1]) && isF32Nchw(outputs[0]))
-                e = new BinaryAddF32Exec(this);   // equal sizes only (the residual add); broadcasts are declined
+            else if (!quantOut && op->main_as_BinaryOp() && BinaryF32Exec::supports(op->main_as_BinaryOp()->opType()) &&
+                     (op->main_as_BinaryOp()->activationType() == 0 || op->main_as_BinaryOp()->activationType() == 1) &&
+                     BinaryF32Exec::takes(inputs, outputs))
+                e = new BinaryF32Exec(this, op->main_as_BinaryOp()->opType(), op->main_as_BinaryOp()->activationType());
             break;
+        case OpType_Eltwise: {
+            // no coeff: the CPU takes only the {1, 0} copy form of one and fails the rest (CPUEltwise.cpp:35-45)
+            auto el = op->main_as_Eltwise();
+            bool ok = !quantOut && el && !(el->coeff() && el->coeff()->size() > 0) && EltwiseF32Exec::binaryOp(el->type()) >= 0 &&
+                      inputs.size() >= 2 && outputs.size() == 1 && isF32(outputs[0]);
+            for (auto t : inputs) ok = ok && isF32(t) && elemCount(t) == elemCount(outputs[0]) && sameLinear(t, outputs[0]);
+            if (ok) e = new EltwiseF32Exec(this, EltwiseF32Exec::binaryOp(el->type()));
+            break;
+        }
+        case OpType_UnaryOp:
+            if (!quantOut && op->main_as_UnaryOp() && UnaryF32Exec::supports(op->main_as_UnaryOp()->opType()) && inputs.size() == 1 &&
+                outputs.size() == 1 && isF32(inputs[0]) && isF32(outputs[0]) && elemCount(inputs[0]) == elemCount(outputs[0]) &&
+                sameLinear(inputs[0], outputs[0]))
+                e = new UnaryF32Exec(this, op->main_as_UnaryOp()->opType());
+            break;
+        case OpType_ArgMax:
+        case OpType_ArgMin: {
+            // the CPU's NC4HW4 input branch is the legacy Caffe form (top-k, float indices): declined, as is any top-k > 1 or
+            // value output
+            auto am = op->main_as_ArgMax();
+            if (!quantOut && am && am->topK() == 1 && am->outMaxVal() == 0 && inputs.size() == 1 && outputs.size() == 1 &&
+                isF32(inputs[0]) && outputs[0]->getType().code == halide_type_int && outputs[0]->getType().bytes() == 4 &&
+                TensorUtils::getDescribe(inputs[0])->dimensionFormat != MNN_DATA_FORMAT_NC4HW4) {
+                int axis = am->axis();
+                if (axis < 0) axis += inputs[0]->dimensions();
+                if (axis >= 0 && axis < inputs[0]->dimensions()) e = new ArgMaxExec(this, axis, op->type() == OpType_ArgMin);
+            }
+            break;
+        }
         case OpType_Pooling:
             if (!quantOut && op->main_as_Pool() && outputs.size() == 1 && inputs[0]->getType().code == halide_type_float &&
                 linearFormat(inputs[0]) == MNN_DATA_FORMAT_NCHW && inputs[0]->dimensions() == 4)

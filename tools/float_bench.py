@@ -8,7 +8,8 @@
                 runSession + output copy per iteration), with the plugin's created / declined command counts;
   cpu           img/s of MNN_FORWARD_CPU on the same model and batch;
   card          name and power limit, read in the same call.
-Usage: python tools/float_bench.py [--batch 32] [--iters 50] [--cpu-threads 16]"""
+With --model other than mbv2 (the other fp32 fixtures build() writes) the line has model, batch, card, plugin_e2e and cpu only.
+Usage: python tools/float_bench.py [--model mbv2] [--batch 32] [--iters 50] [--cpu-threads 16]"""
 import argparse
 import ctypes as C
 import json
@@ -21,6 +22,15 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 HBM_BPS, TF32_FLOPS = 3.35e12, 495e12       # H100 SXM data sheet (700 W): the bounds, not reached figures
+MODELS = {   # --model: (fixture under oracle/_ref, name in the JSON line)
+    "mbv2": ("mbv2_f32.mnn", "MobileNet-v2 fp32 (seeded weights)"),
+    "mbv3": ("mbv3_f32.mnn", "MobileNet-v3 fp32 (seeded weights)"),
+    "nasnet": ("nasnet_f32.mnn", "NASNet fp32 (seeded weights)"),
+    "inception_v3": ("inception_v3_f32.mnn", "Inception-v3 fp32 (seeded weights)"),
+    "squeezenet_v10": ("squeezenet_v10_f32.mnn", "SqueezeNet v1.0 fp32 (seeded weights)"),
+    "squeezenet_v11": ("squeezenet_v11_f32.mnn", "SqueezeNet v1.1 fp32 (seeded weights)"),
+    "mbv1": ("mbv1_f32.mnn", "MobileNet-v1 fp32 (seeded weights)"),
+}
 
 
 def shapes_from_cpu_run(model, refdump, env):
@@ -118,21 +128,24 @@ def refdump_bench(refdump, model, batch, threads, env, iters):
 
 def main():
     ap = argparse.ArgumentParser()
+    ap.add_argument("--model", choices=sorted(MODELS), default="mbv2")
     ap.add_argument("--batch", type=int, default=32)
     ap.add_argument("--iters", type=int, default=50)
     ap.add_argument("--cpu-threads", type=int, default=os.cpu_count() or 4)
     a = ap.parse_args()
     from oracle import oracle as O
-    model = os.path.join(O.REF_DIR, "mbv2_f32.mnn")
+    fixture, title = MODELS[a.model]
+    model = os.path.join(O.REF_DIR, fixture)
     if not O.have_reference() or not os.path.exists(model):
-        sys.exit("float_bench: needs oracle/_ref (refdump, libMNN.so, mbv2_f32.mnn) as build() leaves it")
+        sys.exit(f"float_bench: needs oracle/_ref (refdump, libMNN.so, {fixture}) as build() leaves it")
     env = dict(os.environ)
     env["LD_LIBRARY_PATH"] = O.REF_DIR + ":" + os.path.join(ROOT, "mnn_b200") + ":" + env.get("LD_LIBRARY_PATH", "")
     env.pop("REFDUMP_PLUGIN", None)
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                           text=True, check=True).stdout.strip().splitlines()[0]
-    res = dict(model="MobileNet-v2 fp32 (seeded weights)", batch=a.batch, card=card)
-    res.update(time_convs(shapes_from_cpu_run(model, O.REFDUMP, env), a.batch, a.iters))
+    res = dict(model=title, batch=a.batch, card=card)
+    if a.model == "mbv2":
+        res.update(time_convs(shapes_from_cpu_run(model, O.REFDUMP, env), a.batch, a.iters))
     penv = dict(env, REFDUMP_BENCH_WINDOWS="5", REFDUMP_PLUGIN=os.path.join(ROOT, "mnn_b200", "libmnn_b200_plugin.so"))
     p = refdump_bench(O.REFDUMP, model, a.batch, 4, penv, 20)
     res.update(plugin_e2e_img_per_s=p["img_per_s"], plugin_e2e_ms=p["ms_median_window"], plugin_created=p["plugin_created"],
