@@ -27,6 +27,7 @@
 //              -> stores straight to the NHWC16 output rows; per-column constants staged in shared memory per (layer, n chunk)
 #include <cuda.h>
 #include <cstdlib>
+#include <type_traits>
 #include "common.cuh"
 #include "hopper_common.cuh"
 #include "host_util.h"
@@ -91,6 +92,12 @@ __device__ __forceinline__ void decode_item(uint32_t w, int& layer, int& nc, int
     mt = (int)(w & kGroupItemTileMask);
 }
 
+// A global store the compiler does not treat as a memory write (no "memory" clobber): nothing in the kernel reads the output
+// back, and the compiler may then keep shared-memory values in registers and issue later loads across it.
+__device__ __forceinline__ void st_global_u16(int8_t* p, uint16_t v) {
+    asm volatile("st.global.b16 [%0], %1;\n" ::"l"(p), "h"(v));
+}
+
 // One work item on one consumer warpgroup: rows [64 wg, 64 wg + 64) of `cnt` M tiles x BN columns.  BN is a compile-time
 // constant so the accumulator array, the wgmma_span chain and the epilogue's column loop are fixed: a run-time switch on the
 // tile width between two wgmma instructions would make ptxas serialise every one of them.
@@ -113,6 +120,9 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
     const float scale_x = lp.scale_x, minv = lp.minv, maxv = lp.maxv;
     const bool small_acc = lp.K <= 128;    // |sum (x + 128) w| <= 128 * 255 * 128 < 2^22
+    // the layer fields the epilogue uses, held in registers instead of read from lp (shared memory) for every row and column
+    const int OC = lp.OC, M = lp.M, ldy = lp.ldy, mode = lp.mode;
+    int8_t* const y = lp.y;
     for (int t = 0; t < cnt; ++t) {
         const int mt = mt0 + t;
         int prev = -1;
@@ -160,8 +170,8 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
             const int r = r_base + 8 * h;
             int8_t* yrow = nullptr;
             const int32_t* corrp = nullptr;    // border pixel of a padded conv with z_in != 0: + z_in * sum_{OOB taps} w
-            if (lp.mode == 0) {
-                if (mt * kBM + r < lp.M) yrow = lp.y + (size_t)(mt * kBM + r) * lp.ldy + n0;
+            if (mode == 0) {
+                if (mt * kBM + r < M) yrow = y + (size_t)(mt * kBM + r) * ldy + n0;
             } else {
                 // implicit-GEMM layers: which output pixel accumulator row r is, and its border class
                 const GroupConvGeom& g = *gp;
@@ -174,7 +184,7 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
                     const int oh = (tt % g.OHB) * g.BH + brow, n = tt / g.OHB;
                     const int ow = seg * lp.TWp + pcol;
                     if (ow < g.OW) {
-                        yrow = lp.y + (size_t)((n * g.OH + oh) * g.OW + ow) * lp.ldy + n0;
+                        yrow = y + (size_t)((n * g.OH + oh) * g.OW + ow) * ldy + n0;
                         if (g.corr != nullptr) {
                             const int cls = (int)g.hcls[oh] * g.wc_count + (int)g.wcls[ow];
                             if (cls != g.interior_cls) corrp = g.corr + (size_t)cls * lp.N + n0;
@@ -183,26 +193,32 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
                 }
             }
             if (yrow == nullptr) continue;
+            // the requant path is chosen once per row, not once per column pair: one straight run of column pairs whose loads
+            // the compiler can issue ahead of the previous pairs' arithmetic and stores
+            auto columns = [&](auto small) {
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
-                if (j < nblk) {
-                    const int c = j * 8 + 2 * q4;
-                    int k0 = wsum[c], k1 = wsum[c + 1];
-                    if (corrp != nullptr) { k0 += __ldg(corrp + c); k1 += __ldg(corrp + c + 1); }
-                    const int a0 = acc[j * 4 + 2 * h] + k0, a1 = acc[j * 4 + 2 * h + 1] + k1;
-                    int q0, q1;
-                    if (small_acc) {      // |acc_u| < 2^22: int -> float on the FP32 pipe (exact), not on the conversion unit
-                        q0 = requant_fast_small(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
-                        q1 = requant_fast_small(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
-                    } else {
-                        q0 = requant_fast(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
-                        q1 = requant_fast(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                for (int j = 0; j < BN / 8; ++j) {
+                    if (j < nblk) {
+                        const int c = j * 8 + 2 * q4;
+                        int k0 = wsum[c], k1 = wsum[c + 1];
+                        if (corrp != nullptr) { k0 += __ldg(corrp + c); k1 += __ldg(corrp + c + 1); }
+                        const int a0 = acc[j * 4 + 2 * h] + k0, a1 = acc[j * 4 + 2 * h + 1] + k1;
+                        int q0, q1;
+                        if constexpr (decltype(small)::value) {   // |acc_u| < 2^22: int -> float on the FP32 pipe (exact)
+                            q0 = requant_fast_small(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
+                            q1 = requant_fast_small(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                        } else {
+                            q0 = requant_fast(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
+                            q1 = requant_fast(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                        }
+                        if (n0 + c >= OC) q0 = 0;         // NHWC16 channel padding stays zero
+                        if (n0 + c + 1 >= OC) q1 = 0;
+                        st_global_u16(yrow + c, (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8)));
                     }
-                    if (n0 + c >= lp.OC) q0 = 0;         // NHWC16 channel padding stays zero
-                    if (n0 + c + 1 >= lp.OC) q1 = 0;
-                    *reinterpret_cast<uint16_t*>(yrow + c) = (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8));
                 }
-            }
+            };
+            if (small_acc) columns(std::true_type{});
+            else columns(std::false_type{});
         }
     }
 }
