@@ -93,9 +93,10 @@ __device__ __forceinline__ void decode_item(uint32_t w, int& layer, int& nc, int
 }
 
 // A global store the compiler does not treat as a memory write (no "memory" clobber): nothing in the kernel reads the output
-// back, and the compiler may then keep shared-memory values in registers and issue later loads across it.
-__device__ __forceinline__ void st_global_u16(int8_t* p, uint16_t v) {
-    asm volatile("st.global.b16 [%0], %1;\n" ::"l"(p), "h"(v));
+// back, and the compiler may then keep shared-memory values in registers and issue later loads across it.  Predicated on
+// j < lim inside the instruction, so a run of such stores over a column loop stays one straight run of code.
+__device__ __forceinline__ void st_global_u16_if(int8_t* p, uint16_t v, int j, int lim) {
+    asm volatile("{\n .reg .pred q;\n setp.lt.s32 q, %2, %3;\n @q st.global.b16 [%0], %1;\n}\n" ::"l"(p), "h"(v), "r"(j), "r"(lim));
 }
 
 // One work item on one consumer warpgroup: rows [64 wg, 64 wg + 64) of `cnt` M tiles x BN columns.  BN is a compile-time
@@ -164,18 +165,33 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
         if (lane == 0) mbar_arrive(bar0 + 8u * (kStages + prev));
 
         // ---- epilogue from the accumulator fragments: register i = row r_base + 8 * ((i >> 1) & 1),
-        //      column 8 * (i >> 2) + 2 * q4 + (i & 1); two output bytes per store
+        //      column 8 * (i >> 2) + 2 * q4 + (i & 1); two output bytes per store.
+        // Row setup first, for both rows of the thread: the output address, how many 8-column blocks of the row are stored (0 for
+        // a row outside the layer) and, for a padded conv with z_in != 0, the row of the border-correction table.
+        int8_t* yrow[2];
+        int lim[2];
+        const int32_t* corrp[2];
+        bool corr = false;                   // some row of the warp is a border pixel: + z_in * sum_{OOB taps} w
+        if (mode == 0) {
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {
-            const int r = r_base + 8 * h;
-            int8_t* yrow = nullptr;
-            const int32_t* corrp = nullptr;    // border pixel of a padded conv with z_in != 0: + z_in * sum_{OOB taps} w
-            if (mode == 0) {
-                if (mt * kBM + r < M) yrow = y + (size_t)(mt * kBM + r) * ldy + n0;
-            } else {
-                // implicit-GEMM layers: which output pixel accumulator row r is, and its border class
-                const GroupConvGeom& g = *gp;
-                const int box_rows = g.BH * lp.TWp;
+            for (int h = 0; h < 2; ++h) {
+                const int m = mt * kBM + r_base + 8 * h;
+                yrow[h] = y + (size_t)m * ldy + n0;
+                lim[h] = m < M ? nblk : 0;
+                corrp[h] = nullptr;
+            }
+        } else {
+            // implicit-GEMM layers: which output pixel accumulator row r is, and its border class
+            const GroupConvGeom& g = *gp;
+            const int box_rows = g.BH * lp.TWp;
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int r = r_base + 8 * h;
+                yrow[h] = y;
+                lim[h] = 0;
+                // a row without a correction reads the interior class's row of the table, which holds zeros (or, outside the
+                // layer, any row: nothing is stored)
+                corrp[h] = g.corr == nullptr ? nullptr : g.corr + (size_t)(g.interior_cls < 0 ? 0 : g.interior_cls) * lp.N + n0;
                 const int j = r / box_rows, rem = r - j * box_rows;
                 const int brow = rem / lp.TWp, pcol = rem - brow * lp.TWp;
                 const int rb = mt * lp.R + j;
@@ -184,41 +200,54 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
                     const int oh = (tt % g.OHB) * g.BH + brow, n = tt / g.OHB;
                     const int ow = seg * lp.TWp + pcol;
                     if (ow < g.OW) {
-                        yrow = y + (size_t)((n * g.OH + oh) * g.OW + ow) * ldy + n0;
+                        yrow[h] = y + (size_t)((n * g.OH + oh) * g.OW + ow) * ldy + n0;
+                        lim[h] = nblk;
                         if (g.corr != nullptr) {
                             const int cls = (int)g.hcls[oh] * g.wc_count + (int)g.wcls[ow];
-                            if (cls != g.interior_cls) corrp = g.corr + (size_t)cls * lp.N + n0;
+                            if (cls != g.interior_cls) { corrp[h] = g.corr + (size_t)cls * lp.N + n0; corr = true; }
                         }
                     }
                 }
             }
-            if (yrow == nullptr) continue;
-            // the requant path is chosen once per row, not once per column pair: one straight run of column pairs whose loads
-            // the compiler can issue ahead of the previous pairs' arithmetic and stores
-            auto columns = [&](auto small) {
+            corr = __any_sync(0xffffffffu, corr);
+        }
+        // Then one straight run over every column pair of both rows, the BN-wide tile whole: columns past the chunk's valid
+        // ones read zero constants, only their stores are predicated off.  With no control flow inside, ptxas overlaps the
+        // pairs' requant chains.  The requant path and the border correction are chosen once per run.
+        const int ccap = nblk * 8 - 2;       // last valid column pair: the correction table's row ends there
+        auto columns = [&](auto small, auto with_corr) {
 #pragma unroll
-                for (int j = 0; j < BN / 8; ++j) {
-                    if (j < nblk) {
-                        const int c = j * 8 + 2 * q4;
-                        int k0 = wsum[c], k1 = wsum[c + 1];
-                        if (corrp != nullptr) { k0 += __ldg(corrp + c); k1 += __ldg(corrp + c + 1); }
-                        const int a0 = acc[j * 4 + 2 * h] + k0, a1 = acc[j * 4 + 2 * h + 1] + k1;
-                        int q0, q1;
-                        if constexpr (decltype(small)::value) {   // |acc_u| < 2^22: int -> float on the FP32 pipe (exact)
-                            q0 = requant_fast_small(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
-                            q1 = requant_fast_small(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
-                        } else {
-                            q0 = requant_fast(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
-                            q1 = requant_fast(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
-                        }
-                        if (n0 + c >= OC) q0 = 0;         // NHWC16 channel padding stays zero
-                        if (n0 + c + 1 >= OC) q1 = 0;
-                        st_global_u16(yrow + c, (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8)));
+            for (int j = 0; j < BN / 8; ++j) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {        // rows inside: a column pair's constants serve both rows, then die
+                    const int c = j * 8 + 2 * q4;
+                    int k0 = wsum[c], k1 = wsum[c + 1];
+                    if constexpr (decltype(with_corr)::value) {
+                        const int cc = min(c, ccap);
+                        k0 += __ldg(corrp[h] + cc);
+                        k1 += __ldg(corrp[h] + cc + 1);
                     }
+                    const int a0 = acc[j * 4 + 2 * h] + k0, a1 = acc[j * 4 + 2 * h + 1] + k1;
+                    int q0, q1;
+                    if constexpr (decltype(small)::value) {   // |acc_u| < 2^22: int -> float on the FP32 pipe (exact)
+                        q0 = requant_fast_small(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
+                        q1 = requant_fast_small(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                    } else {
+                        q0 = requant_fast(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
+                        q1 = requant_fast(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                    }
+                    if (n0 + c >= OC) q0 = 0;         // NHWC16 channel padding stays zero
+                    if (n0 + c + 1 >= OC) q1 = 0;
+                    st_global_u16_if(yrow[h] + c, (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8)), j, lim[h]);
                 }
-            };
-            if (small_acc) columns(std::true_type{});
-            else columns(std::false_type{});
+            }
+        };
+        if (corr) {
+            if (small_acc) columns(std::true_type{}, std::true_type{});
+            else columns(std::false_type{}, std::true_type{});
+        } else {
+            if (small_acc) columns(std::true_type{}, std::false_type{});
+            else columns(std::false_type{}, std::false_type{});
         }
     }
 }
@@ -444,9 +473,10 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
             const int ncols = (lp.N - n0) < bn ? (lp.N - n0) : bn;      // valid (16-padded) columns of this chunk
             const int nblk = ncols >> 3;
             if ((w >> kGroupItemChunkShift) != cached) {
-                // reload the per-column constants once every consumer is done READING the previous item's, then publish
+                // reload the per-column constants once every consumer is done READING the previous item's, then publish.  The
+                // whole tile width: the epilogue computes every column, zeros past the layer's last channel.
                 named_sync(1, kConsumerThreads);
-                for (int j = ct; j < ncols; j += kConsumerThreads) {
+                for (int j = ct; j < bn; j += kConsumerThreads) {
                     const int n = n0 + j;
                     const bool v = n < lp.OC;
                     cst[j] = v ? lp.wscale[n] : 0.f;

@@ -95,7 +95,8 @@ struct GroupConvGeom {               // mode 1 only; stays in global memory (rea
     int BH, OHB, pad0_, pad1_;       // a TMA box covers BH consecutive output rows of one image (stride_h == 1), OHB = OH / BH boxes per image
     const uint8_t* hcls;             // [OH] border class of an output row   (nullptr: z_in == 0, no correction)
     const uint8_t* wcls;             // [OW] border class of an output column
-    const int32_t* corr;             // [HC*WC][N] z_in * sum over the out-of-image taps of sum_c w[oc][tap][c]
+    const int32_t* corr;             // [HC*WC][N] z_in * sum over the out-of-image taps of sum_c w[oc][tap][c]; the interior
+                                     // class's row is zeros (the epilogue adds it for pixels next to a border pixel)
     int wc_count, interior_cls;
 };
 // schedule: grid rows of sched_stride items, each row ends with kGroupSchedEnd.  item = layer << 26 | n chunk << 20 |
