@@ -160,23 +160,24 @@ static inline int conv_out(int i, int k, int s, int p, int d) { return (i + 2 * 
 // How a resized conv runs, decided once at resize (conv_plan): the kernels that take it and, where the conv-group kernel does,
 // its layer there -- everything but the x / y pointers, which bind (group_build) adds.
 struct ConvPlan {
-    bool gemm = false;    // 1x1, stride 1, no pad: the wgmma GEMM (and mode 0 on the conv-group kernel)
+    bool gemm = false;    // 1x1, stride 1, no pad: mode 0 on the conv-group kernel
     bool stem = false;    // <= 4 input channels: the dp4a stem kernel
     bool group = false;   // the conv-group kernel takes it: q / g / tmap_b hold the layer and the schedule word can address it
     GroupLayerParams q;   // y = nullptr
     GroupConvGeom g;      // mode 1 only; hcls / wcls / corr point into the execution's d_border
     CUtensorMap tmap_b;   // weights, boxes of q.cb bytes x q.bn rows
 };
-enum class ConvPath { Gemm, Stem, Implicit, MmaSync, Refused };
-// variant (mnnb200_conv_int8_set_variant): 0 auto, 1 mma.sync, 2 wgmma -- Refused when neither wgmma kernel takes the conv
+enum class ConvPath { Stem, Group, MmaSync, Refused };
+// variant (mnnb200_conv_int8_set_variant): 0 auto, 1 mma.sync, 2 wgmma -- Refused when the conv-group kernel does not take the conv
 static ConvPath conv_path(const ConvPlan& c, int variant) {
     if (variant == 1) return ConvPath::MmaSync;
-    if (c.gemm) return ConvPath::Gemm;
-    // first-layer convs (<= 4 input channels): the dp4a kernel beats the implicit GEMM, whose K would be 13/16 padding
-    if (variant == 0 && c.stem) return ConvPath::Stem;
-    // k > 1 / strided / dilated convs: implicit GEMM on wgmma (this layer alone on the conv-group kernel); mma.sync takes what
-    // that kernel does not (stride_w > 2, the largest feature maps)
-    if (c.group) return ConvPath::Implicit;
+    // first-layer convs (<= 4 input channels, not GEMM-shaped): the dp4a kernel beats the implicit GEMM, whose K would be 13/16
+    // padding.  Inside a group they also keep the single-thread TMA producers of every CTA busy and slow the whole group down
+    // (measured on MobileNet-v2 B=32: 0.31 ms with the stem inside the group, 0.19 ms with it outside).
+    if (variant == 0 && c.stem && !c.gemm) return ConvPath::Stem;
+    // wgmma on the conv-group kernel, alone as a one-layer group or as a member of a larger one; mma.sync takes what that
+    // kernel does not (stride_w > 2, the largest feature maps)
+    if (c.group) return ConvPath::Group;
     return variant == 0 ? ConvPath::MmaSync : ConvPath::Refused;
 }
 
@@ -191,7 +192,7 @@ struct ConvInt8Exec : mnnb200_exec {
     ConvPlan plan;
     int32_t* d_border = nullptr;           // border-class tables of plan.g, grow-only
     size_t border_cap = 0;
-    struct GroupState* solo = nullptr;     // this layer alone on the conv-group kernel (implicit GEMM on wgmma)
+    struct GroupState* solo = nullptr;     // this layer alone on the conv-group kernel
     const void* solo_x = nullptr;
     const void* solo_y = nullptr;
     ~ConvInt8Exec() override;
@@ -201,11 +202,6 @@ struct ConvInt8Exec : mnnb200_exec {
     ConvParams p;
     int tile = TILE_128x64;
     bool resized = false;
-    // wgmma GEMM (plan.gemm): A = activation [M][Cp], B = weights [OCp][Cp]
-    int bn = 0;
-    CUtensorMap tmap_b;
-    CUtensorMap tmap_a;
-    const void* tmap_a_ptr = nullptr;
 };
 
 static mnnb200_status conv_create_common(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const int8_t* weight,
@@ -854,12 +850,7 @@ mnnb200_status mnnb200_conv_int8_resize(mnnb200_exec* ex, int n, int ih, int iw,
     e->cost_bytes = (double)n * ih * iw * d.ic + (double)p.M * d.oc + (double)d.oc * d.ic * d.kh * d.kw;
     e->cost_macs = (double)p.M * d.oc * d.ic * d.kh * d.kw;
     if ((st = conv_plan(e, in_zero))) return st;
-    e->tmap_a_ptr = nullptr;
     e->solo_x = e->solo_y = nullptr;
-    if (e->plan.gemm) {
-        e->bn = pick_bn(e->OCp, (p.M + 127) / 128, e->rt->prop.multiProcessorCount);
-        if ((st = make_tmap_i8(&e->tmap_b, e->d_w, e->OCp, e->Cp, e->bn))) return st;
-    }
     e->resized = true;
     if (oh) *oh = OH;
     if (ow) *ow = OW;
@@ -875,25 +866,11 @@ mnnb200_status mnnb200_conv_int8_execute(mnnb200_exec* ex, const int8_t* x, int8
     p.y = y;
     switch (conv_path(e->plan, e->variant)) {
     case ConvPath::Refused:
-        return fail(MNNB200_NOT_SUPPORT, "wgmma variant: this conv shape is not taken by the implicit-GEMM kernel (stride_w > 2?)");
-    case ConvPath::Gemm: {
-        if (e->tmap_a_ptr != (const void*)x) {
-            mnnb200_status st = make_tmap_i8(&e->tmap_a, x, p.M, e->Cp, 128);
-            if (st) return st;
-            e->tmap_a_ptr = x;
-        }
-        GemmI8Params g;
-        memset(&g, 0, sizeof(g));
-        g.a = x; g.b = e->d_w; g.M = p.M; g.N = e->OCp; g.K = e->Cp;
-        g.y_i8 = y; g.ldy = e->OCp; g.wscale = e->d_wscale; g.bias = e->d_bias; g.wsum128 = e->d_wsum128;
-        g.scale_x = p.scale_x; g.minv = p.minv; g.maxv = p.maxv; g.OC = e->d.oc;
-        CK(launch_gemm_i8_wgmma(g, &e->tmap_a, &e->tmap_b, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
-        return MNNB200_OK;
-    }
+        return fail(MNNB200_NOT_SUPPORT, "wgmma variant: this conv shape is not taken by the conv-group kernel (stride_w > 2?)");
     case ConvPath::Stem:
         CK(launch_conv_int8_stem(p, e->rt->stream));
         return MNNB200_OK;
-    case ConvPath::Implicit:
+    case ConvPath::Group:
         if (!e->solo || e->solo_x != (const void*)x || e->solo_y != (const void*)y) {
             if (!e->solo) { e->solo = new GroupState; e->solo->rt = e->rt; }
             else CK(cudaStreamSynchronize(e->rt->stream));
@@ -921,10 +898,7 @@ struct ConvGroupExec : mnnb200_exec {
 int mnnb200_conv_int8_groupable(mnnb200_exec* ex) {
     if (!ex || ex->kind != 1) return 0;
     auto* e = static_cast<ConvInt8Exec*>(ex);
-    // first-layer convs (<= 4 input channels) are better off on their own dp4a kernel: as implicit-GEMM items (16-byte K chunks,
-    // 13/16 padding, ~20 TMA issues per tile) they keep the single-thread TMA producers of every CTA busy and slow the whole group
-    // down (measured on MobileNet-v2 B=32: 0.31 ms with the stem inside the group, 0.19 ms with it outside)
-    return e->resized && e->plan.group && (e->plan.gemm || !e->plan.stem);
+    return e->resized && conv_path(e->plan, 0) == ConvPath::Group;
 }
 mnnb200_status mnnb200_conv_int8_group_plan(mnnb200_exec* ex, int* fields, int count) {
     if (!ex || ex->kind != 1 || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_int8_group_plan: bad argument");

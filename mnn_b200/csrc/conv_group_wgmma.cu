@@ -8,7 +8,8 @@
 //
 // Replaces (structure) the per-op Execution::onExecute walk of Pipeline::execute (source/core/Pipeline.cpp:1069-1140)
 // over ConvInt8CutlassExecution::onExecute (source/backend/cuda/execution/int8/ConvInt8CutlassExecution.cu:381-445)
-// for runs of int8 convolutions; arithmetic = the CPU backend's (see gemm_i8_wgmma.cu / common.cuh).
+// for runs of int8 convolutions; a conv executed alone runs here as a one-layer list.  Arithmetic = the CPU backend's
+// (requant_cpu_exact, common.cuh).
 //
 // Layer modes (kernels.h): 0 = GEMM-shaped 1x1 conv (A is the activation itself); 1 = implicit GEMM for any kernel size /
 // stride <= 2 / dilation / padding: the A tile of a K block (tap, channel chunk) is gathered by R TMA boxes of BH output rows x

@@ -5,8 +5,8 @@
 // by cp.async straight into swizzled shared memory (padded taps are filled with the INPUT ZERO POINT, as the
 // CPU backend does -- compute/ConvInt8TiledExecutor.cpp:2269-2271 -- not with 0 as the reference CUDA kernel),
 // the MMA is mma.sync.m16n8k32.s8 and the epilogue is the CPU backend's fp32 sequence, bit for bit.
-// This is the general kernel (any kernel size / stride / dilation / pad); the wgmma kernel in
-// gemm_i8_wgmma.cu takes the GEMM-shaped cases (1x1 stride 1, LLM linear layers).
+// This is the general kernel (any kernel size / stride / dilation / pad): it takes the convs that the wgmma kernel in
+// conv_group_wgmma.cu does not (stride_w > 2, the largest feature maps).
 //
 // GEMM view: M = N*OH*OW output pixels, N = oc, K = KH*KW*Cp (tap-major, channel-minor; Cp = p16(ic)).
 // Roofline: HBM-bound for MobileNet-class layers; algorithmic bytes = |x| + |w| + |y| (SURVEY 8d).

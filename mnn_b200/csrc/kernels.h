@@ -32,21 +32,19 @@ cudaError_t launch_conv_int8_igemm(const ConvParams& p, int tile, cudaStream_t s
 bool conv_int8_stem_supported(const ConvParams& p, int ic);
 cudaError_t launch_conv_int8_stem(const ConvParams& p, cudaStream_t stream);
 
-// wgmma (s8 x s8 -> s32, register accumulators, TMA operand loads) GEMM for 1x1/stride-1 convs and linear layers
+// wgmma (s8 x s8 -> s32, register accumulators, TMA operand loads) GEMM with fp32 output for the linear layers and the
+// Winograd position GEMMs
 struct GemmI8Params {
     const int8_t* a;  // [M][K]  row-major, K % 16 == 0
     const int8_t* b;  // [Nw][K] row-major ("column-major" B), zero padded rows
-    int M, N, K;      // N = number of valid output columns (padded to 16 for int8 out)
-    // int8 epilogue (conv)
-    int8_t* y_i8;     // [M][ldy]
+    int M, N, K;      // N = output columns padded to 16: the n chunks cover N
     int ldy;
     const float* wscale;
     const float* bias;
     const int32_t* wsum128;
-    float scale_x, minv, maxv;
-    int OC;
-    // fp32 epilogue (dynamic-quant linear): y = acc*alpha*dq[m] + (dq[m]*-128)*wsum[n] + srcsum[m]*wzero[n] + bias[n]
-    float* y_f32;     // [M][ldy]
+    int OC;           // valid output columns
+    // dynamic-quant linear: y = acc*alpha*dq[m] + (dq[m]*-128)*wsum[n] + srcsum[m]*wzero[n] + bias[n]
+    float* y_f32;     // [M][ldy], required
     const float* dq;      // [M] per-token dequant scale
     const float* srcsum;  // [M] float(sum_k (xq+128)) * dq
     const float* wsumf;   // [N] weightKernelSum
@@ -59,7 +57,8 @@ struct GemmI8Params {
 };
 cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& p, const void* tmap_a, const void* tmap_b, int bn, cudaStream_t stream,
                                  int sm_count);
-// ---- one persistent launch over a LIST of int8 convolutions (conv_group_wgmma.cu).  Two layer modes:
+// ---- one persistent launch over a LIST of int8 convolutions (conv_group_wgmma.cu); a lone conv runs as a one-layer list.
+//      Two layer modes:
 //   mode 0  GEMM-shaped (1x1, stride 1, no pad): A = the NHWC16 activation as a 2D matrix, one TMA box per K block
 //   mode 1  implicit GEMM (any kernel / stride <= 2 / dilation / padding): an M tile = R whole output rows of TWp pixels each; the
 //           A operand of K block (tap, channel chunk) is gathered by R TMA boxes from a 4D {C, W, H, N} view of the input

@@ -264,12 +264,14 @@ def test_conv_group_width_by_chunk_matrix(backend):
     refs = [L.submit() for L in layers]
     run_group(backend, layers)
     grouped = [L.check(r.result()) for L, r in zip(layers, refs)]
-    for L, y in zip(layers, grouped):       # each member alone: mode 1 on a one-layer group, mode 0 on the wgmma GEMM
-        L.ex.set_variant(2)
-        L.poison()
-        assert L.ex.onExecute([L.xin], [L.yout]) == 0
-        backend.onSync()
-        assert np.array_equal(L.output(), y), L.plan()
+    # each member alone: on a one-layer group (variant 2) and on the mma.sync kernel (variant 1, no code shared with the group)
+    for L, y in zip(layers, grouped):
+        for variant in (2, 1):
+            L.ex.set_variant(variant)
+            L.poison()
+            assert L.ex.onExecute([L.xin], [L.yout]) == 0
+            backend.onSync()
+            assert np.array_equal(L.output(), y), (variant, L.plan())
 
 
 # ---- B. weight-tile reuse: the 4 tagged slots, the resident set, untagged blocks ---------------------------------------
