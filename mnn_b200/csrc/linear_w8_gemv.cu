@@ -317,10 +317,13 @@ cudaError_t launch_t(const GemvW8Params& p, cudaStream_t stream, int sms) {
     return cudaLaunchKernelEx(&cfg, linear_w8_gemv_kernel<T, R, U>, p);
 }
 
-// rows per warp: as many as keep >= ~2 blocks per SM (the small layers are latency-bound: more blocks = more loads in flight)
+// rows per warp: as many as keep >= ~2 blocks per SM (the small layers are latency-bound: more blocks = more loads in flight).
+// Four rows only for <= 2 tokens, decided at compile time so that <4, 4, 4> and <8, 4, 4> are not instantiated at all.
 template <int T>
 cudaError_t launch_r(const GemvW8Params& p, cudaStream_t stream, int sms) {
-    if (T <= 2 && p.oc >= sms * 2 * 8 * 4) return launch_t<T, 4, 4>(p, stream, sms);
+    if constexpr (T <= 2) {
+        if (p.oc >= sms * 2 * 8 * 4) return launch_t<T, 4, 4>(p, stream, sms);
+    }
     if (p.oc >= sms * 2 * 8 * 2) return launch_t<T, 2, 4>(p, stream, sms);
     return launch_t<T, 1, 4>(p, stream, sms);
 }
