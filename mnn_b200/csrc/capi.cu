@@ -197,12 +197,21 @@ struct ConvInt8Exec : mnnb200_exec {
     const void* solo_y = nullptr;
     ~ConvInt8Exec() override;
     int8_t* d_w = nullptr;
+    int8_t* d_wg = nullptr;                // the conv-group kernel's copy: [n_chunks * bn][taps * Cp], rows permuted per chunk
+    float* d_ep = nullptr;                 // its epilogue table (GroupLayerParams::ep), grow-only
+    size_t ep_cap = 0;
     float *d_wscale = nullptr, *d_bias = nullptr;
     int32_t* d_wsum128 = nullptr;
     ConvParams p;
     int tile = TILE_128x64;
     bool resized = false;
 };
+
+// the conv-group kernel's tile width for OCp output channels: equal n chunks of at most kGroupMaxBN columns
+static int group_bn(int OCp) {
+    const int chunks = (OCp + kGroupMaxBN - 1) / kGroupMaxBN;
+    return ((OCp + chunks - 1) / chunks + 15) & ~15;
+}
 
 static mnnb200_status conv_create_common(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const int8_t* weight,
                                          ConvInt8Exec* e) {
@@ -235,6 +244,17 @@ static mnnb200_status conv_create_common(mnnb200_runtime* rt, const mnnb200_conv
     }
     mnnb200_status st = e->upload(wp, &e->d_w);
     if (st) return st;
+    {   // the conv-group kernel's weights: GEMM column c of chunk nc is channel nc * bn + group_column_channel(c, bn)
+        const int bn = group_bn(e->OCp), n_chunks = (e->OCp + bn - 1) / bn;
+        const size_t row = (size_t)taps * e->Cp;
+        std::vector<int8_t> wg((size_t)n_chunks * bn * row, 0);
+        for (int nc = 0; nc < n_chunks; ++nc)
+            for (int c = 0; c < bn; ++c) {
+                const int o = nc * bn + group_column_channel(c, bn);
+                if (o < e->OCp) memcpy(&wg[((size_t)nc * bn + c) * row], &wp[(size_t)o * row], row);
+            }
+        if ((st = e->upload(wg, &e->d_wg))) return st;
+    }
     std::vector<float> z(e->OCp, 0.f);
     std::vector<int32_t> zi(e->OCp, 0);
     if ((st = e->upload(z, &e->d_wscale))) return st;
@@ -263,7 +283,8 @@ ConvInt8Exec::~ConvInt8Exec() { delete solo; }
 
 // Builds the conv's plan: which kernels take it and, for the conv-group kernel, its layer without the x / y pointers.  Every
 // limit of that kernel and of its schedule word is checked here; a layer outside them is not taken (plan.group = false).
-static mnnb200_status conv_plan(ConvInt8Exec* e, int zin) {
+static mnnb200_status conv_plan(ConvInt8Exec* e, int zin, const std::vector<float>& ws, const std::vector<float>& bf,
+                                const std::vector<int32_t>& k128) {
     const ConvParams& p = e->p;
     const auto& d = e->d;
     ConvPlan& plan = e->plan;
@@ -275,10 +296,11 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin) {
     GroupConvGeom& g = plan.g;
     memset(&q, 0, sizeof(q));
     memset(&g, 0, sizeof(g));
-    const int chunks = (e->OCp + kGroupMaxBN - 1) / kGroupMaxBN;
-    q.bn = ((e->OCp + chunks - 1) / chunks + 15) & ~15;
+    q.bn = group_bn(e->OCp);
     q.n_chunks = (e->OCp + q.bn - 1) / q.bn;
-    q.wscale = e->d_wscale; q.bias = e->d_bias; q.wsum128 = e->d_wsum128;
+    // GEMM column c of chunk nc -> output channel (group_column_channel), and whether it is one of the layer's OC
+    auto channel = [&](int nc, int c) { return nc * q.bn + group_column_channel(c, q.bn); };
+    const int ncol = q.n_chunks * q.bn;
     q.M = p.M; q.N = e->OCp; q.OC = d.oc;
     q.ldy = e->OCp; q.scale_x = p.scale_x; q.minv = p.minv; q.maxv = p.maxv;
     q.mode = plan.gemm ? 0 : 1;
@@ -309,11 +331,28 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin) {
     }
     if (q.n_chunks > kGroupMaxNChunks || q.m_tiles > kGroupMaxMTiles) return MNNB200_OK;
     mnnb200_status st;
-    {   // B: [OCp][taps * Cp], chunk-wide boxes of bn rows
-        cuuint64_t dims[2] = {(cuuint64_t)taps * e->Cp, (cuuint64_t)e->OCp};
+    {   // B: the permuted copy [n_chunks * bn][taps * Cp], chunk-wide boxes of bn rows
+        cuuint64_t dims[2] = {(cuuint64_t)taps * e->Cp, (cuuint64_t)ncol};
         cuuint64_t strides[1] = {(cuuint64_t)taps * e->Cp};
         cuuint32_t box[2] = {(cuuint32_t)q.cb, (cuuint32_t)q.bn};
-        if ((st = make_tmap_u8(&plan.tmap_b, e->d_w, 2, dims, strides, box))) return st;
+        if ((st = make_tmap_u8(&plan.tmap_b, e->d_wg, 2, dims, strides, box))) return st;
+    }
+    {   // epilogue table [n_chunks][3][bn]: wscale, biasFloat, preset = 128 sum w (+ 0x4B400000 for requant_fast_small)
+        const int32_t magic = q.K <= 128 ? 0x4B400000 : 0;
+        std::vector<float> ep((size_t)3 * ncol, 0.f);
+        for (int nc = 0; nc < q.n_chunks; ++nc)
+            for (int c = 0; c < q.bn; ++c) {
+                const int o = channel(nc, c);
+                if (o >= d.oc) continue;
+                float* row = &ep[(size_t)nc * 3 * q.bn];
+                row[c] = ws[o];
+                row[q.bn + c] = bf[o];
+                const int32_t pre = (int32_t)((uint32_t)k128[o] + (uint32_t)magic);
+                memcpy(&row[2 * q.bn + c], &pre, 4);
+            }
+        if ((st = e->grow_scratch((void**)&e->d_ep, &e->ep_cap, ep.size() * 4))) return st;
+        if ((st = e->update(ep, e->d_ep))) return st;
+        q.ep = e->d_ep;
     }
     // padding correction (input zero point != 0): the reference fills padded taps with z_in (ConvInt8TiledExecutor.cpp:2269-2271),
     // the TMA unit fills zeros -> add z_in * sum_{out-of-image taps} sum_c w[oc][tap][c] per border class
@@ -342,20 +381,22 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin) {
         for (uint32_t m : hu) any_border |= m != fullh;
         for (uint32_t m : wu) any_border |= m != fullw;
         if (any_border) {
-            // one buffer: corr [HC * WC][OCp], then hcls [OH] and wcls [OW] bytes
+            // one buffer: corr [HC * WC][n_chunks * bn] in GEMM-column order, then hcls [OH] and wcls [OW] bytes
             const int HC = (int)hu.size(), WC = (int)wu.size();
-            const size_t ncorr = (size_t)HC * WC * e->OCp;
+            const size_t ncorr = (size_t)HC * WC * ncol;
             std::vector<int32_t> tab(ncorr + (p.OH + p.OW + 3) / 4, 0);
             g.interior_cls = -1;
             for (int a = 0; a < HC; ++a)
                 for (int b = 0; b < WC; ++b) {
                     if (hu[a] == fullh && wu[b] == fullw) { g.interior_cls = a * WC + b; continue; }
-                    for (int o = 0; o < d.oc; ++o) {
+                    for (int col = 0; col < ncol; ++col) {
+                        const int o = channel(col / q.bn, col % q.bn);
+                        if (o >= d.oc) continue;
                         int32_t sum = 0;
                         for (int kh = 0; kh < p.KH; ++kh)
                             for (int kw = 0; kw < p.KW; ++kw)
                                 if (!((hu[a] >> kh) & 1u) || !((wu[b] >> kw) & 1u)) sum += e->h_tapsum[(size_t)o * taps + kh * p.KW + kw];
-                        tab[((size_t)a * WC + b) * e->OCp + o] = zin * sum;
+                        tab[((size_t)a * WC + b) * ncol + col] = zin * sum;
                     }
                 }
             memcpy(tab.data() + ncorr, hc.data(), p.OH);
@@ -393,6 +434,7 @@ static mnnb200_status group_build(GroupState& gs, const std::vector<ConvInt8Exec
         if (!e->resized || !e->plan.group) return fail(MNNB200_NOT_SUPPORT, "conv group: a member is not a resized conv the wgmma group kernel takes");
         const ConvParams& p = e->p;
         const GroupLayerParams& q = e->plan.q;
+        if ((uintptr_t)ys[l] % 8) return fail(MNNB200_INVALID_VALUE, "conv group: an output is not 8-byte aligned");
         prm[l] = q;
         prm[l].y = ys[l];
         geo[l] = e->plan.g;
@@ -849,7 +891,7 @@ mnnb200_status mnnb200_conv_int8_resize(mnnb200_exec* ex, int n, int ih, int iw,
     // algorithmic bytes: logical (unpadded) int8 input + output + weights, once each (SURVEY 8d)
     e->cost_bytes = (double)n * ih * iw * d.ic + (double)p.M * d.oc + (double)d.oc * d.ic * d.kh * d.kw;
     e->cost_macs = (double)p.M * d.oc * d.ic * d.kh * d.kw;
-    if ((st = conv_plan(e, in_zero))) return st;
+    if ((st = conv_plan(e, in_zero, ws, bf, k128))) return st;
     e->solo_x = e->solo_y = nullptr;
     e->resized = true;
     if (oh) *oh = OH;

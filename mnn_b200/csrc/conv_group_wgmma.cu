@@ -25,7 +25,8 @@
 //              16 KB activation tiles)
 //   warps 0-7: two consumer warpgroups, 64 rows of the 128-row tile each: wgmma.mma_async m64nNk32 s8 (N = bn <= 128,
 //              accumulators in registers; the per-item work is instantiated per bn, see consume_item) -> CPU-exact requant
-//              -> stores straight to the NHWC16 output rows; per-column constants staged in shared memory per (layer, n chunk)
+//              -> 8-byte stores straight to the NHWC16 output rows; per-column constants staged in shared memory per
+//              (layer, n chunk), the next one copied in with cp.async while the current item runs
 #include <cuda.h>
 #include <cstdlib>
 #include <type_traits>
@@ -48,13 +49,13 @@ constexpr int kStageB = kMaxBN * kBK;             // 16 KB
 constexpr int kStageBytes = kStageA;               // the stage ring holds ACTIVATION tiles only
 constexpr int kBSlots = 4;                        // weight-tile cache: (layer, n chunk, K block) -> slot
 constexpr int kOffB = kStages * kStageA;
-constexpr int kConstBytes = 3 * kMaxBN * 4;       // wscale, bias, wsum128 per column
+constexpr int kConstBytes = 3 * kMaxBN * 4;       // one slot: wscale, biasFloat, preset per column
 
 constexpr int kOffResident = kOffB + kBSlots * kStageB;  // the RESIDENT weight set
 constexpr int kResidentBytes = 36 * 1024;
 static_assert(kOffResident % 1024 == 0, "resident weight tiles need 1 KB alignment");
 constexpr int kOffConsts = kOffResident + kResidentBytes;
-constexpr int kOffLayers = kOffConsts + kConstBytes;
+constexpr int kOffLayers = kOffConsts + 2 * kConstBytes;
 constexpr int kOffRbTab = kOffLayers + kGroupMaxLayers * (int)sizeof(GroupLayerParams);   // producer: [3][16] row-box coordinates
 constexpr int kOffBSlot = kOffRbTab + 3 * 16 * 4;                                          // [kStages] weight slot of the block in each stage
 constexpr int kOffBars = kOffBSlot + 32;                                                   // (kStages ints, padded)
@@ -74,8 +75,9 @@ __device__ __forceinline__ int requant_fast(int acc_u, float wscale, float scale
 }
 // the same sequence for accumulators with |acc_u| < 2^22: float(acc_u) = as_float(0x4B400000 + acc_u) - 1.5 * 2^23 is exact (the
 // integer lands in the mantissa of a float in [2^23, 2^24)): one IADD + one FADD instead of an I2F on the conversion unit
-__device__ __forceinline__ int requant_fast_small(int acc_u, float wscale, float scale_x, float bias_float, float minv, float maxv) {
-    float f = __fmul_rn(__fsub_rn(__int_as_float(0x4B400000 + acc_u), 12582912.0f), wscale);
+// (the conv-group kernel's accumulators start at 0x4B400000 + 128 sum w, so acc_m here is already 0x4B400000 + acc_u)
+__device__ __forceinline__ int requant_fast_small(int acc_m, float wscale, float scale_x, float bias_float, float minv, float maxv) {
+    float f = __fmul_rn(__fsub_rn(__int_as_float(acc_m), 12582912.0f), wscale);
     f = __fmul_rn(f, scale_x);
     f = __fadd_rn(f, bias_float);
     f = fminf(f, maxv);
@@ -96,15 +98,20 @@ __device__ __forceinline__ void decode_item(uint32_t w, int& layer, int& nc, int
 // A global store the compiler does not treat as a memory write (no "memory" clobber): nothing in the kernel reads the output
 // back, and the compiler may then keep shared-memory values in registers and issue later loads across it.  Predicated on
 // j < lim inside the instruction, so a run of such stores over a column loop stays one straight run of code.
-__device__ __forceinline__ void st_global_u16_if(int8_t* p, uint16_t v, int j, int lim) {
-    asm volatile("{\n .reg .pred q;\n setp.lt.s32 q, %2, %3;\n @q st.global.b16 [%0], %1;\n}\n" ::"l"(p), "h"(v), "r"(j), "r"(lim));
+__device__ __forceinline__ void st_global_v2_if(int8_t* p, uint32_t lo, uint32_t hi, int j, int lim) {
+    asm volatile("{\n .reg .pred q;\n setp.lt.s32 q, %3, %4;\n @q st.global.v2.b32 [%0], {%1, %2};\n}\n" ::"l"(p), "r"(lo), "r"(hi),
+                 "r"(j), "r"(lim));
+}
+__device__ __forceinline__ void st_global_b32_if(int8_t* p, uint32_t v, int j, int lim) {
+    asm volatile("{\n .reg .pred q;\n setp.lt.s32 q, %2, %3;\n @q st.global.b32 [%0], %1;\n}\n" ::"l"(p), "r"(v), "r"(j), "r"(lim));
 }
 
 // One work item on one consumer warpgroup: rows [64 wg, 64 wg + 64) of `cnt` M tiles x BN columns.  BN is a compile-time
 // constant so the accumulator array, the wgmma_span chain and the epilogue's column loop are fixed: a run-time switch on the
 // tile width between two wgmma instructions would make ptxas serialise every one of them.
+// cst = the (layer, n chunk)'s row of the epilogue table, [3][BN] in GEMM-column order: wscale, biasFloat, preset.
 template <int BN>
-__device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const GroupConvGeom* __restrict__ gp, int n0, int nblk, int mt0,
+__device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const GroupConvGeom* __restrict__ gp, int n0, int ncols, int mt0,
                                              int cnt, uint32_t base, const uint8_t* smem, const float* cst, int& stage, int& phase) {
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wg = threadIdx.x >> 7;
@@ -114,12 +121,11 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
     // around the wgmmas provably warp-uniform
     const int cb = __shfl_sync(0xffffffffu, lp.cb, 0);
     const int num_kb = __shfl_sync(0xffffffffu, lp.num_kb, 0);
-    const int* wsum = reinterpret_cast<const int*>(cst) + 2 * kMaxBN;
+    const float* wscale = cst;
+    const float* bias = cst + BN;
+    const int* preset = reinterpret_cast<const int*>(cst) + 2 * BN;
     const uint32_t bar0 = base + kOffBars;
     int acc[BN / 2];
-    // defined before the first fence: an undefined accumulator would be live from the kernel's entry, in every instantiation
-#pragma unroll
-    for (int i = 0; i < BN / 2; ++i) acc[i] = 0;
     const float scale_x = lp.scale_x, minv = lp.minv, maxv = lp.maxv;
     const bool small_acc = lp.K <= 128;    // |sum (x + 128) w| <= 128 * 255 * 128 < 2^22
     // the layer fields the epilogue uses, held in registers instead of read from lp (shared memory) for every row and column
@@ -127,6 +133,13 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
     int8_t* const y = lp.y;
     for (int t = 0; t < cnt; ++t) {
         const int mt = mt0 + t;
+        // the accumulators start at their column's preset (128 sum w, + 0x4B400000 for requant_fast_small), so every wgmma
+        // accumulates and the epilogue adds no per-column integer
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) {
+            const int2 v = *reinterpret_cast<const int2*>(preset + 8 * j + 2 * q4);
+            acc[4 * j] = v.x; acc[4 * j + 1] = v.y; acc[4 * j + 2] = v.x; acc[4 * j + 3] = v.y;
+        }
         int prev = -1;
         for (int kb = 0; kb < num_kb; ++kb) {
             mbar_wait(bar0 + 8u * stage, phase);
@@ -140,18 +153,17 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
             if (cb == 128) {
 #pragma unroll
                 for (int k = 0; k < 4; ++k)
-                    wgmma_span<Kind::S8, BN, 0>(acc, gdesc_sw128(a_addr + wg * 64 * 128 + k * 32), gdesc_sw128(b_addr + k * 32), 128,
-                                                (kb | k) != 0);
+                    wgmma_span<Kind::S8, BN, 0>(acc, gdesc_sw128(a_addr + wg * 64 * 128 + k * 32), gdesc_sw128(b_addr + k * 32), 128, 1);
             } else if (cb == 64) {
 #pragma unroll
                 for (int k = 0; k < 2; ++k)
                     wgmma_span<Kind::S8, BN, 0>(acc, gdesc(a_addr + wg * 64 * 64 + k * 32, kSw64, 16, 512),
-                                                gdesc(b_addr + k * 32, kSw64, 16, 512), 64, (kb | k) != 0);
+                                                gdesc(b_addr + k * 32, kSw64, 16, 512), 64, 1);
             } else {
 #pragma unroll
                 for (int u = 0; u < 4; ++u)
                     wgmma_span<Kind::S8, BN, 0>(acc, gdesc(a_addr + 2 * u * (kBM * 16) + wg * 64 * 16, kSwNone, kBM * 16, 128),
-                                                gdesc(b_addr + 2 * u * (BN * 16), kSwNone, BN * 16, 128), 16, (kb | u) != 0);
+                                                gdesc(b_addr + 2 * u * (BN * 16), kSwNone, BN * 16, 128), 16, 1);
             }
             wgmma_commit();
             wgmma_wait<1>();                 // the previous stage's MMAs are done: hand its slot back
@@ -166,8 +178,10 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
         if (lane == 0) mbar_arrive(bar0 + 8u * (kStages + prev));
 
         // ---- epilogue from the accumulator fragments: register i = row r_base + 8 * ((i >> 1) & 1),
-        //      column 8 * (i >> 2) + 2 * q4 + (i & 1); two output bytes per store.
-        // Row setup first, for both rows of the thread: the output address, how many 8-column blocks of the row are stored (0 for
+        //      GEMM column 8 * (i >> 2) + 2 * q4 + (i & 1).  The chunk's columns are permuted (group_column_channel, kernels.h):
+        //      in each 32-column group G the thread holds channels 32 G + 8 q4 ... + 7 of its rows (a 16-wide last group:
+        //      32 G + 4 q4 ... + 3), stored with one 8-byte (4-byte) store per row and group.
+        // Row setup first, for both rows of the thread: the output address, how many channels of the chunk the row stores (0 for
         // a row outside the layer) and, for a padded conv with z_in != 0, the row of the border-correction table.
         int8_t* yrow[2];
         int lim[2];
@@ -178,13 +192,14 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
             for (int h = 0; h < 2; ++h) {
                 const int m = mt * kBM + r_base + 8 * h;
                 yrow[h] = y + (size_t)m * ldy + n0;
-                lim[h] = m < M ? nblk : 0;
+                lim[h] = m < M ? ncols : 0;
                 corrp[h] = nullptr;
             }
         } else {
             // implicit-GEMM layers: which output pixel accumulator row r is, and its border class
             const GroupConvGeom& g = *gp;
             const int box_rows = g.BH * lp.TWp;
+            const int corr_ld = lp.n_chunks * BN;   // the table's columns are in the same permuted order as the weights
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
                 const int r = r_base + 8 * h;
@@ -192,7 +207,7 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
                 lim[h] = 0;
                 // a row without a correction reads the interior class's row of the table, which holds zeros (or, outside the
                 // layer, any row: nothing is stored)
-                corrp[h] = g.corr == nullptr ? nullptr : g.corr + (size_t)(g.interior_cls < 0 ? 0 : g.interior_cls) * lp.N + n0;
+                corrp[h] = g.corr == nullptr ? nullptr : g.corr + (size_t)(g.interior_cls < 0 ? 0 : g.interior_cls) * corr_ld + n0;
                 const int j = r / box_rows, rem = r - j * box_rows;
                 const int brow = rem / lp.TWp, pcol = rem - brow * lp.TWp;
                 const int rb = mt * lp.R + j;
@@ -202,44 +217,64 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
                     const int ow = seg * lp.TWp + pcol;
                     if (ow < g.OW) {
                         yrow[h] = y + (size_t)((n * g.OH + oh) * g.OW + ow) * ldy + n0;
-                        lim[h] = nblk;
+                        lim[h] = ncols;
                         if (g.corr != nullptr) {
                             const int cls = (int)g.hcls[oh] * g.wc_count + (int)g.wcls[ow];
-                            if (cls != g.interior_cls) { corrp[h] = g.corr + (size_t)cls * lp.N + n0; corr = true; }
+                            if (cls != g.interior_cls) { corrp[h] = g.corr + (size_t)cls * corr_ld + n0; corr = true; }
                         }
                     }
                 }
             }
             corr = __any_sync(0xffffffffu, corr);
         }
-        // Then one straight run over every column pair of both rows, the BN-wide tile whole: columns past the chunk's valid
-        // ones read zero constants, only their stores are predicated off.  With no control flow inside, ptxas overlaps the
-        // pairs' requant chains.  The requant path and the border correction are chosen once per run.
-        const int ccap = nblk * 8 - 2;       // last valid column pair: the correction table's row ends there
+        // Then one straight run over every column group of both rows, the BN-wide tile whole: columns past the chunk's valid
+        // ones read zero constants, only their stores are predicated off (a thread's run of channels is valid or not as a
+        // whole: valid columns come in multiples of 16).  With no control flow inside, ptxas overlaps the requant chains.  The
+        // requant path and the border correction are chosen once per run.
         auto columns = [&](auto small, auto with_corr) {
 #pragma unroll
-            for (int j = 0; j < BN / 8; ++j) {
+            for (int G = 0; G < (BN + 31) / 32; ++G) {
+                constexpr int kFull = 4;
+                const int S = BN - 32 * G >= 32 ? kFull : 2;      // column pairs of the thread per row in this group
+                const int ch = 32 * G + 2 * S * q4;              // its first channel
+                // NHWC16 pad channels (>= OC) stay zero: the clamp would give them minv, which is the output zero point with ReLU
+                const int nv = OC - n0 - ch;
+                const uint32_t mlo = nv >= 4 ? 0xffffffffu : (nv <= 0 ? 0u : (1u << (8 * nv)) - 1u);
+                const uint32_t mhi = nv >= 8 ? 0xffffffffu : (nv <= 4 ? 0u : (1u << (8 * (nv - 4))) - 1u);
+                float2 ws[kFull], bs[kFull];
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {        // rows inside: a column pair's constants serve both rows, then die
-                    const int c = j * 8 + 2 * q4;
-                    int k0 = wsum[c], k1 = wsum[c + 1];
-                    if constexpr (decltype(with_corr)::value) {
-                        const int cc = min(c, ccap);
-                        k0 += __ldg(corrp[h] + cc);
-                        k1 += __ldg(corrp[h] + cc + 1);
+                for (int s = 0; s < S; ++s) {
+                    const int c = 8 * (4 * G + s) + 2 * q4;
+                    ws[s] = *reinterpret_cast<const float2*>(wscale + c);
+                    bs[s] = *reinterpret_cast<const float2*>(bias + c);
+                }
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {        // rows inside: a group's constants serve both rows, then die
+                    int q[2 * kFull];
+#pragma unroll
+                    for (int s = 0; s < S; ++s) {
+                        const int j = 4 * G + s;
+                        int a0 = acc[j * 4 + 2 * h], a1 = acc[j * 4 + 2 * h + 1];
+                        if constexpr (decltype(with_corr)::value) {
+                            const int2 k = __ldg(reinterpret_cast<const int2*>(corrp[h] + 8 * j + 2 * q4));
+                            a0 += k.x;
+                            a1 += k.y;
+                        }
+                        if constexpr (decltype(small)::value) {   // |acc_u| < 2^22: int -> float on the FP32 pipe (exact)
+                            q[2 * s] = requant_fast_small(a0, ws[s].x, scale_x, bs[s].x, minv, maxv);
+                            q[2 * s + 1] = requant_fast_small(a1, ws[s].y, scale_x, bs[s].y, minv, maxv);
+                        } else {
+                            q[2 * s] = requant_fast(a0, ws[s].x, scale_x, bs[s].x, minv, maxv);
+                            q[2 * s + 1] = requant_fast(a1, ws[s].y, scale_x, bs[s].y, minv, maxv);
+                        }
                     }
-                    const int a0 = acc[j * 4 + 2 * h] + k0, a1 = acc[j * 4 + 2 * h + 1] + k1;
-                    int q0, q1;
-                    if constexpr (decltype(small)::value) {   // |acc_u| < 2^22: int -> float on the FP32 pipe (exact)
-                        q0 = requant_fast_small(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
-                        q1 = requant_fast_small(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                    const uint32_t lo = __byte_perm(__byte_perm(q[0], q[1], 0x0040), __byte_perm(q[2], q[3], 0x0040), 0x5410) & mlo;
+                    if (S == kFull) {
+                        const uint32_t hi = __byte_perm(__byte_perm(q[4], q[5], 0x0040), __byte_perm(q[6], q[7], 0x0040), 0x5410) & mhi;
+                        st_global_v2_if(yrow[h] + ch, lo, hi, ch, lim[h]);
                     } else {
-                        q0 = requant_fast(a0, cst[c], scale_x, cst[kMaxBN + c], minv, maxv);
-                        q1 = requant_fast(a1, cst[c + 1], scale_x, cst[kMaxBN + c + 1], minv, maxv);
+                        st_global_b32_if(yrow[h] + ch, lo, ch, lim[h]);
                     }
-                    if (n0 + c >= OC) q0 = 0;         // NHWC16 channel padding stays zero
-                    if (n0 + c + 1 >= OC) q1 = 0;
-                    st_global_u16_if(yrow[h] + c, (uint16_t)((q0 & 0xff) | ((q1 & 0xff) << 8)), j, lim[h]);
                 }
             }
         };
@@ -460,44 +495,51 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
     } else {
         // ================= two consumer warpgroups: wgmma main loop + epilogue =================
         const int ct = threadIdx.x;                  // 0..255
-        float* cst = reinterpret_cast<float*>(smem + kOffConsts);
-        uint32_t cached = 0xffffffffu;            // (layer, n chunk) whose constants are in cst
+        // two slots of epilogue constants: the current (layer, n chunk)'s table row, and the next distinct one in this CTA's
+        // schedule, copied with cp.async while the current item runs
+        const uint32_t slot0 = base + kOffConsts;
+        auto fetch = [&](uint32_t w, int slot) {
+            const GroupLayerParams& lp = sl[w >> kGroupItemLayerShift];
+            const int nc = (int)((w >> kGroupItemChunkShift) & kGroupItemChunkMask);
+            if (ct < 3 * lp.bn / 4)         // 3 x bn words, 16 bytes per thread
+                cp_async16(slot0 + slot * kConstBytes + 16u * ct, lp.ep + (size_t)nc * 3 * lp.bn + 4 * ct, true);
+            cp_async_commit();
+        };
+        uint32_t cached = 0xffffffffu;            // (layer, n chunk) whose constants are in slot cur
+        int cur = 1;
         int stage = 0, phase = 0;
 
-        for (int i = 0;; ++i) {
-            const uint32_t w = my[i];
-            if (w == kGroupSchedEnd) break;
+        uint32_t w = my[0];
+        if (w != kGroupSchedEnd) fetch(w, 0);
+        for (int i = 0; w != kGroupSchedEnd; ++i) {
+            const uint32_t w_next = my[i + 1];    // a row ends with two end markers: my[i + 1] exists
             int L, nc, mt0, cnt;
             decode_item(w, L, nc, mt0, cnt);
             const GroupLayerParams& lp = sl[L];
             const int bn = lp.bn, n0 = nc * bn;
             const int ncols = (lp.N - n0) < bn ? (lp.N - n0) : bn;      // valid (16-padded) columns of this chunk
-            const int nblk = ncols >> 3;
             if ((w >> kGroupItemChunkShift) != cached) {
-                // reload the per-column constants once every consumer is done READING the previous item's, then publish.  The
-                // whole tile width: the epilogue computes every column, zeros past the layer's last channel.
+                // this item's constants were fetched into the other slot during the previous item: once every consumer's copies
+                // have landed (and so every consumer is done reading the old slot), switch
+                cp_async_wait<0>();
                 named_sync(1, kConsumerThreads);
-                for (int j = ct; j < bn; j += kConsumerThreads) {
-                    const int n = n0 + j;
-                    const bool v = n < lp.OC;
-                    cst[j] = v ? lp.wscale[n] : 0.f;
-                    cst[kMaxBN + j] = v ? lp.bias[n] : 0.f;
-                    reinterpret_cast<int*>(cst)[2 * kMaxBN + j] = v ? lp.wsum128[n] : 0;
-                }
-                named_sync(1, kConsumerThreads);
+                cur ^= 1;
                 cached = w >> kGroupItemChunkShift;
             }
+            if (w_next != kGroupSchedEnd && (w_next >> kGroupItemChunkShift) != cached) fetch(w_next, cur ^ 1);
+            const float* cst = reinterpret_cast<const float*>(smem + kOffConsts + cur * kConstBytes);
             switch (lp.bn >> 4) {     // conv_plan: bn is a multiple of 16 <= kGroupMaxBN
-                case 1: consume_item<16>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 2: consume_item<32>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 3: consume_item<48>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 4: consume_item<64>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 5: consume_item<80>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 6: consume_item<96>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 7: consume_item<112>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 8: consume_item<128>(lp, geom + L, n0, nblk, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 1: consume_item<16>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 2: consume_item<32>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 3: consume_item<48>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 4: consume_item<64>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 5: consume_item<80>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 6: consume_item<96>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 7: consume_item<112>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 8: consume_item<128>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
                 default: __trap();
             }
+            w = w_next;
         }
     }
 }

@@ -75,11 +75,19 @@ struct GroupMapsParam {
     CUtensorMap_st_opaque b[kGroupMaxLayers];
     CUtensorMap_st_opaque a1[kGroupMaxLayers];   // odd-column view (stride 2, mode 1)
 };
+// Inside an n chunk of bn columns the kernel's GEMM columns are permuted so that the wgmma fragment gives each thread
+// contiguous output channels: in every 32-column group, GEMM column 32 G + 8 s + 2 q + e computes channel 32 G + 8 q + 2 s + e
+// (a 16-wide last group, bn % 32 == 16: 32 G + 4 q + 2 s + e).  The weight rows, the epilogue table and the border-correction
+// table are laid out in this order.
+inline int group_column_channel(int c, int bn) {
+    const int g = c & ~31, s = (c >> 3) & 3, q = (c >> 1) & 3, e = c & 1;
+    return bn - g >= 32 ? g + 8 * q + 2 * s + e : g + 4 * q + 2 * s + e;
+}
 struct GroupLayerParams {            // copied to shared memory by every CTA
     int8_t* y;
-    const float* wscale;
-    const float* bias;
-    const int32_t* wsum128;
+    // epilogue table [n_chunks][3][bn], GEMM-column order, zero past OC: wscale, biasFloat (float) and the accumulators' start
+    // value preset = 128 sum w (+ 0x4B400000 when K <= 128, for the exact int -> float trick of the small-K requant) (int32)
+    const float* ep;
     int M, N, K, bn;                 // mode 0: M rows, K = Cp.  mode 1: M = N*OH*OW, K = taps*Cp
     int n_chunks, m_tiles, num_kb, OC;
     int ldy;
@@ -94,7 +102,8 @@ struct GroupConvGeom {               // mode 1 only; stays in global memory (rea
     int BH, OHB, pad0_, pad1_;       // a TMA box covers BH consecutive output rows of one image (stride_h == 1), OHB = OH / BH boxes per image
     const uint8_t* hcls;             // [OH] border class of an output row   (nullptr: z_in == 0, no correction)
     const uint8_t* wcls;             // [OW] border class of an output column
-    const int32_t* corr;             // [HC*WC][N] z_in * sum over the out-of-image taps of sum_c w[oc][tap][c]; the interior
+    const int32_t* corr;             // [HC*WC][n_chunks*bn] z_in * sum over the out-of-image taps of sum_c w[oc][tap][c], in
+                                     // GEMM-column order (group_column_channel), zero past OC; the interior
                                      // class's row is zeros (the epilogue adds it for pixels next to a border pixel)
     int wc_count, interior_cls;
 };
