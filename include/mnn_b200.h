@@ -264,6 +264,15 @@ MNNB200_API mnnb200_status mnnb200_memcpy_d2d(mnnb200_runtime* rt, void* dst_dev
 MNNB200_API mnnb200_status mnnb200_linear_w8_create(mnnb200_runtime* rt, int ic, int oc, const int8_t* wq,
                                                     const float* alpha, const float* wzero, const float* bias,
                                                     int relu, int relu6, mnnb200_exec** out);
+/* K-blocked weight scales (MNN-LLM's quant_block export; ConvInt8TiledExecutor.cpp mBlockNum): K is split into `blocks` equal runs
+ * of bs = ic / blocks channels, alpha and wzero are [oc][blocks] (wzero NULL when symmetric).  Each block's int32 accumulator is
+ * finished into an fp32 running sum in block order, the arithmetic of mnn_oracle_linear_w8_dynamic_blocks bit for bit, on the same
+ * GEMM and GEMV kernels; resize / execute / set_variant as above.  blocks < 1 or ic % blocks != 0: INVALID_VALUE; bs % 32 != 0
+ * (a wgmma k-step is 32 bytes), or bs not a power of two up to 512: NOT_SUPPORT.  blocks == 1 is the per-channel layer.  The
+ * CTA-pair variant (3) returns NOT_SUPPORT for blocked layers; auto runs >= 9 tokens on the single-CTA GEMM. */
+MNNB200_API mnnb200_status mnnb200_linear_w8_create_blocked(mnnb200_runtime* rt, int ic, int oc, int blocks, const int8_t* wq,
+                                                            const float* alpha, const float* wzero, const float* bias,
+                                                            int relu, int relu6, mnnb200_exec** out);
 MNNB200_API mnnb200_status mnnb200_linear_w8_resize(mnnb200_exec* e, int tokens);
 MNNB200_API mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* e, const float* x, float* y);
 

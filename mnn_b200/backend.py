@@ -373,10 +373,15 @@ class LinearW8Execution(Execution):
         al = np.ascontiguousarray(op.wscale, np.float32)
         wz = None if op.wzero is None else np.ascontiguousarray(op.wzero, np.float32)
         b = None if op.bias is None else np.ascontiguousarray(op.bias, np.float32)
-        check(_capi.lib().mnnb200_linear_w8_create(backend.runtime._h, op.conv["ic"], op.conv["oc"], _np_ptr(wq),
-                                                   _np_ptr(al), _np_ptr(wz), _np_ptr(b),
-                                                   int(bool(op.conv.get("relu", False))), int(op.relu6),
-                                                   C.byref(self._h)), "linear_w8_create")
+        relu = int(bool(op.conv.get("relu", False)))
+        if al.ndim == 2:        # [oc, blocks]: K-blocked weight scales (quant_block), wzero of the same shape or None
+            check(_capi.lib().mnnb200_linear_w8_create_blocked(backend.runtime._h, op.conv["ic"], op.conv["oc"], al.shape[1],
+                                                               _np_ptr(wq), _np_ptr(al), _np_ptr(wz), _np_ptr(b), relu,
+                                                               int(op.relu6), C.byref(self._h)), "linear_w8_create_blocked")
+        else:
+            check(_capi.lib().mnnb200_linear_w8_create(backend.runtime._h, op.conv["ic"], op.conv["oc"], _np_ptr(wq),
+                                                       _np_ptr(al), _np_ptr(wz), _np_ptr(b), relu, int(op.relu6),
+                                                       C.byref(self._h)), "linear_w8_create")
         self.oc = op.conv["oc"]
 
     def onResize(self, inputs, outputs):

@@ -141,8 +141,8 @@ static mnnb200_status make_tmap_u8(CUtensorMap* m, const void* ptr, int rank, co
 // When the M tiles alone cannot fill the GPU (the 7x7 / 14x14 feature maps of MobileNet: 13 / 49 tiles), N is split
 // further (down to 32 columns) so that m_tiles * n_chunks approaches the SM count: a lone CTA streaming a whole K x (A + B)
 // panel through one SM's L2 port is what bounds those layers, not the math.
-static int pick_bn(int n_padded, int m_tiles = 1 << 30, int sm_count = 1) {
-    int chunks = (n_padded + 255) / 256;
+static int pick_bn(int n_padded, int m_tiles = 1 << 30, int sm_count = 1, int max_bn = 256) {
+    int chunks = (n_padded + max_bn - 1) / max_bn;
     if ((long)m_tiles * chunks < sm_count) {
         int want = sm_count / m_tiles, cap = n_padded / 32;
         if (want > cap) want = cap;
@@ -1110,6 +1110,13 @@ struct LinearW8Exec : mnnb200_exec {
     size_t xq_cap = 0, dq_cap = 0, ss_cap = 0;
     int bn = 0, bn2 = 0;            // bn2 != 0: the CTA-pair kernel is usable for this shape
     CUtensorMap tmap_a, tmap_b, tmap_b_half;
+    // K-blocked weight scales (mnnb200_linear_w8_create_blocked): blocks of bs input channels, bs = 0 per channel
+    int bs = 0, blocks = 1;
+    float *d_balpha = nullptr, *d_bwzero = nullptr;                     // [ocp][blocks]: the GEMV's layout
+    float *d_talpha = nullptr, *d_twzero = nullptr, *d_tws = nullptr;   // [blocks][ocp]: the GEMM's layout, ws_b precomputed
+    int32_t* d_tw128 = nullptr;                                         // [blocks][ocp] 128 * sum_b w
+    float* d_xsb = nullptr;                                             // [tokens][blocks] xsum_b * dq (GEMM path)
+    size_t xsb_cap = 0;
 };
 
 extern "C" {
@@ -1142,6 +1149,48 @@ mnnb200_status mnnb200_linear_w8_create(mnnb200_runtime* rt, int ic, int oc, con
     return MNNB200_OK;
 }
 
+mnnb200_status mnnb200_linear_w8_create_blocked(mnnb200_runtime* rt, int ic, int oc, int blocks, const int8_t* wq,
+                                                const float* alpha, const float* wzero, const float* bias, int relu, int relu6,
+                                                mnnb200_exec** out) {
+    if (!rt || !wq || !alpha || !out || ic <= 0 || oc <= 0 || blocks < 1 || ic % blocks)
+        return fail(MNNB200_INVALID_VALUE, "linear_w8_create_blocked: bad argument (blocks must divide ic)");
+    if (blocks == 1) return mnnb200_linear_w8_create(rt, ic, oc, wq, alpha, wzero, bias, relu, relu6, out);
+    const int bs = ic / blocks;
+    if (bs % 32) return fail(MNNB200_NOT_SUPPORT, "linear_w8_create_blocked: a block must be a multiple of 32 channels (one wgmma k-step)");
+    if (bs > 512 || (bs & (bs - 1)))
+        return fail(MNNB200_NOT_SUPPORT, "linear_w8_create_blocked: the GEMV takes power-of-two blocks of at most 512 channels");
+    auto* e = new LinearW8Exec;
+    e->rt = rt; e->kind = 3; e->ic = ic; e->oc = oc; e->icp = up16(ic); e->ocp = up16(oc); e->relu = relu; e->relu6 = relu6;
+    e->has_zero = wzero != nullptr; e->has_bias = bias != nullptr; e->bs = bs; e->blocks = blocks;
+    const size_t nt = (size_t)e->ocp * blocks;
+    std::vector<int8_t> wp((size_t)e->ocp * e->icp, 0);
+    std::vector<float> bsv(e->ocp, 0.f), ba(nt, 0.f), bz(nt, 0.f), ta(nt, 0.f), tz(nt, 0.f), tws(nt, 0.f);
+    std::vector<int32_t> tw128(nt, 0);
+    for (int o = 0; o < oc; ++o) {
+        for (int k = 0; k < ic; ++k) wp[(size_t)o * e->icp + k] = wq[(size_t)o * ic + k];
+        if (bias) bsv[o] = bias[o];
+        for (int b = 0; b < blocks; ++b) {
+            int32_t isum = 0;
+            for (int k = b * bs; k < (b + 1) * bs; ++k) isum += wq[(size_t)o * ic + k];
+            const size_t ob = (size_t)o * blocks + b, bo = (size_t)b * e->ocp + o;
+            const float a = alpha[ob], z = wzero ? wzero[ob] : 0.0f;
+            ba[ob] = a; bz[ob] = z;
+            ta[bo] = a; tz[bo] = z;
+            tws[bo] = (float)isum * a + (float)bs * z;   // the block's weightKernelSum
+            tw128[bo] = 128 * isum;
+        }
+    }
+    mnnb200_status st;
+    if ((st = e->upload(wp, &e->d_w)) || (st = e->upload(bsv, &e->d_bias)) || (st = e->upload(ba, &e->d_balpha)) ||
+        (st = e->upload(bz, &e->d_bwzero)) || (st = e->upload(ta, &e->d_talpha)) || (st = e->upload(tz, &e->d_twzero)) ||
+        (st = e->upload(tws, &e->d_tws)) || (st = e->upload(tw128, &e->d_tw128))) {
+        delete e;
+        return st;
+    }
+    *out = e;
+    return MNNB200_OK;
+}
+
 mnnb200_status mnnb200_linear_w8_resize(mnnb200_exec* ex, int tokens) {
     if (!ex || ex->kind != 3) return fail(MNNB200_INVALID_VALUE, "linear_w8_resize: not a linear execution");
     auto* e = static_cast<LinearW8Exec*>(ex);
@@ -1152,20 +1201,23 @@ mnnb200_status mnnb200_linear_w8_resize(mnnb200_exec* ex, int tokens) {
             (st = e->grow_scratch((void**)&e->d_dq, &e->dq_cap, (size_t)tokens * sizeof(float))) ||
             (st = e->grow_scratch((void**)&e->d_srcsum, &e->ss_cap, (size_t)tokens * sizeof(float))))
             return st;
+        if (e->bs && (st = e->grow_scratch((void**)&e->d_xsb, &e->xsb_cap, (size_t)tokens * e->blocks * sizeof(float)))) return st;
     }
     e->tokens = tokens;
-    e->bn = pick_bn(e->ocp, (tokens + 127) / 128, e->rt->prop.multiProcessorCount);
+    // blocked: at most 128 columns per tile, the other half of the accumulator registers holds the fp32 block sums
+    e->bn = pick_bn(e->ocp, (tokens + 127) / 128, e->rt->prop.multiProcessorCount, e->bs ? 128 : 256);
     mnnb200_status st;
     if ((st = make_tmap_i8(&e->tmap_a, e->d_xq, tokens, e->icp, 128))) return st;
     if ((st = make_tmap_i8(&e->tmap_b, e->d_w, e->ocp, e->icp, e->bn))) return st;
     // tensor-bound shapes run on CTA pairs (2-CTA cluster, 256 rows): needs >= 256 rows and a B tile that splits into two halves
     e->bn2 = 0;
-    if (tokens >= 256 && e->ocp >= 64) {
+    if (tokens >= 256 && e->ocp >= 64 && !e->bs) {
         int chunks = (e->ocp + 255) / 256;
         e->bn2 = (((e->ocp + chunks - 1) / chunks) + 31) & ~31;
         if ((st = make_tmap_i8(&e->tmap_b_half, e->d_w, e->ocp, e->icp, e->bn2 / 2))) return st;
     }
-    e->cost_bytes = (double)tokens * e->ic * 4 + (double)tokens * e->oc * 4 + (double)e->oc * e->ic;
+    e->cost_bytes = (double)tokens * e->ic * 4 + (double)tokens * e->oc * 4 + (double)e->oc * e->ic +
+                    (e->bs ? (double)e->oc * e->blocks * 8 : 0.0);
     e->cost_macs = (double)tokens * e->oc * e->ic;
     return MNNB200_OK;
 }
@@ -1174,21 +1226,23 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
     if (!ex || ex->kind != 3) return fail(MNNB200_INVALID_VALUE, "linear_w8_execute: not a linear execution");
     auto* e = static_cast<LinearW8Exec*>(ex);
     if (e->tokens <= 0) return fail(MNNB200_NO_EXECUTION, "linear_w8_execute before resize");
+    if (e->bs && e->variant == 3) return fail(MNNB200_NOT_SUPPORT, "the CTA-pair variant takes per-channel weight scales only");
     // decode (<= 8 tokens): weight-streaming GEMV, bit-identical to the tensor-core kernels (variant 4 forces it)
-    if (e->variant == 4 && !linear_w8_gemv_supported(e->tokens, e->icp)) return fail(MNNB200_NOT_SUPPORT, "the GEMV variant takes 1..8 tokens");
+    if (e->variant == 4 && !linear_w8_gemv_supported(e->tokens, e->icp, e->bs)) return fail(MNNB200_NOT_SUPPORT, "the GEMV variant takes 1..8 tokens");
     // ONE token is a different ARITHMETIC in the reference (asymmetric single-quant, input zero folded into the bias: see
     // linear_w8_gemv.cu), which only the GEMV kernel implements: the tensor-core kernels would silently compute the multi-token form
-    if (e->tokens == 1 && (e->variant == 2 || e->variant == 3 || !linear_w8_gemv_supported(1, e->icp)))
+    if (e->tokens == 1 && (e->variant == 2 || e->variant == 3 || !linear_w8_gemv_supported(1, e->icp, e->bs)))
         return fail(MNNB200_NOT_SUPPORT, "a single token runs the reference's decode arithmetic: GEMV kernel only (variant 0 or 4, ic <= 25600)");
-    if (e->variant == 4 || e->tokens == 1 || (e->variant == 0 && linear_w8_gemv_supported(e->tokens, e->icp))) {
+    if (e->variant == 4 || e->tokens == 1 || (e->variant == 0 && linear_w8_gemv_supported(e->tokens, e->icp, e->bs))) {
         GemvW8Params g;
         g.x = x; g.w = e->d_w; g.y = y; g.alpha = e->d_alpha; g.bias = e->has_bias ? e->d_bias : nullptr; g.wsumf = e->d_wsumf;
         g.wzero = e->has_zero ? e->d_wzero : nullptr; g.wsum128 = e->d_wsum128;
         g.tokens = e->tokens; g.ic = e->ic; g.oc = e->oc; g.ocp = e->ocp; g.icp = e->icp; g.ldy = e->oc; g.relu = e->relu; g.relu6 = e->relu6;
+        g.bs = e->bs; g.balpha = e->d_balpha; g.bwzero = e->d_bwzero;
         CK(launch_linear_w8_gemv(g, e->rt->stream, e->rt->prop.multiProcessorCount));
         return MNNB200_OK;
     }
-    CK(launch_dynamic_quant(x, e->tokens, e->ic, e->icp, e->d_xq, e->d_dq, e->d_srcsum, e->rt->stream));
+    CK(launch_dynamic_quant(x, e->tokens, e->ic, e->icp, e->d_xq, e->d_dq, e->d_srcsum, e->rt->stream, e->bs, e->d_xsb));
     if (e->variant == 3 && !e->bn2) return fail(MNNB200_NOT_SUPPORT, "the CTA-pair variant needs >= 256 tokens and >= 64 output channels");
     GemmI8Params g;
     memset(&g, 0, sizeof(g));
@@ -1196,6 +1250,8 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
     g.y_f32 = y; g.ldy = e->oc; g.wscale = e->d_alpha; g.bias = e->has_bias ? e->d_bias : nullptr; g.wsum128 = e->d_wsum128;
     g.OC = e->oc; g.dq = e->d_dq; g.srcsum = e->d_srcsum; g.wsumf = e->d_wsumf; g.wzero = e->has_zero ? e->d_wzero : nullptr;
     g.relu = e->relu; g.relu6 = e->relu6;
+    g.bs = e->bs; g.blocks = e->blocks; g.balpha = e->d_talpha; g.bwzero = e->d_twzero; g.bws = e->d_tws; g.bw128 = e->d_tw128;
+    g.xsb = e->d_xsb;
     if (e->variant == 3 || (e->variant == 0 && e->bn2)) {
         CK(launch_gemm_i8_2cta(g, &e->tmap_a, &e->tmap_b_half, e->bn2, e->rt->stream, e->rt->prop.multiProcessorCount));
         return MNNB200_OK;

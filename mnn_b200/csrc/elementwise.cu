@@ -573,9 +573,24 @@ cudaError_t launch_softmax_int8(const int8_t* x, int rows, int c, int cp, float 
 //       _AVX512_DynamicQuant x86_x64/avx512/PackedFunction.cpp:288-348: x*qscale, round-to-nearest-even)
 //      also emits srcsum[token] = float(sum_k (xq_k + 128)) * dq (MNNSumByAxisLForMatmul_A,
 //      compute/Int8FunctionsOpt.cpp:2584-2650) for the asymmetric-weight term.
+//      bs > 0 (K-blocked weight scales): xsb[token][b] = float(sum_{k in block b} (xq_k + 128)) * dq per block of bs channels,
+//      the block's share of srcsum, summed from the quantised row this CTA has just written (visible after __syncthreads)
+__device__ __forceinline__ void quant_block_sums(const int8_t* qr, int ic, int bs, float dqv, float* xsb) {
+    for (int b = threadIdx.x; b * bs < ic; b += blockDim.x) {
+        const int4* q4 = reinterpret_cast<const int4*>(qr + (size_t)b * bs);
+        int s = 0;
+        for (int i = 0; i < (bs >> 4); ++i) {
+            const int4 v = q4[i];
+            s = __dp4a(v.x, 0x01010101, s); s = __dp4a(v.y, 0x01010101, s);
+            s = __dp4a(v.z, 0x01010101, s); s = __dp4a(v.w, 0x01010101, s);
+        }
+        xsb[b] = __fmul_rn(__int2float_rn(s + 128 * bs), dqv);
+    }
+}
+
 __global__ void __launch_bounds__(256) dynamic_quant_kernel(const float* __restrict__ x, int ic, int icp,
                                                             int8_t* __restrict__ xq, float* __restrict__ dq,
-                                                            float* __restrict__ srcsum) {
+                                                            float* __restrict__ srcsum, int bs, float* __restrict__ xsb) {
     __shared__ float s_max[8];
     __shared__ int s_sum[8];
     const int tkn = blockIdx.x;
@@ -615,6 +630,7 @@ __global__ void __launch_bounds__(256) dynamic_quant_kernel(const float* __restr
         dq[tkn] = dqv;
         srcsum[tkn] = __fmul_rn(__int2float_rn(tot), dqv);
     }
+    if (bs) quant_block_sums(xq + (size_t)tkn * icp, ic, bs, dqv, xsb + (size_t)tkn * (ic / bs));
 }
 
 // Same arithmetic, one pass over HBM: the token's row stays in registers between the abs-max and the quantise step
@@ -622,7 +638,7 @@ __global__ void __launch_bounds__(256) dynamic_quant_kernel(const float* __restr
 template <int NV>
 __global__ void __launch_bounds__(256) dynamic_quant_vec_kernel(const float* __restrict__ x, int ic, int icp,
                                                                 int8_t* __restrict__ xq, float* __restrict__ dq,
-                                                                float* __restrict__ srcsum) {
+                                                                float* __restrict__ srcsum, int bs, float* __restrict__ xsb) {
     __shared__ float s_max[8];
     __shared__ int s_sum[8];
     const int tkn = blockIdx.x;
@@ -675,16 +691,17 @@ __global__ void __launch_bounds__(256) dynamic_quant_vec_kernel(const float* __r
         dq[tkn] = dqv;
         srcsum[tkn] = __fmul_rn(__int2float_rn(tot), dqv);
     }
+    if (bs) quant_block_sums(xq + (size_t)tkn * icp, ic, bs, dqv, xsb + (size_t)tkn * (ic / bs));
 }
 
 cudaError_t launch_dynamic_quant(const float* x, int tokens, int ic, int icp, int8_t* xq, float* dq, float* srcsum,
-                                 cudaStream_t s) {
+                                 cudaStream_t s, int bs, float* xsb) {
     const bool vec = (ic & 3) == 0 && (reinterpret_cast<uintptr_t>(x) & 15) == 0;
-    if (vec && icp <= 1024 * 2) dynamic_quant_vec_kernel<2><<<tokens, 256, 0, s>>>(x, ic, icp, xq, dq, srcsum);
-    else if (vec && icp <= 1024 * 4) dynamic_quant_vec_kernel<4><<<tokens, 256, 0, s>>>(x, ic, icp, xq, dq, srcsum);
-    else if (vec && icp <= 1024 * 8) dynamic_quant_vec_kernel<8><<<tokens, 256, 0, s>>>(x, ic, icp, xq, dq, srcsum);
+    if (vec && icp <= 1024 * 2) dynamic_quant_vec_kernel<2><<<tokens, 256, 0, s>>>(x, ic, icp, xq, dq, srcsum, bs, xsb);
+    else if (vec && icp <= 1024 * 4) dynamic_quant_vec_kernel<4><<<tokens, 256, 0, s>>>(x, ic, icp, xq, dq, srcsum, bs, xsb);
+    else if (vec && icp <= 1024 * 8) dynamic_quant_vec_kernel<8><<<tokens, 256, 0, s>>>(x, ic, icp, xq, dq, srcsum, bs, xsb);
     else
-    dynamic_quant_kernel<<<tokens, 256, 0, s>>>(x, ic, icp, xq, dq, srcsum);
+    dynamic_quant_kernel<<<tokens, 256, 0, s>>>(x, ic, icp, xq, dq, srcsum, bs, xsb);
     ++g_launch_count;
     return cudaGetLastError();
 }

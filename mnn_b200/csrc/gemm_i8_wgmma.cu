@@ -65,6 +65,10 @@ struct KParams {
     const float* wsumf;
     const float* wzero;
     int relu, relu6, has_bias;
+    // K-blocked weight scales (EPI 1, single CTA, bn <= 128): bsteps = 32-byte k-steps per block (0: per channel)
+    int bsteps, blocks;
+    const float *balpha, *bwzero, *bws, *xsb;
+    const int32_t* bw128;
     // batched mode (Winograd: one GEMM per transform position): work item = (batch, m_tile, n_chunk)
     int batch, a_batch_rows, b_batch_rows, c_batch_stride;
     int one_tile;   // grid == number of work items: every CTA owns exactly one (batch, m tile, n chunk)
@@ -150,12 +154,17 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
         const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
         const int q4 = lane & 3;
         float* cst = reinterpret_cast<float*>(smem + pl.off_consts);
+        const bool blocked = EPI == 1 && !PAIR && p.bsteps != 0;   // K-blocked weight scales (finish_block below)
         const int* wsum = reinterpret_cast<const int*>(cst) + 2 * kMaxBN;
         auto load_consts = [&](int n0, int cb) {
             for (int j = ct; j < p.bn; j += kConsumerThreads) {
                 int n = n0 + j;
                 const bool v = n < p.OC;
                 n += cb;
+                if (blocked) {                   // the per-block tables are read from global memory by finish_block
+                    cst[kMaxBN + j] = (v && p.has_bias) ? p.bias[n] : 0.f;
+                    continue;
+                }
                 cst[j] = v ? p.wscale[n] : 0.f;
                 cst[kMaxBN + j] = (v && p.has_bias) ? p.bias[n] : 0.f;
                 reinterpret_cast<int*>(cst)[2 * kMaxBN + j] = v ? p.wsum128[n] : 0;
@@ -183,6 +192,46 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
         int acc[MAXBN / 2];
 #pragma unroll
         for (int i = 0; i < MAXBN / 2; ++i) acc[i] = 0;
+        // K-blocked weight scales: the MMAs use acc[0, bn / 2) (bn <= MAXBN / 2), acc[MAXBN / 4 + i] holds the fp32 running sum
+        // of accumulator i as bits.  Block b's int32 accumulators are finished in the order of mnn_oracle_linear_w8_dynamic_blocks:
+        //   part = float(acc + 128 sum_b w) * alpha_b;  part *= dq;  part += (dq * -128) * ws_b;  part = xsb * wzero_b + part;  f += part
+        auto finish_block = [&](int b, int mt, int n0) {
+            float dqm[2], corr[2], xs[2];
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+                const int m = mt * kBM + r_base + 8 * h;
+                const bool v = m < p.M;
+                dqm[h] = v ? p.dq[m] : 0.f;
+                xs[h] = v ? p.xsb[(size_t)m * p.blocks + b] : 0.f;
+                corr[h] = __fmul_rn(dqm[h], -128.f);
+            }
+            const size_t tb = (size_t)b * p.N;
+#pragma unroll
+            for (int j = 0; j < MAXBN / 16; ++j) {
+                if (j < nblk) {
+                    const int n = n0 + j * 8 + 2 * q4;
+                    float2 al = make_float2(0.f, 0.f), wz = al, ws = al;
+                    int2 w128 = make_int2(0, 0);
+                    if (n < p.N) {
+                        al = __ldg(reinterpret_cast<const float2*>(p.balpha + tb + n));
+                        wz = __ldg(reinterpret_cast<const float2*>(p.bwzero + tb + n));
+                        ws = __ldg(reinterpret_cast<const float2*>(p.bws + tb + n));
+                        w128 = __ldg(reinterpret_cast<const int2*>(p.bw128 + tb + n));
+                    }
+#pragma unroll
+                    for (int h = 0; h < 2; ++h)
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const int i = j * 4 + 2 * h + e;
+                            float part = __fmul_rn(__int2float_rn(acc[i] + (e ? w128.y : w128.x)), e ? al.y : al.x);
+                            part = __fmul_rn(part, dqm[h]);
+                            part = __fadd_rn(part, __fmul_rn(corr[h], e ? ws.y : ws.x));
+                            part = __fadd_rn(__fmul_rn(xs[h], e ? wz.y : wz.x), part);
+                            acc[MAXBN / 4 + i] = __float_as_int(__fadd_rn(__int_as_float(acc[MAXBN / 4 + i]), part));
+                        }
+                }
+            }
+        };
         for (int w = unit; w < work_total; w += units) {
             const int nc = w % p.n_chunks, wq = w / p.n_chunks;
             const int mt = wq % p.m_tiles, bt = wq / p.m_tiles;
@@ -193,6 +242,10 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
                 named_sync(1, kConsumerThreads);
             }
             int prev = -1;
+            if (blocked) {
+#pragma unroll
+                for (int i = MAXBN / 4; i < MAXBN / 2; ++i) acc[i] = 0;   // the fp32 running sums (+0.0f)
+            }
             for (int kb = 0; kb < num_kb; ++kb) {
                 mbar_wait(full_bar(stage), phase);  // TMA bytes have landed
                 const uint32_t a_addr = base + stage * pl.stage_bytes + wg * 64 * kBK;
@@ -201,8 +254,26 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
                 const int nmma = kleft >= kBK ? 4 : (kleft + 31) / 32;
                 fence_acc(acc);
                 wgmma_fence();
-                for (int k = 0; k < nmma; ++k)
-                    wgmma_bn<Kind::S8, MAXBN>(acc, p.bn, gdesc_sw128(a_addr + k * 32), gdesc_sw128(b_addr + k * 32), kBK, (kb | k) != 0);
+                if (blocked) {
+                    // every block's first k-step starts its int32 accumulators from zero; its last one is waited for and the
+                    // block finished into the fp32 sums before the next block's MMAs are issued
+                    for (int k = 0; k < nmma; ++k) {
+                        const int ks = kb * 4 + k;
+                        wgmma_bn<Kind::S8, MAXBN>(acc, p.bn, gdesc_sw128(a_addr + k * 32), gdesc_sw128(b_addr + k * 32), kBK,
+                                                  ks % p.bsteps != 0);
+                        if ((ks + 1) % p.bsteps == 0) {
+                            wgmma_commit();
+                            wgmma_wait<0>();
+                            fence_acc(acc);
+                            finish_block(ks / p.bsteps, mt, n0);
+                            fence_acc(acc);
+                            wgmma_fence();
+                        }
+                    }
+                } else {
+                    for (int k = 0; k < nmma; ++k)
+                        wgmma_bn<Kind::S8, MAXBN>(acc, p.bn, gdesc_sw128(a_addr + k * 32), gdesc_sw128(b_addr + k * 32), kBK, (kb | k) != 0);
+                }
                 wgmma_commit();
                 wgmma_wait<1>();                     // the previous stage's MMAs are done: hand its slot back
                 fence_acc(acc);
@@ -221,7 +292,7 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
                 const int m = mt * tile_rows + (int)rank * kBM + r_base + 8 * h;
                 if (m >= p.M) continue;
                 float dqm = 0.f, ss = 0.f, corr = 0.f;
-                if (EPI == 1) { dqm = p.dq[m]; ss = p.srcsum[m]; corr = __fmul_rn(dqm, -128.f); }
+                if (EPI == 1 && !blocked) { dqm = p.dq[m]; ss = p.srcsum[m]; corr = __fmul_rn(dqm, -128.f); }
                 float* yrow = p.y_f32 + ((size_t)bt * p.a_batch_rows + m) * p.ldy;
                 const bool vec_ok = (p.ldy & 1) == 0;
 #pragma unroll
@@ -233,11 +304,18 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
 #pragma unroll
                             for (int e = 0; e < 2; ++e) {
                                 const int jj = c + e;
-                                float f = __fmul_rn(__int2float_rn(acc[j * 4 + 2 * h + e] + wsum[jj]), cst[jj]);
+                                float f;
+                                if (blocked) {
+                                    f = __int_as_float(acc[(MAXBN / 4 + j * 4 + 2 * h + e) & (MAXBN / 2 - 1)]);
+                                } else {
+                                    f = __fmul_rn(__int2float_rn(acc[j * 4 + 2 * h + e] + wsum[jj]), cst[jj]);
+                                    if (EPI == 1) {
+                                        f = __fmul_rn(f, dqm);
+                                        f = __fadd_rn(f, __fmul_rn(corr, cst[3 * kMaxBN + jj]));
+                                        f = __fadd_rn(__fmul_rn(ss, cst[4 * kMaxBN + jj]), f);
+                                    }
+                                }
                                 if (EPI == 1) {
-                                    f = __fmul_rn(f, dqm);
-                                    f = __fadd_rn(f, __fmul_rn(corr, cst[3 * kMaxBN + jj]));
-                                    f = __fadd_rn(__fmul_rn(ss, cst[4 * kMaxBN + jj]), f);
                                     if (p.has_bias) f = __fadd_rn(f, cst[kMaxBN + jj]);
                                     if (p.relu | p.relu6) { f = fminf(f, p.relu6 ? 6.0f : 3.4028234663852886e38f); f = fmaxf(f, 0.f); }
                                 } else {
@@ -296,6 +374,8 @@ KParams make_params(const GemmI8Params& g, int bn) {
     p.wscale = g.wscale; p.bias = g.bias; p.wsum128 = g.wsum128; p.OC = g.OC; p.ldy = g.ldy;
     p.y_f32 = g.y_f32; p.dq = g.dq; p.srcsum = g.srcsum; p.wsumf = g.wsumf; p.wzero = g.wzero;
     p.relu = g.relu; p.relu6 = g.relu6; p.has_bias = g.bias != nullptr;
+    p.bsteps = g.bs / 32; p.blocks = g.blocks;
+    p.balpha = g.balpha; p.bwzero = g.bwzero; p.bws = g.bws; p.xsb = g.xsb; p.bw128 = g.bw128;
     p.batch = g.batch > 0 ? g.batch : 1;
     p.a_batch_rows = g.a_batch_rows; p.b_batch_rows = g.b_batch_rows; p.c_batch_stride = g.c_batch_stride;
     p.one_tile = 0;
@@ -307,6 +387,7 @@ KParams make_params(const GemmI8Params& g, int bn) {
 cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& g, const void* tmap_a, const void* tmap_b, int bn, cudaStream_t stream,
                                  int sm_count) {
     if (bn < 16 || bn > kMaxBN || (bn & 15) || g.y_f32 == nullptr) return cudaErrorInvalidValue;
+    if (g.bs && (g.wino || bn > kMaxBN / 2 || g.bs % 32 || g.K % g.bs || g.blocks != g.K / g.bs)) return cudaErrorInvalidValue;
     KParams p = make_params(g, bn);
     const int num_kb = (g.K + kBK - 1) / kBK;
     const int work = p.batch * p.m_tiles * p.n_chunks;
@@ -322,7 +403,7 @@ cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& g, const void* tmap_a, cons
 
 cudaError_t launch_gemm_i8_2cta(const GemmI8Params& g, const void* tmap_a, const void* tmap_b_half, int bn, cudaStream_t stream,
                                 int sm_count) {
-    if (bn < 32 || bn > kMaxBN || (bn & 31) || g.y_f32 == nullptr || g.wino) return cudaErrorInvalidValue;
+    if (bn < 32 || bn > kMaxBN || (bn & 31) || g.y_f32 == nullptr || g.wino || g.bs) return cudaErrorInvalidValue;
     KParams p = make_params(g, bn);
     p.batch = 1;
     p.m_tiles = (g.M + 2 * kBM - 1) / (2 * kBM);

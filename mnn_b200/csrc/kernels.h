@@ -50,6 +50,13 @@ struct GemmI8Params {
     const float* wsumf;   // [N] weightKernelSum
     const float* wzero;   // [N] or nullptr
     int relu, relu6;
+    // K-blocked weight scales (bs = 0: per channel, the fields above): K runs in blocks of bs bytes (bs % 32 == 0, bn <= 128),
+    // each block's int32 accumulator is finished into an fp32 running sum (mnn_oracle_linear_w8_dynamic_blocks):
+    //   f += float(acc_b + bw128[b][n]) * balpha[b][n] * dq[m] + (dq[m] * -128) * bws[b][n] + xsb[m][b] * bwzero[b][n]
+    // then + bias[n].  Tables [blocks][N], zero past OC; xsb = float(sum_{k in b} (xq + 128)) * dq.
+    int bs, blocks;
+    const float *balpha, *bwzero, *bws, *xsb;
+    const int32_t* bw128;
     // batched mode (int8 Winograd: one GEMM per transform position a).  A = [batch][a_batch_rows][K],
     // B = [batch][b_batch_rows][K], per-column constants [batch][c_batch_stride], fp32 out [batch][a_batch_rows][ldy]:
     //   y = float(acc + wsum128[a][n]) * wscale[a][n] + bias[a][n]        (wino = 1)
@@ -262,12 +269,18 @@ struct GemvW8Params {
     const float *alpha, *bias, *wsumf, *wzero;   // bias / wzero may be null
     const int32_t* wsum128;
     int tokens, ic, oc, ocp, icp, ldy, relu, relu6;
+    // K-blocked weight scales (bs = 0: per channel): blocks of bs bytes, bs a power of two in [32, 512]; balpha / bwzero
+    // [ocp][ic / bs] (bwzero zeros when symmetric).  The per-block weight sums are taken from the streamed weights, and
+    // alpha / wsumf / wzero / wsum128 are not read.
+    int bs;
+    const float *balpha, *bwzero;
 };
-bool linear_w8_gemv_supported(int tokens, int icp);
+bool linear_w8_gemv_supported(int tokens, int icp, int bs = 0);
 cudaError_t launch_linear_w8_gemv(const GemvW8Params& p, cudaStream_t s, int sm_count);
 
-// dynamic per-token quantisation (MNNAbsMax + MNNQuantScale + MNNDynamicQuant fused)
+// dynamic per-token quantisation (MNNAbsMax + MNNQuantScale + MNNDynamicQuant fused); bs > 0 also writes
+// xsb[token][b] = float(sum_{k in block b} (xq_k + 128)) * dq for the blocks of bs channels (ic % bs == 0, bs % 16 == 0)
 cudaError_t launch_dynamic_quant(const float* x, int tokens, int ic, int icp, int8_t* xq, float* dq, float* srcsum,
-                                 cudaStream_t s);
+                                 cudaStream_t s, int bs = 0, float* xsb = nullptr);
 
 }  // namespace mnnb200

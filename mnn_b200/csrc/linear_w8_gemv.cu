@@ -8,6 +8,8 @@
 //   * every warp streams R weight rows with 16-byte non-allocating loads (each weight byte is read exactly once: HBM-bound),
 //     dp4a into int32, butterfly reduce, then the SAME fp32 epilogue as gemm_i8_wgmma's EPI 1 -- int32 sums are
 //     order-independent, so the result is bit-identical to the tensor-core path;
+//   * K-blocked weight scales (p.bs != 0, MNN-LLM's quant_block export) take a run-time branch of the same kernel: exact int32
+//     sums per block, finished in block order as gemm_i8_wgmma's blocked EPI 1 does, so again bit-identical to it;
 //   * programmatic dependent launch: the first weight chunk is requested before griddepcontrol.wait, so the next layer's blocks
 //     are resident and loading while this layer drains (a decode step is ~120 dependent launches of 2-10 us each).
 #include "common.cuh"
@@ -16,8 +18,10 @@
 namespace mnnb200 {
 namespace {
 
+// two blocks per SM: at most 128 registers, which the per-channel path fits in on its own; the blocked path's extra values
+// would otherwise lift <2, 4, 4> past it and halve its occupancy
 template <int T, int R, int U>
-__global__ void __launch_bounds__(256) linear_w8_gemv_kernel(GemvW8Params p) {
+__global__ void __launch_bounds__(256, 2) linear_w8_gemv_kernel(GemvW8Params p) {
     extern __shared__ __align__(16) uint8_t smem_x[];      // [T][icp] int8
     __shared__ float s_max[8];
     __shared__ int s_sum[8];
@@ -46,7 +50,7 @@ __global__ void __launch_bounds__(256) linear_w8_gemv_kernel(GemvW8Params p) {
     int c_wsum128 = 0;
     {
         const int n = n0 + lane % R;
-        if (lane < T * R && n < p.oc) {
+        if (lane < T * R && n < p.oc && !p.bs) {
             c_alpha = __ldg(p.alpha + n); c_wsumf = __ldg(p.wsumf + n); c_wsum128 = __ldg(p.wsum128 + n);
             if (p.wzero) c_wzero = __ldg(p.wzero + n);
             if (p.bias) c_bias = __ldg(p.bias + n);
@@ -216,6 +220,117 @@ __global__ void __launch_bounds__(256) linear_w8_gemv_kernel(GemvW8Params p) {
     __syncthreads();
 
     bool first = true;
+    if (p.bs) {
+        // ---- K-blocked weight scales (mnn_oracle_linear_w8_dynamic_blocks): every output sums, block after block, the fp32
+        //      finish of its exact int32 block accumulator.  The quantisation above is unchanged; the per-block input sums
+        //      xsum_b * scale come from the quantised rows in shared memory.  In a 512-byte window of K the G = bs / 16 lanes of a
+        //      block reduce its int32 sums with a butterfly, the group's first lane finishes the block (sum_b w is dp4a'd from the
+        //      streamed weights, not stored) into shared memory, and the lane owning the output adds the parts in block order.
+        const int bs = p.bs, G = bs >> 4, nb = ic / bs;
+        float* s_xs = reinterpret_cast<float*>(smem_x + T * icp);                 // [T][nb]
+        float* s_part = s_xs + T * nb + warp * (T * R + R) * 16;                 // [T * R][16] parts, then [R][16] ws_b
+        float* s_wsb = s_part + T * R * 16;
+        for (int i = threadIdx.x; i < T * nb; i += blockDim.x) {
+            const int t = i / nb, b = i - t * nb;
+            float v = 0.f;
+            if (t < p.tokens) {
+                const int4* q4 = reinterpret_cast<const int4*>(smem_x + t * icp + b * bs);
+                int sum = 0;
+                for (int j = 0; j < (bs >> 4); ++j) {
+                    const int4 q = q4[j];
+                    sum = __dp4a(q.x, 0x01010101, sum); sum = __dp4a(q.y, 0x01010101, sum);
+                    sum = __dp4a(q.z, 0x01010101, sum); sum = __dp4a(q.w, 0x01010101, sum);
+                }
+                v = __fmul_rn(__int2float_rn(sum + 128 * bs), s_dq[t]);
+            }
+            s_xs[i] = v;
+        }
+        __syncthreads();
+        for (; n0 < p.oc; n0 += gridDim.x * warps * R) {
+            if (!first) {
+#pragma unroll
+                for (int r = 0; r < R; ++r) wrow[r] = p.w + (size_t)min(n0 + r, p.ocp - 1) * icp;
+            }
+            float f = 0.f, wtot = 0.f;
+            for (int kbase = 0; kbase < icp; kbase += 512 * U) {
+                if (!(first && kbase == 0)) {
+#pragma unroll
+                    for (int r = 0; r < R; ++r)
+#pragma unroll
+                        for (int u = 0; u < U; ++u) {
+                            const int k = kbase + lane * 16 + u * 512;
+                            wv[r][u] = k < icp ? ld_nc_16(wrow[r] + k) : make_int4(0, 0, 0, 0);
+                        }
+                }
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    const int kw = kbase + u * 512, k = kw + lane * 16;
+                    if (kw >= icp) break;
+                    // one weight row at a time: its T block sums and sum_b w are the only new values live next to the weights
+#pragma unroll
+                    for (int r = 0; r < R; ++r) {
+                        const int4 w = wv[r][u];
+                        int sw = __dp4a(w.x, 0x01010101, 0);
+                        sw = __dp4a(w.y, 0x01010101, sw);
+                        sw = __dp4a(w.z, 0x01010101, sw);
+                        sw = __dp4a(w.w, 0x01010101, sw);
+                        int a[T];
+#pragma unroll
+                        for (int t = 0; t < T; ++t) {
+                            const int4 xv = k < icp ? *reinterpret_cast<const int4*>(smem_x + t * icp + k) : make_int4(0, 0, 0, 0);
+                            int v = __dp4a(xv.x, w.x, 0);
+                            v = __dp4a(xv.y, w.y, v);
+                            v = __dp4a(xv.z, w.z, v);
+                            a[t] = __dp4a(xv.w, w.w, v);
+                        }
+                        for (int o = 1; o < G; o <<= 1) {
+                            sw += __shfl_xor_sync(0xffffffffu, sw, o);
+#pragma unroll
+                            for (int t = 0; t < T; ++t) a[t] += __shfl_xor_sync(0xffffffffu, a[t], o);
+                        }
+                        if ((lane & (G - 1)) == 0 && k < icp) {
+                            const int g = lane / G, b = k / bs;
+                            const size_t ci = (size_t)min(n0 + r, p.ocp - 1) * nb + b;   // alpha_b / wzero_b (zero past oc)
+                            const float c_al = __ldg(p.balpha + ci), c_wz = __ldg(p.bwzero + ci);
+                            // ws_b = float(sum_b w) * alpha_b + bs * wzero_b;  the block's accumulator includes the +128 offset
+                            const float ws = __fadd_rn(__fmul_rn(__int2float_rn(sw), c_al), __fmul_rn((float)bs, c_wz));
+                            s_wsb[r * 16 + g] = ws;
+#pragma unroll
+                            for (int t = 0; t < T; ++t) {
+                                const float sc = s_dq[t];
+                                float part = __fmul_rn(__int2float_rn(a[t] + 128 * sw), c_al);
+                                part = __fmul_rn(part, sc);
+                                part = __fadd_rn(part, __fmul_rn(__fmul_rn(sc, -128.f), ws));
+                                part = __fadd_rn(__fmul_rn(s_xs[t * nb + b], c_wz), part);
+                                s_part[(t * R + r) * 16 + g] = part;
+                            }
+                        }
+                    }
+                    __syncwarp();
+                    if (lane < T * R) {
+                        const int nbw = min(32 / G, nb - kw / bs);     // blocks in this window, in order
+                        for (int g = 0; g < nbw; ++g) {
+                            f = __fadd_rn(f, s_part[lane * 16 + g]);
+                            wtot = __fadd_rn(wtot, s_wsb[(lane % R) * 16 + g]);
+                        }
+                    }
+                    __syncwarp();
+                }
+            }
+            first = false;
+            if (lane < T * R) {
+                const int n = n0 + lane % R, m = lane / R;
+                if (n < p.oc && m < p.tokens) {
+                    const float bias = p.bias ? __ldg(p.bias + n) : 0.f;
+                    if (p.tokens == 1) f = __fadd_rn(f, __fadd_rn(bias, __fmul_rn(wtot, s_izf)));   // bias' = bias + sum_b ws_b * izf
+                    else if (p.bias) f = __fadd_rn(f, bias);
+                    if (p.relu | p.relu6) { f = fminf(f, p.relu6 ? 6.0f : 3.4028234663852886e38f); f = fmaxf(f, 0.f); }
+                    p.y[(size_t)m * p.ldy + n] = f;
+                }
+            }
+        }
+        return;
+    }
     for (; n0 < p.oc; n0 += gridDim.x * warps * R) {
         int acc[T][R];
 #pragma unroll
@@ -294,7 +409,8 @@ __global__ void __launch_bounds__(256) linear_w8_gemv_kernel(GemvW8Params p) {
 
 template <int T, int R, int U>
 cudaError_t launch_t(const GemvW8Params& p, cudaStream_t stream, int sms) {
-    const size_t smem = (size_t)T * p.icp;
+    // blocked: + the per-block input sums [T][ic / bs] and each warp's block parts
+    const size_t smem = (size_t)T * p.icp + (p.bs ? ((size_t)T * (p.ic / p.bs) + 8 * (T * R + R) * 16) * sizeof(float) : 0);
     if (smem > 40 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(linear_w8_gemv_kernel<T, R, U>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
@@ -330,7 +446,11 @@ cudaError_t launch_r(const GemvW8Params& p, cudaStream_t stream, int sms) {
 
 }  // namespace
 
-bool linear_w8_gemv_supported(int tokens, int icp) { return tokens >= 1 && tokens <= 8 && (size_t)8 * icp <= 200 * 1024; }
+// blocked (bs > 0): the shared memory also holds the per-block input sums and every warp's block parts (launch_t)
+bool linear_w8_gemv_supported(int tokens, int icp, int bs) {
+    const size_t extra = bs ? ((size_t)8 * (icp / bs) + 8 * 18 * 16) * sizeof(float) : 0;
+    return tokens >= 1 && tokens <= 8 && (size_t)8 * icp + extra <= 200 * 1024;
+}
 
 cudaError_t launch_linear_w8_gemv(const GemvW8Params& p, cudaStream_t stream, int sms) {
     if (p.tokens <= 1) return launch_r<1>(p, stream, sms);

@@ -599,22 +599,26 @@ public:
         if (ic <= 0 || q->weight.size() != (size_t)oc * ic) return nullptr;
         const float* al = q->getAlphaFloat();
         const int per = q->asymmetric ? 2 : 1;
-        if (q->alphaSize != per * oc) return nullptr;             // block-wise quantisation: not on this path yet
-        std::vector<float> alpha(oc), wzero(oc, 0.f), bias(oc, 0.f);
-        for (int o = 0; o < oc; ++o) {
+        // per-channel scales, or K-blocked ones (quant_block): [oc][blocks], blocks = alphaSize / (per * oc)
+        if (q->alphaSize <= 0 || q->alphaSize % (per * oc) != 0) return nullptr;
+        const int blocks = q->alphaSize / (per * oc);
+        const size_t n = (size_t)oc * blocks;
+        std::vector<float> alpha(n), wzero(n, 0.f), bias(oc, 0.f);
+        for (size_t i = 0; i < n; ++i) {
             if (q->asymmetric) {   // {offset, scale}: load() has already turned the wire "min" into the offset of SIGNED int8
                                    // weights, min - clampMin * scale (ConvolutionCommon.cpp:757-766), so w = q * scale + offset
-                alpha[o] = al[2 * o + 1];
-                wzero[o] = al[2 * o];
+                alpha[i] = al[2 * i + 1];
+                wzero[i] = al[2 * i];
             } else {
-                alpha[o] = al[o];
+                alpha[i] = al[i];
             }
         }
         const bool hasBias = conv->bias() && (int)conv->bias()->size() == oc;
         if (hasBias) ::memcpy(bias.data(), conv->bias()->data(), sizeof(float) * oc);
         std::shared_ptr<Resource> res(new Resource);
-        if (mnnb200_linear_w8_create(bn->handle(), ic, oc, q->weight.get(), alpha.data(), q->asymmetric ? wzero.data() : nullptr,
-                                     hasBias ? bias.data() : nullptr, cm->relu() ? 1 : 0, cm->relu6() ? 1 : 0, &res->h) != MNNB200_OK) {
+        if (mnnb200_linear_w8_create_blocked(bn->handle(), ic, oc, blocks, q->weight.get(), alpha.data(),
+                                             q->asymmetric ? wzero.data() : nullptr, hasBias ? bias.data() : nullptr,
+                                             cm->relu() ? 1 : 0, cm->relu6() ? 1 : 0, &res->h) != MNNB200_OK) {
             MNN_ERROR("mnn_b200 linear create: %s\n", mnnb200_last_error());
             return nullptr;
         }
