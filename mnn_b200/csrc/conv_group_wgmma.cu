@@ -21,10 +21,10 @@
 // for layers whose K blocks all fit): with round-robin scheduling all CTAs work on the same layer at the same time, and
 // re-fetching the same few weight lines for every item from every SM serialises in L2.
 //
-//   warp 8:    TMA producer (cp.async.bulk.tensor.2d/4d, 128B / 64B swizzle or 16-byte interleaved chunks, 6-stage ring of
+//   warps 8-11: producer warpgroup (setmaxnreg.dec); one thread issues the TMA loads (cp.async.bulk.tensor.2d/4d, 128B / 64B swizzle or 16-byte interleaved chunks, 6-stage ring of
 //              16 KB activation tiles)
 //   warps 0-7: two consumer warpgroups, 64 rows of the 128-row tile each: wgmma.mma_async m64nNk32 s8 (N = bn <= 128,
-//              accumulators in registers; the per-item work is instantiated per bn, see consume_item) -> CPU-exact requant
+//              accumulators in registers; the per-run work is instantiated per bn, see consume_run) -> CPU-exact requant
 //              -> 8-byte stores straight to the NHWC16 output rows; per-column constants staged in shared memory per
 //              (layer, n chunk), the next one copied in with cp.async while the current item runs
 #include <cuda.h>
@@ -62,6 +62,14 @@ constexpr int kOffBars = kOffBSlot + 32;                                        
 constexpr int kSmemTotal = kOffBars + 256;
 static_assert(kSmemTotal + 1024 <= 227 * 1024, "conv group kernel: shared memory plan does not fit");
 static_assert(sizeof(GroupLayerParams) % 16 == 0, "layer params are copied with 16-byte loads");
+// Two consumer warpgroups and a producer WARPGROUP (warps 8-11, one thread of warp 8 issues the TMA loads).  With nine warps
+// ptxas caps a thread at 168 registers (three warps share one of the SM's four 64 KB register files), too few for two
+// accumulator sets; with whole warpgroups setmaxnreg moves the producer's registers to the consumers: per register file one
+// producer warp at 88 and two consumer warps at 208, 504 x 32 <= 16 K registers.  (The TMA thread's bookkeeping spills below
+// 88; two bn-96 sets and the epilogue fit 208.)
+constexpr int kCgThreads = kConsumerThreads + 128;
+constexpr int kProducerRegs = 88, kConsumerRegs = 208;
+static_assert(kProducerRegs + 2 * kConsumerRegs <= 512, "conv group kernel: register split does not fit");
 
 // requant_cpu_exact (common.cuh) with the +-0.5 select done as copysign(0.5, f): one LOP3, identical result
 __device__ __forceinline__ int requant_fast(int acc_u, float wscale, float scale_x, float bias_float, float minv, float maxv) {
@@ -106,13 +114,42 @@ __device__ __forceinline__ void st_global_b32_if(int8_t* p, uint32_t v, int j, i
     asm volatile("{\n .reg .pred q;\n setp.lt.s32 q, %2, %3;\n @q st.global.b32 [%0], %1;\n}\n" ::"l"(p), "r"(v), "r"(j), "r"(lim));
 }
 
-// One work item on one consumer warpgroup: rows [64 wg, 64 wg + 64) of `cnt` M tiles x BN columns.  BN is a compile-time
-// constant so the accumulator array, the wgmma_span chain and the epilogue's column loop are fixed: a run-time switch on the
-// tile width between two wgmma instructions would make ptxas serialise every one of them.
+// Has the phase of parity `parity` of barrier `bar` completed, in EVERY thread of this consumer warpgroup?  test_wait does not
+// block; the AND over the warpgroup's 128 threads (named barrier 2 + wg) makes the answer the same in every warp, as the wgmmas
+// it decides about need.  A completed phase stays completed until this warpgroup releases the stage, so a 'no' from one warp
+// only means the stage is taken through the blocking wait later.  The barrier id is a register, so ptxas reserves all 16
+// named barriers (harmless at one CTA per SM): immediate ids behind a branch or a predicate on wg make it serialise the wgmmas.
+__device__ __forceinline__ bool stage_landed(uint32_t bar, uint32_t parity, int wg) {
+    uint32_t all;
+    asm volatile(
+        "{\n"
+        ".reg .pred p, q;\n"
+        "mbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n"
+        "bar.red.and.pred q, %3, 128, p;\n"
+        "selp.u32 %0, 1, 0, q;\n"
+        "}\n"
+        : "=r"(all)
+        : "r"(bar), "r"(parity), "r"(2 + wg)
+        : "memory");
+    return all != 0;
+}
+
+// Widths up to this one keep a second accumulator set: the next tile's first K block is issued into it before the current
+// tile's epilogue, so the tensor core works while the epilogue runs.  Two sets of a wider tile do not fit the registers; such
+// layers have few tiles per CTA, so there is little to overlap.
+constexpr int kOverlapMaxBN = 64;
+
+// One RUN on one consumer warpgroup: the consecutive items my[i], my[i + 1], ... of the CTA's schedule row with the same
+// (layer, n chunk), each `cnt` M tiles of rows [64 wg, 64 wg + 64) x BN columns; on return i is the run's last item.  BN is a
+// compile-time constant so the accumulator arrays, the wgmma_span chain and the epilogue's column loop are fixed: a run-time
+// switch on the tile width between two wgmma instructions would make ptxas serialise every one of them.
 // cst = the (layer, n chunk)'s row of the epilogue table, [3][BN] in GEMM-column order: wscale, biasFloat, preset.
-template <int BN>
-__device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const GroupConvGeom* __restrict__ gp, int n0, int ncols, int mt0,
-                                             int cnt, uint32_t base, const uint8_t* smem, const float* cst, int& stage, int& phase) {
+// fetch_next(w) is called once, with the item that follows the run, when the run's last item starts.
+template <int BN, class FetchNext>
+__device__ __forceinline__ void consume_run(const GroupLayerParams& lp, const GroupConvGeom* __restrict__ gp, int n0, int ncols,
+                                            const uint32_t* __restrict__ my, int& i, uint32_t base, const uint8_t* smem,
+                                            const float* cst, int& stage, int& phase, FetchNext fetch_next) {
+    constexpr bool kTwoSets = BN <= kOverlapMaxBN;
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int wg = threadIdx.x >> 7;
     const int r_base = wg * 64 + (warp & 3) * 16 + (lane >> 2);
@@ -126,56 +163,112 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
     const int* preset = reinterpret_cast<const int*>(cst) + 2 * BN;
     const uint32_t bar0 = base + kOffBars;
     int acc[BN / 2];
+    // the next tile's first K block while acc's epilogue runs.  Only wgmmas write it: a register write to an accumulator
+    // while a wgmma pipeline is open makes ptxas serialise every wgmma of the kernel
+    int nxt[kTwoSets ? BN / 2 : 1];
     const float scale_x = lp.scale_x, minv = lp.minv, maxv = lp.maxv;
-    const bool small_acc = lp.K <= 128;    // |sum (x + 128) w| <= 128 * 255 * 128 < 2^22
+    // |sum (x + 128) w| <= 128 * 255 * 128 < 2^22.  Broadcast like cb: the epilogue branches on it and on mode while the next
+    // tile's wgmmas run, and a branch ptxas cannot prove uniform there makes it serialise the wgmmas
+    const bool small_acc = __shfl_sync(0xffffffffu, lp.K, 0) <= 128;
     // the layer fields the epilogue uses, held in registers instead of read from lp (shared memory) for every row and column
-    const int OC = lp.OC, M = lp.M, ldy = lp.ldy, mode = lp.mode;
+    const int OC = lp.OC, M = lp.M, ldy = lp.ldy, mode = __shfl_sync(0xffffffffu, lp.mode, 0);
     int8_t* const y = lp.y;
-    for (int t = 0; t < cnt; ++t) {
-        const int mt = mt0 + t;
-        // the accumulators start at their column's preset (128 sum w, + 0x4B400000 for requant_fast_small), so every wgmma
-        // accumulates and the epilogue adds no per-column integer
+
+    // the accumulators start at their column's preset (128 sum w, + 0x4B400000 for requant_fast_small), so every wgmma
+    // accumulates and the epilogue adds no per-column integer
+    auto init = [&](int (&a)[BN / 2]) {
 #pragma unroll
         for (int j = 0; j < BN / 8; ++j) {
             const int2 v = *reinterpret_cast<const int2*>(preset + 8 * j + 2 * q4);
-            acc[4 * j] = v.x; acc[4 * j + 1] = v.y; acc[4 * j + 2] = v.x; acc[4 * j + 3] = v.y;
+            a[4 * j] = v.x; a[4 * j + 1] = v.y; a[4 * j + 2] = v.x; a[4 * j + 3] = v.y;
         }
-        int prev = -1;
-        for (int kb = 0; kb < num_kb; ++kb) {
+    };
+    // the wgmmas of the K block in the current stage into a (after wgmma_fence, before the commit); scale0 = 0: the first
+    // k-step overwrites a instead of accumulating
+    auto mma_block = [&](int (&a)[BN / 2], int scale0) {
+        const uint32_t a_addr = base + stage * kStageBytes;
+        const uint32_t b_addr = base + kOffB + (uint32_t)(*reinterpret_cast<const volatile int*>(smem + kOffBSlot + 4 * stage));
+        // every K block runs its full count of k-steps in one straight run: a condition per k-step would make ptxas
+        // serialise the wgmmas.  Past the end of a layer's K the weight tile holds zeros from the TMA unit (out-of-bounds
+        // fill), so those k-steps add nothing.
+        if (cb == 128) {
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                wgmma_span<Kind::S8, BN, 0>(a, gdesc_sw128(a_addr + wg * 64 * 128 + k * 32), gdesc_sw128(b_addr + k * 32), 128, k ? 1 : scale0);
+        } else if (cb == 64) {
+#pragma unroll
+            for (int k = 0; k < 2; ++k)
+                wgmma_span<Kind::S8, BN, 0>(a, gdesc(a_addr + wg * 64 * 64 + k * 32, kSw64, 16, 512),
+                                            gdesc(b_addr + k * 32, kSw64, 16, 512), 64, k ? 1 : scale0);
+        } else {
+#pragma unroll
+            for (int u = 0; u < 4; ++u)
+                wgmma_span<Kind::S8, BN, 0>(a, gdesc(a_addr + 2 * u * (kBM * 16) + wg * 64 * 16, kSwNone, kBM * 16, 128),
+                                            gdesc(b_addr + 2 * u * (BN * 16), kSwNone, BN * 16, 128), 16,
+                                            u ? 1 : scale0);
+        }
+    };
+    // prev = the stage whose MMAs were issued last and which is not released yet (-1: none)
+    int prev = -1;
+    auto release_prev = [&]() {
+        if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar0 + 8u * (kStages + prev)); }
+    };
+    auto next_stage = [&]() {
+        prev = stage;
+        if (++stage == kStages) { stage = 0; phase ^= 1; }
+    };
+
+    // the run's tiles: M tile mt of item my[i], `left` tiles of the item from mt on; last_item = my[i + 1] is not in the run
+    // (a row ends with two end markers: my[i + 1] exists)
+    const uint32_t key = my[i] >> kGroupItemChunkShift;
+    int mt, left;
+    bool last_item;
+    auto start_item = [&]() {
+        int L, nc;
+        decode_item(my[i], L, nc, mt, left);
+        const uint32_t wn = my[i + 1];
+        last_item = wn == kGroupSchedEnd || (wn >> kGroupItemChunkShift) != key;
+        if (last_item && wn != kGroupSchedEnd) fetch_next(wn);
+    };
+    start_item();
+    init(acc);
+    bool ahead = false;                      // the tile's first K block was issued (into acc) before the previous epilogue
+    for (;;) {
+        for (int kb = ahead ? 1 : 0; kb < num_kb; ++kb) {
             mbar_wait(bar0 + 8u * stage, phase);
-            const uint32_t a_addr = base + stage * kStageBytes;
-            const uint32_t b_addr = base + kOffB + (uint32_t)(*reinterpret_cast<const volatile int*>(smem + kOffBSlot + 4 * stage));
             fence_acc(acc);
             wgmma_fence();
-            // every K block runs its full count of k-steps in one straight run: a condition per k-step would make ptxas
-            // serialise the wgmmas.  Past the end of a layer's K the weight tile holds zeros from the TMA unit (out-of-bounds
-            // fill), so those k-steps add nothing.
-            if (cb == 128) {
-#pragma unroll
-                for (int k = 0; k < 4; ++k)
-                    wgmma_span<Kind::S8, BN, 0>(acc, gdesc_sw128(a_addr + wg * 64 * 128 + k * 32), gdesc_sw128(b_addr + k * 32), 128, 1);
-            } else if (cb == 64) {
-#pragma unroll
-                for (int k = 0; k < 2; ++k)
-                    wgmma_span<Kind::S8, BN, 0>(acc, gdesc(a_addr + wg * 64 * 64 + k * 32, kSw64, 16, 512),
-                                                gdesc(b_addr + k * 32, kSw64, 16, 512), 64, 1);
-            } else {
-#pragma unroll
-                for (int u = 0; u < 4; ++u)
-                    wgmma_span<Kind::S8, BN, 0>(acc, gdesc(a_addr + 2 * u * (kBM * 16) + wg * 64 * 16, kSwNone, kBM * 16, 128),
-                                                gdesc(b_addr + 2 * u * (BN * 16), kSwNone, BN * 16, 128), 16, 1);
-            }
+            mma_block(acc, 1);
             wgmma_commit();
             wgmma_wait<1>();                 // the previous stage's MMAs are done: hand its slot back
             fence_acc(acc);
-            if (prev >= 0) { __syncwarp(); if (lane == 0) mbar_arrive(bar0 + 8u * (kStages + prev)); }
-            prev = stage;
-            if (++stage == kStages) { stage = 0; phase ^= 1; }
+            release_prev();
+            next_stage();
         }
-        wgmma_wait<0>();
+        const int mt_cur = mt;
+        bool more = true;                    // the run has another tile: it becomes (mt, ...)
+        if (--left > 0) ++mt;
+        else if (!last_item) { ++i; start_item(); }
+        else more = false;
+        more = __shfl_sync(0xffffffffu, more, 0);      // (the schedule is the same in every lane; see cb)
+        bool issued = false;                 // the next tile's first K block is in flight, into nxt
+        if constexpr (kTwoSets) {
+            // only if its stage has landed already: the epilogue never waits for a future stage.  Both ways commit one group
+            // (empty if nothing was issued) and wait for all but it, so ptxas sees the same wgmma pipeline on either side.
+            // (the result is the same in every lane; the broadcast lets ptxas see that, like cb's)
+            if (more) issued = __shfl_sync(0xffffffffu, stage_landed(bar0 + 8u * stage, phase, wg), 0);
+            fence_acc(nxt);
+            wgmma_fence();
+            if (issued) mma_block(nxt, 0);
+            wgmma_commit();
+            wgmma_wait<1>();                 // this tile's MMAs are done, the next tile's keep running
+        } else {
+            wgmma_wait<0>();
+        }
         fence_acc(acc);
-        __syncwarp();
-        if (lane == 0) mbar_arrive(bar0 + 8u * (kStages + prev));
+        release_prev();                      // this tile's last stage goes back before its epilogue
+        if (issued) next_stage();
+        else prev = -1;
 
         // ---- epilogue from the accumulator fragments: register i = row r_base + 8 * ((i >> 1) & 1),
         //      GEMM column 8 * (i >> 2) + 2 * q4 + (i & 1).  The chunk's columns are permuted (group_column_channel, kernels.h):
@@ -190,7 +283,7 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
         if (mode == 0) {
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int m = mt * kBM + r_base + 8 * h;
+                const int m = mt_cur * kBM + r_base + 8 * h;
                 yrow[h] = y + (size_t)m * ldy + n0;
                 lim[h] = m < M ? ncols : 0;
                 corrp[h] = nullptr;
@@ -210,7 +303,7 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
                 corrp[h] = g.corr == nullptr ? nullptr : g.corr + (size_t)(g.interior_cls < 0 ? 0 : g.interior_cls) * corr_ld + n0;
                 const int j = r / box_rows, rem = r - j * box_rows;
                 const int brow = rem / lp.TWp, pcol = rem - brow * lp.TWp;
-                const int rb = mt * lp.R + j;
+                const int rb = mt_cur * lp.R + j;
                 if (j < lp.R && rb < g.rowboxes) {
                     const int seg = rb % g.SEG, tt = rb / g.SEG;
                     const int oh = (tt % g.OHB) * g.BH + brow, n = tt / g.OHB;
@@ -285,10 +378,27 @@ __device__ __forceinline__ void consume_item(const GroupLayerParams& lp, const G
             if (small_acc) columns(std::true_type{}, std::false_type{});
             else columns(std::false_type{}, std::false_type{});
         }
+        if constexpr (kTwoSets) {
+            // the next tile starts in acc: the preset, + its first K block if that was issued (into nxt, which is written by
+            // wgmmas only); that block's stage goes back.  The wait comes before the run can end, so no path leaves the loop
+            // with a wgmma in flight.
+            wgmma_wait<0>();
+            fence_acc(nxt);
+            if (!more) break;
+            release_prev();
+            prev = -1;
+            init(acc);
+#pragma unroll
+            for (int j = 0; j < BN / 2; ++j) acc[j] += issued ? nxt[j] : 0;
+        } else {
+            if (!more) break;
+            init(acc);
+        }
+        ahead = issued;
     }
 }
 
-__global__ void __launch_bounds__(kThreads, 1)
+__global__ void __launch_bounds__(kCgThreads, 1)
 conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLayerParams* __restrict__ params,
                         const GroupConvGeom* __restrict__ geom, int n_layers, const uint32_t* __restrict__ sched, int sched_stride) {
     extern __shared__ __align__(1024) uint8_t smem_raw[];
@@ -309,7 +419,7 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
         const int4* src = reinterpret_cast<const int4*>(params);
         int4* dst = reinterpret_cast<int4*>(smem + kOffLayers);
         const int n16 = n_layers * (int)(sizeof(GroupLayerParams) / 16);
-        for (int i = threadIdx.x; i < n16; i += kThreads) dst[i] = src[i];
+        for (int i = threadIdx.x; i < n16; i += kCgThreads) dst[i] = src[i];
     }
     if (warp == 8 && lane == 0) {
         for (int s = 0; s < kStages; ++s) { mbar_init(full_bar(s), 1); mbar_init(empty_bar(s), 8); }
@@ -317,9 +427,10 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
     }
     __syncthreads();
 
-    if (warp == 8) {
+    if (warp >= 8) {
         // ================= TMA producer =================
-        if (lane == 0) {
+        asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;\n" ::"n"(kProducerRegs));
+        if (warp == 8 && lane == 0) {
             int stage = 0, phase = 0;
             // weight-tile cache, all bookkeeping in registers (this thread's instruction count per K block is what bounds the kernel
             // on short K loops; a shared-memory tag table measured 8-30 % slower):
@@ -494,6 +605,7 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
         }
     } else {
         // ================= two consumer warpgroups: wgmma main loop + epilogue =================
+        asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;\n" ::"n"(kConsumerRegs));
         const int ct = threadIdx.x;                  // 0..255
         // two slots of epilogue constants: the current (layer, n chunk)'s table row, and the next distinct one in this CTA's
         // schedule, copied with cp.async while the current item runs
@@ -505,41 +617,36 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                 cp_async16(slot0 + slot * kConstBytes + 16u * ct, lp.ep + (size_t)nc * 3 * lp.bn + 4 * ct, true);
             cp_async_commit();
         };
-        uint32_t cached = 0xffffffffu;            // (layer, n chunk) whose constants are in slot cur
         int cur = 1;
         int stage = 0, phase = 0;
 
         uint32_t w = my[0];
         if (w != kGroupSchedEnd) fetch(w, 0);
-        for (int i = 0; w != kGroupSchedEnd; ++i) {
-            const uint32_t w_next = my[i + 1];    // a row ends with two end markers: my[i + 1] exists
+        for (int i = 0; w != kGroupSchedEnd; w = my[++i]) {
+            // a run of items with the same (layer, n chunk) starts at my[i]
             int L, nc, mt0, cnt;
             decode_item(w, L, nc, mt0, cnt);
             const GroupLayerParams& lp = sl[L];
             const int bn = lp.bn, n0 = nc * bn;
             const int ncols = (lp.N - n0) < bn ? (lp.N - n0) : bn;      // valid (16-padded) columns of this chunk
-            if ((w >> kGroupItemChunkShift) != cached) {
-                // this item's constants were fetched into the other slot during the previous item: once every consumer's copies
-                // have landed (and so every consumer is done reading the old slot), switch
-                cp_async_wait<0>();
-                named_sync(1, kConsumerThreads);
-                cur ^= 1;
-                cached = w >> kGroupItemChunkShift;
-            }
-            if (w_next != kGroupSchedEnd && (w_next >> kGroupItemChunkShift) != cached) fetch(w_next, cur ^ 1);
+            // this run's constants were fetched into the other slot during the previous run: once every consumer's copies have
+            // landed (and so every consumer is done reading the old slot), switch
+            cp_async_wait<0>();
+            named_sync(1, kConsumerThreads);
+            cur ^= 1;
+            auto fetch_next = [&](uint32_t wn) { fetch(wn, cur ^ 1); };
             const float* cst = reinterpret_cast<const float*>(smem + kOffConsts + cur * kConstBytes);
             switch (lp.bn >> 4) {     // conv_plan: bn is a multiple of 16 <= kGroupMaxBN
-                case 1: consume_item<16>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 2: consume_item<32>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 3: consume_item<48>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 4: consume_item<64>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 5: consume_item<80>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 6: consume_item<96>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 7: consume_item<112>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
-                case 8: consume_item<128>(lp, geom + L, n0, ncols, mt0, cnt, base, smem, cst, stage, phase); break;
+                case 1: consume_run<16>(lp, geom + L, n0, ncols, my, i, base, smem, cst, stage, phase, fetch_next); break;
+                case 2: consume_run<32>(lp, geom + L, n0, ncols, my, i, base, smem, cst, stage, phase, fetch_next); break;
+                case 3: consume_run<48>(lp, geom + L, n0, ncols, my, i, base, smem, cst, stage, phase, fetch_next); break;
+                case 4: consume_run<64>(lp, geom + L, n0, ncols, my, i, base, smem, cst, stage, phase, fetch_next); break;
+                case 5: consume_run<80>(lp, geom + L, n0, ncols, my, i, base, smem, cst, stage, phase, fetch_next); break;
+                case 6: consume_run<96>(lp, geom + L, n0, ncols, my, i, base, smem, cst, stage, phase, fetch_next); break;
+                case 7: consume_run<112>(lp, geom + L, n0, ncols, my, i, base, smem, cst, stage, phase, fetch_next); break;
+                case 8: consume_run<128>(lp, geom + L, n0, ncols, my, i, base, smem, cst, stage, phase, fetch_next); break;
                 default: __trap();
             }
-            w = w_next;
         }
     }
 }
@@ -551,7 +658,7 @@ cudaError_t launch_conv_group(const GroupMapsParam* maps_host, const GroupLayerP
     cudaError_t e = ensure_max_dynamic_smem((const void*)conv_group_wgmma_kernel, 227 * 1024);
     if (e != cudaSuccess) return e;
     ++g_launch_count;
-    conv_group_wgmma_kernel<<<grid, kThreads, kSmemTotal + 1024, stream>>>(*maps_host, params, geom, n_layers, sched, sched_stride);
+    conv_group_wgmma_kernel<<<grid, kCgThreads, kSmemTotal + 1024, stream>>>(*maps_host, params, geom, n_layers, sched, sched_stride);
     return cudaGetLastError();
 }
 
