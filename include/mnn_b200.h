@@ -303,6 +303,11 @@ MNNB200_API mnnb200_status mnnb200_conv_f32_create(mnnb200_runtime* rt, const mn
 MNNB200_API mnnb200_status mnnb200_conv_f32_set_pad(mnnb200_exec* e, int pad_h, int pad_w);
 MNNB200_API mnnb200_status mnnb200_conv_f32_resize(mnnb200_exec* e, int n, int ih, int iw, int* oh, int* ow);
 MNNB200_API mnnb200_status mnnb200_conv_f32_execute(mnnb200_exec* e, const float* x_nchw, float* y_nchw);
+/* read-only view of the resized conv_f32 execution's launch, as resize planned it: the first `count` (at most 7) of
+ * {bn (tile width 32 / 64 / 128), n_chunks, m_tiles (128-pixel M tiles), num_kb (32-wide K blocks per tile), stages (K blocks the
+ * bn-wide kernel's shared-memory ring holds), cp8 (ic rounded up to 8), taps (kh * kw)} go to fields.  NO_EXECUTION before resize,
+ * INVALID_VALUE for any other kind of execution.  Changes nothing. */
+MNNB200_API mnnb200_status mnnb200_conv_f32_plan(mnnb200_exec* e, int* fields, int count);
 MNNB200_API mnnb200_status mnnb200_dwconv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight,
                                                      const float* bias, int relu6, mnnb200_exec** out);
 MNNB200_API mnnb200_status mnnb200_dwconv_f32_resize(mnnb200_exec* e, int n, int ih, int iw, int* oh, int* ow);

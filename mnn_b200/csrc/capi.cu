@@ -1689,6 +1689,16 @@ mnnb200_status mnnb200_conv_f32_execute(mnnb200_exec* ex, const float* x, float*
     return MNNB200_OK;
 }
 
+mnnb200_status mnnb200_conv_f32_plan(mnnb200_exec* ex, int* fields, int count) {
+    if (!ex || ex->kind != 8 || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_f32_plan: bad argument");
+    auto* e = static_cast<ConvF32Exec*>(ex);
+    if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_f32_plan before resize");
+    const ConvF32Params& p = e->p;
+    const int v[] = {e->bn, p.n_chunks, p.m_tiles, p.num_kb, conv_f32_stages(e->bn), p.Cp8, p.taps};
+    for (int i = 0; i < count && i < (int)(sizeof(v) / sizeof(v[0])); ++i) fields[i] = v[i];
+    return MNNB200_OK;
+}
+
 mnnb200_status mnnb200_dwconv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight, const float* bias,
                                          int relu6, mnnb200_exec** out) {
     if (!rt || !desc || !weight || !out) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_create: NULL argument");

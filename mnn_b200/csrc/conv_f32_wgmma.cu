@@ -260,4 +260,13 @@ cudaError_t launch_conv_f32_wgmma(const ConvF32Params& p, const void* tmap_hi, c
     }
 }
 
+int conv_f32_stages(int bn) {
+    switch (bn) {
+        case 32: return Layout<32>::stages;
+        case 64: return Layout<64>::stages;
+        case 128: return Layout<128>::stages;
+        default: return 0;
+    }
+}
+
 }  // namespace mnnb200

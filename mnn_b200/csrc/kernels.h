@@ -156,6 +156,8 @@ cudaError_t launch_pack_conv_w_f32(const float* w, int oc, int ic, int taps, int
 // tmap_hi / tmap_lo: 2D maps over the [ocp][kp * 4 bytes] weight arrays with {128 bytes, bn rows} boxes, 128B swizzle; bn 32 / 64 / 128
 cudaError_t launch_conv_f32_wgmma(const ConvF32Params& p, const void* tmap_hi, const void* tmap_lo, int bn, cudaStream_t s,
                                   int sm_count);
+// pipeline stages of the bn-wide kernel (how many K blocks its shared-memory ring holds); 0 for a width it does not compile
+int conv_f32_stages(int bn);
 
 // fp32 neighbours of the float conv, all NCHW-linear.  dwconv: w [C][KH*KW]; act 0 none, 1 ReLU, 2 ReLU6
 struct DwF32Params {
