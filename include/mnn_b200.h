@@ -203,6 +203,16 @@ MNNB200_API mnnb200_status mnnb200_conv_int8_wino_execute(mnnb200_exec* e, const
  * transform); execute() == phases 7.  bench.py times each kernel class alone against its own roofline (SURVEY 8d C3). */
 MNNB200_API mnnb200_status mnnb200_conv_int8_wino_execute_phases(mnnb200_exec* e, const int8_t* x_nhwc16,
                                                                  int8_t* y_nhwc16, int phases);
+/* resize checks everything before it changes anything: a refusal (COMPUTE_SIZE_ERROR for an empty output or more tiles than
+ * 32-bit row coordinates reach, INVALID_VALUE for a zero scale) keeps the previous plan; a failure while building the new one
+ * (out of memory) leaves none, and execute returns NO_EXECUTION until a resize succeeds.  execute / execute_phases return
+ * INVALID_VALUE unless x and y are 4-byte aligned.
+ * Read-only view of the resized execution's launch: the first `count` (at most 13) of {unit, T (Winograd tiles), m_tiles
+ * (128-tile rows of the position GEMMs), Cp, OCp (ic / oc rounded up to 16), bn (columns per work item), n_chunks, items
+ * (work items), grid (persistent CTAs), one_tile (grid == items), resident_b (the weights stay in shared memory), stages
+ * (operand ring), num_kb (128-byte K blocks per item)} go to fields.  F(2,3) reports its fused kernel (bn 8, B streamed);
+ * F(4,3) / F(6,3) the batched position GEMM.  NO_EXECUTION before resize, INVALID_VALUE for any other kind of execution. */
+MNNB200_API mnnb200_status mnnb200_conv_int8_wino_plan(mnnb200_exec* e, int* fields, int count);
 
 /* ---- Depthwise int8 conv: replaces DepthwiseConvInt8Execution (execution/int8/DepthwiseConvInt8Execution.cu)
  *      with CPUDepthwiseConvInt8 arithmetic (CPUConvolution.cpp:181-192, Int8FunctionsOpt.cpp:1767-1814). */

@@ -71,6 +71,7 @@ SIGNATURES = {
     "mnnb200_conv_int8_wino_resize": (C.c_int, _RESIZE),
     "mnnb200_conv_int8_wino_execute": (C.c_int, [P, P, P]),
     "mnnb200_conv_int8_wino_execute_phases": (C.c_int, [P, P, P, C.c_int]),
+    "mnnb200_conv_int8_wino_plan": (C.c_int, [P, C.POINTER(C.c_int), C.c_int]),
     "mnnb200_exec_cost": (C.c_int, [P, C.POINTER(C.c_double), C.POINTER(C.c_double)]),
     "mnnb200_dwconv_int8_create": (C.c_int, [P, C.POINTER(ConvDesc), P, P, P, C.POINTER(P)]),
     "mnnb200_dwconv_int8_resize": (C.c_int, _RESIZE),

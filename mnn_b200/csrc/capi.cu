@@ -1407,10 +1407,20 @@ mnnb200_status mnnb200_conv_int8_wino_resize(mnnb200_exec* ex, int n, int ih, in
     if (!ex || ex->kind != 4) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_resize: not a Winograd execution");
     auto* e = static_cast<WinoConvInt8Exec*>(ex);
     const auto& d = e->d;
-    int OH = (oh && *oh > 0) ? *oh : conv_out(ih, 3, 1, d.pad_h, 1);
-    int OW = (ow && *ow > 0) ? *ow : conv_out(iw, 3, 1, d.pad_w, 1);
+    // every check first, on locals: a refused resize leaves the previous plan, fused bias and tensor maps as they were
+    const int OH = (oh && *oh > 0) ? *oh : conv_out(ih, 3, 1, d.pad_h, 1);
+    const int OW = (ow && *ow > 0) ? *ow : conv_out(iw, 3, 1, d.pad_w, 1);
     if (n <= 0 || OH <= 0 || OW <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "conv_int8_wino_resize: empty output");
     if (in_scale == 0.f || out_scale == 0.f) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_resize: zero quant scale");
+    const int hU = (OH + e->unit - 1) / e->unit, wU = (OW + e->unit - 1) / e->unit;
+    // the V / U tensor maps' row counts and the position GEMMs' row coordinates (a * Mpad + m, a * OCb + n) are 32-bit:
+    // Mpad * alpha2 and OCb * alpha2 <= INT32_MAX (hU * wU is bounded first, so that n * hU * wU cannot overflow)
+    const long long lim = 0x7fffffffLL / e->alpha2, tiles = (long long)hU * wU;
+    if (tiles > lim || (n * tiles + 127) / 128 * 128 > lim || e->OCb > lim)
+        return fail(MNNB200_COMPUTE_SIZE_ERROR, "conv_int8_wino_resize: too many tiles");
+    const long long T = n * tiles, Mpad = (T + 127) / 128 * 128;
+    // commit; a failure from here on (out of memory, tensor-map encode) leaves no plan, so execute returns NO_EXECUTION
+    e->resized = false;
     std::vector<float> fused(e->OCp, 0.f);
     for (int o = 0; o < d.oc; ++o) fused[o] = e->h_bias[o] / out_scale + (float)out_zero;   // mFusedBias, :215-217
     mnnb200_status st;
@@ -1419,10 +1429,9 @@ mnnb200_status mnnb200_conv_int8_wino_resize(mnnb200_exec* ex, int n, int ih, in
     memset(&p, 0, sizeof(p));
     p.N = n; p.IH = ih; p.IW = iw; p.Cp = e->Cp; p.OH = OH; p.OW = OW; p.OC = d.oc; p.OCp = e->OCp;
     p.pad_h = d.pad_h; p.pad_w = d.pad_w; p.unit = e->unit;
-    p.hU = (OH + e->unit - 1) / e->unit; p.wU = (OW + e->unit - 1) / e->unit;
-    p.T = (long long)n * p.hU * p.wU;
-    if (p.T * e->alpha2 > 0x7fffffffLL - 128) return fail(MNNB200_COMPUTE_SIZE_ERROR, "conv_int8_wino_resize: too many tiles");
-    p.Mpad = (int)((p.T + 127) / 128 * 128);
+    p.hU = hU; p.wU = wU;
+    p.T = T;
+    p.Mpad = (int)Mpad;
     p.s_in = in_scale; p.z_in = in_zero;
     p.out_inv = (float)(1.0 / (double)out_scale);                 // float outputdequantScale = 1.0 / mOutputScale, :340
     p.minv = (float)(d.relu ? out_zero : clamp_min);              // :347-351
@@ -1455,6 +1464,20 @@ mnnb200_status mnnb200_conv_int8_set_pad(mnnb200_exec* ex, int pad_h, int pad_w)
     else return fail(MNNB200_INVALID_VALUE, "set_pad: not a convolution execution");
     return MNNB200_OK;
 }
+}  // extern "C"
+
+// the alpha^2 batched position GEMMs of a resized F(4,3) / F(6,3) execution (and of F(2,3)'s three-kernel form)
+static GemmI8Params wino_gemm_params(const WinoConvInt8Exec* e) {
+    const WinoParams& p = e->p;
+    GemmI8Params g;
+    memset(&g, 0, sizeof(g));
+    g.a = e->d_v; g.b = e->d_u; g.M = (int)p.T; g.N = e->OCp; g.K = e->Cp;
+    g.y_f32 = e->d_m; g.ldy = e->OCp; g.wscale = e->d_scale; g.bias = e->d_offset; g.wsum128 = e->d_wsum128; g.OC = e->d.oc;
+    g.batch = e->alpha2; g.a_batch_rows = p.Mpad; g.b_batch_rows = e->OCb; g.c_batch_stride = e->OCp; g.wino = 1;
+    return g;
+}
+
+extern "C" {
 mnnb200_status mnnb200_conv_int8_wino_execute(mnnb200_exec* ex, const int8_t* x, int8_t* y) {
     return mnnb200_conv_int8_wino_execute_phases(ex, x, y, 7);
 }
@@ -1462,6 +1485,9 @@ mnnb200_status mnnb200_conv_int8_wino_execute_phases(mnnb200_exec* ex, const int
     if (!ex || ex->kind != 4) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_execute: not a Winograd execution");
     auto* e = static_cast<WinoConvInt8Exec*>(ex);
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_int8_wino_execute before resize");
+    // the transforms move 4 input channels and up to 4 output channels per access
+    if (!x || !y || ((uintptr_t)x & 3) || ((uintptr_t)y & 3))
+        return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_execute: x and y must be 4-byte aligned");
     WinoParams p = e->p;
     p.x = x; p.y = y;
     if (phases & 1) CK(launch_wino_input(p, e->rt->stream));
@@ -1480,13 +1506,28 @@ mnnb200_status mnnb200_conv_int8_wino_execute_phases(mnnb200_exec* ex, const int
         if (phases & 4) CK(launch_wino_output(p, e->rt->stream));
         return MNNB200_OK;
     }
-    GemmI8Params g;
-    memset(&g, 0, sizeof(g));
-    g.a = e->d_v; g.b = e->d_u; g.M = (int)p.T; g.N = e->OCp; g.K = e->Cp;
-    g.y_f32 = e->d_m; g.ldy = e->OCp; g.wscale = e->d_scale; g.bias = e->d_offset; g.wsum128 = e->d_wsum128; g.OC = e->d.oc;
-    g.batch = e->alpha2; g.a_batch_rows = p.Mpad; g.b_batch_rows = e->OCb; g.c_batch_stride = e->OCp; g.wino = 1;
-    CK(launch_gemm_i8_wgmma(g, &e->tmap_a, &e->tmap_b, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
+    CK(launch_gemm_i8_wgmma(wino_gemm_params(e), &e->tmap_a, &e->tmap_b, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
     if (phases & 4) CK(launch_wino_output(p, e->rt->stream));
+    return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_conv_int8_wino_plan(mnnb200_exec* ex, int* fields, int count) {
+    if (!ex || ex->kind != 4 || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_plan: bad argument");
+    auto* e = static_cast<WinoConvInt8Exec*>(ex);
+    if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_int8_wino_plan before resize");
+    const WinoParams& p = e->p;
+    const int sm = e->rt->prop.multiProcessorCount, m_tiles = p.Mpad / 128, num_kb = (e->Cp + 127) / 128;
+    int bn, n_chunks, items, grid, one_tile, resident_b, stages;
+    if (e->unit == 2) {            // the fused kernel: (m tile, 8-channel chunk) items over a persistent grid, B streamed
+        bn = kWinoFusedBN; n_chunks = e->OCp / kWinoFusedBN; items = m_tiles * n_chunks;
+        grid = std::min(items, sm); one_tile = grid == items; resident_b = 0; stages = kWinoFusedStages;
+    } else {
+        const GemmI8Launch l = gemm_i8_wgmma_launch(wino_gemm_params(e), e->bn, sm);
+        bn = e->bn; n_chunks = e->OCb / e->bn; items = l.items;
+        grid = l.grid; one_tile = l.one_tile; resident_b = l.resident_b; stages = l.stages;
+    }
+    const int v[] = {e->unit, (int)p.T, m_tiles, e->Cp, e->OCp, bn, n_chunks, items, grid, one_tile, resident_b, stages, num_kb};
+    for (int i = 0; i < count && i < (int)(sizeof(v) / sizeof(v[0])); ++i) fields[i] = v[i];
     return MNNB200_OK;
 }
 }  // extern "C"

@@ -384,21 +384,32 @@ KParams make_params(const GemmI8Params& g, int bn) {
 
 }  // namespace
 
+GemmI8Launch gemm_i8_wgmma_launch(const GemmI8Params& g, int bn, int sm_count) {
+    const KParams p = make_params(g, bn);
+    GemmI8Launch l;
+    l.num_kb = (g.K + kBK - 1) / kBK;
+    l.items = p.batch * p.m_tiles * p.n_chunks;
+    l.grid = l.items < sm_count ? l.items : sm_count;
+    l.one_tile = l.grid == l.items ? 1 : 0;
+    const bool fixed_tile = l.one_tile || p.n_chunks * p.batch == 1;
+    const SmemPlan pl = make_plan(bn, fixed_tile ? 1 : p.n_chunks * p.batch, l.num_kb, false);
+    l.resident_b = pl.resident_b;
+    l.stages = pl.stages;
+    l.smem = pl.total + 1024;
+    return l;
+}
+
 cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& g, const void* tmap_a, const void* tmap_b, int bn, cudaStream_t stream,
                                  int sm_count) {
     if (bn < 16 || bn > kMaxBN || (bn & 15) || g.y_f32 == nullptr) return cudaErrorInvalidValue;
     if (g.bs && (g.wino || bn > kMaxBN / 2 || g.bs % 32 || g.K % g.bs || g.blocks != g.K / g.bs)) return cudaErrorInvalidValue;
     KParams p = make_params(g, bn);
-    const int num_kb = (g.K + kBK - 1) / kBK;
-    const int work = p.batch * p.m_tiles * p.n_chunks;
-    const int grid = work < sm_count ? work : sm_count;
-    p.one_tile = grid == work ? 1 : 0;
-    const bool fixed_tile = p.one_tile || p.n_chunks * p.batch == 1;
-    const int smem = make_plan(bn, fixed_tile ? 1 : p.n_chunks * p.batch, num_kb, false).total + 1024;
+    const GemmI8Launch l = gemm_i8_wgmma_launch(g, bn, sm_count);
+    p.one_tile = l.one_tile;
     const CUtensorMap* ta = reinterpret_cast<const CUtensorMap*>(tmap_a);
     const CUtensorMap* tb = reinterpret_cast<const CUtensorMap*>(tmap_b);
-    if (g.wino) return launch(gemm_i8_wgmma_kernel<2, false, 256>, ta, tb, p, grid, smem, 227 * 1024, false, stream);
-    return launch(gemm_i8_wgmma_kernel<1, false, 256>, ta, tb, p, grid, smem, 227 * 1024, false, stream);
+    if (g.wino) return launch(gemm_i8_wgmma_kernel<2, false, 256>, ta, tb, p, l.grid, l.smem, 227 * 1024, false, stream);
+    return launch(gemm_i8_wgmma_kernel<1, false, 256>, ta, tb, p, l.grid, l.smem, 227 * 1024, false, stream);
 }
 
 cudaError_t launch_gemm_i8_2cta(const GemmI8Params& g, const void* tmap_a, const void* tmap_b_half, int bn, cudaStream_t stream,

@@ -64,6 +64,13 @@ struct GemmI8Params {
 };
 cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& p, const void* tmap_a, const void* tmap_b, int bn, cudaStream_t stream,
                                  int sm_count);
+// the launch launch_gemm_i8_wgmma makes for (p, bn) on sm_count SMs: work items (batch, m tile, n chunk), persistent grid,
+// one_tile (every CTA owns exactly one item), resident_b (the weights stay in shared memory for the whole launch), the
+// operand ring's stages, 128-byte K blocks per item and the dynamic shared memory
+struct GemmI8Launch {
+    int items, grid, one_tile, resident_b, stages, num_kb, smem;
+};
+GemmI8Launch gemm_i8_wgmma_launch(const GemmI8Params& p, int bn, int sm_count);
 // ---- one persistent launch over a LIST of int8 convolutions (conv_group_wgmma.cu); a lone conv runs as a one-layer list.
 //      Two layer modes:
 //   mode 0  GEMM-shaped (1x1, stride 1, no pad): A = the NHWC16 activation as a 2D matrix, one TMA box per K block
@@ -250,8 +257,8 @@ struct WinoParams {
 };
 cudaError_t launch_wino_input(const WinoParams& p, cudaStream_t s);
 // F(2,3): the 16 position GEMMs + output transform + requantise fused (all 16 accumulators in registers, no fp32 M tensor);
-// tmap_u has boxes of kWinoFusedBN rows
-constexpr int kWinoFusedBN = 8;
+// tmap_u has boxes of kWinoFusedBN rows; its operand ring has kWinoFusedStages stages
+constexpr int kWinoFusedBN = 8, kWinoFusedStages = 6;
 struct WinoFusedParams {
     int8_t* y;
     const float *scale, *offset, *fused_bias;   // [16][OCp], [16][OCp], [OCp]

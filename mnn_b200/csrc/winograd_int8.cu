@@ -255,7 +255,7 @@ __global__ void __launch_bounds__(256) wino_output_kernel(const WinoParams p) {
 // Arithmetic identical to gemm_i8_wgmma_kernel<2> + wino_output_kernel<4,4>, bit for bit.
 // =====================================================================================================================
 using namespace hop;
-constexpr int kFStages = 6, kFBN = kWinoFusedBN, kFStageBytes = 128 * 128 + kFBN * 128;
+constexpr int kFStages = kWinoFusedStages, kFBN = kWinoFusedBN, kFStageBytes = 128 * 128 + kFBN * 128;
 
 __global__ void __launch_bounds__(kThreads, 1)
 wino_f23_fused_kernel(const __grid_constant__ CUtensorMap tmap_v, const __grid_constant__ CUtensorMap tmap_u, const WinoFusedParams p) {

@@ -671,7 +671,8 @@ static void wino_dst(int alpha, const float* s, float* m) {
 
 /* ConvInt8Winograd::onExecute + WinoExecution::onExecute + mergeAddBiasScaleQuantize
  * (ConvInt8Winograd.cpp:306-356, 396-651, 243-259).  x [n][ic][ih][iw] int8, y [n][oc][oh][ow] int8,
- * stride 1, dilation 1, kernel r x r, symmetric pads.  clamp: min = relu ? z_out : clamp_min. */
+ * stride 1, dilation 1, kernel r x r, begin pads pad_h (rows) and pad_w (columns), each also added at the end (CAFFE).
+ * clamp: min = relu ? z_out : clamp_min. */
 ORACLE_API void mnn_oracle_wino_conv_int8(const int8_t* x, int n, int ic, int ih, int iw, const int8_t* w, int oc, int r,
                                           int pad_h, int pad_w, int unit, const float* wscale, const float* bias,
                                           const float* in_scales, const int32_t* in_zeros, const float* w_scales,

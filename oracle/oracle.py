@@ -336,14 +336,20 @@ def wino_weights(w, wscale, in_scales, in_zeros, w_scales, unit):
     return wq, sc, of
 
 
+def _wino_pads(pad):
+    """pad: one int for both axes or (pad_h, pad_w)"""
+    return (int(pad[0]), int(pad[1])) if isinstance(pad, (tuple, list)) else (int(pad), int(pad))
+
+
 def wino_conv_int8(x, w, wscale, bias, in_scales, in_zeros, w_scales, unit, pad=1, s_in=1.0, z_in=0, s_out=1.0, z_out=0,
                    clamp_min=-127, clamp_max=127, relu=False):
     x, w, wscale, bias, in_scales, in_zeros, w_scales = _wino_args(x, w, wscale, bias, in_scales, in_zeros, w_scales, unit)
     n, ic, ih, iw = x.shape
     oc, r = w.shape[0], w.shape[2]
-    oh, ow = ih + 2 * pad - r + 1, iw + 2 * pad - r + 1
+    ph, pw = _wino_pads(pad)
+    oh, ow = ih + 2 * ph - r + 1, iw + 2 * pw - r + 1
     y = np.empty((n, oc, oh, ow), np.int8)
-    lib().mnn_oracle_wino_conv_int8(_p(x, C.c_int8), n, ic, ih, iw, _p(w, C.c_int8), oc, r, pad, pad, unit,
+    lib().mnn_oracle_wino_conv_int8(_p(x, C.c_int8), n, ic, ih, iw, _p(w, C.c_int8), oc, r, ph, pw, unit,
                                     _p(wscale, C.c_float), _p(bias, C.c_float), _p(in_scales, C.c_float),
                                     _p(in_zeros, C.c_int32), _p(w_scales, C.c_float), C.c_float(s_in), int(z_in),
                                     C.c_float(s_out), int(z_out), int(clamp_min), int(clamp_max), int(relu), _p(y, C.c_int8))
@@ -356,7 +362,8 @@ def ref_wino(x, w, wscale, bias, in_scales, in_zeros, w_scales, unit, pad=1, s_i
     x, w, wscale, bias, in_scales, in_zeros, w_scales = _wino_args(x, w, wscale, bias, in_scales, in_zeros, w_scales, unit)
     n, ic, ih, iw = x.shape
     oc, r = w.shape[0], w.shape[2]
-    hdr = struct.pack("<13i2f", n, ic, ih, iw, oc, r, pad, unit, int(relu), z_in, z_out, clamp_min, clamp_max, s_in, s_out)
+    ph, pw = _wino_pads(pad)
+    hdr = struct.pack("<13i2fi", n, ic, ih, iw, oc, r, ph, unit, int(relu), z_in, z_out, clamp_min, clamp_max, s_in, s_out, pw)
     payload = hdr + x.tobytes() + w.tobytes() + bias.tobytes() + wscale.tobytes() + in_scales.tobytes() + \
         in_zeros.tobytes() + w_scales.tobytes()
     env = dict(os.environ)

@@ -218,7 +218,8 @@ static int cmdConv(const char* reqPath, const char* outPath) {
     return 0;
 }
 
-struct WinoReq { int32_t n, ic, ih, iw, oc, k, pad, unit, relu, zin, zout, minv, maxv; float scaleIn, scaleOut; };
+// pad = padY (rows), padW = padX (columns)
+struct WinoReq { int32_t n, ic, ih, iw, oc, k, pad, unit, relu, zin, zout, minv, maxv; float scaleIn, scaleOut; int32_t padW; };
 // wino <req.bin> <out.bin>: OpType_ConvInt8 carrying a winogradAttr => ConvInt8Winograd on the CPU backend
 // (source/backend/cpu/CPUConvolution.cpp:336-339).  Op built exactly as test/op/ConvInt8Test.cpp:585-610 does
 // (_Conv float-bias overload + WinogradInt8Attr::turnToWinogradConv).  Must be linked against the AVX2 build
@@ -244,7 +245,7 @@ static int cmdWino(const char* reqPath, const char* outPath) {
     memcpy(xin->writeMap<int8_t>(), x.data(), xs);
     auto xC4 = _Convert(xin, NC4HW4);
     xC4 = _FloatToInt8(_Cast<float>(xC4), _Scalar<float>(1.0f), -128, 127);
-    INTS channel = {r.ic, r.oc}, kernel = {r.k, r.k}, pads = {r.pad, r.pad};
+    INTS channel = {r.ic, r.oc}, kernel = {r.k, r.k}, pads = {r.padW, r.pad};   // {padX, padY}, as convModern
     WinogradInt8Attr attrs;
     attrs.add(0, 0, r.k, r.k, r.unit, r.unit, inS, wS, inZ);
     auto y = _Conv(std::move(w), std::move(bias), std::move(wscale), xC4, channel, kernel, CAFFE, {1, 1}, {1, 1}, 1, pads,

@@ -42,7 +42,7 @@ KERNEL_TESTS = {
     ("dynamic_quant_vec_kernel", (8,)): f"{HERE}::test_prefill_dynamic_quant",
     ("gemm_i8_wgmma_kernel", (1, 0, 256)): f"{HERE}::test_prefill_dynamic_quant",
     ("gemm_i8_wgmma_kernel", (1, 1, 256)): "tests/test_gpu_parity.py::test_linear_w8_cta_pair_variant_bit_exact",
-    ("gemm_i8_wgmma_kernel", (2, 0, 256)): "tests/test_winograd.py::test_gpu_vs_oracle",
+    ("gemm_i8_wgmma_kernel", (2, 0, 256)): "tests/test_gpu_winograd.py::test_wino_cell_matrix",
     # mma.sync implicit GEMM: (BM, BN, WM, WN)
     **{("conv_int8_igemm_kernel", t): f"{HERE}::test_mma_sync_tiles"
        for t in ((128, 64, 4, 2), (128, 32, 8, 1), (128, 16, 8, 1), (64, 64, 2, 2), (64, 32, 4, 1), (128, 128, 4, 2))},
@@ -50,16 +50,16 @@ KERNEL_TESTS = {
     ("dwconv3x3_int8_kernel", (1,)): f"{HERE}::test_depthwise_strip",
     ("dwconv3x3_int8_kernel", (2,)): f"{HERE}::test_depthwise_strip",
     ("dwconv_int8_kernel", ()): f"{HERE}::test_depthwise_generic",
-    # the conv-group kernel, Winograd, fp32 conv / GEMM and the elementwise kernels: their own modules (F(2,3) Winograd's
-    # three-kernel form runs only through the per-phase entry point: checked here)
+    # the conv-group kernel, Winograd, fp32 conv / GEMM and the elementwise kernels: their own modules (the Winograd cell matrix
+    # also runs every cell as three kernels, F(2,3)'s output transform only reachable that way)
     ("conv_group_wgmma_kernel", ()): "tests/test_gpu_conv_group.py::test_conv_group_width_by_chunk_matrix",
-    ("wino_input_kernel", (4, 4)): "tests/test_winograd.py::test_gpu_vs_oracle",
-    ("wino_input_kernel", (8, 1)): "tests/test_winograd.py::test_gpu_vs_oracle",
-    ("wino_input_seq4_kernel", (6,)): "tests/test_winograd.py::test_gpu_vs_oracle",
-    ("wino_output_kernel", (4, 4)): f"{HERE}::test_winograd_f23_three_kernel_form",
-    ("wino_output_kernel", (6, 2)): "tests/test_winograd.py::test_gpu_vs_oracle",
-    ("wino_output_kernel", (8, 1)): "tests/test_winograd.py::test_gpu_vs_oracle",
-    ("wino_f23_fused_kernel", ()): "tests/test_winograd.py::test_gpu_vs_oracle",
+    ("wino_input_kernel", (4, 4)): "tests/test_gpu_winograd.py::test_wino_cell_matrix",
+    ("wino_input_kernel", (8, 1)): "tests/test_gpu_winograd.py::test_wino_cell_matrix",
+    ("wino_input_seq4_kernel", (6,)): "tests/test_gpu_winograd.py::test_wino_cell_matrix",
+    ("wino_output_kernel", (4, 4)): "tests/test_gpu_winograd.py::test_wino_cell_matrix",
+    ("wino_output_kernel", (6, 2)): "tests/test_gpu_winograd.py::test_wino_cell_matrix",
+    ("wino_output_kernel", (8, 1)): "tests/test_gpu_winograd.py::test_wino_cell_matrix",
+    ("wino_f23_fused_kernel", ()): "tests/test_gpu_winograd.py::test_wino_cell_matrix",
     ("conv_f32_wgmma_kernel", (32,)): "tests/test_gpu_conv_f32.py::test_conv_f32_cell_matrix",
     ("conv_f32_wgmma_kernel", (64,)): "tests/test_gpu_conv_f32.py::test_conv_f32_cell_matrix",
     ("conv_f32_wgmma_kernel", (128,)): "tests/test_gpu_conv_f32.py::test_conv_f32_cell_matrix",

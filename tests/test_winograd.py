@@ -64,6 +64,21 @@ def test_oracle_bit_exact_vs_live_reference_avx2():
         assert np.array_equal(wino_oracle(O, c, unit), wino_oracle(O, c, unit, O.ref_wino)), (unit, ic, oc)
 
 
+@needs_ref2
+@pytest.mark.reference
+@pytest.mark.parametrize("unit,n,ic,oc,ih,iw,pad", [
+    (2, 2, 21, 19, 9, 7, (0, 2)),
+    (4, 1, 24, 17, 11, 13, (2, 1)),
+    (6, 1, 16, 20, 7, 15, (1, 3)),
+])
+def test_oracle_asymmetric_pads_bit_exact_vs_live_reference_avx2(unit, n, ic, oc, ih, iw, pad):
+    """pad_h != pad_w: ConvInt8Winograd takes padY for the rows and padX for the columns, and the output size follows each"""
+    c = dict(random_wino_case(np.random.default_rng(unit * 31 + ic), unit, n, ic, oc, ih, iw, 1, False), pad=pad)
+    y = wino_oracle(O, c, unit)
+    assert y.shape == (n, oc, ih + 2 * pad[0] - 2, iw + 2 * pad[1] - 2)
+    assert np.array_equal(y, wino_oracle(O, c, unit, O.ref_wino)), (unit, pad)
+
+
 # ------------------------------------------------------------------------------------------------------------- GPU
 def run_wino(backend, c, unit):
     from mnn_b200.backend import Op, QuantAttr, Tensor, encode_winograd_attr
