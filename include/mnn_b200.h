@@ -163,8 +163,8 @@ MNNB200_API mnnb200_status mnnb200_reduce_f32(mnnb200_runtime* rt, const float* 
  *      per-command Execution::onExecute walk of Pipeline::execute (source/core/Pipeline.cpp:1069-1140) over
  *      ConvInt8CutlassExecution::onExecute
  *      (execution/int8/ConvInt8CutlassExecution.cu:381-445) for such a run of commands: the members' TMA descriptors and
- *      epilogue constants go into a device-side layer table and all (layer, tile) work items into one schedule dealt
- *      round-robin to one CTA per SM.  The members stay owned by the caller and must outlive the group.
+ *      epilogue constants go into a device-side layer table and all (layer, tile) work items into one schedule that gives
+ *      every CTA (one per SM) an equal share of every layer's tiles (mnnb200_conv_group_schedule).  The members stay owned by the caller and must outlive the group.
  *      create: every member must be a conv execution (mnnb200_conv_int8_create*), count <= 64.
  *      bind:   after every member's resize; xs[i] / ys[i] = member i's NHWC16 input / output (must not alias another
  *              member's output: members are NOT ordered against each other).  NOT_SUPPORT if the conv-group kernel does
@@ -177,10 +177,17 @@ MNNB200_API mnnb200_status mnnb200_conv_group_execute(mnnb200_exec* group);
 /* 1 if auto execute runs the (resized) conv on the conv-group kernel; such a conv can be a member of a conv group */
 MNNB200_API int mnnb200_conv_int8_groupable(mnnb200_exec* e);
 /* read-only view of the resized conv's layer on the conv-group kernel, as resize planned it: the first `count` (at most 10) of
- * {mode (0 = 1x1 GEMM, 1 = implicit GEMM), cb (bytes of K per TMA chunk: 128 / 64 / 16), bn (tile width), n_chunks, m_tiles,
+ * {mode (0 = 1x1 GEMM, 1 = implicit GEMM), cb (bytes of K per TMA chunk: 128 / 64 / 32 / 16), bn (tile width), n_chunks, m_tiles,
  * num_kb (K blocks per tile), K, R (row boxes per M tile), TWp (pixels per row box), BH (output rows per box)} go to fields.
  * NO_EXECUTION before resize, NOT_SUPPORT if the conv-group kernel does not take the conv.  Changes nothing. */
 MNNB200_API mnnb200_status mnnb200_conv_int8_group_plan(mnnb200_exec* e, int* fields, int count);
+/* the schedule bind builds for a list of `layers` (<= 64) members with m_tiles[l] M tiles and n_chunks[l] n chunks (both from
+ * mnnb200_conv_int8_group_plan) on a device with sm_count SMs: *grid CTAs, one row of *stride words each, a row's items
+ * followed by 0xffffffff up to its end.  item = layer << 26 | n chunk << 20 | (tiles - 1) << 14 | first M tile: `tiles`
+ * consecutive M tiles of one (layer, n chunk).  items == NULL: only *grid and *stride; otherwise capacity >= grid * stride
+ * words.  Needs no device. */
+MNNB200_API mnnb200_status mnnb200_conv_group_schedule(const int* m_tiles, const int* n_chunks, int layers, int sm_count,
+                                                       uint32_t* items, int capacity, int* grid, int* stride);
 
 /* ---- Int8 Winograd Conv2D F(m x m, 3 x 3), m = 2 / 4 / 6: the op carries a winogradAttr (per-position input scales /
  *      zero points and per-(position, oc) weight scales).  Replaces the structure of ConvWinogradExecution {Resource,

@@ -67,6 +67,8 @@ SIGNATURES = {
     "mnnb200_conv_group_execute": (C.c_int, [P]),
     "mnnb200_conv_int8_groupable": (C.c_int, [P]),
     "mnnb200_conv_int8_group_plan": (C.c_int, [P, C.POINTER(C.c_int), C.c_int]),
+    "mnnb200_conv_group_schedule": (C.c_int, [C.POINTER(C.c_int), C.POINTER(C.c_int), C.c_int, C.c_int, C.POINTER(C.c_uint32), C.c_int,
+                                              C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "mnnb200_conv_int8_wino_create": (C.c_int, [P, C.POINTER(ConvDesc), P, P, P, P, C.c_int, C.POINTER(P)]),
     "mnnb200_conv_int8_wino_resize": (C.c_int, _RESIZE),
     "mnnb200_conv_int8_wino_execute": (C.c_int, [P, P, P]),

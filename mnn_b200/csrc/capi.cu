@@ -131,7 +131,9 @@ static mnnb200_status make_tmap_u8(CUtensorMap* m, const void* ptr, int rank, co
     PFN_encodeTiled enc = get_encode();
     if (!enc) return fail(MNNB200_CUDA_ERROR, "cuTensorMapEncodeTiled entry point not available");
     cuuint32_t estr[5] = {1u, 1u, 1u, 1u, 1u};
-    const CUtensorMapSwizzle sw = box[0] == 128 ? CU_TENSOR_MAP_SWIZZLE_128B : (box[0] == 64 ? CU_TENSOR_MAP_SWIZZLE_64B : CU_TENSOR_MAP_SWIZZLE_NONE);
+    const CUtensorMapSwizzle sw = box[0] == 128 ? CU_TENSOR_MAP_SWIZZLE_128B
+                                  : box[0] == 64 ? CU_TENSOR_MAP_SWIZZLE_64B
+                                  : box[0] == 32 ? CU_TENSOR_MAP_SWIZZLE_32B : CU_TENSOR_MAP_SWIZZLE_NONE;
     CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, (cuuint32_t)rank, const_cast<void*>(ptr), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, sw, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail(MNNB200_CUDA_ERROR, "cuTensorMapEncodeTiled (rank " + std::to_string(rank) + ") failed: " + std::to_string((int)r));
@@ -306,8 +308,10 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin, const std::vector<floa
     q.mode = plan.gemm ? 0 : 1;
     const int taps = p.KH * p.KW;
     if (plan.gemm) {
-        q.K = e->Cp; q.cb = 128; q.TWp = 128; q.R = 1;
-        q.m_tiles = (p.M + 127) / 128; q.num_kb = (e->Cp + 127) / 128;
+        // a layer whose whole K fits a narrower K block gets that one: a 128-byte block of a 16 ... 64 byte K is mostly TMA
+        // zero fill in the stage and the weight tile, and k-steps that multiply it (Cp = 16: a k-step eats 32 bytes, half fill)
+        q.K = e->Cp; q.cb = e->Cp <= 32 ? 32 : (e->Cp <= 64 ? 64 : 128); q.TWp = 128; q.R = 1;
+        q.m_tiles = (p.M + 127) / 128; q.num_kb = (e->Cp + q.cb - 1) / q.cb;
     } else {
         g.KH = p.KH; g.KW = p.KW; g.Cp = e->Cp; g.NB = p.N;
         g.sh = p.sh; g.sw = p.sw; g.ph = p.ph; g.pw = p.pw; g.dh = p.dh; g.dw = p.dw; g.OH = p.OH; g.OW = p.OW;
@@ -413,6 +417,62 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin, const std::vector<floa
     return MNNB200_OK;
 }
 
+// The schedule of a list of layers (M tiles, n chunks each) on at most sm_count CTAs: *stride words per CTA row.  Layers go in
+// list order in every row, so all CTAs work on the same layer at the same time (the kernel's weight cache depends on that;
+// a contiguous cost-balanced partition over layers measured 0.81 ms against 0.28 ms on MobileNet-v2 B=32) and every CTA
+// gets the same mix of layers: the balance needs no cost model.
+//  * a layer of ONE n chunk with at least one M tile per CTA is dealt as CONTIGUOUS ranges of T / grid tiles, T mod grid
+//    CTAs getting one more, in items of up to 64 tiles: the kernel pays its per-item bookkeeping once per range, and a
+//    CTA's activation and output rows of the layer are one contiguous piece of memory;
+//  * the tiles of any other layer go one per item to consecutive CTAs, the n chunks of an M tile next to each other: the
+//    chunks of a tile write parts of the same output rows, and written a whole range apart those leave L2 as partial lines
+//    (K = 32, OC = 144, M = 32 x 112 x 112 on an H100 at 700 W: 118 us with ranges per chunk, 80 us with single tiles).
+// One cursor serves both: the extra tiles of a range-dealt layer start at the CTA the last single tile stopped at and move
+// it on, so neither piles up on the same CTAs from layer to layer.
+static std::vector<uint32_t> group_schedule(const int* m_tiles, const int* n_chunks, int layers, int sm_count, int* grid_out,
+                                            int* stride_out) {
+    long total = 0;
+    for (int l = 0; l < layers; ++l) total += (long)m_tiles[l] * n_chunks[l];
+    const int grid = (int)std::max(1L, std::min(total, (long)sm_count));
+    std::vector<std::vector<uint32_t>> rows(grid);
+    auto item = [](int l, int nc, int mt, int cnt) {
+        return ((uint32_t)l << kGroupItemLayerShift) | ((uint32_t)nc << kGroupItemChunkShift) |
+               ((uint32_t)(cnt - 1) << kGroupItemCountShift) | (uint32_t)mt;
+    };
+    const int max_cnt = (int)kGroupItemCountMask + 1;
+    int cursor = 0;
+    for (int l = 0; l < layers; ++l) {
+        const int T = m_tiles[l];
+        if (T < grid || n_chunks[l] > 1) {
+            for (int mt = 0; mt < T; ++mt)
+                for (int nc = 0; nc < n_chunks[l]; ++nc) {
+                    rows[cursor].push_back(item(l, nc, mt, 1));
+                    cursor = (cursor + 1) % grid;
+                }
+            continue;
+        }
+        const int each = T / grid, extra = T % grid;
+        int mt = 0;
+        for (int k = 0; k < grid; ++k) {
+            const int n = each + (k < extra ? 1 : 0);
+            for (int done = 0; done < n; done += max_cnt)
+                rows[(cursor + k) % grid].push_back(item(l, 0, mt + done, std::min(max_cnt, n - done)));
+            mt += n;
+        }
+        cursor = (cursor + extra) % grid;
+    }
+    // Every role of a CTA walks its whole row up to the first terminator.  The row keeps a second one: the consumers read
+    // the item after the current one.
+    size_t longest = 0;
+    for (const auto& r : rows) longest = std::max(longest, r.size());
+    const size_t stride = longest + 2;
+    std::vector<uint32_t> sched(stride * grid, kGroupSchedEnd);
+    for (int c = 0; c < grid; ++c) std::copy(rows[c].begin(), rows[c].end(), sched.begin() + c * stride);
+    *grid_out = grid;
+    *stride_out = (int)stride;
+    return sched;
+}
+
 // Binds planned convs to their activations: the A tensor maps, the y pointers and the schedule.
 static mnnb200_status group_build(GroupState& gs, const std::vector<ConvInt8Exec*>& members, const int8_t* const* xs,
                                   int8_t* const* ys, double* cost_bytes, double* cost_macs) {
@@ -425,7 +485,7 @@ static mnnb200_status group_build(GroupState& gs, const std::vector<ConvInt8Exec
     static_assert(sizeof(CUtensorMap) == sizeof(CUtensorMap_st_opaque), "tensor map size");
     std::vector<GroupLayerParams> prm(L);
     std::vector<GroupConvGeom> geo(L);
-    std::vector<uint32_t> items;
+    std::vector<int> m_tiles(L), n_chunks(L);
     if (cost_bytes) *cost_bytes = 0;
     if (cost_macs) *cost_macs = 0;
     mnnb200_status st;
@@ -442,7 +502,10 @@ static mnnb200_status group_build(GroupState& gs, const std::vector<ConvInt8Exec
         CUtensorMap* ta1 = reinterpret_cast<CUtensorMap*>(&gs.h_maps->a1[l]);
         memcpy(&gs.h_maps->b[l], &e->plan.tmap_b, sizeof(CUtensorMap));
         if (q.mode == 0) {
-            if ((st = make_tmap_i8(ta, xs[l], p.M, e->Cp, 128))) return st;
+            cuuint64_t dims[2] = {(cuuint64_t)e->Cp, (cuuint64_t)p.M};
+            cuuint64_t strides[1] = {(cuuint64_t)e->Cp};
+            cuuint32_t box[2] = {(cuuint32_t)q.cb, 128u};
+            if ((st = make_tmap_u8(ta, xs[l], 2, dims, strides, box))) return st;
         } else {
             // A: one 4D {C, W', H, N} view of the NHWC16 input per column parity (W' = every sw-th column)
             for (int par = 0; par < p.sw; ++par) {
@@ -455,19 +518,11 @@ static mnnb200_status group_build(GroupState& gs, const std::vector<ConvInt8Exec
         if (p.sw == 1) *ta1 = *ta;
         if (cost_bytes) *cost_bytes += e->cost_bytes;
         if (cost_macs) *cost_macs += e->cost_macs;
-        // an item = ONE M tile of one n chunk: measured on MobileNet-v2 B=32, 1 tile per item is best (0.184 ms; 2: 0.186, 8: 0.192)
-        for (int mt = 0; mt < q.m_tiles; ++mt)
-            for (int nc = 0; nc < q.n_chunks; ++nc)
-                items.push_back(((uint32_t)l << kGroupItemLayerShift) | ((uint32_t)nc << kGroupItemChunkShift) | (uint32_t)mt);
+        m_tiles[l] = q.m_tiles;
+        n_chunks[l] = q.n_chunks;
     }
-    // round-robin, item i -> CTA i mod grid: every CTA gets the same mix of layers, so the balance needs no cost model
-    // (measured on MobileNet-v2 B=32: 0.28 ms against 0.81 ms for a contiguous cost-balanced partition).
-    // Every role of a CTA walks its whole row up to the first terminator.  The row keeps a second one so that a walk over
-    // alternate items (i = g, g + 2, ..., one per consumer warpgroup) would also meet an end marker inside the row.
-    const int grid = (int)std::min<size_t>(items.size(), (size_t)rt->prop.multiProcessorCount);
-    const size_t stride = (items.size() + grid - 1) / grid + 2;
-    std::vector<uint32_t> sched(stride * grid, kGroupSchedEnd);
-    for (size_t i = 0; i < items.size(); ++i) sched[(i % grid) * stride + i / grid] = items[i];
+    int grid = 0, stride = 0;
+    const std::vector<uint32_t> sched = group_schedule(m_tiles.data(), n_chunks.data(), L, rt->prop.multiProcessorCount, &grid, &stride);
     if (sched.size() > gs.sched_cap) {
         if (gs.d_sched) cudaFree(gs.d_sched);
         gs.d_sched = nullptr;
@@ -477,7 +532,7 @@ static mnnb200_status group_build(GroupState& gs, const std::vector<ConvInt8Exec
     CK(cudaMemcpy(gs.d_params, prm.data(), sizeof(GroupLayerParams) * L, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(gs.d_geom, geo.data(), sizeof(GroupConvGeom) * L, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(gs.d_sched, sched.data(), sched.size() * 4, cudaMemcpyHostToDevice));
-    gs.sched_stride = (int)stride;
+    gs.sched_stride = stride;
     gs.grid = grid;
     gs.n_layers = L;
     return MNNB200_OK;
@@ -950,6 +1005,20 @@ mnnb200_status mnnb200_conv_int8_group_plan(mnnb200_exec* ex, int* fields, int c
     const GroupLayerParams& q = e->plan.q;
     const int v[] = {q.mode, q.cb, q.bn, q.n_chunks, q.m_tiles, q.num_kb, q.K, q.R, q.TWp, e->plan.g.BH};
     for (int i = 0; i < count && i < (int)(sizeof(v) / sizeof(v[0])); ++i) fields[i] = v[i];
+    return MNNB200_OK;
+}
+mnnb200_status mnnb200_conv_group_schedule(const int* m_tiles, const int* n_chunks, int layers, int sm_count, uint32_t* items,
+                                           int capacity, int* grid, int* stride) {
+    if (!m_tiles || !n_chunks || !grid || !stride || layers <= 0 || layers > kGroupMaxLayers || sm_count <= 0 || capacity < 0)
+        return fail(MNNB200_INVALID_VALUE, "conv_group_schedule: bad argument");
+    for (int l = 0; l < layers; ++l)
+        if (m_tiles[l] <= 0 || m_tiles[l] > kGroupMaxMTiles || n_chunks[l] <= 0 || n_chunks[l] > kGroupMaxNChunks)
+            return fail(MNNB200_INVALID_VALUE, "conv_group_schedule: a layer is outside the schedule word's fields");
+    const std::vector<uint32_t> sched = group_schedule(m_tiles, n_chunks, layers, sm_count, grid, stride);
+    if (items) {
+        if ((size_t)capacity < sched.size()) return fail(MNNB200_INVALID_VALUE, "conv_group_schedule: items holds fewer than grid * stride words");
+        std::copy(sched.begin(), sched.end(), items);
+    }
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_conv_group_create(mnnb200_runtime* rt, mnnb200_exec* const* members, int count, mnnb200_exec** out) {

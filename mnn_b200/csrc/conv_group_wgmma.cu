@@ -2,8 +2,8 @@
 //
 // One launch per 1x1 convolution pays the launch -> barrier init -> cold TMA -> epilogue -> teardown chain for a few MB of
 // traffic per layer.  Here the per-layer state (TMA descriptors + epilogue constants) lives in a device-side layer table
-// and the tiles of ALL layers form one host-built schedule dealt round-robin to the CTAs (every CTA, one per SM, gets the
-// same mix of layers), so barriers are set up once per step, the TMA producer runs ahead across layer boundaries (the next
+// and the tiles of ALL layers form one host-built schedule that gives every CTA, one per SM, an equal share of every layer's
+// tiles in list order (group_schedule, capi.cu), so barriers are set up once per step, the TMA producer runs ahead across layer boundaries (the next
 // layer's operands are already in flight while the current tile's epilogue drains) and there is no per-layer tail.
 //
 // Replaces (structure) the per-op Execution::onExecute walk of Pipeline::execute (source/core/Pipeline.cpp:1069-1140)
@@ -18,10 +18,10 @@
 // zero point is not 0, put back in the epilogue as z_in * sum_{OOB taps} w from a small per-border-class table.
 //
 // Weight tiles are CACHED in shared memory across work items (4 slots tagged (layer, n chunk, K block) + a 36 KB resident set
-// for layers whose K blocks all fit): with round-robin scheduling all CTAs work on the same layer at the same time, and
+// for layers whose K blocks all fit): the schedule keeps all CTAs on the same layer at the same time, and
 // re-fetching the same few weight lines for every item from every SM serialises in L2.
 //
-//   warps 8-11: producer warpgroup (setmaxnreg.dec); one thread issues the TMA loads (cp.async.bulk.tensor.2d/4d, 128B / 64B swizzle or 16-byte interleaved chunks, 6-stage ring of
+//   warps 8-11: producer warpgroup (setmaxnreg.dec); one thread issues the TMA loads (cp.async.bulk.tensor.2d/4d, 128B / 64B / 32B swizzle or 16-byte interleaved chunks, 6-stage ring of
 //              16 KB activation tiles)
 //   warps 0-7: two consumer warpgroups, 64 rows of the 128-row tile each: wgmma.mma_async m64nNk32 s8 (N = bn <= 128,
 //              accumulators in registers; the per-run work is instantiated per bn, see consume_run) -> CPU-exact requant
@@ -59,7 +59,9 @@ constexpr int kOffLayers = kOffConsts + 2 * kConstBytes;
 constexpr int kOffRbTab = kOffLayers + kGroupMaxLayers * (int)sizeof(GroupLayerParams);   // producer: [3][16] row-box coordinates
 constexpr int kOffBSlot = kOffRbTab + 3 * 16 * 4;                                          // [kStages] weight slot of the block in each stage
 constexpr int kOffBars = kOffBSlot + 32;                                                   // (kStages ints, padded)
-constexpr int kSmemTotal = kOffBars + 256;
+constexpr int kOffSched = kOffBars + 256;                                                  // the CTA's schedule row
+constexpr int kSchedSmemWords = 512;
+constexpr int kSmemTotal = kOffSched + kSchedSmemWords * 4;
 static_assert(kSmemTotal + 1024 <= 227 * 1024, "conv group kernel: shared memory plan does not fit");
 static_assert(sizeof(GroupLayerParams) % 16 == 0, "layer params are copied with 16-byte loads");
 // Two consumer warpgroups and a producer WARPGROUP (warps 8-11, one thread of warp 8 issues the TMA loads).  With nine warps
@@ -190,7 +192,8 @@ __device__ __forceinline__ void consume_run(const GroupLayerParams& lp, const Gr
         const uint32_t b_addr = base + kOffB + (uint32_t)(*reinterpret_cast<const volatile int*>(smem + kOffBSlot + 4 * stage));
         // every K block runs its full count of k-steps in one straight run: a condition per k-step would make ptxas
         // serialise the wgmmas.  Past the end of a layer's K the weight tile holds zeros from the TMA unit (out-of-bounds
-        // fill), so those k-steps add nothing.
+        // fill), so those k-steps add nothing.  A mode-0 layer's K block is as narrow as its K allows (conv_plan): 64 bytes are
+        // two k-steps, 32 bytes one.
         if (cb == 128) {
 #pragma unroll
             for (int k = 0; k < 4; ++k)
@@ -200,6 +203,8 @@ __device__ __forceinline__ void consume_run(const GroupLayerParams& lp, const Gr
             for (int k = 0; k < 2; ++k)
                 wgmma_span<Kind::S8, BN, 0>(a, gdesc(a_addr + wg * 64 * 64 + k * 32, kSw64, 16, 512),
                                             gdesc(b_addr + k * 32, kSw64, 16, 512), 64, k ? 1 : scale0);
+        } else if (cb == 32) {
+            wgmma_span<Kind::S8, BN, 0>(a, gdesc(a_addr + wg * 64 * 32, kSw32, 16, 256), gdesc(b_addr, kSw32, 16, 256), 32, scale0);
         } else {
 #pragma unroll
             for (int u = 0; u < 4; ++u)
@@ -410,7 +415,15 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
     auto full_bar = [&](int s) { return bar0 + 8u * s; };
     auto empty_bar = [&](int s) { return bar0 + 8u * (kStages + s); };
     const GroupLayerParams* sl = reinterpret_cast<const GroupLayerParams*>(smem + kOffLayers);
-    const uint32_t* my = sched + (size_t)blockIdx.x * sched_stride;
+    // every role reads its schedule row item by item, two dependent loads per tile in the consumers: a row that fits is read
+    // from shared memory (contiguous multi-tile items keep rows to a few words per layer), a longer one from global memory
+    const uint32_t* grow = sched + (size_t)blockIdx.x * sched_stride;
+    const bool fits = sched_stride <= kSchedSmemWords;
+    if (fits) {
+        uint32_t* row = reinterpret_cast<uint32_t*>(smem + kOffSched);
+        for (int i = threadIdx.x; i < sched_stride; i += kCgThreads) row[i] = grow[i];
+    }
+    const uint32_t* const my = fits ? reinterpret_cast<const uint32_t*>(smem + kOffSched) : grow;
 
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
@@ -486,7 +499,8 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                 const void* ta = &mp.a[L];
                 const void* tb = &mp.b[L];
                 if (lp.mode == 0) {
-                    const int num_kb = lp.num_kb, bn = lp.bn;
+                    const int num_kb = lp.num_kb, cb = lp.cb, brow = nc * lp.bn;
+                    const uint32_t a_bytes = (uint32_t)(kBM * cb), b_bytes = (uint32_t)(lp.bn * cb);
                     const uint32_t key0 = ((uint32_t)L << 16) | ((uint32_t)nc << 8);
                     for (int t = 0; t < cnt; ++t) {
                         const int row0 = (mt0 + t) * kBM;
@@ -495,10 +509,10 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
                             bool miss;
                             const int bs = b_lookup(key0 | (uint32_t)kb, &miss);
                             stage_bslot[stage] = bs;
-                            mbar_expect_tx(full_bar(stage), (uint32_t)(kStageA + (miss ? bn * kBK : 0)));
+                            mbar_expect_tx(full_bar(stage), a_bytes + (miss ? b_bytes : 0u));
                             const uint32_t a_dst = base + stage * kStageBytes;
-                            tma_load_2d(a_dst, ta, full_bar(stage), kb * kBK, row0);
-                            if (miss) tma_load_2d(base + kOffB + bs, tb, full_bar(stage), kb * kBK, nc * bn);
+                            tma_load_2d(a_dst, ta, full_bar(stage), kb * cb, row0);
+                            if (miss) tma_load_2d(base + kOffB + bs, tb, full_bar(stage), kb * cb, brow);
                             if (++stage == kStages) { stage = 0; phase ^= 1; }
                             ++blk;
                         }

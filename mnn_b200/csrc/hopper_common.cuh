@@ -100,7 +100,7 @@ __device__ __forceinline__ void pdl_wait() {
 // K-major shared-memory matrix descriptor of wgmma: [0,14) start >> 4 | [16,30) LBO >> 4 | [32,46) SBO >> 4 | [62,64) layout.
 // layout 1 = 128B swizzle (SBO 1024 between 8-row groups), 2 = 64B swizzle (SBO 512), 0 = no swizzle: 8 x 16 B core
 // matrices, LBO = distance of the two 16-byte K halves, SBO = distance of 8-row groups.
-enum : uint32_t { kSwNone = 0, kSw128 = 1, kSw64 = 2 };
+enum : uint32_t { kSwNone = 0, kSw128 = 1, kSw64 = 2, kSw32 = 3 };
 __device__ __forceinline__ uint64_t gdesc(uint32_t smem_addr, uint32_t layout, uint32_t lbo, uint32_t sbo) {
     return (uint64_t)((smem_addr & 0x3FFFF) >> 4) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) |
            ((uint64_t)((sbo >> 4) & 0x3FFF) << 32) | ((uint64_t)layout << 62);

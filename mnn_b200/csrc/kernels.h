@@ -106,7 +106,7 @@ struct GroupLayerParams {            // copied to shared memory by every CTA
     int n_chunks, m_tiles, num_kb, OC;
     int ldy;
     float scale_x, minv, maxv;
-    int mode, cb, TWp, R;            // cb: bytes of K per TMA chunk (128 / 64 / 16); mode 1: R boxes of BH rows x TWp pixels per M tile
+    int mode, cb, TWp, R;            // cb: bytes of K per TMA chunk (128 / 64 / 16, mode 0 also 32); mode 1: R boxes of BH rows x TWp pixels per M tile
 };
 struct GroupConvGeom {               // mode 1 only; stays in global memory (read once per tile)
     int KH, KW, Cp, NB;
@@ -122,8 +122,8 @@ struct GroupConvGeom {               // mode 1 only; stays in global memory (rea
     int wc_count, interior_cls;
 };
 // schedule: grid rows of sched_stride items, each row ends with kGroupSchedEnd.  item = layer << 26 | n chunk << 20 |
-// (tiles - 1) << 14 | first m tile; the host puts one M tile in every item (tile count field 0).  A layer whose n chunks or
-// M tiles these fields cannot hold is not taken by the conv-group kernel.
+// (tiles - 1) << 14 | first m tile: `tiles` consecutive M tiles of one (layer, n chunk) (group_schedule, capi.cu).  A layer
+// whose n chunks or M tiles these fields cannot hold is not taken by the conv-group kernel.
 constexpr int kGroupItemLayerShift = 26, kGroupItemChunkShift = 20, kGroupItemCountShift = 14;
 constexpr uint32_t kGroupItemChunkMask = 0x3fu, kGroupItemCountMask = 0x3fu, kGroupItemTileMask = 0x3fffu;
 constexpr int kGroupMaxNChunks = 63, kGroupMaxMTiles = 16383;

@@ -1,6 +1,6 @@
 """Cost of one work item of the persistent conv-group launch (conv_group_wgmma.cu), per CTA: single-layer groups of a 1x1 int8
 conv at M = 32 x 112 x 112 rows (about 24 items of 128 rows per CTA on a 132-SM part), swept over the tile width (OC at
-K = 16) and over K (at OC = 32).  Each configuration is one group launch captured in a CUDA graph and replayed back to back;
+K = 16) and over K (at OC = 32), plus the shallow 1x1 shapes of MobileNet-v2's first blocks.  Each configuration is one group launch captured in a CUDA graph and replayed back to back;
 the time is the median of several windows.  Cycles use the SM clock read while the replays run.  Next to each: the
 algorithmic bytes (input + output activations, weights) and the time they take at the data-sheet HBM bandwidth.
 Usage (on the GPU): python tools/group_item_costs.py > item_costs.json"""
@@ -19,6 +19,7 @@ PEAK_GBS = 3350.0     # H100 SXM data-sheet HBM3 bandwidth
 N, H, W = 32, 112, 112
 SWEEP_OC = [(16, oc) for oc in (16, 32, 64, 96, 128)]          # (K, OC)
 SWEEP_K = [(k, 32) for k in (16, 64, 128, 256, 576)]
+SHALLOW = [(16, 16), (32, 16), (16, 96), (32, 144)]
 
 
 def smi(query):
@@ -87,7 +88,8 @@ def main():
     with torch.cuda.stream(stream):
         backend = Runtime(torch.cuda.current_device()).onCreate()
     rows = {"oc_at_k16": [measure(backend, stream, k, oc) for k, oc in SWEEP_OC],
-            "k_at_oc32": [measure(backend, stream, k, oc) for k, oc in SWEEP_K]}
+            "k_at_oc32": [measure(backend, stream, k, oc) for k, oc in SWEEP_K],
+            "shallow_1x1": [measure(backend, stream, k, oc) for k, oc in SHALLOW]}
     print(json.dumps({"device": torch.cuda.get_device_name(), "power_limit_w": smi("power.limit"),
                       "sm_count": backend.runtime.sm_count, "M": N * H * W, **rows}, indent=1))
 
