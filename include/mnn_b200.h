@@ -169,7 +169,8 @@ MNNB200_API mnnb200_status mnnb200_reduce_f32(mnnb200_runtime* rt, const float* 
  *      bind:   after every member's resize; xs[i] / ys[i] = member i's NHWC16 input / output (must not alias another
  *              member's output: members are NOT ordered against each other).  NOT_SUPPORT if the conv-group kernel does
  *              not take a member (mnnb200_conv_int8_group_plan says which).
- *      execute: enqueue the one launch on the runtime's stream. */
+ *      execute: enqueue the one launch on the runtime's stream.  NO_EXECUTION until bound, and again once a member has been
+ *              resized since the last bind: bind again first. */
 MNNB200_API mnnb200_status mnnb200_conv_group_create(mnnb200_runtime* rt, mnnb200_exec* const* members, int count,
                                                      mnnb200_exec** out);
 MNNB200_API mnnb200_status mnnb200_conv_group_bind(mnnb200_exec* group, const int8_t* const* xs, int8_t* const* ys);

@@ -13,6 +13,7 @@
 #include <cmath>
 #include <cstdio>
 #include <cstring>
+#include <memory>
 #include <mutex>
 #include <string>
 #include <vector>
@@ -53,48 +54,86 @@ struct mnnb200_graph {
     cudaGraphExec_t exec = nullptr;
 };
 
-struct mnnb200_exec {
-    mnnb200_runtime* rt = nullptr;
-    int kind = 0;  // 1 conv, 2 depthwise, 3 linear
-    int variant = 0;  // mnnb200_conv_int8_set_variant: 0 auto, 1 mma.sync implicit GEMM (conv), 2 wgmma, 3 CTA pair, 4 GEMV (linear)
-    double cost_bytes = 0, cost_macs = 0;
-    std::vector<void*> dev_bufs;  // everything freed at destroy
-    virtual ~mnnb200_exec() {
-        for (void* p : dev_bufs)
-            if (p) cudaFree(p);
-    }
-    // grow-only scratch owned by the execution: the previous buffer is released (cudaFree waits for the device, so kernels still
-    // reading it have finished) and replaced in dev_bufs -- repeated resizes do not accumulate device memory
-    mnnb200_status grow_scratch(void** slot, size_t* cap, size_t bytes) {
-        if (bytes <= *cap && *slot) return MNNB200_OK;
+// One device allocation, owned by the execution (or conv group) that holds it and freed with it.  Zero elements allocate 16
+// bytes, so every buffer has an address.  It converts to T* where a kernel's parameter block takes the pointer.
+template <class T>
+class DevBuf {
+  public:
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete;
+    DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { reset(); }
+    operator T*() const { return p_; }
+    // grow-only: a new allocation only when n elements do not fit.  The old one is released then (cudaFree waits for the
+    // device, so kernels still reading it have finished): repeated resizes do not accumulate device memory.
+    mnnb200_status reserve(size_t n) {
+        if (p_ && n <= cap_) return MNNB200_OK;
         void* q = nullptr;
-        CK(cudaMalloc(&q, bytes ? bytes : 16));
-        if (*slot) {
-            for (auto& b : dev_bufs)
-                if (b == *slot) b = nullptr;
-            cudaFree(*slot);
-        }
-        dev_bufs.push_back(q);
-        *slot = q;
-        *cap = bytes;
+        CK(cudaMalloc(&q, n ? n * sizeof(T) : 16));
+        reset();
+        p_ = static_cast<T*>(q);
+        cap_ = n;
         return MNNB200_OK;
     }
-    template <class T>
-    mnnb200_status upload(const std::vector<T>& h, T** d) {
-        size_t bytes = h.size() * sizeof(T);
-        CK(cudaMalloc((void**)d, bytes ? bytes : 16));
-        dev_bufs.push_back(*d);
-        if (bytes) CK(cudaMemcpyAsync(*d, h.data(), bytes, cudaMemcpyHostToDevice, rt->stream));
-        CK(cudaStreamSynchronize(rt->stream));  // h may be a temporary
+    // reserve(h.size()), then copy h to the front of the buffer and wait for the copy: h may be a temporary
+    mnnb200_status upload(const std::vector<T>& h, cudaStream_t s) {
+        if (mnnb200_status st = reserve(h.size())) return st;
+        if (!h.empty()) CK(cudaMemcpyAsync(p_, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, s));
+        CK(cudaStreamSynchronize(s));
         return MNNB200_OK;
     }
-    template <class T>
-    mnnb200_status update(const std::vector<T>& h, T* d) {
-        CK(cudaMemcpyAsync(d, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, rt->stream));
-        CK(cudaStreamSynchronize(rt->stream));
-        return MNNB200_OK;
+    void reset() {
+        if (p_) cudaFree(p_);
+        p_ = nullptr;
+        cap_ = 0;
     }
+
+  private:
+    T* p_ = nullptr;
+    size_t cap_ = 0;
 };
+
+// The execution types, one bit each: a handle is tested against the types an entry point takes before it is cast (exec_as).
+enum ExecType : unsigned {
+    kConvInt8 = 1u << 0, kDwConvInt8 = 1u << 1, kLinearW8 = 1u << 2, kWinoInt8 = 1u << 3, kMatMul = 1u << 4,
+    kConvGroup = 1u << 5, kScaleInt8 = 1u << 6, kConvF32 = 1u << 7, kDwConvF32 = 1u << 8, kScaleF32 = 1u << 9,
+};
+struct mnnb200_exec {
+    unsigned type = 0;  // the ExecType of the struct new_exec made
+    mnnb200_runtime* rt = nullptr;
+    int variant = 0;  // mnnb200_conv_int8_set_variant: 0 auto, 1 mma.sync implicit GEMM (conv), 2 wgmma, 3 CTA pair, 4 GEMV (linear)
+    bool resized = false;
+    double cost_bytes = 0, cost_macs = 0;
+    virtual ~mnnb200_exec() = default;
+};
+// The five convolutions: the descriptor that set_pad edits.
+struct ConvExec : mnnb200_exec {
+    mnnb200_conv_desc d;
+};
+// An execution struct derives from Tagged<its ExecType, its base>.
+template <unsigned Type, class Base = mnnb200_exec>
+struct Tagged : Base {
+    static constexpr unsigned kTypes = Type;
+};
+template <class T>
+static std::unique_ptr<T> new_exec(mnnb200_runtime* rt) {
+    auto e = std::make_unique<T>();
+    e->type = T::kTypes;
+    e->rt = rt;
+    return e;
+}
+// The handle as a T, or null for a NULL handle or a handle of a type outside `types`.  A tag compare rather than
+// dynamic_cast: nothing depends on RTTI across the library's hidden symbols.
+template <class T>
+static T* exec_as(mnnb200_exec* ex, unsigned types = T::kTypes) {
+    return ex && (ex->type & types) ? static_cast<T*>(ex) : nullptr;
+}
+// a plan query: the first `count` (at most N) of the plan's fields go to `fields`
+template <size_t N>
+static mnnb200_status copy_fields(const int (&v)[N], int* fields, int count) {
+    for (int i = 0; i < count && i < (int)N; ++i) fields[i] = v[i];
+    return MNNB200_OK;
+}
 
 // ---- TMA descriptors (driver entry point fetched through the runtime: no link-time libcuda dependency)
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
@@ -155,6 +194,21 @@ static int pick_bn(int n_padded, int m_tiles = 1 << 30, int sm_count = 1, int ma
 }
 
 static inline int conv_out(int i, int k, int s, int p, int d) { return (i + 2 * p - (d * (k - 1) + 1)) / s + 1; }
+// A conv resize's output size.  MNN's shape inference owns it (SAME padding pads more at the end than at the beginning): a
+// caller that knows it passes it in through *oh / *ow (> 0), pad_h / pad_w being the BEGIN pads; otherwise the descriptor
+// gives it.  done() writes it back once the resize has succeeded.
+struct ConvOutSize {
+    int *oh, *ow;
+    int H, W;
+    ConvOutSize(const mnnb200_conv_desc& d, int ih, int iw, int* oh, int* ow)
+        : oh(oh), ow(ow), H(oh && *oh > 0 ? *oh : conv_out(ih, d.kh, d.stride_h, d.pad_h, d.dilate_h)),
+          W(ow && *ow > 0 ? *ow : conv_out(iw, d.kw, d.stride_w, d.pad_w, d.dilate_w)) {}
+    mnnb200_status done() const {
+        if (oh) *oh = H;
+        if (ow) *ow = W;
+        return MNNB200_OK;
+    }
+};
 
 // =================================================================================================
 // Int8 Conv2D
@@ -183,8 +237,7 @@ static ConvPath conv_path(const ConvPlan& c, int variant) {
     return variant == 0 ? ConvPath::MmaSync : ConvPath::Refused;
 }
 
-struct ConvInt8Exec : mnnb200_exec {
-    mnnb200_conv_desc d;
+struct ConvInt8Exec : Tagged<kConvInt8, ConvExec> {
     bool legacy = false;
     int Cp = 0, OCp = 0, kernel_len = 0;
     std::vector<float> h_wscale, h_bias;   // modern: alpha + float bias; legacy: fused scale
@@ -192,21 +245,19 @@ struct ConvInt8Exec : mnnb200_exec {
     std::vector<int32_t> h_isum;           // sum_k w[oc][k]
     std::vector<int32_t> h_tapsum;         // [OCp][taps] sum_c w[oc][tap][c]: padding correction of the implicit-GEMM kernel
     ConvPlan plan;
-    int32_t* d_border = nullptr;           // border-class tables of plan.g, grow-only
-    size_t border_cap = 0;
-    struct GroupState* solo = nullptr;     // this layer alone on the conv-group kernel
+    unsigned resizes = 0;                  // resizes that passed their checks: a group built before the last one is stale
+    DevBuf<int32_t> d_border;              // border-class tables of plan.g, grow-only
+    std::unique_ptr<struct GroupState> solo;   // this layer alone on the conv-group kernel
     const void* solo_x = nullptr;
     const void* solo_y = nullptr;
     ~ConvInt8Exec() override;
-    int8_t* d_w = nullptr;
-    int8_t* d_wg = nullptr;                // the conv-group kernel's copy: [n_chunks * bn][taps * Cp], rows permuted per chunk
-    float* d_ep = nullptr;                 // its epilogue table (GroupLayerParams::ep), grow-only
-    size_t ep_cap = 0;
-    float *d_wscale = nullptr, *d_bias = nullptr;
-    int32_t* d_wsum128 = nullptr;
+    DevBuf<int8_t> d_w;
+    DevBuf<int8_t> d_wg;                   // the conv-group kernel's copy: [n_chunks * bn][taps * Cp], rows permuted per chunk
+    DevBuf<float> d_ep;                    // its epilogue table (GroupLayerParams::ep), grow-only
+    DevBuf<float> d_wscale, d_bias;
+    DevBuf<int32_t> d_wsum128;
     ConvParams p;
     int tile = TILE_128x64;
-    bool resized = false;
 };
 
 // the conv-group kernel's tile width for OCp output channels: equal n chunks of at most kGroupMaxBN columns
@@ -215,10 +266,7 @@ static int group_bn(int OCp) {
     return ((OCp + chunks - 1) / chunks + 15) & ~15;
 }
 
-static mnnb200_status conv_create_common(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const int8_t* weight,
-                                         ConvInt8Exec* e) {
-    e->rt = rt;
-    e->kind = 1;
+static mnnb200_status conv_create_common(const mnnb200_conv_desc* desc, const int8_t* weight, ConvInt8Exec* e) {
     e->d = *desc;
     const auto& d = e->d;
     if (d.group != 1) return fail(MNNB200_NOT_SUPPORT, "conv_int8: group != 1 (use dwconv for depthwise)");
@@ -244,7 +292,8 @@ static mnnb200_status conv_create_common(mnnb200_runtime* rt, const mnnb200_conv
             }
         e->h_isum[o] = s;
     }
-    mnnb200_status st = e->upload(wp, &e->d_w);
+    const cudaStream_t s = e->rt->stream;
+    mnnb200_status st = e->d_w.upload(wp, s);
     if (st) return st;
     {   // the conv-group kernel's weights: GEMM column c of chunk nc is channel nc * bn + group_column_channel(c, bn)
         const int bn = group_bn(e->OCp), n_chunks = (e->OCp + bn - 1) / bn;
@@ -255,33 +304,33 @@ static mnnb200_status conv_create_common(mnnb200_runtime* rt, const mnnb200_conv
                 const int o = nc * bn + group_column_channel(c, bn);
                 if (o < e->OCp) memcpy(&wg[((size_t)nc * bn + c) * row], &wp[(size_t)o * row], row);
             }
-        if ((st = e->upload(wg, &e->d_wg))) return st;
+        if ((st = e->d_wg.upload(wg, s))) return st;
     }
     std::vector<float> z(e->OCp, 0.f);
     std::vector<int32_t> zi(e->OCp, 0);
-    if ((st = e->upload(z, &e->d_wscale))) return st;
-    if ((st = e->upload(z, &e->d_bias))) return st;
-    if ((st = e->upload(zi, &e->d_wsum128))) return st;
+    if ((st = e->d_wscale.upload(z, s)) || (st = e->d_bias.upload(z, s)) || (st = e->d_wsum128.upload(zi, s))) return st;
     return MNNB200_OK;
 }
 
 // ---- conv group: one persistent launch over a list of convolutions (conv_group_wgmma.cu) ----------------------------
 struct GroupState {
-    mnnb200_runtime* rt = nullptr;
-    GroupMapsParam* h_maps = nullptr;       // host: passed by value as the kernel's __grid_constant__ parameter
-    GroupLayerParams* d_params = nullptr;
-    GroupConvGeom* d_geom = nullptr;
-    uint32_t* d_sched = nullptr;
-    size_t sched_cap = 0;
+    std::vector<ConvInt8Exec*> members;
+    std::vector<unsigned> built_resizes;    // each member's resize count at the last successful build; empty: not built
+    std::unique_ptr<GroupMapsParam> h_maps; // host: passed by value as the kernel's __grid_constant__ parameter
+    DevBuf<GroupLayerParams> d_params;
+    DevBuf<GroupConvGeom> d_geom;
+    DevBuf<uint32_t> d_sched;               // grow-only
     int n_layers = 0, sched_stride = 0, grid = 0;
-    ~GroupState() {
-        delete h_maps;
-        if (d_params) cudaFree(d_params);
-        if (d_geom) cudaFree(d_geom);
-        if (d_sched) cudaFree(d_sched);
+    // Built, and no member resized since: a resize rebuilds the epilogue and border tables the layer table points at (and
+    // may free them) and changes the layer's geometry.
+    bool current() const {
+        if (built_resizes.size() != members.size()) return false;
+        for (size_t l = 0; l < members.size(); ++l)
+            if (members[l]->resizes != built_resizes[l]) return false;
+        return true;
     }
 };
-ConvInt8Exec::~ConvInt8Exec() { delete solo; }
+ConvInt8Exec::~ConvInt8Exec() = default;
 
 // Builds the conv's plan: which kernels take it and, for the conv-group kernel, its layer without the x / y pointers.  Every
 // limit of that kernel and of its schedule word is checked here; a layer outside them is not taken (plan.group = false).
@@ -354,8 +403,7 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin, const std::vector<floa
                 const int32_t pre = (int32_t)((uint32_t)k128[o] + (uint32_t)magic);
                 memcpy(&row[2 * q.bn + c], &pre, 4);
             }
-        if ((st = e->grow_scratch((void**)&e->d_ep, &e->ep_cap, ep.size() * 4))) return st;
-        if ((st = e->update(ep, e->d_ep))) return st;
+        if ((st = e->d_ep.upload(ep, e->rt->stream))) return st;
         q.ep = e->d_ep;
     }
     // padding correction (input zero point != 0): the reference fills padded taps with z_in (ConvInt8TiledExecutor.cpp:2269-2271),
@@ -405,8 +453,7 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin, const std::vector<floa
                 }
             memcpy(tab.data() + ncorr, hc.data(), p.OH);
             memcpy((uint8_t*)(tab.data() + ncorr) + p.OH, wc.data(), p.OW);
-            if ((st = e->grow_scratch((void**)&e->d_border, &e->border_cap, tab.size() * 4))) return st;
-            if ((st = e->update(tab, e->d_border))) return st;
+            if ((st = e->d_border.upload(tab, e->rt->stream))) return st;
             g.corr = e->d_border;
             g.hcls = (const uint8_t*)(e->d_border + ncorr);
             g.wcls = g.hcls + p.OH;
@@ -473,24 +520,23 @@ static std::vector<uint32_t> group_schedule(const int* m_tiles, const int* n_chu
     return sched;
 }
 
-// Binds planned convs to their activations: the A tensor maps, the y pointers and the schedule.
-static mnnb200_status group_build(GroupState& gs, const std::vector<ConvInt8Exec*>& members, const int8_t* const* xs,
-                                  int8_t* const* ys, double* cost_bytes, double* cost_macs) {
-    mnnb200_runtime* rt = gs.rt;
-    const int L = (int)members.size();
+// Binds the members' plans to their activations: the A tensor maps, the y pointers and the schedule.
+static mnnb200_status group_build(GroupState& gs, mnnb200_runtime* rt, const int8_t* const* xs, int8_t* const* ys,
+                                  double* cost_bytes, double* cost_macs) {
+    const int L = (int)gs.members.size();
+    gs.built_resizes.clear();
     CK(cudaSetDevice(rt->device));
-    if (!gs.h_maps) { gs.h_maps = new GroupMapsParam; memset(gs.h_maps, 0, sizeof(GroupMapsParam)); }
-    if (!gs.d_params) CK(cudaMalloc((void**)&gs.d_params, sizeof(GroupLayerParams) * kGroupMaxLayers));
-    if (!gs.d_geom) CK(cudaMalloc((void**)&gs.d_geom, sizeof(GroupConvGeom) * kGroupMaxLayers));
+    if (!gs.h_maps) gs.h_maps = std::make_unique<GroupMapsParam>();
+    mnnb200_status st;
+    if ((st = gs.d_params.reserve(kGroupMaxLayers)) || (st = gs.d_geom.reserve(kGroupMaxLayers))) return st;
     static_assert(sizeof(CUtensorMap) == sizeof(CUtensorMap_st_opaque), "tensor map size");
     std::vector<GroupLayerParams> prm(L);
     std::vector<GroupConvGeom> geo(L);
     std::vector<int> m_tiles(L), n_chunks(L);
     if (cost_bytes) *cost_bytes = 0;
     if (cost_macs) *cost_macs = 0;
-    mnnb200_status st;
     for (int l = 0; l < L; ++l) {
-        const ConvInt8Exec* e = members[l];
+        const ConvInt8Exec* e = gs.members[l];
         if (!e->resized || !e->plan.group) return fail(MNNB200_NOT_SUPPORT, "conv group: a member is not a resized conv the wgmma group kernel takes");
         const ConvParams& p = e->p;
         const GroupLayerParams& q = e->plan.q;
@@ -523,22 +569,18 @@ static mnnb200_status group_build(GroupState& gs, const std::vector<ConvInt8Exec
     }
     int grid = 0, stride = 0;
     const std::vector<uint32_t> sched = group_schedule(m_tiles.data(), n_chunks.data(), L, rt->prop.multiProcessorCount, &grid, &stride);
-    if (sched.size() > gs.sched_cap) {
-        if (gs.d_sched) cudaFree(gs.d_sched);
-        gs.d_sched = nullptr;
-        CK(cudaMalloc((void**)&gs.d_sched, sched.size() * 4));
-        gs.sched_cap = sched.size();
-    }
+    if ((st = gs.d_sched.reserve(sched.size()))) return st;
     CK(cudaMemcpy(gs.d_params, prm.data(), sizeof(GroupLayerParams) * L, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(gs.d_geom, geo.data(), sizeof(GroupConvGeom) * L, cudaMemcpyHostToDevice));
     CK(cudaMemcpy(gs.d_sched, sched.data(), sched.size() * 4, cudaMemcpyHostToDevice));
     gs.sched_stride = stride;
     gs.grid = grid;
     gs.n_layers = L;
+    for (const ConvInt8Exec* e : gs.members) gs.built_resizes.push_back(e->resizes);
     return MNNB200_OK;
 }
-static mnnb200_status group_launch(const GroupState& gs) {
-    CK(launch_conv_group(gs.h_maps, gs.d_params, gs.d_geom, gs.n_layers, gs.d_sched, gs.sched_stride, gs.grid, gs.rt->stream));
+static mnnb200_status group_launch(const GroupState& gs, cudaStream_t stream) {
+    CK(launch_conv_group(gs.h_maps.get(), gs.d_params, gs.d_geom, gs.n_layers, gs.d_sched, gs.sched_stride, gs.grid, stream));
     return MNNB200_OK;
 }
 
@@ -592,10 +634,12 @@ void mnnb200_runtime_destroy(mnnb200_runtime* rt) {
 }
 void* mnnb200_runtime_stream(mnnb200_runtime* rt) { return rt ? (void*)rt->stream : nullptr; }
 mnnb200_status mnnb200_runtime_sync(mnnb200_runtime* rt) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "runtime_sync: NULL runtime");
     CK(cudaStreamSynchronize(rt->stream));
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_runtime_info(mnnb200_runtime* rt, int* sm_count, int* cc_major, int* cc_minor, size_t* total_mem) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "runtime_info: NULL runtime");
     if (sm_count) *sm_count = rt->prop.multiProcessorCount;
     if (cc_major) *cc_major = rt->prop.major;
     if (cc_minor) *cc_minor = rt->prop.minor;
@@ -603,20 +647,23 @@ mnnb200_status mnnb200_runtime_info(mnnb200_runtime* rt, int* sm_count, int* cc_
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_alloc(mnnb200_runtime* rt, size_t bytes, void** dev_ptr) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "alloc: NULL runtime");
     CK(cudaSetDevice(rt->device));
     CK(cudaMalloc(dev_ptr, bytes ? bytes : 16));
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_free(mnnb200_runtime* rt, void* dev_ptr) {
-    (void)rt;
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "free: NULL runtime");
     CK(cudaFree(dev_ptr));
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_memcpy_h2d(mnnb200_runtime* rt, void* dst, const void* src, size_t bytes) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "memcpy_h2d: NULL runtime");
     CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyHostToDevice, rt->stream));
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_memcpy_d2h(mnnb200_runtime* rt, void* dst, const void* src, size_t bytes) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "memcpy_d2h: NULL runtime");
     CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToHost, rt->stream));
     return MNNB200_OK;
 }
@@ -666,7 +713,7 @@ mnnb200_status mnnb200_host_register(mnnb200_runtime* rt, void* p, size_t bytes)
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_host_unregister(mnnb200_runtime* rt, void* p) {
-    (void)rt;
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "host_unregister: NULL runtime");
     cudaError_t e = cudaHostUnregister(p);
     if (e != cudaSuccess) { cudaGetLastError(); return fail(MNNB200_INVALID_VALUE, std::string("cudaHostUnregister: ") + cudaGetErrorString(e)); }
     return MNNB200_OK;
@@ -678,7 +725,7 @@ mnnb200_status mnnb200_alloc_host(mnnb200_runtime* rt, size_t bytes, void** p) {
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_free_host(mnnb200_runtime* rt, void* p) {
-    (void)rt;
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "free_host: NULL runtime");
     CK(cudaFreeHost(p));
     return MNNB200_OK;
 }
@@ -708,20 +755,24 @@ float mnnb200_runtime_last_gpu_ms(mnnb200_runtime* rt) {
 // ---- casts ---------------------------------------------------------------------------------------
 mnnb200_status mnnb200_float_to_int8(mnnb200_runtime* rt, const float* x, int n, int c, int h, int w, float scale,
                                      float zero, int min_v, int max_v, int8_t* y) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "float_to_int8: NULL runtime");
     float inv = scale == 0.f ? 0.f : 1.f / scale;  // CPUCast.cpp:24
     CK(launch_float_to_int8(x, n, c, h, w, inv, zero, (float)min_v, (float)max_v, y, rt->stream));
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_int8_to_float(mnnb200_runtime* rt, const int8_t* x, int n, int c, int h, int w, float scale,
                                      float zero, float* y) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "int8_to_float: NULL runtime");
     CK(launch_int8_to_float(x, n, c, h, w, scale, zero, y, rt->stream));
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_pack_nchw_int8(mnnb200_runtime* rt, const int8_t* x, int n, int c, int h, int w, int8_t* y) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "pack_nchw_int8: NULL runtime");
     CK(launch_pack_nchw_int8(x, n, c, h, w, y, rt->stream));
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_unpack_nchw_int8(mnnb200_runtime* rt, const int8_t* x, int n, int c, int h, int w, int8_t* y) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "unpack_nchw_int8: NULL runtime");
     CK(launch_unpack_nchw_int8(x, n, c, h, w, y, rt->stream));
     return MNNB200_OK;
 }
@@ -730,6 +781,7 @@ mnnb200_status mnnb200_unpack_nchw_int8(mnnb200_runtime* rt, const int8_t* x, in
 mnnb200_status mnnb200_binary_add_int8(mnnb200_runtime* rt, const int8_t* x0, float s0, int z0, const int8_t* x1, float s1,
                                        int z1, int8_t* y, float s_out, int z_out, int min_v, int max_v, int n, int c, int h,
                                        int w) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "binary_add_int8: NULL runtime");
     float inv = s_out != 0 ? 1 / s_out : 0;   // CPUBinaryInt8.cpp:37-41
     CK(launch_binary_add_int8(x0, s0, z0, x1, s1, z1, y, inv, z_out, min_v, max_v, (size_t)n * h * w, c, up16(c), rt->stream));
     return MNNB200_OK;
@@ -737,6 +789,7 @@ mnnb200_status mnnb200_binary_add_int8(mnnb200_runtime* rt, const int8_t* x0, fl
 mnnb200_status mnnb200_avgpool_int8(mnnb200_runtime* rt, const int8_t* x, int n, int c, int ih, int iw, int kh, int kw,
                                     int stride_h, int stride_w, int pad_h, int pad_w, int pad_type, int count_type, float s_in,
                                     float z_in, float s_out, float z_out, int min_v, int max_v, int8_t* y, int oh, int ow) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "avgpool_int8: NULL runtime");
     PoolParams p;
     p.x = x; p.y = y; p.N = n; p.C = c; p.Cp = up16(c); p.IH = ih; p.IW = iw; p.OH = oh; p.OW = ow; p.KH = kh; p.KW = kw;
     p.sh = stride_h; p.sw = stride_w; p.ph = pad_h; p.pw = pad_w;
@@ -749,6 +802,7 @@ mnnb200_status mnnb200_avgpool_int8(mnnb200_runtime* rt, const int8_t* x, int n,
 mnnb200_status mnnb200_pool_f32(mnnb200_runtime* rt, const float* x, int n, int c, int ih, int iw, int kh, int kw, int stride_h,
                                 int stride_w, int pad_h, int pad_w, int pad_type, int count_type, int is_avg, float* y, int oh,
                                 int ow) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "pool_f32: NULL runtime");
     PoolParams p;
     memset(&p, 0, sizeof(p));
     p.N = n; p.C = c; p.Cp = c; p.IH = ih; p.IW = iw; p.OH = oh; p.OW = ow; p.KH = kh; p.KW = kw;
@@ -775,34 +829,34 @@ mnnb200_status mnnb200_transpose_b32(mnnb200_runtime* rt, const void* src, int b
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_memcpy_d2d(mnnb200_runtime* rt, void* dst, const void* src, size_t bytes) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "memcpy_d2d: NULL runtime");
     CK(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, rt->stream));
     return MNNB200_OK;
 }
 // ---- ResNet-50 neighbours: int8 Scale, int8 pooling (equal attrs), float ReLU / Reduction ----------------------------------
-struct ScaleInt8Exec : mnnb200_exec {
+struct ScaleInt8Exec : Tagged<kScaleInt8> {
     int c = 0, cp = 0;
     std::vector<float> h_scale, h_bias;
-    int32_t *d_alpha = nullptr, *d_bias = nullptr;
+    DevBuf<int32_t> d_alpha, d_bias;
     int zin = 0, zout = 0, minv = -127, maxv = 127;
-    bool resized = false;
 };
 mnnb200_status mnnb200_scale_int8_create(mnnb200_runtime* rt, int channels, const float* scale, const float* bias, mnnb200_exec** out) {
     if (!rt || !scale || !out || channels <= 0) return fail(MNNB200_INVALID_VALUE, "scale_int8_create: bad argument");
-    auto* e = new ScaleInt8Exec;
-    e->rt = rt; e->kind = 7; e->c = channels; e->cp = up16(channels);
+    auto e = new_exec<ScaleInt8Exec>(rt);
+    e->c = channels; e->cp = up16(channels);
     e->h_scale.assign(scale, scale + channels);
     e->h_bias.assign(channels, 0.f);
     if (bias) e->h_bias.assign(bias, bias + channels);
     std::vector<int32_t> z(e->cp, 0);
     mnnb200_status st;
-    if ((st = e->upload(z, &e->d_alpha)) || (st = e->upload(z, &e->d_bias))) { delete e; return st; }
-    *out = e;
+    if ((st = e->d_alpha.upload(z, rt->stream)) || (st = e->d_bias.upload(z, rt->stream))) return st;
+    *out = e.release();
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_scale_int8_resize(mnnb200_exec* ex, float in_scale, int in_zero, float out_scale, int out_zero, int clamp_min,
                                          int clamp_max) {
-    if (!ex || ex->kind != 7) return fail(MNNB200_INVALID_VALUE, "scale_int8_resize: not a Scale execution");
-    auto* e = static_cast<ScaleInt8Exec*>(ex);
+    auto* e = exec_as<ScaleInt8Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "scale_int8_resize: not a Scale execution");
     // CPUScaleInt8::onResize (CPUScaleInt8.cpp:60-90): 15-bit fixed point, float products left to right, roundf
     const float inv_out = out_scale == 0.f ? 0.f : 1.f / out_scale;
     std::vector<int32_t> al(e->cp, 0), bi(e->cp, 0);
@@ -816,14 +870,14 @@ mnnb200_status mnnb200_scale_int8_resize(mnnb200_exec* ex, float in_scale, int i
         bi[i] = (int32_t)roundf(b);
     }
     mnnb200_status st;
-    if ((st = e->update(al, e->d_alpha)) || (st = e->update(bi, e->d_bias))) return st;
+    if ((st = e->d_alpha.upload(al, e->rt->stream)) || (st = e->d_bias.upload(bi, e->rt->stream))) return st;
     e->zin = (int)(int8_t)in_zero; e->zout = (int)(int8_t)out_zero; e->minv = clamp_min; e->maxv = clamp_max;
     e->resized = true;
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_scale_int8_execute(mnnb200_exec* ex, const int8_t* x, int n, int h, int w, int8_t* y) {
-    if (!ex || ex->kind != 7) return fail(MNNB200_INVALID_VALUE, "scale_int8_execute: not a Scale execution");
-    auto* e = static_cast<ScaleInt8Exec*>(ex);
+    auto* e = exec_as<ScaleInt8Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "scale_int8_execute: not a Scale execution");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "scale_int8_execute before resize");
     CK(launch_scale_int8(x, y, e->d_alpha, e->d_bias, e->zin, e->zout, e->minv, e->maxv, (size_t)n * h * w, e->c, e->cp, e->rt->stream));
     return MNNB200_OK;
@@ -853,6 +907,7 @@ mnnb200_status mnnb200_reduce_f32(mnnb200_runtime* rt, const float* x, int outsi
 }
 mnnb200_status mnnb200_softmax_int8(mnnb200_runtime* rt, const int8_t* x, int rows, int c, float s_in, float z_in, float s_out,
                                     float z_out, int min_v, int max_v, int8_t* y) {
+    if (!rt) return fail(MNNB200_INVALID_VALUE, "softmax_int8: NULL runtime");
     CK(launch_softmax_int8(x, rows, c, up16(c), s_in, z_in, s_out == 0.f ? 0.f : 1.f / s_out, z_out, (float)min_v, (float)max_v,
                            y, rt->stream));
     return MNNB200_OK;
@@ -862,39 +917,37 @@ mnnb200_status mnnb200_softmax_int8(mnnb200_runtime* rt, const int8_t* x, int ro
 mnnb200_status mnnb200_conv_int8_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const int8_t* weight,
                                         const float* wscale, const float* bias, mnnb200_exec** out) {
     if (!rt || !desc || !weight || !wscale || !out) return fail(MNNB200_INVALID_VALUE, "conv_int8_create: NULL argument");
-    auto* e = new ConvInt8Exec;
-    mnnb200_status st = conv_create_common(rt, desc, weight, e);
-    if (st) { delete e; return st; }
+    auto e = new_exec<ConvInt8Exec>(rt);
+    mnnb200_status st = conv_create_common(desc, weight, e.get());
+    if (st) return st;
     e->legacy = false;
     e->h_wscale.assign(wscale, wscale + desc->oc);
     e->h_bias.assign(desc->oc, 0.f);
     if (bias) e->h_bias.assign(bias, bias + desc->oc);
-    *out = e;
+    *out = e.release();
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_conv_int8_create_legacy(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const int8_t* weight,
                                                const float* scale, const int32_t* bias_i32, mnnb200_exec** out) {
     if (!rt || !desc || !weight || !scale || !out) return fail(MNNB200_INVALID_VALUE, "conv_int8_create_legacy: NULL argument");
-    auto* e = new ConvInt8Exec;
-    mnnb200_status st = conv_create_common(rt, desc, weight, e);
-    if (st) { delete e; return st; }
+    auto e = new_exec<ConvInt8Exec>(rt);
+    mnnb200_status st = conv_create_common(desc, weight, e.get());
+    if (st) return st;
     e->legacy = true;
     e->h_wscale.assign(scale, scale + desc->oc);
     e->h_bias_i32.assign(desc->oc, 0);
     if (bias_i32) e->h_bias_i32.assign(bias_i32, bias_i32 + desc->oc);
-    *out = e;
+    *out = e.release();
     return MNNB200_OK;
 }
 
 mnnb200_status mnnb200_conv_int8_resize(mnnb200_exec* ex, int n, int ih, int iw, float in_scale, int in_zero,
                                         float out_scale, int out_zero, int clamp_min, int clamp_max, int* oh, int* ow) {
-    if (!ex || ex->kind != 1) return fail(MNNB200_INVALID_VALUE, "conv_int8_resize: not a conv execution");
-    auto* e = static_cast<ConvInt8Exec*>(ex);
+    auto* e = exec_as<ConvInt8Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "conv_int8_resize: not a conv execution");
     const auto& d = e->d;
-    // MNN's shape inference owns the output size (SAME padding pads more at the end than at the beginning);
-    // a caller that knows it passes it in through *oh/*ow (> 0), pad_h/pad_w being the BEGIN pads.
-    int OH = (oh && *oh > 0) ? *oh : conv_out(ih, d.kh, d.stride_h, d.pad_h, d.dilate_h);
-    int OW = (ow && *ow > 0) ? *ow : conv_out(iw, d.kw, d.stride_w, d.pad_w, d.dilate_w);
+    const ConvOutSize out(d, ih, iw, oh, ow);
+    const int OH = out.H, OW = out.W;
     if (n <= 0 || OH <= 0 || OW <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "conv_int8_resize: empty output");
     // ---- fold (CPU backend arithmetic; see file header)
     std::vector<float> ws(e->OCp, 0.f), bf(e->OCp, 0.f);
@@ -925,9 +978,9 @@ mnnb200_status mnnb200_conv_int8_resize(mnnb200_exec* ex, int n, int ih, int iw,
     for (int o = 0; o < d.oc; ++o) k128[o] = 128 * e->h_isum[o];
     mnnb200_status st;
     e->resized = false;   // until the new plan is complete
-    if ((st = e->update(ws, e->d_wscale))) return st;
-    if ((st = e->update(bf, e->d_bias))) return st;
-    if ((st = e->update(k128, e->d_wsum128))) return st;
+    ++e->resizes;         // from here on the tables a group built before may point at change, or are freed
+    const cudaStream_t s = e->rt->stream;
+    if ((st = e->d_wscale.upload(ws, s)) || (st = e->d_bias.upload(bf, s)) || (st = e->d_wsum128.upload(k128, s))) return st;
 
     ConvParams& p = e->p;
     memset(&p, 0, sizeof(p));
@@ -947,16 +1000,13 @@ mnnb200_status mnnb200_conv_int8_resize(mnnb200_exec* ex, int n, int ih, int iw,
     e->cost_bytes = (double)n * ih * iw * d.ic + (double)p.M * d.oc + (double)d.oc * d.ic * d.kh * d.kw;
     e->cost_macs = (double)p.M * d.oc * d.ic * d.kh * d.kw;
     if ((st = conv_plan(e, in_zero, ws, bf, k128))) return st;
-    e->solo_x = e->solo_y = nullptr;
     e->resized = true;
-    if (oh) *oh = OH;
-    if (ow) *ow = OW;
-    return MNNB200_OK;
+    return out.done();
 }
 
 mnnb200_status mnnb200_conv_int8_execute(mnnb200_exec* ex, const int8_t* x, int8_t* y) {
-    if (!ex || ex->kind != 1) return fail(MNNB200_INVALID_VALUE, "conv_int8_execute: not a conv execution");
-    auto* e = static_cast<ConvInt8Exec*>(ex);
+    auto* e = exec_as<ConvInt8Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "conv_int8_execute: not a conv execution");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_int8_execute before resize");
     ConvParams p = e->p;
     p.x = x;
@@ -968,17 +1018,16 @@ mnnb200_status mnnb200_conv_int8_execute(mnnb200_exec* ex, const int8_t* x, int8
         CK(launch_conv_int8_stem(p, e->rt->stream));
         return MNNB200_OK;
     case ConvPath::Group:
-        if (!e->solo || e->solo_x != (const void*)x || e->solo_y != (const void*)y) {
-            if (!e->solo) { e->solo = new GroupState; e->solo->rt = e->rt; }
+        if (!e->solo || !e->solo->current() || e->solo_x != (const void*)x || e->solo_y != (const void*)y) {
+            if (!e->solo) { e->solo = std::make_unique<GroupState>(); e->solo->members = {e}; }
             else CK(cudaStreamSynchronize(e->rt->stream));
-            std::vector<ConvInt8Exec*> one{e};
             const int8_t* xs[1] = {x};
             int8_t* ys[1] = {y};
-            mnnb200_status st = group_build(*e->solo, one, xs, ys, nullptr, nullptr);
+            mnnb200_status st = group_build(*e->solo, e->rt, xs, ys, nullptr, nullptr);
             if (st) return st;
             e->solo_x = x; e->solo_y = y;
         }
-        return group_launch(*e->solo);
+        return group_launch(*e->solo, e->rt->stream);
     case ConvPath::MmaSync:
         break;
     }
@@ -986,26 +1035,22 @@ mnnb200_status mnnb200_conv_int8_execute(mnnb200_exec* ex, const int8_t* x, int8
     return MNNB200_OK;
 }
 // ---- conv group C ABI (GroupState / group_build are defined above, before the conv entry points)
-struct ConvGroupExec : mnnb200_exec {
-    std::vector<ConvInt8Exec*> members;
+struct ConvGroupExec : Tagged<kConvGroup> {
     GroupState gs;
-    bool bound = false;
 };
 
 int mnnb200_conv_int8_groupable(mnnb200_exec* ex) {
-    if (!ex || ex->kind != 1) return 0;
-    auto* e = static_cast<ConvInt8Exec*>(ex);
-    return e->resized && conv_path(e->plan, 0) == ConvPath::Group;
+    auto* e = exec_as<ConvInt8Exec>(ex);
+    return e && e->resized && conv_path(e->plan, 0) == ConvPath::Group;
 }
 mnnb200_status mnnb200_conv_int8_group_plan(mnnb200_exec* ex, int* fields, int count) {
-    if (!ex || ex->kind != 1 || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_int8_group_plan: bad argument");
-    auto* e = static_cast<ConvInt8Exec*>(ex);
+    auto* e = exec_as<ConvInt8Exec>(ex);
+    if (!e || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_int8_group_plan: bad argument");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_int8_group_plan before resize");
     if (!e->plan.group) return fail(MNNB200_NOT_SUPPORT, "conv_int8_group_plan: the conv-group kernel does not take this conv");
     const GroupLayerParams& q = e->plan.q;
     const int v[] = {q.mode, q.cb, q.bn, q.n_chunks, q.m_tiles, q.num_kb, q.K, q.R, q.TWp, e->plan.g.BH};
-    for (int i = 0; i < count && i < (int)(sizeof(v) / sizeof(v[0])); ++i) fields[i] = v[i];
-    return MNNB200_OK;
+    return copy_fields(v, fields, count);
 }
 mnnb200_status mnnb200_conv_group_schedule(const int* m_tiles, const int* n_chunks, int layers, int sm_count, uint32_t* items,
                                            int capacity, int* grid, int* stride) {
@@ -1024,38 +1069,32 @@ mnnb200_status mnnb200_conv_group_schedule(const int* m_tiles, const int* n_chun
 mnnb200_status mnnb200_conv_group_create(mnnb200_runtime* rt, mnnb200_exec* const* members, int count, mnnb200_exec** out) {
     if (!rt || !members || !out || count <= 0) return fail(MNNB200_INVALID_VALUE, "conv_group_create: bad argument");
     if (count > kGroupMaxLayers) return fail(MNNB200_NOT_SUPPORT, "conv_group_create: more than 64 members");
-    auto* g = new ConvGroupExec;
-    g->rt = rt;
-    g->kind = 6;
-    g->gs.rt = rt;
+    auto g = new_exec<ConvGroupExec>(rt);
     for (int i = 0; i < count; ++i) {
-        if (!members[i] || members[i]->kind != 1 || members[i]->rt != rt) {
-            delete g;
-            return fail(MNNB200_INVALID_VALUE, "conv_group_create: member is not a conv execution of this runtime");
-        }
-        g->members.push_back(static_cast<ConvInt8Exec*>(members[i]));
+        auto* m = exec_as<ConvInt8Exec>(members[i]);
+        if (!m || m->rt != rt) return fail(MNNB200_INVALID_VALUE, "conv_group_create: member is not a conv execution of this runtime");
+        g->gs.members.push_back(m);
     }
-    *out = g;
+    *out = g.release();
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_conv_group_bind(mnnb200_exec* ex, const int8_t* const* xs, int8_t* const* ys) {
-    if (!ex || ex->kind != 6 || !xs || !ys) return fail(MNNB200_INVALID_VALUE, "conv_group_bind: bad argument");
-    auto* g = static_cast<ConvGroupExec*>(ex);
+    auto* g = exec_as<ConvGroupExec>(ex);
+    if (!g || !xs || !ys) return fail(MNNB200_INVALID_VALUE, "conv_group_bind: bad argument");
     CK(cudaStreamSynchronize(g->rt->stream));       // a previous launch may still read the layer table and schedule being replaced
-    mnnb200_status st = group_build(g->gs, g->members, xs, ys, &g->cost_bytes, &g->cost_macs);
-    g->bound = st == MNNB200_OK;
-    return st;
+    return group_build(g->gs, g->rt, xs, ys, &g->cost_bytes, &g->cost_macs);
 }
 mnnb200_status mnnb200_conv_group_execute(mnnb200_exec* ex) {
-    if (!ex || ex->kind != 6) return fail(MNNB200_INVALID_VALUE, "conv_group_execute: not a conv group");
-    auto* g = static_cast<ConvGroupExec*>(ex);
-    if (!g->bound) return fail(MNNB200_NO_EXECUTION, "conv_group_execute before bind");
-    return group_launch(g->gs);
+    auto* g = exec_as<ConvGroupExec>(ex);
+    if (!g) return fail(MNNB200_INVALID_VALUE, "conv_group_execute: not a conv group");
+    if (g->gs.built_resizes.empty()) return fail(MNNB200_NO_EXECUTION, "conv_group_execute before bind");
+    if (!g->gs.current()) return fail(MNNB200_NO_EXECUTION, "conv_group_execute: a member was resized since bind");
+    return group_launch(g->gs, g->rt->stream);
 }
 
 mnnb200_status mnnb200_conv_int8_set_variant(mnnb200_exec* ex, int variant) {
-    if (!ex || (ex->kind != 1 && ex->kind != 3)) return fail(MNNB200_INVALID_VALUE, "set_variant: not a conv/linear execution");
-    const bool ok = ex->kind == 1 ? (variant >= 0 && variant <= 2) : (variant == 0 || (variant >= 2 && variant <= 4));
+    if (!exec_as<mnnb200_exec>(ex, kConvInt8 | kLinearW8)) return fail(MNNB200_INVALID_VALUE, "set_variant: not a conv/linear execution");
+    const bool ok = ex->type == kConvInt8 ? (variant >= 0 && variant <= 2) : (variant == 0 || (variant >= 2 && variant <= 4));
     if (!ok) return fail(MNNB200_INVALID_VALUE, "set_variant: a conv takes variant 0, 1 or 2, a linear 0, 2, 3 or 4");
     ex->variant = variant;
     return MNNB200_OK;
@@ -1073,16 +1112,14 @@ void mnnb200_exec_destroy(mnnb200_exec* e) { delete e; }
 // =================================================================================================
 // Depthwise int8 conv
 // =================================================================================================
-struct DwConvInt8Exec : mnnb200_exec {
-    mnnb200_conv_desc d;
+struct DwConvInt8Exec : Tagged<kDwConvInt8, ConvExec> {
     int Cp = 0;
     std::vector<float> h_wscale, h_bias;
     std::vector<int32_t> h_isum;
-    int8_t* d_w = nullptr;
-    float* d_scale = nullptr;
-    int32_t* d_bias = nullptr;
+    DevBuf<int8_t> d_w;
+    DevBuf<float> d_scale;
+    DevBuf<int32_t> d_bias;
     DwParams p;
-    bool resized = false;
 };
 
 extern "C" {
@@ -1090,8 +1127,8 @@ mnnb200_status mnnb200_dwconv_int8_create(mnnb200_runtime* rt, const mnnb200_con
                                           const float* wscale, const float* bias, mnnb200_exec** out) {
     if (!rt || !desc || !weight || !wscale || !out) return fail(MNNB200_INVALID_VALUE, "dwconv_int8_create: NULL argument");
     if (desc->group != desc->ic || desc->ic != desc->oc) return fail(MNNB200_NOT_SUPPORT, "dwconv: group == ic == oc required");
-    auto* e = new DwConvInt8Exec;
-    e->rt = rt; e->kind = 2; e->d = *desc;
+    auto e = new_exec<DwConvInt8Exec>(rt);
+    e->d = *desc;
     const int C = desc->oc, taps = desc->kh * desc->kw;
     e->Cp = up16(C);
     std::vector<int8_t> wp((size_t)taps * e->Cp, 0);
@@ -1107,20 +1144,19 @@ mnnb200_status mnnb200_dwconv_int8_create(mnnb200_runtime* rt, const mnnb200_con
     mnnb200_status st;
     std::vector<float> z(e->Cp, 0.f);
     std::vector<int32_t> zi(e->Cp, 0);
-    if ((st = e->upload(wp, &e->d_w)) || (st = e->upload(z, &e->d_scale)) || (st = e->upload(zi, &e->d_bias))) { delete e; return st; }
-    *out = e;
+    if ((st = e->d_w.upload(wp, rt->stream)) || (st = e->d_scale.upload(z, rt->stream)) || (st = e->d_bias.upload(zi, rt->stream)))
+        return st;
+    *out = e.release();
     return MNNB200_OK;
 }
 
 mnnb200_status mnnb200_dwconv_int8_resize(mnnb200_exec* ex, int n, int ih, int iw, float in_scale, int in_zero,
                                           float out_scale, int out_zero, int clamp_min, int clamp_max, int* oh, int* ow) {
-    if (!ex || ex->kind != 2) return fail(MNNB200_INVALID_VALUE, "dwconv_int8_resize: not a depthwise execution");
-    auto* e = static_cast<DwConvInt8Exec*>(ex);
+    auto* e = exec_as<DwConvInt8Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "dwconv_int8_resize: not a depthwise execution");
     const auto& d = e->d;
-    // MNN's shape inference owns the output size (SAME padding pads more at the end than at the beginning);
-    // a caller that knows it passes it in through *oh/*ow (> 0), pad_h/pad_w being the BEGIN pads.
-    int OH = (oh && *oh > 0) ? *oh : conv_out(ih, d.kh, d.stride_h, d.pad_h, d.dilate_h);
-    int OW = (ow && *ow > 0) ? *ow : conv_out(iw, d.kw, d.stride_w, d.pad_w, d.dilate_w);
+    const ConvOutSize out(d, ih, iw, oh, ow);
+    const int OH = out.H, OW = out.W;
     if (n <= 0 || OH <= 0 || OW <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "dwconv_int8_resize: empty output");
     if (in_scale == 0.f || out_scale == 0.f) return fail(MNNB200_INVALID_VALUE, "dwconv_int8_resize: zero quant scale");
     // depthwise branch of updateInputOutputScale, CPUConvolution.cpp:181-192
@@ -1137,7 +1173,7 @@ mnnb200_status mnnb200_dwconv_int8_resize(mnnb200_exec* ex, int n, int ih, int i
         bi[c] = b + 128 * e->h_isum[c];  // device activations are plain int8: fold the x86 +128 storage offset here
     }
     mnnb200_status st;
-    if ((st = e->update(sc, e->d_scale)) || (st = e->update(bi, e->d_bias))) return st;
+    if ((st = e->d_scale.upload(sc, e->rt->stream)) || (st = e->d_bias.upload(bi, e->rt->stream))) return st;
     DwParams& p = e->p;
     memset(&p, 0, sizeof(p));
     p.w = e->d_w; p.scale = e->d_scale; p.bias_i32 = e->d_bias;
@@ -1149,14 +1185,12 @@ mnnb200_status mnnb200_dwconv_int8_resize(mnnb200_exec* ex, int n, int ih, int i
     e->cost_bytes = (double)n * ih * iw * e->Cp + (double)n * OH * OW * e->Cp + (double)d.kh * d.kw * e->Cp;
     e->cost_macs = (double)n * OH * OW * d.oc * d.kh * d.kw;
     e->resized = true;
-    if (oh) *oh = OH;
-    if (ow) *ow = OW;
-    return MNNB200_OK;
+    return out.done();
 }
 
 mnnb200_status mnnb200_dwconv_int8_execute(mnnb200_exec* ex, const int8_t* x, int8_t* y) {
-    if (!ex || ex->kind != 2) return fail(MNNB200_INVALID_VALUE, "dwconv_int8_execute: not a depthwise execution");
-    auto* e = static_cast<DwConvInt8Exec*>(ex);
+    auto* e = exec_as<DwConvInt8Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "dwconv_int8_execute: not a depthwise execution");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "dwconv_int8_execute before resize");
     DwParams p = e->p;
     p.x = x; p.y = y;
@@ -1168,32 +1202,30 @@ mnnb200_status mnnb200_dwconv_int8_execute(mnnb200_exec* ex, const int8_t* x, in
 // =================================================================================================
 // LLM linear: W8 weights, dynamic per-token A8
 // =================================================================================================
-struct LinearW8Exec : mnnb200_exec {
+struct LinearW8Exec : Tagged<kLinearW8> {
     int ic = 0, oc = 0, icp = 0, ocp = 0, relu = 0, relu6 = 0, tokens = 0;
     bool has_zero = false, has_bias = false;
-    int8_t* d_w = nullptr;
-    float *d_alpha = nullptr, *d_wzero = nullptr, *d_bias = nullptr, *d_wsumf = nullptr;
-    int32_t* d_wsum128 = nullptr;
-    int8_t* d_xq = nullptr;
-    float *d_dq = nullptr, *d_srcsum = nullptr;
-    size_t xq_cap = 0, dq_cap = 0, ss_cap = 0;
+    DevBuf<int8_t> d_w;
+    DevBuf<float> d_alpha, d_wzero, d_bias, d_wsumf;
+    DevBuf<int32_t> d_wsum128;
+    DevBuf<int8_t> d_xq;                  // grow-only, as d_dq, d_srcsum and d_xsb
+    DevBuf<float> d_dq, d_srcsum;
     int bn = 0, bn2 = 0;            // bn2 != 0: the CTA-pair kernel is usable for this shape
     CUtensorMap tmap_a, tmap_b, tmap_b_half;
     // K-blocked weight scales (mnnb200_linear_w8_create_blocked): blocks of bs input channels, bs = 0 per channel
     int bs = 0, blocks = 1;
-    float *d_balpha = nullptr, *d_bwzero = nullptr;                     // [ocp][blocks]: the GEMV's layout
-    float *d_talpha = nullptr, *d_twzero = nullptr, *d_tws = nullptr;   // [blocks][ocp]: the GEMM's layout, ws_b precomputed
-    int32_t* d_tw128 = nullptr;                                         // [blocks][ocp] 128 * sum_b w
-    float* d_xsb = nullptr;                                             // [tokens][blocks] xsum_b * dq (GEMM path)
-    size_t xsb_cap = 0;
+    DevBuf<float> d_balpha, d_bwzero;             // [ocp][blocks]: the GEMV's layout
+    DevBuf<float> d_talpha, d_twzero, d_tws;      // [blocks][ocp]: the GEMM's layout, ws_b precomputed
+    DevBuf<int32_t> d_tw128;                      // [blocks][ocp] 128 * sum_b w
+    DevBuf<float> d_xsb;                          // [tokens][blocks] xsum_b * dq (GEMM path)
 };
 
 extern "C" {
 mnnb200_status mnnb200_linear_w8_create(mnnb200_runtime* rt, int ic, int oc, const int8_t* wq, const float* alpha,
                                         const float* wzero, const float* bias, int relu, int relu6, mnnb200_exec** out) {
     if (!rt || !wq || !alpha || !out || ic <= 0 || oc <= 0) return fail(MNNB200_INVALID_VALUE, "linear_w8_create: bad argument");
-    auto* e = new LinearW8Exec;
-    e->rt = rt; e->kind = 3; e->ic = ic; e->oc = oc; e->icp = up16(ic); e->ocp = up16(oc); e->relu = relu; e->relu6 = relu6;
+    auto e = new_exec<LinearW8Exec>(rt);
+    e->ic = ic; e->oc = oc; e->icp = up16(ic); e->ocp = up16(oc); e->relu = relu; e->relu6 = relu6;
     e->has_zero = wzero != nullptr; e->has_bias = bias != nullptr;
     std::vector<int8_t> wp((size_t)e->ocp * e->icp, 0);
     std::vector<float> al(e->ocp, 0.f), wz(e->ocp, 0.f), bs(e->ocp, 0.f), wsf(e->ocp, 0.f);
@@ -1208,13 +1240,12 @@ mnnb200_status mnnb200_linear_w8_create(mnnb200_runtime* rt, int ic, int oc, con
         wsf[o] = (float)s * alpha[o] + (float)ic * zb;  // _computeReorderQuantInfo, ConvInt8TiledExecutor.cpp:226-267
         k128[o] = 128 * s;
     }
+    const cudaStream_t s = rt->stream;
     mnnb200_status st;
-    if ((st = e->upload(wp, &e->d_w)) || (st = e->upload(al, &e->d_alpha)) || (st = e->upload(wz, &e->d_wzero)) ||
-        (st = e->upload(bs, &e->d_bias)) || (st = e->upload(wsf, &e->d_wsumf)) || (st = e->upload(k128, &e->d_wsum128))) {
-        delete e;
+    if ((st = e->d_w.upload(wp, s)) || (st = e->d_alpha.upload(al, s)) || (st = e->d_wzero.upload(wz, s)) ||
+        (st = e->d_bias.upload(bs, s)) || (st = e->d_wsumf.upload(wsf, s)) || (st = e->d_wsum128.upload(k128, s)))
         return st;
-    }
-    *out = e;
+    *out = e.release();
     return MNNB200_OK;
 }
 
@@ -1228,8 +1259,8 @@ mnnb200_status mnnb200_linear_w8_create_blocked(mnnb200_runtime* rt, int ic, int
     if (bs % 32) return fail(MNNB200_NOT_SUPPORT, "linear_w8_create_blocked: a block must be a multiple of 32 channels (one wgmma k-step)");
     if (bs > 512 || (bs & (bs - 1)))
         return fail(MNNB200_NOT_SUPPORT, "linear_w8_create_blocked: the GEMV takes power-of-two blocks of at most 512 channels");
-    auto* e = new LinearW8Exec;
-    e->rt = rt; e->kind = 3; e->ic = ic; e->oc = oc; e->icp = up16(ic); e->ocp = up16(oc); e->relu = relu; e->relu6 = relu6;
+    auto e = new_exec<LinearW8Exec>(rt);
+    e->ic = ic; e->oc = oc; e->icp = up16(ic); e->ocp = up16(oc); e->relu = relu; e->relu6 = relu6;
     e->has_zero = wzero != nullptr; e->has_bias = bias != nullptr; e->bs = bs; e->blocks = blocks;
     const size_t nt = (size_t)e->ocp * blocks;
     std::vector<int8_t> wp((size_t)e->ocp * e->icp, 0);
@@ -1249,33 +1280,27 @@ mnnb200_status mnnb200_linear_w8_create_blocked(mnnb200_runtime* rt, int ic, int
             tw128[bo] = 128 * isum;
         }
     }
+    const cudaStream_t s = rt->stream;
     mnnb200_status st;
-    if ((st = e->upload(wp, &e->d_w)) || (st = e->upload(bsv, &e->d_bias)) || (st = e->upload(ba, &e->d_balpha)) ||
-        (st = e->upload(bz, &e->d_bwzero)) || (st = e->upload(ta, &e->d_talpha)) || (st = e->upload(tz, &e->d_twzero)) ||
-        (st = e->upload(tws, &e->d_tws)) || (st = e->upload(tw128, &e->d_tw128))) {
-        delete e;
+    if ((st = e->d_w.upload(wp, s)) || (st = e->d_bias.upload(bsv, s)) || (st = e->d_balpha.upload(ba, s)) ||
+        (st = e->d_bwzero.upload(bz, s)) || (st = e->d_talpha.upload(ta, s)) || (st = e->d_twzero.upload(tz, s)) ||
+        (st = e->d_tws.upload(tws, s)) || (st = e->d_tw128.upload(tw128, s)))
         return st;
-    }
-    *out = e;
+    *out = e.release();
     return MNNB200_OK;
 }
 
 mnnb200_status mnnb200_linear_w8_resize(mnnb200_exec* ex, int tokens) {
-    if (!ex || ex->kind != 3) return fail(MNNB200_INVALID_VALUE, "linear_w8_resize: not a linear execution");
-    auto* e = static_cast<LinearW8Exec*>(ex);
+    auto* e = exec_as<LinearW8Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "linear_w8_resize: not a linear execution");
     if (tokens <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "linear_w8_resize: tokens <= 0");
-    {
-        mnnb200_status st;
-        if ((st = e->grow_scratch((void**)&e->d_xq, &e->xq_cap, (size_t)tokens * e->icp)) ||
-            (st = e->grow_scratch((void**)&e->d_dq, &e->dq_cap, (size_t)tokens * sizeof(float))) ||
-            (st = e->grow_scratch((void**)&e->d_srcsum, &e->ss_cap, (size_t)tokens * sizeof(float))))
-            return st;
-        if (e->bs && (st = e->grow_scratch((void**)&e->d_xsb, &e->xsb_cap, (size_t)tokens * e->blocks * sizeof(float)))) return st;
-    }
+    mnnb200_status st;
+    if ((st = e->d_xq.reserve((size_t)tokens * e->icp)) || (st = e->d_dq.reserve(tokens)) || (st = e->d_srcsum.reserve(tokens)))
+        return st;
+    if (e->bs && (st = e->d_xsb.reserve((size_t)tokens * e->blocks))) return st;
     e->tokens = tokens;
     // blocked: at most 128 columns per tile, the other half of the accumulator registers holds the fp32 block sums
     e->bn = pick_bn(e->ocp, (tokens + 127) / 128, e->rt->prop.multiProcessorCount, e->bs ? 128 : 256);
-    mnnb200_status st;
     if ((st = make_tmap_i8(&e->tmap_a, e->d_xq, tokens, e->icp, 128))) return st;
     if ((st = make_tmap_i8(&e->tmap_b, e->d_w, e->ocp, e->icp, e->bn))) return st;
     // tensor-bound shapes run on CTA pairs (2-CTA cluster, 256 rows): needs >= 256 rows and a B tile that splits into two halves
@@ -1292,8 +1317,8 @@ mnnb200_status mnnb200_linear_w8_resize(mnnb200_exec* ex, int tokens) {
 }
 
 mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float* y) {
-    if (!ex || ex->kind != 3) return fail(MNNB200_INVALID_VALUE, "linear_w8_execute: not a linear execution");
-    auto* e = static_cast<LinearW8Exec*>(ex);
+    auto* e = exec_as<LinearW8Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "linear_w8_execute: not a linear execution");
     if (e->tokens <= 0) return fail(MNNB200_NO_EXECUTION, "linear_w8_execute before resize");
     if (e->bs && e->variant == 3) return fail(MNNB200_NOT_SUPPORT, "the CTA-pair variant takes per-channel weight scales only");
     // decode (<= 8 tokens): weight-streaming GEMV, bit-identical to the tensor-core kernels (variant 4 forces it)
@@ -1304,8 +1329,8 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
         return fail(MNNB200_NOT_SUPPORT, "a single token runs the reference's decode arithmetic: GEMV kernel only (variant 0 or 4, ic <= 25600)");
     if (e->variant == 4 || e->tokens == 1 || (e->variant == 0 && linear_w8_gemv_supported(e->tokens, e->icp, e->bs))) {
         GemvW8Params g;
-        g.x = x; g.w = e->d_w; g.y = y; g.alpha = e->d_alpha; g.bias = e->has_bias ? e->d_bias : nullptr; g.wsumf = e->d_wsumf;
-        g.wzero = e->has_zero ? e->d_wzero : nullptr; g.wsum128 = e->d_wsum128;
+        g.x = x; g.w = e->d_w; g.y = y; g.alpha = e->d_alpha; g.bias = e->has_bias ? static_cast<float*>(e->d_bias) : nullptr; g.wsumf = e->d_wsumf;
+        g.wzero = e->has_zero ? static_cast<float*>(e->d_wzero) : nullptr; g.wsum128 = e->d_wsum128;
         g.tokens = e->tokens; g.ic = e->ic; g.oc = e->oc; g.ocp = e->ocp; g.icp = e->icp; g.ldy = e->oc; g.relu = e->relu; g.relu6 = e->relu6;
         g.bs = e->bs; g.balpha = e->d_balpha; g.bwzero = e->d_bwzero;
         CK(launch_linear_w8_gemv(g, e->rt->stream, e->rt->prop.multiProcessorCount));
@@ -1316,8 +1341,8 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
     GemmI8Params g;
     memset(&g, 0, sizeof(g));
     g.a = e->d_xq; g.b = e->d_w; g.M = e->tokens; g.N = e->ocp; g.K = e->icp;
-    g.y_f32 = y; g.ldy = e->oc; g.wscale = e->d_alpha; g.bias = e->has_bias ? e->d_bias : nullptr; g.wsum128 = e->d_wsum128;
-    g.OC = e->oc; g.dq = e->d_dq; g.srcsum = e->d_srcsum; g.wsumf = e->d_wsumf; g.wzero = e->has_zero ? e->d_wzero : nullptr;
+    g.y_f32 = y; g.ldy = e->oc; g.wscale = e->d_alpha; g.bias = e->has_bias ? static_cast<float*>(e->d_bias) : nullptr; g.wsum128 = e->d_wsum128;
+    g.OC = e->oc; g.dq = e->d_dq; g.srcsum = e->d_srcsum; g.wsumf = e->d_wsumf; g.wzero = e->has_zero ? static_cast<float*>(e->d_wzero) : nullptr;
     g.relu = e->relu; g.relu6 = e->relu6;
     g.bs = e->bs; g.blocks = e->blocks; g.balpha = e->d_talpha; g.bwzero = e->d_twzero; g.bws = e->d_tws; g.bw128 = e->d_tw128;
     g.xsb = e->d_xsb;
@@ -1336,20 +1361,17 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
 // per-(position, oc) requantisation, scale/offset tables -- then three enqueues per execute:
 // input transform -> alpha^2 batched wgmma int8 GEMMs -> output transform + requantise.
 // =================================================================================================
-struct WinoConvInt8Exec : mnnb200_exec {
-    mnnb200_conv_desc d;
+struct WinoConvInt8Exec : Tagged<kWinoInt8, ConvExec> {
     int unit = 0, alpha = 0, alpha2 = 0, Cp = 0, OCp = 0, OCb = 0, bn = 0;
     std::vector<float> h_bias, h_in_scale;
     std::vector<int32_t> h_in_zero;
-    int8_t* d_u = nullptr;                 // [alpha2][OCb][Cp]
-    float *d_scale = nullptr, *d_offset = nullptr, *d_fused = nullptr;   // [alpha2][OCp], [alpha2][OCp], [OCp]
-    int32_t* d_wsum128 = nullptr;          // [alpha2][OCp]
-    int8_t* d_v = nullptr;
-    float* d_m = nullptr;
-    size_t v_bytes = 0, m_bytes = 0;
+    DevBuf<int8_t> d_u;                    // [alpha2][OCb][Cp]
+    DevBuf<float> d_scale, d_offset, d_fused;   // [alpha2][OCp], [alpha2][OCp], [OCp]
+    DevBuf<int32_t> d_wsum128;             // [alpha2][OCp]
+    DevBuf<int8_t> d_v;                    // grow-only, as d_m
+    DevBuf<float> d_m;
     WinoParams p;
     CUtensorMap tmap_a, tmap_b, tmap_u_fused;   // tmap_u_fused: kWinoFusedBN-row boxes of U for the fused F(2,3) kernel
-    bool resized = false;
 };
 
 // Math::WinogradGenerater(unit, kernel, interp = 1, dividedInG = true), G only: source/math/WingoradGenerater.cpp:96-135,
@@ -1395,14 +1417,12 @@ mnnb200_status mnnb200_conv_int8_wino_create(mnnb200_runtime* rt, const mnnb200_
     if (ky0 != 0 || kx0 != 0 || kys != d.kh || kxs != d.kw || d.kh != 3 || d.kw != 3 || unit_y != unit_x ||
         (unit_y != 2 && unit_y != 4 && unit_y != 6))
         return fail(MNNB200_NOT_SUPPORT, "conv_int8_wino: only one full-kernel 3x3 unit with F(2/4/6, 3) is supported");
-    auto* e = new WinoConvInt8Exec;
-    e->rt = rt; e->kind = 4; e->d = d;
+    auto e = new_exec<WinoConvInt8Exec>(rt);
+    e->d = d;
     e->unit = unit_y; e->alpha = unit_y + 2; e->alpha2 = e->alpha * e->alpha;
     const int a2 = e->alpha2, alpha = e->alpha, oc = d.oc, ic = d.ic, r = 3;
-    if (unit_size != 6 + 2 * a2 + a2 * oc || attr_len < 3 + unit_size) {
-        delete e;
+    if (unit_size != 6 + 2 * a2 + a2 * oc || attr_len < 3 + unit_size)
         return fail(MNNB200_INVALID_VALUE, "conv_int8_wino: winogradAttr size does not match alpha^2 and oc");
-    }
     const float* in_scales = reinterpret_cast<const float*>(u + 6);
     const int32_t* in_zeros = u + 6 + a2;
     const float* w_scales = reinterpret_cast<const float*>(u + 6 + 2 * a2);
@@ -1461,24 +1481,23 @@ mnnb200_status mnnb200_conv_int8_wino_create(mnnb200_runtime* rt, const mnnb200_
             k128[(size_t)a * e->OCp + o] = 128 * isum;
         }
     std::vector<float> zf(e->OCp, 0.f);
+    const cudaStream_t s = rt->stream;
     mnnb200_status st;
-    if ((st = e->upload(uq, &e->d_u)) || (st = e->upload(sc, &e->d_scale)) || (st = e->upload(of, &e->d_offset)) ||
-        (st = e->upload(k128, &e->d_wsum128)) || (st = e->upload(zf, &e->d_fused))) {
-        delete e;
+    if ((st = e->d_u.upload(uq, s)) || (st = e->d_scale.upload(sc, s)) || (st = e->d_offset.upload(of, s)) ||
+        (st = e->d_wsum128.upload(k128, s)) || (st = e->d_fused.upload(zf, s)))
         return st;
-    }
-    *out = e;
+    *out = e.release();
     return MNNB200_OK;
 }
 
 mnnb200_status mnnb200_conv_int8_wino_resize(mnnb200_exec* ex, int n, int ih, int iw, float in_scale, int in_zero,
                                              float out_scale, int out_zero, int clamp_min, int clamp_max, int* oh, int* ow) {
-    if (!ex || ex->kind != 4) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_resize: not a Winograd execution");
-    auto* e = static_cast<WinoConvInt8Exec*>(ex);
+    auto* e = exec_as<WinoConvInt8Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_resize: not a Winograd execution");
     const auto& d = e->d;
     // every check first, on locals: a refused resize leaves the previous plan, fused bias and tensor maps as they were
-    const int OH = (oh && *oh > 0) ? *oh : conv_out(ih, 3, 1, d.pad_h, 1);
-    const int OW = (ow && *ow > 0) ? *ow : conv_out(iw, 3, 1, d.pad_w, 1);
+    const ConvOutSize out(d, ih, iw, oh, ow);   // 3x3, stride 1, dilation 1: create checked them
+    const int OH = out.H, OW = out.W;
     if (n <= 0 || OH <= 0 || OW <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "conv_int8_wino_resize: empty output");
     if (in_scale == 0.f || out_scale == 0.f) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_resize: zero quant scale");
     const int hU = (OH + e->unit - 1) / e->unit, wU = (OW + e->unit - 1) / e->unit;
@@ -1493,7 +1512,7 @@ mnnb200_status mnnb200_conv_int8_wino_resize(mnnb200_exec* ex, int n, int ih, in
     std::vector<float> fused(e->OCp, 0.f);
     for (int o = 0; o < d.oc; ++o) fused[o] = e->h_bias[o] / out_scale + (float)out_zero;   // mFusedBias, :215-217
     mnnb200_status st;
-    if ((st = e->update(fused, e->d_fused))) return st;
+    if ((st = e->d_fused.upload(fused, e->rt->stream))) return st;
     WinoParams& p = e->p;
     memset(&p, 0, sizeof(p));
     p.N = n; p.IH = ih; p.IW = iw; p.Cp = e->Cp; p.OH = OH; p.OW = OW; p.OC = d.oc; p.OCp = e->OCp;
@@ -1510,8 +1529,8 @@ mnnb200_status mnnb200_conv_int8_wino_resize(mnnb200_exec* ex, int n, int ih, in
         p.in_zero[a] = (float)e->h_in_zero[a];
     }
     p.fused_bias = e->d_fused;
-    const size_t vb = (size_t)e->alpha2 * p.Mpad * e->Cp, mb = (size_t)e->alpha2 * p.Mpad * e->OCp * sizeof(float);
-    if ((st = e->grow_scratch((void**)&e->d_v, &e->v_bytes, vb)) || (st = e->grow_scratch((void**)&e->d_m, &e->m_bytes, mb))) return st;
+    if ((st = e->d_v.reserve((size_t)e->alpha2 * p.Mpad * e->Cp)) || (st = e->d_m.reserve((size_t)e->alpha2 * p.Mpad * e->OCp)))
+        return st;
     p.v = e->d_v; p.m = e->d_m;
     if ((st = make_tmap_i8(&e->tmap_a, e->d_v, e->alpha2 * p.Mpad, e->Cp, 128))) return st;
     if ((st = make_tmap_i8(&e->tmap_b, e->d_u, e->alpha2 * e->OCb, e->Cp, e->bn))) return st;
@@ -1520,17 +1539,13 @@ mnnb200_status mnnb200_conv_int8_wino_resize(mnnb200_exec* ex, int n, int ih, in
     e->cost_bytes = (double)n * ih * iw * d.ic + (double)n * OH * OW * d.oc + (double)d.oc * d.ic * 9;
     e->cost_macs = (double)n * OH * OW * d.oc * d.ic * 9;
     e->resized = true;
-    if (oh) *oh = OH;
-    if (ow) *ow = OW;
-    return MNNB200_OK;
+    return out.done();
 }
 
 mnnb200_status mnnb200_conv_int8_set_pad(mnnb200_exec* ex, int pad_h, int pad_w) {
-    if (!ex) return fail(MNNB200_INVALID_VALUE, "set_pad: NULL");
-    if (ex->kind == 1) { auto* e = static_cast<ConvInt8Exec*>(ex); e->d.pad_h = pad_h; e->d.pad_w = pad_w; }
-    else if (ex->kind == 2) { auto* e = static_cast<DwConvInt8Exec*>(ex); e->d.pad_h = pad_h; e->d.pad_w = pad_w; }
-    else if (ex->kind == 4) { auto* e = static_cast<WinoConvInt8Exec*>(ex); e->d.pad_h = pad_h; e->d.pad_w = pad_w; }
-    else return fail(MNNB200_INVALID_VALUE, "set_pad: not a convolution execution");
+    auto* e = exec_as<ConvExec>(ex, kConvInt8 | kDwConvInt8 | kWinoInt8);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "set_pad: not a convolution execution");
+    e->d.pad_h = pad_h; e->d.pad_w = pad_w;
     return MNNB200_OK;
 }
 }  // extern "C"
@@ -1551,8 +1566,8 @@ mnnb200_status mnnb200_conv_int8_wino_execute(mnnb200_exec* ex, const int8_t* x,
     return mnnb200_conv_int8_wino_execute_phases(ex, x, y, 7);
 }
 mnnb200_status mnnb200_conv_int8_wino_execute_phases(mnnb200_exec* ex, const int8_t* x, int8_t* y, int phases) {
-    if (!ex || ex->kind != 4) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_execute: not a Winograd execution");
-    auto* e = static_cast<WinoConvInt8Exec*>(ex);
+    auto* e = exec_as<WinoConvInt8Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_execute: not a Winograd execution");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_int8_wino_execute before resize");
     // the transforms move 4 input channels and up to 4 output channels per access
     if (!x || !y || ((uintptr_t)x & 3) || ((uintptr_t)y & 3))
@@ -1581,8 +1596,8 @@ mnnb200_status mnnb200_conv_int8_wino_execute_phases(mnnb200_exec* ex, const int
 }
 
 mnnb200_status mnnb200_conv_int8_wino_plan(mnnb200_exec* ex, int* fields, int count) {
-    if (!ex || ex->kind != 4 || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_plan: bad argument");
-    auto* e = static_cast<WinoConvInt8Exec*>(ex);
+    auto* e = exec_as<WinoConvInt8Exec>(ex);
+    if (!e || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_int8_wino_plan: bad argument");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_int8_wino_plan before resize");
     const WinoParams& p = e->p;
     const int sm = e->rt->prop.multiProcessorCount, m_tiles = p.Mpad / 128, num_kb = (e->Cp + 127) / 128;
@@ -1596,8 +1611,7 @@ mnnb200_status mnnb200_conv_int8_wino_plan(mnnb200_exec* ex, int* fields, int co
         grid = l.grid; one_tile = l.one_tile; resident_b = l.resident_b; stages = l.stages;
     }
     const int v[] = {e->unit, (int)p.T, m_tiles, e->Cp, e->OCp, bn, n_chunks, items, grid, one_tile, resident_b, stages, num_kb};
-    for (int i = 0; i < count && i < (int)(sizeof(v) / sizeof(v[0])); ++i) fields[i] = v[i];
-    return MNNB200_OK;
+    return copy_fields(v, fields, count);
 }
 }  // extern "C"
 
@@ -1605,10 +1619,10 @@ mnnb200_status mnnb200_conv_int8_wino_plan(mnnb200_exec* ex, int* fields, int co
 // Float (batched) MatMul (SURVEY a9): C[b][e][h] = A x B (+ bias), MatMul / BatchMatMul semantics of
 // source/backend/cpu/CPUMatMul.cpp (transposeA / transposeB) and CPUBatchMatMul (adjX / adjY).
 // =================================================================================================
-struct MatMulExec : mnnb200_exec {
+struct MatMulExec : Tagged<kMatMul> {
     int batch = 0, e = 0, l = 0, h = 0, lp = 0, ta = 0, tb = 0, bn = 0;
     int tf32 = 0, esize = 2;               // tf32: fp32 operands consumed as tf32 (no conversion pass); else fp16 operands
-    void *d_a = nullptr, *d_b = nullptr;   // K-major scratch operands [batch][e][lp], [batch][h][lp] (only when a pack is needed)
+    DevBuf<uint8_t> d_a, d_b;              // K-major scratch operands [batch][e][lp], [batch][h][lp] (only when a pack is needed)
     CUtensorMap tmap_a, tmap_b;
     const void *tmap_a_ptr = nullptr, *tmap_b_ptr = nullptr;
 };
@@ -1617,8 +1631,8 @@ extern "C" {
 mnnb200_status mnnb200_matmul_create(mnnb200_runtime* rt, int batch, int e, int l, int h, int transpose_a, int transpose_b,
                                      int inputs_are_f16, mnnb200_exec** out) {
     if (!rt || !out || batch <= 0 || e <= 0 || l <= 0 || h <= 0) return fail(MNNB200_INVALID_VALUE, "matmul_create: bad argument");
-    auto* m = new MatMulExec;
-    m->rt = rt; m->kind = 5; m->batch = batch; m->e = e; m->l = l; m->h = h; m->ta = transpose_a; m->tb = transpose_b;
+    auto m = new_exec<MatMulExec>(rt);
+    m->batch = batch; m->e = e; m->l = l; m->h = h; m->ta = transpose_a; m->tb = transpose_b;
     // fp32 operands: tf32 wgmma reads them in place (K-major operands need no pass at all)
     m->tf32 = inputs_are_f16 ? 0 : 1;
     m->esize = m->tf32 ? 4 : 2;
@@ -1627,40 +1641,37 @@ mnnb200_status mnnb200_matmul_create(mnnb200_runtime* rt, int batch, int e, int 
     m->bn = pick_bn(up16(h), batch * ((e + 127) / 128), rt->prop.multiProcessorCount);
     m->cost_bytes = (double)batch * ((double)e * l + (double)l * h + (double)e * h) * 4;
     m->cost_macs = (double)batch * e * l * h;
-    *out = m;
+    *out = m.release();
     return MNNB200_OK;
 }
 mnnb200_status mnnb200_matmul_execute(mnnb200_exec* ex, const void* a, const void* b, const float* bias, float* c) {
-    if (!ex || ex->kind != 5) return fail(MNNB200_INVALID_VALUE, "matmul_execute: not a matmul execution");
-    auto* m = static_cast<MatMulExec*>(ex);
+    auto* m = exec_as<MatMulExec>(ex);
+    if (!m) return fail(MNNB200_INVALID_VALUE, "matmul_execute: not a matmul execution");
     // A logical [e][l]: memory [e][l] (ta = 0) or [l][e] (ta = 1).  B logical [l][h]; the kernel wants B^T = [h][l]:
     // memory [l][h] (tb = 0) is the transposed form, memory [h][l] (tb = 1) is already K-major.
     const bool aligned = m->lp == m->l;
     const bool a_direct = m->tf32 && !m->ta && aligned && ((uintptr_t)a & 15) == 0;
     const bool b_direct = m->tf32 && m->tb && aligned && ((uintptr_t)b & 15) == 0;
     const size_t row_bytes = (size_t)m->lp * m->esize;
-    auto scratch = [&](void** p, size_t rows) -> mnnb200_status {
-        if (*p) return MNNB200_OK;
-        // one extra tile of rows: the last tile of the last batch reads past the operand
-        CK(cudaMalloc(p, (rows + 256) * row_bytes));
-        CK(cudaMemsetAsync(*p, 0, (rows + 256) * row_bytes, m->rt->stream));
-        m->dev_bufs.push_back(*p);
+    // packs an operand of `rows` rows per batch K-major into its scratch and points *dst at it.  The scratch is zeroed when
+    // first allocated and has one extra tile of rows: the last tile of the last batch reads past the operand.
+    auto pack = [&](DevBuf<uint8_t>& buf, const void* src, int rows, int trans, const void** dst) -> mnnb200_status {
+        const size_t bytes = ((size_t)m->batch * rows + 256) * row_bytes;
+        if (!buf) {
+            mnnb200_status st = buf.reserve(bytes);
+            if (st) return st;
+            CK(cudaMemsetAsync(buf, 0, bytes, m->rt->stream));
+        }
+        void* d = buf;
+        if (m->tf32) CK(launch_pack_kmajor_f32((const float*)src, (float*)d, m->batch, rows, m->l, m->lp, trans, m->rt->stream));
+        else CK(launch_pack_kmajor_f16(src, d, m->batch, rows, m->l, m->lp, trans, m->rt->stream));
+        *dst = d;
         return MNNB200_OK;
     };
     mnnb200_status st;
     const void *pa = a, *pb = b;
-    if (!a_direct) {
-        if ((st = scratch(&m->d_a, (size_t)m->batch * m->e))) return st;
-        if (m->tf32) CK(launch_pack_kmajor_f32((const float*)a, (float*)m->d_a, m->batch, m->e, m->l, m->lp, m->ta ? 1 : 0, m->rt->stream));
-        else CK(launch_pack_kmajor_f16(a, m->d_a, m->batch, m->e, m->l, m->lp, m->ta ? 1 : 0, m->rt->stream));
-        pa = m->d_a;
-    }
-    if (!b_direct) {
-        if ((st = scratch(&m->d_b, (size_t)m->batch * m->h))) return st;
-        if (m->tf32) CK(launch_pack_kmajor_f32((const float*)b, (float*)m->d_b, m->batch, m->h, m->l, m->lp, m->tb ? 0 : 1, m->rt->stream));
-        else CK(launch_pack_kmajor_f16(b, m->d_b, m->batch, m->h, m->l, m->lp, m->tb ? 0 : 1, m->rt->stream));
-        pb = m->d_b;
-    }
+    if (!a_direct && (st = pack(m->d_a, a, m->e, m->ta ? 1 : 0, &pa))) return st;
+    if (!b_direct && (st = pack(m->d_b, b, m->h, m->tb ? 0 : 1, &pb))) return st;
     if (m->tmap_a_ptr != pa) {
         // direct operands are exactly batch*e rows (TMA zero-fills rows past the end); scratch has a padded tail
         if ((st = make_tmap_i8(&m->tmap_a, pa, m->batch * m->e + (a_direct ? 0 : 128), (int)row_bytes, 128))) return st;
@@ -1682,26 +1693,21 @@ mnnb200_status mnnb200_matmul_execute(mnnb200_exec* ex, const void* a, const voi
 // =================================================================================================
 static int float_act(const mnnb200_conv_desc* d, int relu6) { return relu6 ? 2 : (d->relu ? 1 : 0); }
 
-struct ConvF32Exec : mnnb200_exec {
-    mnnb200_conv_desc d;
+struct ConvF32Exec : Tagged<kConvF32, ConvExec> {
     int act = 0, cp8 = 0, taps = 0, kp = 0, ocp = 0, bn = 0;
-    float *d_hi = nullptr, *d_lo = nullptr, *d_bias = nullptr;
+    DevBuf<float> d_hi, d_lo, d_bias;
     CUtensorMap tmap_hi, tmap_lo;
     ConvF32Params p;
-    bool resized = false;
 };
-struct DwConvF32Exec : mnnb200_exec {
-    mnnb200_conv_desc d;
+struct DwConvF32Exec : Tagged<kDwConvF32, ConvExec> {
     int act = 0;
-    float *d_w = nullptr, *d_bias = nullptr;
+    DevBuf<float> d_w, d_bias;
     DwF32Params p;
-    bool resized = false;
 };
-struct ScaleF32Exec : mnnb200_exec {
+struct ScaleF32Exec : Tagged<kScaleF32> {
     int c = 0, n = 0;
     size_t plane = 0;
-    float *d_scale = nullptr, *d_bias = nullptr;
-    bool resized = false;
+    DevBuf<float> d_scale, d_bias;
 };
 
 static bool conv_desc_valid(const mnnb200_conv_desc* d) {
@@ -1715,8 +1721,8 @@ mnnb200_status mnnb200_conv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_d
     if (!rt || !desc || !weight || !out) return fail(MNNB200_INVALID_VALUE, "conv_f32_create: NULL argument");
     if (!conv_desc_valid(desc)) return fail(MNNB200_INVALID_VALUE, "conv_f32_create: bad descriptor");
     if (desc->group != 1) return fail(MNNB200_NOT_SUPPORT, "conv_f32: group > 1 (depthwise has its own execution)");
-    auto* e = new ConvF32Exec;
-    e->rt = rt; e->kind = 8; e->d = *desc; e->act = float_act(desc, relu6);
+    auto e = new_exec<ConvF32Exec>(rt);
+    e->d = *desc; e->act = float_act(desc, relu6);
     e->taps = desc->kh * desc->kw;
     e->cp8 = (desc->ic + 7) & ~7;
     e->kp = (e->taps * e->cp8 + 31) & ~31;
@@ -1724,39 +1730,32 @@ mnnb200_status mnnb200_conv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_d
     const size_t wn = (size_t)desc->oc * desc->ic * e->taps, packed = (size_t)e->ocp * e->kp;
     std::vector<float> hw(weight, weight + wn), hb(desc->oc, 0.f);
     if (bias) hb.assign(bias, bias + desc->oc);
-    float* d_raw = nullptr;
+    DevBuf<float> raw;
     mnnb200_status st;
-    if ((st = e->upload(hw, &d_raw)) || (st = e->upload(hb, &e->d_bias))) { delete e; return st; }
-    auto packed_buf = [&](float** p) -> mnnb200_status {
-        CK(cudaMalloc((void**)p, packed * sizeof(float)));
-        e->dev_bufs.push_back(*p);
-        return MNNB200_OK;
-    };
-    if ((st = packed_buf(&e->d_hi)) || (st = packed_buf(&e->d_lo))) { delete e; return st; }
-    cudaError_t ce = launch_pack_conv_w_f32(d_raw, desc->oc, desc->ic, e->taps, e->cp8, e->kp, e->ocp, e->d_hi, e->d_lo, rt->stream);
+    if ((st = raw.upload(hw, rt->stream)) || (st = e->d_bias.upload(hb, rt->stream)) || (st = e->d_hi.reserve(packed)) ||
+        (st = e->d_lo.reserve(packed)))
+        return st;
+    cudaError_t ce = launch_pack_conv_w_f32(raw, desc->oc, desc->ic, e->taps, e->cp8, e->kp, e->ocp, e->d_hi, e->d_lo, rt->stream);
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(rt->stream);
-    for (auto& b : e->dev_bufs)                  // the unpacked weights are not needed after the split
-        if (b == d_raw) b = nullptr;
-    cudaFree(d_raw);
-    if (ce != cudaSuccess) { delete e; return fail(MNNB200_CUDA_ERROR, std::string("conv_f32_create: ") + cudaGetErrorString(ce)); }
-    *out = e;
+    raw.reset();                                 // the unpacked weights are not needed after the split
+    if (ce != cudaSuccess) return fail(MNNB200_CUDA_ERROR, std::string("conv_f32_create: ") + cudaGetErrorString(ce));
+    *out = e.release();
     return MNNB200_OK;
 }
 
 mnnb200_status mnnb200_conv_f32_set_pad(mnnb200_exec* ex, int pad_h, int pad_w) {
-    if (!ex || pad_h < 0 || pad_w < 0) return fail(MNNB200_INVALID_VALUE, "conv_f32_set_pad: bad argument");
-    if (ex->kind == 8) { auto* e = static_cast<ConvF32Exec*>(ex); e->d.pad_h = pad_h; e->d.pad_w = pad_w; }
-    else if (ex->kind == 9) { auto* e = static_cast<DwConvF32Exec*>(ex); e->d.pad_h = pad_h; e->d.pad_w = pad_w; }
-    else return fail(MNNB200_INVALID_VALUE, "conv_f32_set_pad: not a float convolution execution");
+    auto* e = exec_as<ConvExec>(ex, kConvF32 | kDwConvF32);
+    if (!e || pad_h < 0 || pad_w < 0) return fail(MNNB200_INVALID_VALUE, "conv_f32_set_pad: bad argument (a float convolution, pads >= 0)");
+    e->d.pad_h = pad_h; e->d.pad_w = pad_w;
     return MNNB200_OK;
 }
 
 mnnb200_status mnnb200_conv_f32_resize(mnnb200_exec* ex, int n, int ih, int iw, int* oh, int* ow) {
-    if (!ex || ex->kind != 8) return fail(MNNB200_INVALID_VALUE, "conv_f32_resize: not a float conv execution");
-    auto* e = static_cast<ConvF32Exec*>(ex);
+    auto* e = exec_as<ConvF32Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "conv_f32_resize: not a float conv execution");
     const auto& d = e->d;
-    const int OH = (oh && *oh > 0) ? *oh : conv_out(ih, d.kh, d.stride_h, d.pad_h, d.dilate_h);
-    const int OW = (ow && *ow > 0) ? *ow : conv_out(iw, d.kw, d.stride_w, d.pad_w, d.dilate_w);
+    const ConvOutSize out(d, ih, iw, oh, ow);
+    const int OH = out.H, OW = out.W;
     if (n <= 0 || ih <= 0 || iw <= 0 || OH <= 0 || OW <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "conv_f32_resize: empty output");
     const long long M = (long long)n * OH * OW;
     if (M > 0x7fffffffLL - 128 || (long long)n * d.ic * ih * iw > 0x7fffffffLL || (long long)n * d.oc * OH * OW > 0x7fffffffLL)
@@ -1783,14 +1782,12 @@ mnnb200_status mnnb200_conv_f32_resize(mnnb200_exec* ex, int n, int ih, int iw, 
     e->cost_bytes = 4.0 * ((double)n * d.ic * ih * iw + (double)M * d.oc + (double)d.oc * d.ic * e->taps);
     e->cost_macs = (double)M * d.oc * d.ic * e->taps;
     e->resized = true;
-    if (oh) *oh = OH;
-    if (ow) *ow = OW;
-    return MNNB200_OK;
+    return out.done();
 }
 
 mnnb200_status mnnb200_conv_f32_execute(mnnb200_exec* ex, const float* x, float* y) {
-    if (!ex || ex->kind != 8) return fail(MNNB200_INVALID_VALUE, "conv_f32_execute: not a float conv execution");
-    auto* e = static_cast<ConvF32Exec*>(ex);
+    auto* e = exec_as<ConvF32Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "conv_f32_execute: not a float conv execution");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_f32_execute before resize");
     if (!x || !y) return fail(MNNB200_INVALID_VALUE, "conv_f32_execute: NULL tensor");
     ConvF32Params p = e->p;
@@ -1800,13 +1797,12 @@ mnnb200_status mnnb200_conv_f32_execute(mnnb200_exec* ex, const float* x, float*
 }
 
 mnnb200_status mnnb200_conv_f32_plan(mnnb200_exec* ex, int* fields, int count) {
-    if (!ex || ex->kind != 8 || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_f32_plan: bad argument");
-    auto* e = static_cast<ConvF32Exec*>(ex);
+    auto* e = exec_as<ConvF32Exec>(ex);
+    if (!e || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_f32_plan: bad argument");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_f32_plan before resize");
     const ConvF32Params& p = e->p;
     const int v[] = {e->bn, p.n_chunks, p.m_tiles, p.num_kb, conv_f32_stages(e->bn), p.Cp8, p.taps};
-    for (int i = 0; i < count && i < (int)(sizeof(v) / sizeof(v[0])); ++i) fields[i] = v[i];
-    return MNNB200_OK;
+    return copy_fields(v, fields, count);
 }
 
 mnnb200_status mnnb200_dwconv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight, const float* bias,
@@ -1814,22 +1810,22 @@ mnnb200_status mnnb200_dwconv_f32_create(mnnb200_runtime* rt, const mnnb200_conv
     if (!rt || !desc || !weight || !out) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_create: NULL argument");
     if (!conv_desc_valid(desc)) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_create: bad descriptor");
     if (desc->group != desc->ic || desc->ic != desc->oc) return fail(MNNB200_NOT_SUPPORT, "dwconv_f32: group == ic == oc required");
-    auto* e = new DwConvF32Exec;
-    e->rt = rt; e->kind = 9; e->d = *desc; e->act = float_act(desc, relu6);
+    auto e = new_exec<DwConvF32Exec>(rt);
+    e->d = *desc; e->act = float_act(desc, relu6);
     std::vector<float> hw(weight, weight + (size_t)desc->oc * desc->kh * desc->kw), hb(desc->oc, 0.f);
     if (bias) hb.assign(bias, bias + desc->oc);
     mnnb200_status st;
-    if ((st = e->upload(hw, &e->d_w)) || (st = e->upload(hb, &e->d_bias))) { delete e; return st; }
-    *out = e;
+    if ((st = e->d_w.upload(hw, rt->stream)) || (st = e->d_bias.upload(hb, rt->stream))) return st;
+    *out = e.release();
     return MNNB200_OK;
 }
 
 mnnb200_status mnnb200_dwconv_f32_resize(mnnb200_exec* ex, int n, int ih, int iw, int* oh, int* ow) {
-    if (!ex || ex->kind != 9) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_resize: not a float depthwise execution");
-    auto* e = static_cast<DwConvF32Exec*>(ex);
+    auto* e = exec_as<DwConvF32Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_resize: not a float depthwise execution");
     const auto& d = e->d;
-    const int OH = (oh && *oh > 0) ? *oh : conv_out(ih, d.kh, d.stride_h, d.pad_h, d.dilate_h);
-    const int OW = (ow && *ow > 0) ? *ow : conv_out(iw, d.kw, d.stride_w, d.pad_w, d.dilate_w);
+    const ConvOutSize out(d, ih, iw, oh, ow);
+    const int OH = out.H, OW = out.W;
     if (n <= 0 || ih <= 0 || iw <= 0 || OH <= 0 || OW <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "dwconv_f32_resize: empty output");
     DwF32Params& p = e->p;
     memset(&p, 0, sizeof(p));
@@ -1839,14 +1835,12 @@ mnnb200_status mnnb200_dwconv_f32_resize(mnnb200_exec* ex, int n, int ih, int iw
     e->cost_bytes = 4.0 * ((double)n * d.oc * ih * iw + (double)n * d.oc * OH * OW + (double)d.oc * d.kh * d.kw);
     e->cost_macs = (double)n * OH * OW * d.oc * d.kh * d.kw;
     e->resized = true;
-    if (oh) *oh = OH;
-    if (ow) *ow = OW;
-    return MNNB200_OK;
+    return out.done();
 }
 
 mnnb200_status mnnb200_dwconv_f32_execute(mnnb200_exec* ex, const float* x, float* y) {
-    if (!ex || ex->kind != 9) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_execute: not a float depthwise execution");
-    auto* e = static_cast<DwConvF32Exec*>(ex);
+    auto* e = exec_as<DwConvF32Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_execute: not a float depthwise execution");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "dwconv_f32_execute before resize");
     if (!x || !y) return fail(MNNB200_INVALID_VALUE, "dwconv_f32_execute: NULL tensor");
     DwF32Params p = e->p;
@@ -1887,19 +1881,19 @@ mnnb200_status mnnb200_argmax_f32(mnnb200_runtime* rt, const float* x, int outsi
 
 mnnb200_status mnnb200_scale_f32_create(mnnb200_runtime* rt, int channels, const float* scale, const float* bias, mnnb200_exec** out) {
     if (!rt || !scale || !out || channels <= 0) return fail(MNNB200_INVALID_VALUE, "scale_f32_create: bad argument");
-    auto* e = new ScaleF32Exec;
-    e->rt = rt; e->kind = 10; e->c = channels;
+    auto e = new_exec<ScaleF32Exec>(rt);
+    e->c = channels;
     std::vector<float> hs(scale, scale + channels), hb(channels, 0.f);
     if (bias) hb.assign(bias, bias + channels);
     mnnb200_status st;
-    if ((st = e->upload(hs, &e->d_scale)) || (st = e->upload(hb, &e->d_bias))) { delete e; return st; }
-    *out = e;
+    if ((st = e->d_scale.upload(hs, rt->stream)) || (st = e->d_bias.upload(hb, rt->stream))) return st;
+    *out = e.release();
     return MNNB200_OK;
 }
 
 mnnb200_status mnnb200_scale_f32_resize(mnnb200_exec* ex, int n, int h, int w) {
-    if (!ex || ex->kind != 10) return fail(MNNB200_INVALID_VALUE, "scale_f32_resize: not a float Scale execution");
-    auto* e = static_cast<ScaleF32Exec*>(ex);
+    auto* e = exec_as<ScaleF32Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "scale_f32_resize: not a float Scale execution");
     if (n <= 0 || h <= 0 || w <= 0) return fail(MNNB200_COMPUTE_SIZE_ERROR, "scale_f32_resize: empty tensor");
     e->n = n; e->plane = (size_t)h * w;
     e->cost_bytes = 8.0 * n * e->c * (double)e->plane;
@@ -1909,8 +1903,8 @@ mnnb200_status mnnb200_scale_f32_resize(mnnb200_exec* ex, int n, int h, int w) {
 }
 
 mnnb200_status mnnb200_scale_f32_execute(mnnb200_exec* ex, const float* x, float* y) {
-    if (!ex || ex->kind != 10) return fail(MNNB200_INVALID_VALUE, "scale_f32_execute: not a float Scale execution");
-    auto* e = static_cast<ScaleF32Exec*>(ex);
+    auto* e = exec_as<ScaleF32Exec>(ex);
+    if (!e) return fail(MNNB200_INVALID_VALUE, "scale_f32_execute: not a float Scale execution");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "scale_f32_execute before resize");
     if (!x || !y) return fail(MNNB200_INVALID_VALUE, "scale_f32_execute: NULL tensor");
     CK(launch_scale_f32(x, e->d_scale, e->d_bias, y, e->n, e->c, e->plane, e->rt->stream));
