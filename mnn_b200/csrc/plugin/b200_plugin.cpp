@@ -85,6 +85,39 @@ size_t deviceBytes(const Tensor* t) {
 }
 inline void* dev(const Tensor* t) { return (void*)(uintptr_t)t->deviceId(); }
 
+// The one owner of a C ABI execution: destroyed exactly once, with the execution that holds it
+struct ExecDeleter { void operator()(mnnb200_exec* h) const { mnnb200_exec_destroy(h); } };
+typedef std::unique_ptr<mnnb200_exec, ExecDeleter> ExecHandle;
+
+// A grow-only scratch allocation (device or pinned host, by Alloc / Free): reallocated only when a request does not fit, the
+// old allocation freed after a sync because the device may still read it; a failed allocation leaves it empty
+template <mnnb200_status (*Alloc)(mnnb200_runtime*, size_t, void**), mnnb200_status (*Free)(mnnb200_runtime*, void*)>
+class Scratch {
+public:
+    explicit Scratch(mnnb200_runtime* h) : mH(h) {}
+    Scratch(const Scratch&) = delete;
+    Scratch& operator=(const Scratch&) = delete;
+    ~Scratch() { release(); }
+    void* get(size_t bytes) {
+        if (bytes > mBytes) {
+            release();
+            if (Alloc(mH, bytes, &mP) != MNNB200_OK) { mP = nullptr; return nullptr; }
+            mBytes = bytes;
+        }
+        return mP;
+    }
+    void* data() const { return mP; }
+private:
+    void release() {
+        if (mP) { mnnb200_runtime_sync(mH); Free(mH, mP); mP = nullptr; mBytes = 0; }
+    }
+    mnnb200_runtime* mH;
+    void* mP = nullptr;
+    size_t mBytes = 0;
+};
+typedef Scratch<mnnb200_alloc, mnnb200_free> DeviceScratch;
+typedef Scratch<mnnb200_alloc_host, mnnb200_free_host> PinnedScratch;
+
 class B200Runtime;
 
 // ------------------------------------------------------------------------------------------------ Backend
@@ -93,7 +126,7 @@ class B200Exec;
 class B200Backend : public Backend {
 public:
     B200Backend(const B200Runtime* rt, mnnb200_runtime* h, bool memoryLow)
-        : Backend(MNN_FORWARD_CUDA), mRuntime(rt), mH(h), mMemoryLow(memoryLow) {
+        : Backend(MNN_FORWARD_CUDA), mRuntime(rt), mH(h), mMemoryLow(memoryLow), mStageDev(h), mStageHost(h) {
         if (const char* v = getenv("MNNB200_PLUGIN_GRAPH")) mGraphEnabled = atoi(v) != 0;
         if (const char* v = getenv("MNNB200_PLUGIN_HOSTREG")) mHostRegEnabled = atoi(v) != 0;
     }
@@ -102,11 +135,7 @@ public:
         mnnb200_runtime_sync(mH);
         dropGraph();
         for (auto& kv : mRegistered) mnnb200_host_unregister(mH, kv.first);
-        if (mStageDev) mnnb200_free(mH, mStageDev);
-        if (mStageHost) mnnb200_free_host(mH, mStageHost);
-        for (auto& c : mPool->chunks) mnnb200_free(mH, c.ptr);
-        mPool->chunks.clear();
-        ++mPool->epoch;
+        freePool();
     }
     mnnb200_runtime* handle() const { return mH; }
 
@@ -187,10 +216,14 @@ public:
     bool onClearBuffer() override {
         dropGraph();
         mnnb200_runtime_sync(mH);
+        freePool();
+        return true;
+    }
+    // every dynamic chunk back to the driver; a DynamicMem that outlives this sees the new epoch and leaves the list alone
+    void freePool() {
         for (auto& c : mPool->chunks) mnnb200_free(mH, c.ptr);
         mPool->chunks.clear();
         ++mPool->epoch;
-        return true;
     }
     void onCopyBuffer(const Tensor* src, const Tensor* dst) const override;
     int onSync(Tensor::MapType, bool toCpu, const Tensor*) override {
@@ -203,20 +236,14 @@ public:
     //      malloc/free per copy), and the user's own host tensors pinned in place on first sight (cudaHostRegister) so that
     //      the H2D/D2H DMA runs at PCIe speed instead of through the driver's pageable-memory bounce buffers
     void* stageDev(size_t bytes) const {
-        if (bytes > mStageDevBytes) {
-            if (mStageDev) { mnnb200_runtime_sync(mH); mnnb200_free(mH, mStageDev); mStageDev = nullptr; mStageDevBytes = 0; }
-            if (mnnb200_alloc(mH, bytes, &mStageDev) != MNNB200_OK) { MNN_ERROR("mnn_b200: staging alloc of %zu bytes failed: %s\n", bytes, mnnb200_last_error()); return nullptr; }
-            mStageDevBytes = bytes;
-        }
-        return mStageDev;
+        void* p = mStageDev.get(bytes);
+        if (!p) MNN_ERROR("mnn_b200: staging alloc of %zu bytes failed: %s\n", bytes, mnnb200_last_error());
+        return p;
     }
     void* stageHost(size_t bytes) const {
-        if (bytes > mStageHostBytes) {
-            if (mStageHost) { mnnb200_runtime_sync(mH); mnnb200_free_host(mH, mStageHost); mStageHost = nullptr; mStageHostBytes = 0; }
-            if (mnnb200_alloc_host(mH, bytes, &mStageHost) != MNNB200_OK) { MNN_ERROR("mnn_b200: pinned staging alloc failed: %s\n", mnnb200_last_error()); return nullptr; }
-            mStageHostBytes = bytes;
-        }
-        return mStageHost;
+        void* p = mStageHost.get(bytes);
+        if (!p) MNN_ERROR("mnn_b200: pinned staging alloc failed: %s\n", mnnb200_last_error());
+        return p;
     }
     // true when [p, p+bytes) is pinned (registered now or before); copies below 1 MiB are not worth a registration.
     // OFF by default (MNNB200_PLUGIN_HOSTREG=1 opts in): the backend cannot see a user tensor die.  A host tensor that is freed
@@ -246,8 +273,7 @@ public:
     bool h2d(void* devDst, const void* hostSrc, size_t bytes) const {
         if (pinned(const_cast<void*>(hostSrc), bytes)) {
             if (mnnb200_memcpy_h2d(mH, devDst, hostSrc, bytes) == MNNB200_OK) return mnnb200_runtime_sync(mH) == MNNB200_OK;
-            mnnb200_host_unregister(mH, const_cast<void*>(hostSrc));      // stale registration (the tensor was freed and its address
-            mRegistered.erase(const_cast<void*>(hostSrc));                // reused): the copy fails cleanly, redo it unpinned
+            unpin(const_cast<void*>(hostSrc));
         }
         if (mnnb200_memcpy_h2d(mH, devDst, hostSrc, bytes) != MNNB200_OK) return false;
         return mnnb200_runtime_sync(mH) == MNNB200_OK;
@@ -255,14 +281,19 @@ public:
     bool d2h(void* hostDst, const void* devSrc, size_t bytes) const {
         if (pinned(hostDst, bytes)) {
             if (mnnb200_memcpy_d2h(mH, hostDst, devSrc, bytes) == MNNB200_OK) return mnnb200_runtime_sync(mH) == MNNB200_OK;
-            mnnb200_host_unregister(mH, hostDst);
-            mRegistered.erase(hostDst);
+            unpin(hostDst);
         }
         void* st = stageHost(bytes);
         if (!st) return false;
         if (mnnb200_memcpy_d2h(mH, st, devSrc, bytes) != MNNB200_OK || mnnb200_runtime_sync(mH) != MNNB200_OK) return false;
         ::memcpy(hostDst, st, bytes);
         return true;
+    }
+    // a pinned copy that failed: the registration is stale (the tensor was freed and its address reused), the copy failed
+    // cleanly, and the caller redoes it unpinned
+    void unpin(void* p) const {
+        mnnb200_host_unregister(mH, p);
+        mRegistered.erase(p);
     }
     float lastGpuMs() const { return mnnb200_runtime_last_gpu_ms(mH); }
 
@@ -278,10 +309,8 @@ private:
     mutable mnnb200_graph* mGraph = nullptr;
     mutable std::vector<Call> mPending;
     mutable std::vector<uint64_t> mTrace;   // signature of the captured forward
-    mutable void* mStageDev = nullptr;
-    mutable size_t mStageDevBytes = 0;
-    mutable void* mStageHost = nullptr;
-    mutable size_t mStageHostBytes = 0;
+    mutable DeviceScratch mStageDev;
+    mutable PinnedScratch mStageHost;
     mutable std::map<void*, size_t> mRegistered;
 };
 
@@ -290,11 +319,27 @@ class B200Exec : public Execution {
 public:
     explicit B200Exec(Backend* bn) : Execution(bn) {}
     ErrorCode onExecute(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) final {
-        auto b = static_cast<B200Backend*>(backend());
-        if (b->deferring()) { b->log(this, inputs, outputs); return NO_ERROR; }
+        if (owner()->deferring()) { owner()->log(this, inputs, outputs); return NO_ERROR; }
         return launch(inputs, outputs);
     }
     virtual ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) = 0;
+protected:
+    B200Backend* owner() const { return static_cast<B200Backend*>(backend()); }
+    mnnb200_runtime* rt() const { return owner()->handle(); }
+};
+
+// Execution::onClone (source/core/Execution.hpp:63) for an execution that T::create(backend, op) makes from the op alone.  A clone
+// makes its weights again from the op: the C ABI keeps the launch plan and epilogue constants per execution and has no way to
+// share its device weights.  dst == nullptr asks whether the execution can be cloned.
+template <class T>
+class ClonedFromOp : public B200Exec {
+public:
+    explicit ClonedFromOp(Backend* bn) : B200Exec(bn) {}
+    bool onClone(Backend* bn, const Op* op, Execution** dst) override {
+        if (dst == nullptr) return true;
+        *dst = T::create(static_cast<B200Backend*>(bn), op);
+        return *dst != nullptr;
+    }
 };
 
 void B200Backend::onExecuteBegin() const {
@@ -358,12 +403,13 @@ void B200Backend::onExecuteEnd() const {
 
 // host tensor <-> linear fp32/int32 device layout.  User host tensors are NCHW (Tensor::CAFFE), NHWC (TENSORFLOW) or
 // NC4HW4 with pack 4 (CAFFE_C4); the device keeps NCHW-linear for NCHW/NC4HW4-format tensors and NHWC-linear for NHWC.
-static void hostToLinear(const Tensor* host, MNN_DATA_FORMAT devFmt, std::vector<uint8_t>& out, bool toHost, const uint8_t* in = nullptr) {
+// Calls copy(host tensor's byte offset, linear layout's byte offset, element bytes) for every element.
+template <class F>
+static void forEachElement(const Tensor* host, MNN_DATA_FORMAT devFmt, F copy) {
     auto hfmt = TensorUtils::getDescribe(host)->dimensionFormat;
-    const int bytes = host->getType().bytes();
+    const size_t bytes = host->getType().bytes();
     auto d = dims4(host);
     const size_t area = (size_t)d.h * d.w;
-    auto hostPtr = host->host<uint8_t>();
     auto devIndex = [&](int n, int c, size_t a) -> size_t {
         return devFmt == MNN_DATA_FORMAT_NHWC ? ((size_t)n * area + a) * d.c + c : ((size_t)n * d.c + c) * area + a;
     };
@@ -372,13 +418,9 @@ static void hostToLinear(const Tensor* host, MNN_DATA_FORMAT devFmt, std::vector
         if (hfmt == MNN_DATA_FORMAT_NC4HW4) return (((size_t)n * ((d.c + 3) / 4) + c / 4) * area + a) * 4 + c % 4;
         return ((size_t)n * d.c + c) * area + a;
     };
-    if (!toHost) out.assign((size_t)d.n * d.c * area * bytes, 0);
     for (int n = 0; n < d.n; ++n)
         for (int c = 0; c < d.c; ++c)
-            for (size_t a = 0; a < area; ++a) {
-                if (toHost) ::memcpy(hostPtr + hostIndex(n, c, a) * bytes, in + devIndex(n, c, a) * bytes, bytes);
-                else ::memcpy(out.data() + devIndex(n, c, a) * bytes, hostPtr + hostIndex(n, c, a) * bytes, bytes);
-            }
+            for (size_t a = 0; a < area; ++a) copy(hostIndex(n, c, a) * bytes, devIndex(n, c, a) * bytes, bytes);
 }
 static MNN_DATA_FORMAT linearFormat(const Tensor* t) {
     auto f = TensorUtils::getDescribe(t)->dimensionFormat;
@@ -416,13 +458,17 @@ void B200Backend::onCopyBuffer(const Tensor* src, const Tensor* dst) const {
         return;
     }
     if (!srcDev && dstDev) {   // host -> device
+        const void* from = src->host<void>();
+        const size_t bytes = elemCount(src) * (size_t)src->getType().bytes();
+        const auto devFmt = isInt8(dst) ? MNN_DATA_FORMAT_NCHW : linearFormat(dst);
         std::vector<uint8_t> lin;
+        if (!hostIsLinear(src, devFmt)) {
+            lin.assign(bytes, 0);
+            forEachElement(src, devFmt, [&](size_t h, size_t l, size_t n) { ::memcpy(&lin[l], src->host<uint8_t>() + h, n); });
+            from = lin.data();
+        }
         if (isInt8(dst)) {
             auto d = dims4(dst);
-            const bool direct = hostIsLinear(src, MNN_DATA_FORMAT_NCHW);
-            const void* from = src->host<void>();
-            size_t bytes = elemCount(src) * (size_t)src->getType().bytes();
-            if (!direct) { hostToLinear(src, MNN_DATA_FORMAT_NCHW, lin, false); from = lin.data(); bytes = lin.size(); }
             void* stage = stageDev(bytes);
             if (!stage || !h2d(stage, from, bytes)) { MNN_ERROR("mnn_b200 onCopyBuffer h2d failed: %s\n", mnnb200_last_error()); return; }
             if (src->getType().bytes() == 1) {   // int8 host, logical NCHW -> NHWC16
@@ -436,9 +482,6 @@ void B200Backend::onCopyBuffer(const Tensor* src, const Tensor* dst) const {
             if (st != MNNB200_OK) MNN_ERROR("mnn_b200 onCopyBuffer cast: %s\n", mnnb200_last_error());
             return;
         }
-        const void* from = src->host<void>();
-        size_t bytes = elemCount(src) * (size_t)src->getType().bytes();
-        if (!hostIsLinear(src, linearFormat(dst))) { hostToLinear(src, linearFormat(dst), lin, false); from = lin.data(); bytes = lin.size(); }
         if (!h2d(dev(dst), from, bytes)) MNN_ERROR("mnn_b200 onCopyBuffer h2d failed: %s\n", mnnb200_last_error());
         return;
     }
@@ -462,9 +505,9 @@ void B200Backend::onCopyBuffer(const Tensor* src, const Tensor* dst) const {
         if (hostIsLinear(dst, devFmt)) {
             if (!d2h(dst->host<void>(), from, bytes)) MNN_ERROR("mnn_b200 onCopyBuffer d2h failed: %s\n", mnnb200_last_error());
         } else {
-            std::vector<uint8_t> lin(bytes), unused;
+            std::vector<uint8_t> lin(bytes);
             if (!d2h(lin.data(), from, bytes)) { MNN_ERROR("mnn_b200 onCopyBuffer d2h failed: %s\n", mnnb200_last_error()); return; }
-            hostToLinear(dst, devFmt, unused, true, lin.data());
+            forEachElement(dst, devFmt, [&](size_t h, size_t l, size_t n) { ::memcpy(dst->host<uint8_t>() + h, &lin[l], n); });
         }
         return;
     }
@@ -479,15 +522,12 @@ static ErrorCode toErr(mnnb200_status s, const char* what) {
 }
 
 // Convolution / ConvolutionDepthwise / ConvInt8 / DepthwiseConvInt8 with int8 tensors (ConvInt8CutlassExecution's role)
-class ConvInt8Exec : public B200Exec {
+class ConvInt8Exec : public ClonedFromOp<ConvInt8Exec> {
 public:
-    struct Resource {   // immutable, shared by clones (Execution::onClone contract)
-        mnnb200_exec* h = nullptr;
-        ~Resource() { if (h) mnnb200_exec_destroy(h); }
-    };
-    ConvInt8Exec(Backend* bn, const Op* op, std::shared_ptr<Resource> res, bool dw, bool wino)
-        : B200Exec(bn), mOp(op), mRes(res), mDepthwise(dw), mWino(wino) {}
-    static Execution* create(B200Backend* bn, const Op* op, bool depthwise) {
+    ConvInt8Exec(Backend* bn, const Op* op, mnnb200_exec* h, bool dw, bool wino)
+        : ClonedFromOp(bn), mOp(op), mH(h), mDepthwise(dw), mWino(wino) {}
+    static Execution* create(B200Backend* bn, const Op* op) {
+        const bool depthwise = op->type() == OpType_ConvolutionDepthwise || op->type() == OpType_DepthwiseConvInt8;
         auto conv = op->main_as_Convolution2D();
         if (!conv || !conv->common()) return nullptr;
         auto cm = conv->common();
@@ -509,27 +549,25 @@ public:
         d.pad_h = cm->padY(); d.pad_w = cm->padX(); d.dilate_h = cm->dilateY(); d.dilate_w = cm->dilateX();
         d.group = depthwise ? oc : 1; d.relu = (cm->relu() || cm->relu6()) ? 1 : 0;
         if (!depthwise && cm->group() != 1) return nullptr;
-        std::shared_ptr<Resource> res(new Resource);
         const bool wino = !depthwise && conv->symmetricQuan() && conv->symmetricQuan()->winogradAttr();
+        mnnb200_exec* h = nullptr;
         mnnb200_status st;
         if (wino) {
             auto a = conv->symmetricQuan()->winogradAttr();
-            st = mnnb200_conv_int8_wino_create(bn->handle(), &d, w, scale.data(), (const float*)bias.data(), a->data(), (int)a->size(), &res->h);
+            st = mnnb200_conv_int8_wino_create(bn->handle(), &d, w, scale.data(), (const float*)bias.data(), a->data(), (int)a->size(), &h);
         } else if (depthwise) {
             if (legacy) return nullptr;
-            st = mnnb200_dwconv_int8_create(bn->handle(), &d, w, scale.data(), (const float*)bias.data(), &res->h);
+            st = mnnb200_dwconv_int8_create(bn->handle(), &d, w, scale.data(), (const float*)bias.data(), &h);
         } else if (legacy) {
-            st = mnnb200_conv_int8_create_legacy(bn->handle(), &d, w, scale.data(), bias.data(), &res->h);
+            st = mnnb200_conv_int8_create_legacy(bn->handle(), &d, w, scale.data(), bias.data(), &h);
         } else {
-            st = mnnb200_conv_int8_create(bn->handle(), &d, w, scale.data(), (const float*)bias.data(), &res->h);
+            st = mnnb200_conv_int8_create(bn->handle(), &d, w, scale.data(), (const float*)bias.data(), &h);
         }
         if (st != MNNB200_OK) {
             if (st != MNNB200_NOT_SUPPORT) MNN_ERROR("mnn_b200 conv create: %s\n", mnnb200_last_error());
             return nullptr;
         }
-        auto e = new ConvInt8Exec(bn, op, res, depthwise, wino);
-        e->mLegacy = legacy;
-        return e;
+        return new ConvInt8Exec(bn, op, h, depthwise, wino);
     }
     ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto in = inputs[0], out = outputs[0];
@@ -547,34 +585,25 @@ public:
             }
         }
         int oh = out->height(), ow = out->width();
-        mnnb200_status st = mnnb200_conv_int8_set_pad(mRes->h, pad.second, pad.first);
+        mnnb200_status st = mnnb200_conv_int8_set_pad(mH.get(), pad.second, pad.first);
         if (st == MNNB200_OK) {
-            if (mWino) st = mnnb200_conv_int8_wino_resize(mRes->h, in->batch(), in->height(), in->width(), si, zi, so, zo, cmin, cmax, &oh, &ow);
-            else if (mDepthwise) st = mnnb200_dwconv_int8_resize(mRes->h, in->batch(), in->height(), in->width(), si, zi, so, zo, cmin, cmax, &oh, &ow);
-            else st = mnnb200_conv_int8_resize(mRes->h, in->batch(), in->height(), in->width(), si, zi, so, zo, cmin, cmax, &oh, &ow);
+            if (mWino) st = mnnb200_conv_int8_wino_resize(mH.get(), in->batch(), in->height(), in->width(), si, zi, so, zo, cmin, cmax, &oh, &ow);
+            else if (mDepthwise) st = mnnb200_dwconv_int8_resize(mH.get(), in->batch(), in->height(), in->width(), si, zi, so, zo, cmin, cmax, &oh, &ow);
+            else st = mnnb200_conv_int8_resize(mH.get(), in->batch(), in->height(), in->width(), si, zi, so, zo, cmin, cmax, &oh, &ow);
         }
         return toErr(st, "conv resize");
     }
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto x = (const int8_t*)dev(inputs[0]);
         auto y = (int8_t*)dev(outputs[0]);
-        mnnb200_status st = mWino ? mnnb200_conv_int8_wino_execute(mRes->h, x, y)
-                                  : (mDepthwise ? mnnb200_dwconv_int8_execute(mRes->h, x, y) : mnnb200_conv_int8_execute(mRes->h, x, y));
+        mnnb200_status st = mWino ? mnnb200_conv_int8_wino_execute(mH.get(), x, y)
+                                  : (mDepthwise ? mnnb200_dwconv_int8_execute(mH.get(), x, y) : mnnb200_conv_int8_execute(mH.get(), x, y));
         return toErr(st, "conv execute");
-    }
-    // Execution::onClone (source/core/Execution.hpp:63): a clone owns its own resize state; the packed weights are re-created
-    // from the op (the C ABI keeps epilogue constants per execution), dst == nullptr is the capability query
-    bool onClone(Backend* bn, const Op* op, Execution** dst) override {
-        if (dst) {
-            *dst = create(static_cast<B200Backend*>(bn), op, mDepthwise);
-            if (*dst == nullptr) return false;
-        }
-        return true;
     }
 private:
     const Op* mOp;
-    std::shared_ptr<Resource> mRes;
-    bool mDepthwise, mWino, mLegacy = false;
+    ExecHandle mH;
+    bool mDepthwise, mWino;
 };
 
 // Convolution 1x1 with IDST int8 weights on FLOAT tensors under BackendConfig::Memory_Low = the MNN-LLM linear layer:
@@ -583,9 +612,8 @@ private:
 // wants token-major rows: transposed in and out unless H*W == 1.
 class LinearW8Exec : public B200Exec {
 public:
-    struct Resource { mnnb200_exec* h = nullptr; ~Resource() { if (h) mnnb200_exec_destroy(h); } };
-    LinearW8Exec(Backend* bn, std::shared_ptr<Resource> r, int ic, int oc) : B200Exec(bn), mRes(r), mIc(ic), mOc(oc) {}
-    ~LinearW8Exec() override { release(); }
+    LinearW8Exec(B200Backend* bn, mnnb200_exec* h, int ic, int oc)
+        : B200Exec(bn), mH(h), mIc(ic), mOc(oc), mX(bn->handle()), mY(bn->handle()) {}
     static Execution* create(B200Backend* bn, const Op* op) {
         auto conv = op->main_as_Convolution2D();
         auto cm = conv->common();
@@ -615,51 +643,39 @@ public:
         }
         const bool hasBias = conv->bias() && (int)conv->bias()->size() == oc;
         if (hasBias) ::memcpy(bias.data(), conv->bias()->data(), sizeof(float) * oc);
-        std::shared_ptr<Resource> res(new Resource);
+        mnnb200_exec* h = nullptr;
         if (mnnb200_linear_w8_create_blocked(bn->handle(), ic, oc, blocks, q->weight.get(), alpha.data(),
                                              q->asymmetric ? wzero.data() : nullptr, hasBias ? bias.data() : nullptr,
-                                             cm->relu() ? 1 : 0, cm->relu6() ? 1 : 0, &res->h) != MNNB200_OK) {
+                                             cm->relu() ? 1 : 0, cm->relu6() ? 1 : 0, &h) != MNNB200_OK) {
             MNN_ERROR("mnn_b200 linear create: %s\n", mnnb200_last_error());
             return nullptr;
         }
-        return new LinearW8Exec(bn, res, ic, oc);
+        return new LinearW8Exec(bn, h, ic, oc);
     }
     ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>&) override {
         auto d = dims4(inputs[0]);
         mN = d.n; mArea = d.h * d.w;
         const int tokens = mN * mArea;
-        release();
-        auto rt = static_cast<B200Backend*>(backend())->handle();
-        if (mArea > 1) {
-            if (mnnb200_alloc(rt, (size_t)tokens * mIc * 4, &mX) != MNNB200_OK || mnnb200_alloc(rt, (size_t)tokens * mOc * 4, &mY) != MNNB200_OK)
-                return OUT_OF_MEMORY;
-        }
-        return toErr(mnnb200_linear_w8_resize(mRes->h, tokens), "linear resize");
+        if (mArea > 1 && (!mX.get((size_t)tokens * mIc * 4) || !mY.get((size_t)tokens * mOc * 4))) return OUT_OF_MEMORY;
+        return toErr(mnnb200_linear_w8_resize(mH.get(), tokens), "linear resize");
     }
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        auto rt = static_cast<B200Backend*>(backend())->handle();
-        if (mArea == 1) return toErr(mnnb200_linear_w8_execute(mRes->h, (const float*)dev(inputs[0]), (float*)dev(outputs[0])), "linear");
-        mnnb200_status st = mnnb200_transpose_b32(rt, dev(inputs[0]), mN, mIc, mArea, mX);            // [n][ic][hw] -> [n][hw][ic]
-        if (st == MNNB200_OK) st = mnnb200_linear_w8_execute(mRes->h, (const float*)mX, (float*)mY);
-        if (st == MNNB200_OK) st = mnnb200_transpose_b32(rt, mY, mN, mArea, mOc, dev(outputs[0]));    // [n][hw][oc] -> [n][oc][hw]
+        if (mArea == 1) return toErr(mnnb200_linear_w8_execute(mH.get(), (const float*)dev(inputs[0]), (float*)dev(outputs[0])), "linear");
+        mnnb200_status st = mnnb200_transpose_b32(rt(), dev(inputs[0]), mN, mIc, mArea, mX.data());            // [n][ic][hw] -> [n][hw][ic]
+        if (st == MNNB200_OK) st = mnnb200_linear_w8_execute(mH.get(), (const float*)mX.data(), (float*)mY.data());
+        if (st == MNNB200_OK) st = mnnb200_transpose_b32(rt(), mY.data(), mN, mArea, mOc, dev(outputs[0]));    // [n][hw][oc] -> [n][oc][hw]
         return toErr(st, "linear execute");
     }
 private:
-    void release() {
-        auto rt = static_cast<B200Backend*>(backend())->handle();
-        if (mX) { mnnb200_runtime_sync(rt); mnnb200_free(rt, mX); mX = nullptr; }
-        if (mY) { mnnb200_free(rt, mY); mY = nullptr; }
-    }
-    std::shared_ptr<Resource> mRes;
+    ExecHandle mH;
     int mIc, mOc, mN = 0, mArea = 0;
-    void *mX = nullptr, *mY = nullptr;
+    DeviceScratch mX, mY;   // token-major input and output when H*W > 1
 };
 
 // MatMul on float tensors (MatMulExecution.cu's role): C[e,h] = op(A) op(B) (+ bias input)
 class MatMulExec : public B200Exec {
 public:
     MatMulExec(Backend* bn, bool ta, bool tb) : B200Exec(bn), mTa(ta), mTb(tb) {}
-    ~MatMulExec() override { if (mH) mnnb200_exec_destroy(mH); }
     ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto a = inputs[0], b = inputs[1];
         const int na = a->dimensions(), nb = b->dimensions();
@@ -672,16 +688,19 @@ public:
         const int e = mTa ? a->length(na - 1) : a->length(na - 2), l = mTa ? a->length(na - 2) : a->length(na - 1);
         const int h = mTb ? b->length(nb - 2) : b->length(nb - 1), l2 = mTb ? b->length(nb - 1) : b->length(nb - 2);
         if (l != l2) return COMPUTE_SIZE_ERROR;
-        if (mH) { mnnb200_exec_destroy(mH); mH = nullptr; }
-        return toErr(mnnb200_matmul_create(static_cast<B200Backend*>(backend())->handle(), batch, e, l, h, mTa, mTb, 0, &mH), "matmul create");
+        mH.reset();
+        mnnb200_exec* m = nullptr;
+        const mnnb200_status st = mnnb200_matmul_create(rt(), batch, e, l, h, mTa, mTb, 0, &m);
+        mH.reset(m);
+        return toErr(st, "matmul create");
     }
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         const float* bias = inputs.size() > 2 ? (const float*)dev(inputs[2]) : nullptr;
-        return toErr(mnnb200_matmul_execute(mH, dev(inputs[0]), dev(inputs[1]), bias, (float*)dev(outputs[0])), "matmul");
+        return toErr(mnnb200_matmul_execute(mH.get(), dev(inputs[0]), dev(inputs[1]), bias, (float*)dev(outputs[0])), "matmul");
     }
 private:
     bool mTa, mTb;
-    mnnb200_exec* mH = nullptr;
+    ExecHandle mH;
 };
 
 class FloatToInt8Exec : public B200Exec {
@@ -690,7 +709,7 @@ public:
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto d = dims4(inputs[0]);
         auto q = TensorUtils::getQuantInfo(outputs[0]);   // CPUCast.cpp:17-60: scale = 1/quant.scale, zero, min, max
-        return toErr(mnnb200_float_to_int8(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(inputs[0]), d.n, d.c, d.h, d.w,
+        return toErr(mnnb200_float_to_int8(rt(), (const float*)dev(inputs[0]), d.n, d.c, d.h, d.w,
                                            q[0], q[1], (int)q[2], (int)q[3], (int8_t*)dev(outputs[0])), "FloatToInt8");
     }
 };
@@ -700,7 +719,7 @@ public:
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto d = dims4(inputs[0]);
         auto q = TensorUtils::getQuantInfo(inputs[0]);
-        return toErr(mnnb200_int8_to_float(static_cast<B200Backend*>(backend())->handle(), (const int8_t*)dev(inputs[0]), d.n, d.c, d.h, d.w,
+        return toErr(mnnb200_int8_to_float(rt(), (const int8_t*)dev(inputs[0]), d.n, d.c, d.h, d.w,
                                            q[0], q[1], (float*)dev(outputs[0])), "Int8ToFloat");
     }
 };
@@ -710,64 +729,65 @@ public:
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto d = dims4(outputs[0]);
         auto q0 = TensorUtils::getQuantInfo(inputs[0]), q1 = TensorUtils::getQuantInfo(inputs[1]), qo = TensorUtils::getQuantInfo(outputs[0]);
-        return toErr(mnnb200_binary_add_int8(static_cast<B200Backend*>(backend())->handle(), (const int8_t*)dev(inputs[0]), q0[0], (int)q0[1],
+        return toErr(mnnb200_binary_add_int8(rt(), (const int8_t*)dev(inputs[0]), q0[0], (int)q0[1],
                                              (const int8_t*)dev(inputs[1]), q1[0], (int)q1[1], (int8_t*)dev(outputs[0]), qo[0], (int)qo[1],
                                              (int)qo[2], (int)qo[3], d.n, d.c, d.h, d.w), "BinaryOp add int8");
     }
 };
+// kernel, stride and begin pads of a pooling window: global, SAME and VALID pooling (CPUPool.cpp:45-66, CPUPoolInt8.cpp:180-215)
+struct PoolWindow { int kh, kw, sh, sw, ph, pw; };
+static PoolWindow poolWindow(const Pool* p, const Tensor* in, const Tensor* out) {
+    PoolWindow w = {p->kernelY(), p->kernelX(), p->strideY(), p->strideX(), p->padY(), p->padX()};
+    if (p->isGlobal()) { w.kw = in->width(); w.kh = in->height(); w.sw = w.kw; w.sh = w.kh; w.pw = w.ph = 0; }
+    if (p->padType() == PoolPadType_SAME) {
+        int nw = (out->width() - 1) * w.sw + w.kw - in->width(), nh = (out->height() - 1) * w.sh + w.kh - in->height();
+        w.pw = nw > 0 ? nw / 2 : 0; w.ph = nh > 0 ? nh / 2 : 0;
+    } else if (p->padType() == PoolPadType_VALID) {
+        w.pw = w.ph = 0;
+    }
+    return w;
+}
 class PoolF32Exec : public B200Exec {
 public:
     PoolF32Exec(Backend* bn, const Pool* p) : B200Exec(bn), mP(p) {}
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto in = inputs[0], out = outputs[0];
-        int kw = mP->kernelX(), kh = mP->kernelY(), sw = mP->strideX(), sh = mP->strideY(), pw = mP->padX(), ph = mP->padY();
+        auto w = poolWindow(mP, in, out);
         int padType = (int)mP->padType();
-        if (mP->isGlobal()) { kw = in->width(); kh = in->height(); sw = kw; sh = kh; pw = ph = 0; }   // CPUPool.cpp:45-52
-        if (mP->padType() == PoolPadType_SAME) {
-            int nw = (out->width() - 1) * sw + kw - in->width(), nh = (out->height() - 1) * sh + kh - in->height();
-            pw = nw > 0 ? nw / 2 : 0; ph = nh > 0 ? nh / 2 : 0;
-        } else if (mP->padType() == PoolPadType_VALID) {
-            pw = ph = 0;
-        }
         if (!mP->isGlobal() && mP->pads() != nullptr && mP->padType() == PoolPadType_CAFFE) {   // CPUPool.cpp:67-73
-            if (mP->pads()->size() == 4) { ph = mP->pads()->data()[0]; pw = mP->pads()->data()[1]; }
+            if (mP->pads()->size() == 4) { w.ph = mP->pads()->data()[0]; w.pw = mP->pads()->data()[1]; }
             padType = (int)PoolPadType_VALID;   // any pads vector: DEFAULT counting then excludes the padding
         }
-        return toErr(mnnb200_pool_f32(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(in), in->batch(), in->channel(),
-                                      in->height(), in->width(), kh, kw, sh, sw, ph, pw, padType, (int)mP->countType(),
+        return toErr(mnnb200_pool_f32(rt(), (const float*)dev(in), in->batch(), in->channel(),
+                                      in->height(), in->width(), w.kh, w.kw, w.sh, w.sw, w.ph, w.pw, padType, (int)mP->countType(),
                                       mP->type() == PoolType_AVEPOOL ? 1 : 0, (float*)dev(out), out->height(), out->width()), "Pooling");
     }
 private:
     const Pool* mP;
 };
 // int8 Scale (CPUScaleInt8's role): per-channel fixed-point scale + bias between int8 tensors
-class ScaleInt8Exec : public B200Exec {
+class ScaleInt8Exec : public ClonedFromOp<ScaleInt8Exec> {
 public:
-    struct Resource { mnnb200_exec* h = nullptr; ~Resource() { if (h) mnnb200_exec_destroy(h); } };
-    ScaleInt8Exec(Backend* bn, std::shared_ptr<Resource> r) : B200Exec(bn), mRes(r) {}
+    ScaleInt8Exec(Backend* bn, mnnb200_exec* h) : ClonedFromOp(bn), mH(h) {}
     static Execution* create(B200Backend* bn, const Op* op) {
         auto sc = op->main_as_Scale();
         if (!sc || !sc->scaleData()) return nullptr;
         const int c = (int)sc->scaleData()->size();
         const float* bias = (sc->biasData() && (int)sc->biasData()->size() == c) ? sc->biasData()->data() : nullptr;
-        std::shared_ptr<Resource> res(new Resource);
-        if (mnnb200_scale_int8_create(bn->handle(), c, sc->scaleData()->data(), bias, &res->h) != MNNB200_OK) return nullptr;
-        return new ScaleInt8Exec(bn, res);
+        mnnb200_exec* h = nullptr;
+        if (mnnb200_scale_int8_create(bn->handle(), c, sc->scaleData()->data(), bias, &h) != MNNB200_OK) return nullptr;
+        return new ScaleInt8Exec(bn, h);
     }
     ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto qi = TensorUtils::getQuantInfo(inputs[0]), qo = TensorUtils::getQuantInfo(outputs[0]);
-        return toErr(mnnb200_scale_int8_resize(mRes->h, qi[0], (int)qi[1], qo[0], (int)qo[1], (int)qo[2], (int)qo[3]), "Scale resize");
+        return toErr(mnnb200_scale_int8_resize(mH.get(), qi[0], (int)qi[1], qo[0], (int)qo[1], (int)qo[2], (int)qo[3]), "Scale resize");
     }
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto d = dims4(inputs[0]);
-        return toErr(mnnb200_scale_int8_execute(mRes->h, (const int8_t*)dev(inputs[0]), d.n, d.h, d.w, (int8_t*)dev(outputs[0])), "Scale int8");
-    }
-    bool onClone(Backend* bn, const Op* op, Execution** dst) override {
-        if (dst) *dst = create(static_cast<B200Backend*>(bn), op);
-        return true;
+        return toErr(mnnb200_scale_int8_execute(mH.get(), (const int8_t*)dev(inputs[0]), d.n, d.h, d.w, (int8_t*)dev(outputs[0])), "Scale int8");
     }
 private:
-    std::shared_ptr<Resource> mRes;
+    ExecHandle mH;
 };
 // int8 Pooling between tensors with equal quant attrs (CPUPoolInt8's role, x86 semantics)
 class PoolInt8Exec : public B200Exec {
@@ -775,16 +795,9 @@ public:
     PoolInt8Exec(Backend* bn, const Pool* p) : B200Exec(bn), mP(p) {}
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto in = inputs[0], out = outputs[0];
-        int kw = mP->kernelX(), kh = mP->kernelY(), sw = mP->strideX(), sh = mP->strideY(), pw = mP->padX(), ph = mP->padY();
-        if (mP->isGlobal()) { kw = in->width(); kh = in->height(); sw = kw; sh = kh; pw = ph = 0; }          // CPUPoolInt8.cpp:180-215
-        if (mP->padType() == PoolPadType_SAME) {
-            int nw = (out->width() - 1) * sw + kw - in->width(), nh = (out->height() - 1) * sh + kh - in->height();
-            pw = nw > 0 ? nw / 2 : 0; ph = nh > 0 ? nh / 2 : 0;
-        } else if (mP->padType() == PoolPadType_VALID) {
-            pw = ph = 0;
-        }
-        return toErr(mnnb200_pool_int8(static_cast<B200Backend*>(backend())->handle(), (const int8_t*)dev(in), in->batch(), in->channel(),
-                                       in->height(), in->width(), kh, kw, sh, sw, ph, pw, mP->type() == PoolType_AVEPOOL ? 1 : 0,
+        auto w = poolWindow(mP, in, out);
+        return toErr(mnnb200_pool_int8(rt(), (const int8_t*)dev(in), in->batch(), in->channel(),
+                                       in->height(), in->width(), w.kh, w.kw, w.sh, w.sw, w.ph, w.pw, mP->type() == PoolType_AVEPOOL ? 1 : 0,
                                        (int8_t*)dev(out), out->height(), out->width()), "Pooling int8");
     }
 private:
@@ -794,7 +807,7 @@ class ReluF32Exec : public B200Exec {
 public:
     ReluF32Exec(Backend* bn, float slope) : B200Exec(bn), mSlope(slope) {}
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        return toErr(mnnb200_relu_f32(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(inputs[0]), elemCount(inputs[0]), mSlope,
+        return toErr(mnnb200_relu_f32(rt(), (const float*)dev(inputs[0]), elemCount(inputs[0]), mSlope,
                                       (float*)dev(outputs[0])), "ReLU");
     }
 private:
@@ -806,7 +819,7 @@ public:
     ReduceF32Exec(Backend* bn, int op) : B200Exec(bn), mOp(op) {}
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto in = inputs[0];
-        return toErr(mnnb200_reduce_f32(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(in), in->length(0), in->length(1),
+        return toErr(mnnb200_reduce_f32(rt(), (const float*)dev(in), in->length(0), in->length(1),
                                         in->length(2), mOp, (float*)dev(outputs[0])), "Reduction");
     }
 private:
@@ -818,7 +831,7 @@ public:
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto d = dims4(inputs[0]);
         auto qi = TensorUtils::getQuantInfo(inputs[0]), qo = TensorUtils::getQuantInfo(outputs[0]);
-        return toErr(mnnb200_softmax_int8(static_cast<B200Backend*>(backend())->handle(), (const int8_t*)dev(inputs[0]), d.n, d.c, qi[0], qi[1],
+        return toErr(mnnb200_softmax_int8(rt(), (const int8_t*)dev(inputs[0]), d.n, d.c, qi[0], qi[1],
                                           qo[0], qo[1], (int)qo[2], (int)qo[3], (int8_t*)dev(outputs[0])), "Softmax int8");
     }
 };
@@ -846,7 +859,7 @@ public:
             for (int k = 0; k < 3; ++k) { g.src_stride[k] = r.src.stride[k]; g.dst_stride[k] = r.dst.stride[k]; g.size[k] = r.size[k]; }
             regs.push_back(g);
         }
-        return toErr(mnnb200_raster_b32(static_cast<B200Backend*>(backend())->handle(), regs.data(), (int)regs.size(), dev(out),
+        return toErr(mnnb200_raster_b32(rt(), regs.data(), (int)regs.size(), dev(out),
                                         elemCount(out) * 4, mZero ? 1 : 0), "Raster");
     }
 private:
@@ -858,10 +871,9 @@ static bool isF32Nchw(const Tensor* t) {
     return t->getType().code == halide_type_float && t->getType().bytes() == 4 && linearFormat(t) == MNN_DATA_FORMAT_NCHW;
 }
 // Convolution (group 1, split-TF32 wgmma) and ConvolutionDepthwise (also a Convolution whose group == ic == oc) on float tensors
-class ConvF32Exec : public B200Exec {
+class ConvF32Exec : public ClonedFromOp<ConvF32Exec> {
 public:
-    struct Resource { mnnb200_exec* h = nullptr; ~Resource() { if (h) mnnb200_exec_destroy(h); } };
-    ConvF32Exec(Backend* bn, const Op* op, std::shared_ptr<Resource> res, bool dw) : B200Exec(bn), mOp(op), mRes(res), mDepthwise(dw) {}
+    ConvF32Exec(Backend* bn, const Op* op, mnnb200_exec* h, bool dw, int ic) : ClonedFromOp(bn), mOp(op), mH(h), mDepthwise(dw), mIc(ic) {}
     static Execution* create(B200Backend* bn, const Op* op) {
         auto conv = op->main_as_Convolution2D();
         if (!conv || !conv->common()) return nullptr;
@@ -882,16 +894,14 @@ public:
         d.pad_h = 0; d.pad_w = 0; d.dilate_h = cm->dilateY(); d.dilate_w = cm->dilateX();   // pads: set at resize
         d.group = dw ? oc : 1; d.relu = cm->relu() ? 1 : 0;
         const float* bias = (conv->bias() && (int)conv->bias()->size() == oc) ? conv->bias()->data() : nullptr;
-        std::shared_ptr<Resource> res(new Resource);
-        mnnb200_status st = dw ? mnnb200_dwconv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &res->h)
-                               : mnnb200_conv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &res->h);
+        mnnb200_exec* h = nullptr;
+        mnnb200_status st = dw ? mnnb200_dwconv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &h)
+                               : mnnb200_conv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &h);
         if (st != MNNB200_OK) {
             if (st != MNNB200_NOT_SUPPORT) MNN_ERROR("mnn_b200 float conv create: %s\n", mnnb200_last_error());
             return nullptr;
         }
-        auto e = new ConvF32Exec(bn, op, res, dw);
-        e->mIc = ic;
-        return e;
+        return new ConvF32Exec(bn, op, h, dw, ic);
     }
     ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto in = inputs[0], out = outputs[0];
@@ -901,30 +911,22 @@ public:
         }
         auto pad = ConvolutionCommon::convolutionPad(in, out, mOp->main_as_Convolution2D()->common());   // (padX, padY)
         int oh = out->height(), ow = out->width();
-        mnnb200_status st = mnnb200_conv_f32_set_pad(mRes->h, pad.second, pad.first);
+        mnnb200_status st = mnnb200_conv_f32_set_pad(mH.get(), pad.second, pad.first);
         if (st == MNNB200_OK)
-            st = mDepthwise ? mnnb200_dwconv_f32_resize(mRes->h, in->batch(), in->height(), in->width(), &oh, &ow)
-                            : mnnb200_conv_f32_resize(mRes->h, in->batch(), in->height(), in->width(), &oh, &ow);
+            st = mDepthwise ? mnnb200_dwconv_f32_resize(mH.get(), in->batch(), in->height(), in->width(), &oh, &ow)
+                            : mnnb200_conv_f32_resize(mH.get(), in->batch(), in->height(), in->width(), &oh, &ow);
         return toErr(st, "float conv resize");
     }
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto x = (const float*)dev(inputs[0]);
         auto y = (float*)dev(outputs[0]);
-        return toErr(mDepthwise ? mnnb200_dwconv_f32_execute(mRes->h, x, y) : mnnb200_conv_f32_execute(mRes->h, x, y), "float conv");
-    }
-    // a clone owns its own resize state (the launch plan lives in the C execution), so the packed weights are made again from the op
-    bool onClone(Backend* bn, const Op* op, Execution** dst) override {
-        if (dst) {
-            *dst = create(static_cast<B200Backend*>(bn), op);
-            if (*dst == nullptr) return false;
-        }
-        return true;
+        return toErr(mDepthwise ? mnnb200_dwconv_f32_execute(mH.get(), x, y) : mnnb200_conv_f32_execute(mH.get(), x, y), "float conv");
     }
 private:
     const Op* mOp;
-    std::shared_ptr<Resource> mRes;
+    ExecHandle mH;
     bool mDepthwise;
-    int mIc = 0;
+    int mIc;
 };
 static bool isF32(const Tensor* t) { return t->getType().code == halide_type_float && t->getType().bytes() == 4; }
 // a full-size operand has the output's bytes: the same linear layout, or both of <= 2 dims (NCHW and NHWC are then the same)
@@ -958,7 +960,7 @@ public:
         return full >= 1 || n == 1;
     }
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        return toErr(mnnb200_binary_f32(static_cast<B200Backend*>(backend())->handle(), mOp, (const float*)dev(inputs[0]), elemCount(inputs[0]),
+        return toErr(mnnb200_binary_f32(rt(), mOp, (const float*)dev(inputs[0]), elemCount(inputs[0]),
                                         (const float*)dev(inputs[1]), elemCount(inputs[1]), (float*)dev(outputs[0]), elemCount(outputs[0]),
                                         mRelu), "BinaryOp fp32");
     }
@@ -979,12 +981,11 @@ public:
         }
     }
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        auto rt = static_cast<B200Backend*>(backend())->handle();
         const size_t n = elemCount(outputs[0]);
         auto y = (float*)dev(outputs[0]);
-        mnnb200_status st = mnnb200_binary_f32(rt, mOp, (const float*)dev(inputs[0]), n, (const float*)dev(inputs[1]), n, y, n, 0);
+        mnnb200_status st = mnnb200_binary_f32(rt(), mOp, (const float*)dev(inputs[0]), n, (const float*)dev(inputs[1]), n, y, n, 0);
         for (size_t i = 2; st == MNNB200_OK && i < inputs.size(); ++i)
-            st = mnnb200_binary_f32(rt, mOp, y, n, (const float*)dev(inputs[i]), n, y, n, 0);
+            st = mnnb200_binary_f32(rt(), mOp, y, n, (const float*)dev(inputs[i]), n, y, n, 0);
         return toErr(st, "Eltwise fp32");
     }
 private:
@@ -1005,66 +1006,63 @@ public:
         }
     }
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        return toErr(mnnb200_unary_f32(static_cast<B200Backend*>(backend())->handle(), mOp, (const float*)dev(inputs[0]),
+        return toErr(mnnb200_unary_f32(rt(), mOp, (const float*)dev(inputs[0]),
                                        (float*)dev(outputs[0]), elemCount(outputs[0])), "UnaryOp fp32");
     }
 private:
     int mOp;
 };
+// a tensor as [outside][axis][inside] around one of its dimensions
+struct AxisSplit { int outside, axis, inside; };
+static AxisSplit splitAt(const Tensor* t, int axis) {
+    AxisSplit s = {1, t->length(axis), 1};
+    for (int i = 0; i < axis; ++i) s.outside *= t->length(i);
+    for (int i = axis + 1; i < t->dimensions(); ++i) s.inside *= t->length(i);
+    return s;
+}
 // ArgMax / ArgMin with one index per position and no values (CPUArgMax's non-NC4HW4 branch): int32 output
 class ArgMaxExec : public B200Exec {
 public:
     ArgMaxExec(Backend* bn, int axis, bool isMin) : B200Exec(bn), mAxis(axis), mIsMin(isMin) {}
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        auto in = inputs[0];
-        int outside = 1, inside = 1;
-        for (int i = 0; i < mAxis; ++i) outside *= in->length(i);
-        for (int i = mAxis + 1; i < in->dimensions(); ++i) inside *= in->length(i);
-        return toErr(mnnb200_argmax_f32(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(in), outside, in->length(mAxis),
-                                        inside, mIsMin ? 1 : 0, (int32_t*)dev(outputs[0])), "ArgMax");
+        auto s = splitAt(inputs[0], mAxis);
+        return toErr(mnnb200_argmax_f32(rt(), (const float*)dev(inputs[0]), s.outside, s.axis, s.inside, mIsMin ? 1 : 0,
+                                        (int32_t*)dev(outputs[0])), "ArgMax");
     }
 private:
     int mAxis;
     bool mIsMin;
 };
-class ScaleF32Exec : public B200Exec {
+class ScaleF32Exec : public ClonedFromOp<ScaleF32Exec> {
 public:
-    struct Resource { mnnb200_exec* h = nullptr; ~Resource() { if (h) mnnb200_exec_destroy(h); } };
-    ScaleF32Exec(Backend* bn, std::shared_ptr<Resource> r) : B200Exec(bn), mRes(r) {}
+    ScaleF32Exec(Backend* bn, mnnb200_exec* h) : ClonedFromOp(bn), mH(h) {}
     static Execution* create(B200Backend* bn, const Op* op) {
         auto sc = op->main_as_Scale();
         if (!sc || !sc->scaleData()) return nullptr;
         const int c = (int)sc->scaleData()->size();
         const float* bias = (sc->biasData() && (int)sc->biasData()->size() == c) ? sc->biasData()->data() : nullptr;
-        std::shared_ptr<Resource> res(new Resource);
-        if (mnnb200_scale_f32_create(bn->handle(), c, sc->scaleData()->data(), bias, &res->h) != MNNB200_OK) return nullptr;
-        return new ScaleF32Exec(bn, res);
+        mnnb200_exec* h = nullptr;
+        if (mnnb200_scale_f32_create(bn->handle(), c, sc->scaleData()->data(), bias, &h) != MNNB200_OK) return nullptr;
+        return new ScaleF32Exec(bn, h);
     }
     ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>&) override {
         auto d = dims4(inputs[0]);
-        return toErr(mnnb200_scale_f32_resize(mRes->h, d.n, d.h, d.w), "Scale fp32 resize");
+        return toErr(mnnb200_scale_f32_resize(mH.get(), d.n, d.h, d.w), "Scale fp32 resize");
     }
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        return toErr(mnnb200_scale_f32_execute(mRes->h, (const float*)dev(inputs[0]), (float*)dev(outputs[0])), "Scale fp32");
-    }
-    bool onClone(Backend* bn, const Op* op, Execution** dst) override {
-        if (dst) *dst = create(static_cast<B200Backend*>(bn), op);
-        return true;
+        return toErr(mnnb200_scale_f32_execute(mH.get(), (const float*)dev(inputs[0]), (float*)dev(outputs[0])), "Scale fp32");
     }
 private:
-    std::shared_ptr<Resource> mRes;
+    ExecHandle mH;
 };
 // Softmax over one axis of an [outside][axis][inside] view (CPUSoftmax.cpp)
 class SoftmaxF32Exec : public B200Exec {
 public:
     SoftmaxF32Exec(Backend* bn, int axis) : B200Exec(bn), mAxis(axis) {}
     ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
-        auto in = inputs[0];
-        int outside = 1, inside = 1;
-        for (int i = 0; i < mAxis; ++i) outside *= in->length(i);
-        for (int i = mAxis + 1; i < in->dimensions(); ++i) inside *= in->length(i);
-        return toErr(mnnb200_softmax_f32(static_cast<B200Backend*>(backend())->handle(), (const float*)dev(in), outside, in->length(mAxis),
-                                         inside, (float*)dev(outputs[0])), "Softmax fp32");
+        auto s = splitAt(inputs[0], mAxis);
+        return toErr(mnnb200_softmax_f32(rt(), (const float*)dev(inputs[0]), s.outside, s.axis, s.inside, (float*)dev(outputs[0])),
+                     "Softmax fp32");
     }
 private:
     int mAxis;
@@ -1078,7 +1076,7 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
         case OpType_Convolution:
         case OpType_ConvInt8:
             if (quantOut || op->type() == OpType_ConvInt8) {
-                e = ConvInt8Exec::create(this, op, false);
+                e = ConvInt8Exec::create(this, op);
             } else if (mMemoryLow && inputs.size() == 1 && op->main_as_Convolution2D() && op->main_as_Convolution2D()->quanParameter() &&
                        inputs[0]->getType().code == halide_type_float && linearFormat(inputs[0]) == MNN_DATA_FORMAT_NCHW) {
                 e = LinearW8Exec::create(this, op);   // weight-quantised conv on float tensors: W8A8 only under Memory_Low, like the CPU
@@ -1096,7 +1094,7 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
             break;
         case OpType_ConvolutionDepthwise:
         case OpType_DepthwiseConvInt8:
-            if (quantOut || op->type() == OpType_DepthwiseConvInt8) e = ConvInt8Exec::create(this, op, true);
+            if (quantOut || op->type() == OpType_DepthwiseConvInt8) e = ConvInt8Exec::create(this, op);
             else if (inputs.size() == 1 && isF32Nchw(inputs[0])) e = ConvF32Exec::create(this, op);
             break;
         case OpType_FloatToInt8:   // the cast kernels read/write NCHW-linear fp32 (NHWC-format tensors of <= 2 dims are the same bytes)

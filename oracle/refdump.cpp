@@ -17,6 +17,7 @@
 #include <MNN/expr/ExprCreator.hpp>
 #include <MNN/expr/Executor.hpp>
 #include <MNN/expr/ExecutorScope.hpp>
+#include <MNN/expr/Module.hpp>
 #include "MNN_generated.h"
 #include "core/TensorUtils.hpp"
 #include "core/ConvolutionCommon.hpp"
@@ -531,7 +532,7 @@ static void fillInput(Tensor* input, int seed) {
 // a second time: CPUScaleInt8::onResize folds its float scale/bias into fixed point IN PLACE (CPUScaleInt8.cpp:60-90), a second
 // resize re-reads the folded integers as floats and the op outputs nothing but the zero point from then on -- an upstream bug that
 // has nothing to do with the arithmetic under test.
-static std::shared_ptr<Interpreter> loadWithBatch(const char* model, int batch) {
+static std::vector<uint8_t> netWithBatch(const char* model, int batch) {
     auto buf = readFile(model);
     std::unique_ptr<NetT> net(UnPackNet(buf.data()));
     for (auto& op : net->oplists) {
@@ -541,7 +542,11 @@ static std::shared_ptr<Interpreter> loadWithBatch(const char* model, int batch) 
     }
     flatbuffers::FlatBufferBuilder fb(1024);
     fb.Finish(Net::Pack(fb, net.get()));
-    return std::shared_ptr<Interpreter>(Interpreter::createFromBuffer(fb.GetBufferPointer(), fb.GetSize()), Interpreter::destroy);
+    return std::vector<uint8_t>(fb.GetBufferPointer(), fb.GetBufferPointer() + fb.GetSize());
+}
+static std::shared_ptr<Interpreter> loadWithBatch(const char* model, int batch) {
+    auto buf = netWithBatch(model, batch);
+    return std::shared_ptr<Interpreter>(Interpreter::createFromBuffer(buf.data(), buf.size()), Interpreter::destroy);
 }
 
 // run <model.mnn> <batch> <seed> <outdir> <threads>: dump the input and every command's outputs
@@ -610,6 +615,54 @@ static int cmdRun(const char* model, int batch, int seed, const std::string& dir
         Tensor host(output, Tensor::CAFFE);
         output->copyToHostTensor(&host);
         writeFile(dir + "/output.f32", host.host<float>(), host.size());
+    }
+    pluginStats();
+    return 0;
+}
+
+// clone <model.mnn> <batch> <outdir> [<tensor>]: the model as an Express Module (express/module: StaticModule over one Session) on
+// the forward type, run once so that every execution is created, then copied with Module::clone, which goes StaticModule::clone ->
+// Session::clone -> Execution::onClone for each cached execution (StaticModule.cpp:814-828, Session.cpp:612-625).  The original
+// and the clone then run on the same seeded input (fillInput's values); their first outputs go to output.f32 and
+// output_clone.f32, the original's first forward to output_first.f32.  A plugin's stats are printed after the first forward
+// and at the end.  <tensor>: the module's output is that tensor instead of the model's outputs.
+static int cmdClone(const char* model, int batch, const std::string& dir, const char* output) {
+    const auto buf = netWithBatch(model, batch);   // outlives both modules
+    ScheduleConfig c; c.type = forwardType(); c.numThread = 4; c.backupType = MNN_FORWARD_CPU;
+    BackendConfig bc; bc.precision = BackendConfig::Precision_High; c.backendConfig = &bc;
+    std::shared_ptr<Executor::RuntimeManager> rtm(Executor::RuntimeManager::createRuntimeManager(c));
+    std::vector<std::string> outputs;
+    if (output) outputs.push_back(output);
+    std::shared_ptr<Module> net(Module::load({}, outputs, buf.data(), buf.size(), rtm));
+    if (!net) { fprintf(stderr, "refdump clone: Module::load failed\n"); return 2; }
+    const auto& in = net->getInfo()->inputs[0];
+    VARP x = _Input(in.dim, NCHW, halide_type_of<float>());
+    {
+        std::mt19937 rng(3);
+        std::uniform_real_distribution<float> u(-1.f, 1.f);
+        auto p = x->writeMap<float>();
+        const int n = x->getInfo()->size;
+        for (int i = 0; i < n; ++i) p[i] = u(rng);
+    }
+    if (in.order == NC4HW4) x = _Convert(x, NC4HW4);
+    x.fix(VARP::CONSTANT);
+    auto forward = [&](Module* m, const char* name) {
+        auto outs = m->onForward({x});
+        if (outs.empty() || !outs[0]->getInfo()) return false;
+        VARP y = outs[0];
+        if (y->getInfo()->order == NC4HW4 && y->getInfo()->dim.size() > 1) y = _Convert(y, NCHW);
+        auto p = y->readMap<float>();
+        if (!p) return false;
+        writeFile(dir + "/" + name, p, (size_t)y->getInfo()->size * 4);
+        return true;
+    };
+    if (!forward(net.get(), "output_first.f32")) { fprintf(stderr, "refdump clone: first forward failed\n"); return 2; }
+    pluginStats();   // the original's executions; the last line adds what the clone had to create instead of cloning
+    std::shared_ptr<Module> copy(Module::clone(net.get()));
+    if (!copy) { fprintf(stderr, "refdump clone: Module::clone failed\n"); return 2; }
+    if (!forward(net.get(), "output.f32") || !forward(copy.get(), "output_clone.f32")) {
+        fprintf(stderr, "refdump clone: forward failed\n");
+        return 2;
     }
     pluginStats();
     return 0;
@@ -739,7 +792,7 @@ static int cmdExport(const char* model, const std::string& dir) {
 }
 
 int main(int argc, char** argv) {
-    if (argc < 2) { fprintf(stderr, "usage: refdump conv|linear|revert|run|bench|convbench|export ...\n"); return 1; }
+    if (argc < 2) { fprintf(stderr, "usage: refdump conv|linear|revert|run|clone|bench|convbench|export ...\n"); return 1; }
     std::string cmd = argv[1];
     if (cmd == "conv" && argc >= 4) return cmdConv(argv[2], argv[3]);
     if (cmd == "pool" && argc >= 4) return cmdPool(argv[2], argv[3]);
@@ -749,6 +802,7 @@ int main(int argc, char** argv) {
     if (cmd == "linear" && argc >= 4) return cmdLinear(argv[2], argv[3], argc > 4 ? atoi(argv[4]) : 1);
     if (cmd == "revert" && argc >= 6) return cmdRevert(argv[2], argv[3], atoi(argv[4]), atoi(argv[5]));
     if (cmd == "run" && argc >= 7) return cmdRun(argv[2], atoi(argv[3]), atoi(argv[4]), argv[5], atoi(argv[6]));
+    if (cmd == "clone" && argc >= 5) return cmdClone(argv[2], atoi(argv[3]), argv[4], argc > 5 ? argv[5] : nullptr);
     if (cmd == "bench" && argc >= 7) return cmdBench(argv[2], atoi(argv[3]), atoi(argv[4]), atoi(argv[5]), atoi(argv[6]));
     if (cmd == "convbench" && argc >= 8) return cmdConvBench(argv[2], argv[3], atoi(argv[4]), atoi(argv[5]), atoi(argv[6]), atoi(argv[7]));
     if (cmd == "export" && argc >= 4) return cmdExport(argv[2], argv[3]);

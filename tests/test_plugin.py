@@ -178,6 +178,53 @@ def test_plugin_graph_replay_and_mid_run_interrupt_match_cpu_backend():
 
 
 @pytest.mark.gpu
+@pytest.mark.parametrize("model_name", ["r50_int8.mnn", "r50_f32.mnn"])
+def test_module_clone_on_plugin_matches_original(model_name):
+    """Module::clone of a model loaded as an Express Module reaches Session::clone -> Execution::onClone: the int8 / fp32
+    convolutions and Scales are cloned (made again from their op), the other executions are created again.  After one forward,
+    the original and its clone run on the same input: nothing declined, the clone's logits bit-identical to the original's, and
+    both within the model tests' tolerance of MNN_FORWARD_CPU's original (int8: equal, fp32: 1e-3 of max|ref|).  The [N, 1001]
+    logits, not the model's output: r50_int8's int8 Softmax rounds every probability to the same code.  Not the logits
+    convolution's own NC4HW4 output either: the Module hands it to the host as a CPU-backend NC4HW4 tensor, whose x86 channel
+    pack the plugin does not take (INTEGRATION.md, known limits).
+    The plugin counts only the executions its onCreate makes: the original's first forward must have created at least one per
+    Convolution / Scale op, and the clone's forward must have created at least that many fewer than the original did, so the
+    clone ran on executions that onClone returned."""
+    from mnn_b200 import mnn_file
+    _need_ref_and_plugin()
+    model = os.path.join(O.REF_DIR, model_name)
+    if not os.path.exists(model):
+        pytest.skip(f"{model_name} not generated (build() writes it where the reference exists)")
+    clonable = sum(op.type in ("Convolution", "Scale") for op in mnn_file.load(model).ops)
+    assert clonable >= 70
+    with tempfile.TemporaryDirectory() as d:
+        outs = {}
+        for side, env in (("cpu", {k: v for k, v in _plugin_env().items() if k != "REFDUMP_PLUGIN"}), ("gpu", _plugin_env())):
+            os.makedirs(os.path.join(d, side))
+            r = subprocess.run([O.REFDUMP, "clone", model, "2", os.path.join(d, side), "resnet_v2_50/SpatialSqueeze"],
+                               env=env, capture_output=True, text=True, timeout=900)
+            assert r.returncode == 0, r.stderr[-2000:] + r.stdout[-500:]
+            outs[side] = [np.fromfile(os.path.join(d, side, f), np.float32)
+                          for f in ("output_first.f32", "output.f32", "output_clone.f32")]
+        stats = [json.loads(l) for l in r.stdout.splitlines() if l.startswith("{\"plugin_")]
+    assert len(stats) == 2, r.stdout[-2500:]
+    first, last = stats
+    assert first["plugin_declined"] == 0 and last["plugin_declined"] == 0, f"commands fell back to the CPU backend: {stats}"
+    assert first["plugin_created"] >= clonable, f"the original did not run on the plugin: {stats}"
+    assert last["plugin_created"] - first["plugin_created"] <= first["plugin_created"] - clonable, \
+        f"the clone created its {clonable} Convolution / Scale executions again instead of cloning them: {stats}"
+    ref = outs["cpu"][1]
+    first_run, original, clone = outs["gpu"]
+    assert ref.size == 2 * 1001 and np.unique(ref).size > 10 and original.shape == ref.shape and clone.shape == ref.shape
+    assert np.array_equal(first_run, original), "the original's two forwards differ"
+    assert np.array_equal(original, clone), f"{np.count_nonzero(original != clone)} of {clone.size} logits of the clone differ"
+    if "int8" in model_name:
+        assert np.array_equal(original, ref), f"{np.count_nonzero(original != ref)} of {ref.size} int8 logits differ from the CPU's"
+    else:
+        assert np.abs(original - ref).max() <= 1e-3 * np.abs(ref).max()
+
+
+@pytest.mark.gpu
 @pytest.mark.parametrize("model_name", ["r50_int8.mnn", "r50_int8_eq.mnn"])
 def test_resnet50_int8_on_plugin_matches_cpu_backend(model_name):
     """BASELINE configs[2] as a MODEL: ResNet-50 (v2) int8 from the reference's weight-less benchmark graph + its own Revert tool
