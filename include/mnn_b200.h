@@ -291,6 +291,16 @@ MNNB200_API mnnb200_status mnnb200_linear_w8_create(mnnb200_runtime* rt, int ic,
 MNNB200_API mnnb200_status mnnb200_linear_w8_create_blocked(mnnb200_runtime* rt, int ic, int oc, int blocks, const int8_t* wq,
                                                             const float* alpha, const float* wzero, const float* bias,
                                                             int relu, int relu6, mnnb200_exec** out);
+/* 4-bit weights (MNN-LLM's default export, --quant_bit 4): wpacked is the buffer ConvolutionCommon::load(..., forceInt8 = true)
+ * returns for a 4-bit layer (canUseInt4): oc * ic / 2 bytes of unsigned nibbles u = q + 8, the even index in the high nibble;
+ * alpha / wzero as for mnnb200_linear_w8_create_blocked (wzero as load() returns it, already min - clampMin * scale), blocks == 1
+ * per channel.  The device keeps the nibbles (repacked once, no int8 copy) and the per-block constants; the GEMV streams them and
+ * the GEMM expands each K block in shared memory.  The arithmetic is the reference's 4-bit executor's
+ * (mnn_oracle_linear_w4_dynamic_blocks bit for bit).  Returns a linear execution: resize / execute / set_variant as above, with the
+ * same block rules; an odd ic, and the CTA-pair variant (3), return NOT_SUPPORT. */
+MNNB200_API mnnb200_status mnnb200_linear_w4_create_blocked(mnnb200_runtime* rt, int ic, int oc, int blocks, const uint8_t* wpacked,
+                                                            const float* alpha, const float* wzero, const float* bias,
+                                                            int relu, int relu6, mnnb200_exec** out);
 MNNB200_API mnnb200_status mnnb200_linear_w8_resize(mnnb200_exec* e, int tokens);
 MNNB200_API mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* e, const float* x, float* y);
 

@@ -58,6 +58,7 @@ class Op:
     wscale: Optional[np.ndarray] = None   # quanParameter.alpha (modern) or symmetricQuan.scale (legacy)
     bias: Optional[np.ndarray] = None     # float (modern) or int32 (legacy)
     wzero: Optional[np.ndarray] = None    # asymmetric weight offsets (LinearW8)
+    bits: int = 8                         # LinearW8 weight bits: 4 = weight holds oc * ic / 2 packed nibbles as load() returns them
     legacy: bool = False
     relu6: bool = False
     extra: dict = field(default_factory=dict)
@@ -369,11 +370,23 @@ class LinearW8Execution(Execution):
 
     def __init__(self, backend, op: Op):
         super().__init__(backend)
-        wq = np.ascontiguousarray(op.weight, np.int8).reshape(op.conv["oc"], op.conv["ic"])
         al = np.ascontiguousarray(op.wscale, np.float32)
         wz = None if op.wzero is None else np.ascontiguousarray(op.wzero, np.float32)
         b = None if op.bias is None else np.ascontiguousarray(op.bias, np.float32)
         relu = int(bool(op.conv.get("relu", False)))
+        self.oc = op.conv["oc"]
+        if op.bits == 4:        # alpha [oc] or [oc, blocks], wzero of the same shape or None
+            wp = np.ascontiguousarray(op.weight, np.uint8).reshape(-1)
+            if wp.size * 2 != op.conv["oc"] * op.conv["ic"]:
+                raise MnnB200Error(f"LinearW8 bits=4: {wp.size} packed bytes for oc {op.conv['oc']} x ic {op.conv['ic']}")
+            check(_capi.lib().mnnb200_linear_w4_create_blocked(backend.runtime._h, op.conv["ic"], op.conv["oc"],
+                                                               al.shape[1] if al.ndim == 2 else 1, _np_ptr(wp), _np_ptr(al),
+                                                               _np_ptr(wz), _np_ptr(b), relu, int(op.relu6), C.byref(self._h)),
+                  "linear_w4_create_blocked")
+            return
+        if op.bits != 8:
+            raise MnnB200Error(f"LinearW8: {op.bits}-bit weights are not supported")
+        wq = np.ascontiguousarray(op.weight, np.int8).reshape(op.conv["oc"], op.conv["ic"])
         if al.ndim == 2:        # [oc, blocks]: K-blocked weight scales (quant_block), wzero of the same shape or None
             check(_capi.lib().mnnb200_linear_w8_create_blocked(backend.runtime._h, op.conv["ic"], op.conv["oc"], al.shape[1],
                                                                _np_ptr(wq), _np_ptr(al), _np_ptr(wz), _np_ptr(b), relu,
@@ -382,7 +395,6 @@ class LinearW8Execution(Execution):
             check(_capi.lib().mnnb200_linear_w8_create(backend.runtime._h, op.conv["ic"], op.conv["oc"], _np_ptr(wq),
                                                        _np_ptr(al), _np_ptr(wz), _np_ptr(b), relu, int(op.relu6),
                                                        C.byref(self._h)), "linear_w8_create")
-        self.oc = op.conv["oc"]
 
     def onResize(self, inputs, outputs):
         tokens = inputs[0].shape[0]

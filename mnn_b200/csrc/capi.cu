@@ -164,6 +164,21 @@ static mnnb200_status make_tmap_i8(CUtensorMap* m, const void* ptr, int rows, in
     if (r != CUDA_SUCCESS) return fail(MNNB200_CUDA_ERROR, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
     return MNNB200_OK;
 }
+// 4-bit weights [rows][k / 2] bytes: boxes of 64 bytes (one 128-channel K block) x box_rows, unswizzled (the GEMM expands
+// them into the 128B-swizzled int8 tile itself)
+static mnnb200_status make_tmap_w4(CUtensorMap* m, const void* ptr, int rows, int k, int box_rows) {
+    PFN_encodeTiled enc = get_encode();
+    if (!enc) return fail(MNNB200_CUDA_ERROR, "cuTensorMapEncodeTiled entry point not available");
+    cuuint64_t dims[2] = {(cuuint64_t)k / 2, (cuuint64_t)rows};
+    cuuint64_t strides[1] = {(cuuint64_t)k / 2};
+    cuuint32_t box[2] = {64u, (cuuint32_t)box_rows};
+    cuuint32_t estr[2] = {1u, 1u};
+    CUresult r = enc(m, CU_TENSOR_MAP_DATA_TYPE_UINT8, 2, const_cast<void*>(ptr), dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail(MNNB200_CUDA_ERROR, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
+    return MNNB200_OK;
+}
 // generic tiled map over uint8 data: dims/box innermost first, strides (bytes) for dims 1..rank-1; swizzle by the inner box bytes
 static mnnb200_status make_tmap_u8(CUtensorMap* m, const void* ptr, int rank, const cuuint64_t* dims, const cuuint64_t* strides,
                                    const cuuint32_t* box) {
@@ -1218,6 +1233,7 @@ struct LinearW8Exec : Tagged<kLinearW8> {
     DevBuf<float> d_talpha, d_twzero, d_tws;      // [blocks][ocp]: the GEMM's layout, ws_b precomputed
     DevBuf<int32_t> d_tw128;                      // [blocks][ocp] 128 * sum_b w
     DevBuf<float> d_xsb;                          // [tokens][blocks] xsum_b * dq (GEMM path)
+    int w4 = 0;     // 4-bit weights (mnnb200_linear_w4_create_blocked): d_w holds [ocp][icp / 2] packed nibbles, icp % 32 == 0
 };
 
 extern "C" {
@@ -1290,6 +1306,70 @@ mnnb200_status mnnb200_linear_w8_create_blocked(mnnb200_runtime* rt, int ic, int
     return MNNB200_OK;
 }
 
+// 4-bit weights.  The reference's x86 executor (ConvInt8TiledExecutor.cpp:454-458, 536-616, 807-816; the AVX512 build: GEMM
+// units H = 64, L = 4) runs them as unsigned nibbles u = q + 8 with the per-(oc, block) weight bias wb = wzero - 8 alpha
+// (-8 alpha when symmetric) and one weightKernelSum, summed over the blocks in one of two roundings (_computeReorderQuantInfo,
+// :192-280): the fast int4 reorder (oc % 64 == 0, ic % 4 == 0) sums ks_b alpha_b + bs wb_b, the other form
+// (ks_b - 8 bs) alpha_b + bs wzero_b, with ks_b = sum_b u.  The kernels keep the 8-bit epilogue: the int32 accumulator is
+// sum (xq + 128) u (128 sum u in the tables), wb takes wzero's place, and the weightKernelSum enters with the first block only
+// (_AVX512_MNNGemmInt8AddBiasScale_16x4_w4_Unit_VNNI, avx512/GemmInt8_VNNI.cpp:1626-1900) -- mnn_oracle_linear_w4_dynamic_blocks.
+mnnb200_status mnnb200_linear_w4_create_blocked(mnnb200_runtime* rt, int ic, int oc, int blocks, const uint8_t* wpacked,
+                                                const float* alpha, const float* wzero, const float* bias, int relu, int relu6,
+                                                mnnb200_exec** out) {
+    if (!rt || !wpacked || !alpha || !out || ic <= 0 || oc <= 0 || blocks < 1 || ic % blocks)
+        return fail(MNNB200_INVALID_VALUE, "linear_w4_create_blocked: bad argument (blocks must divide ic)");
+    if (ic & 1) return fail(MNNB200_NOT_SUPPORT, "linear_w4_create_blocked: an odd ic splits a byte of nibbles across two rows");
+    const int bs = ic / blocks;
+    if (blocks > 1 && bs % 32)
+        return fail(MNNB200_NOT_SUPPORT, "linear_w4_create_blocked: a block must be a multiple of 32 channels (one wgmma k-step)");
+    if (blocks > 1 && (bs > 512 || (bs & (bs - 1))))
+        return fail(MNNB200_NOT_SUPPORT, "linear_w4_create_blocked: the GEMV takes power-of-two blocks of at most 512 channels");
+    auto e = new_exec<LinearW8Exec>(rt);
+    e->ic = ic; e->oc = oc; e->icp = (ic + 31) & ~31; e->ocp = up16(oc); e->relu = relu; e->relu6 = relu6;
+    e->has_zero = true; e->has_bias = bias != nullptr; e->w4 = 1;
+    if (blocks > 1) { e->bs = bs; e->blocks = blocks; }
+    const bool fast = oc % 64 == 0 && ic % 4 == 0;
+    const size_t nt = (size_t)e->ocp * blocks;
+    std::vector<uint8_t> wp((size_t)e->ocp * (e->icp / 2), 0);
+    std::vector<float> bsv(e->ocp, 0.f), wks(e->ocp, 0.f), ba(nt, 0.f), bz(nt, 0.f), ta(nt, 0.f), tz(nt, 0.f), tws(nt, 0.f);
+    std::vector<int32_t> tw128(nt, 0);
+    for (int o = 0; o < oc; ++o) {
+        const uint8_t* src = wpacked + (size_t)o * (ic / 2);      // ConvolutionCommon.cpp:367-371: high nibble = even index
+        uint8_t* dst = wp.data() + (size_t)o * (e->icp / 2);
+        for (int k = 0; k < ic; ++k) {
+            const int u = (k & 1) ? (src[k >> 1] & 15) : (src[k >> 1] >> 4);
+            dst[(k >> 5) * 16 + (k & 15)] |= (uint8_t)(u << ((k & 16) ? 4 : 0));
+            tw128[(size_t)(k / bs) * e->ocp + o] += u;
+        }
+        if (bias) bsv[o] = bias[o];
+        float accum = 0.f;
+        for (int b = 0; b < blocks; ++b) {
+            const size_t ob = (size_t)o * blocks + b, bo = (size_t)b * e->ocp + o;
+            const float a = alpha[ob], z = wzero ? wzero[ob] : 0.f;
+            const float wb = wzero ? z + -8.f * a : -8.f * a;
+            const float ks = (float)tw128[bo];
+            accum = accum + (fast ? ks * a + (float)bs * wb : (wzero ? (ks - (float)(bs * 8)) * a + (float)bs * z : (ks - (float)(bs * 8)) * a));
+            ba[ob] = a; bz[ob] = wb;
+            ta[bo] = a; tz[bo] = wb;
+            tw128[bo] *= 128;
+        }
+        wks[o] = accum;
+        tws[o] = accum;      // block 0 carries the weightKernelSum, the others 0
+    }
+    const cudaStream_t s = rt->stream;
+    mnnb200_status st;
+    std::vector<int8_t> wpi(wp.begin(), wp.end());
+    if ((st = e->d_w.upload(wpi, s)) || (st = e->d_bias.upload(bsv, s)) || (st = e->d_wsumf.upload(wks, s))) return st;
+    if (blocks == 1) {       // per channel: the 8-bit per-channel tables
+        if ((st = e->d_alpha.upload(ta, s)) || (st = e->d_wzero.upload(tz, s)) || (st = e->d_wsum128.upload(tw128, s))) return st;
+    } else if ((st = e->d_balpha.upload(ba, s)) || (st = e->d_bwzero.upload(bz, s)) || (st = e->d_talpha.upload(ta, s)) ||
+               (st = e->d_twzero.upload(tz, s)) || (st = e->d_tws.upload(tws, s)) || (st = e->d_tw128.upload(tw128, s))) {
+        return st;
+    }
+    *out = e.release();
+    return MNNB200_OK;
+}
+
 mnnb200_status mnnb200_linear_w8_resize(mnnb200_exec* ex, int tokens) {
     auto* e = exec_as<LinearW8Exec>(ex);
     if (!e) return fail(MNNB200_INVALID_VALUE, "linear_w8_resize: not a linear execution");
@@ -1302,15 +1382,16 @@ mnnb200_status mnnb200_linear_w8_resize(mnnb200_exec* ex, int tokens) {
     // blocked: at most 128 columns per tile, the other half of the accumulator registers holds the fp32 block sums
     e->bn = pick_bn(e->ocp, (tokens + 127) / 128, e->rt->prop.multiProcessorCount, e->bs ? 128 : 256);
     if ((st = make_tmap_i8(&e->tmap_a, e->d_xq, tokens, e->icp, 128))) return st;
-    if ((st = make_tmap_i8(&e->tmap_b, e->d_w, e->ocp, e->icp, e->bn))) return st;
+    if ((st = e->w4 ? make_tmap_w4(&e->tmap_b, e->d_w, e->ocp, e->icp, e->bn) : make_tmap_i8(&e->tmap_b, e->d_w, e->ocp, e->icp, e->bn)))
+        return st;
     // tensor-bound shapes run on CTA pairs (2-CTA cluster, 256 rows): needs >= 256 rows and a B tile that splits into two halves
     e->bn2 = 0;
-    if (tokens >= 256 && e->ocp >= 64 && !e->bs) {
+    if (tokens >= 256 && e->ocp >= 64 && !e->bs && !e->w4) {
         int chunks = (e->ocp + 255) / 256;
         e->bn2 = (((e->ocp + chunks - 1) / chunks) + 31) & ~31;
         if ((st = make_tmap_i8(&e->tmap_b_half, e->d_w, e->ocp, e->icp, e->bn2 / 2))) return st;
     }
-    e->cost_bytes = (double)tokens * e->ic * 4 + (double)tokens * e->oc * 4 + (double)e->oc * e->ic +
+    e->cost_bytes = (double)tokens * e->ic * 4 + (double)tokens * e->oc * 4 + (double)e->oc * e->ic / (1 + e->w4) +
                     (e->bs ? (double)e->oc * e->blocks * 8 : 0.0);
     e->cost_macs = (double)tokens * e->oc * e->ic;
     return MNNB200_OK;
@@ -1321,18 +1402,19 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
     if (!e) return fail(MNNB200_INVALID_VALUE, "linear_w8_execute: not a linear execution");
     if (e->tokens <= 0) return fail(MNNB200_NO_EXECUTION, "linear_w8_execute before resize");
     if (e->bs && e->variant == 3) return fail(MNNB200_NOT_SUPPORT, "the CTA-pair variant takes per-channel weight scales only");
+    if (e->w4 && e->variant == 3) return fail(MNNB200_NOT_SUPPORT, "the CTA-pair variant takes 8-bit weights only");
     // decode (<= 8 tokens): weight-streaming GEMV, bit-identical to the tensor-core kernels (variant 4 forces it)
-    if (e->variant == 4 && !linear_w8_gemv_supported(e->tokens, e->icp, e->bs)) return fail(MNNB200_NOT_SUPPORT, "the GEMV variant takes 1..8 tokens");
+    if (e->variant == 4 && !linear_w8_gemv_supported(e->tokens, e->icp, e->bs, e->w4)) return fail(MNNB200_NOT_SUPPORT, "the GEMV variant takes 1..8 tokens");
     // ONE token is a different ARITHMETIC in the reference (asymmetric single-quant, input zero folded into the bias: see
     // linear_w8_gemv.cu), which only the GEMV kernel implements: the tensor-core kernels would silently compute the multi-token form
-    if (e->tokens == 1 && (e->variant == 2 || e->variant == 3 || !linear_w8_gemv_supported(1, e->icp, e->bs)))
+    if (e->tokens == 1 && (e->variant == 2 || e->variant == 3 || !linear_w8_gemv_supported(1, e->icp, e->bs, e->w4)))
         return fail(MNNB200_NOT_SUPPORT, "a single token runs the reference's decode arithmetic: GEMV kernel only (variant 0 or 4, ic <= 25600)");
-    if (e->variant == 4 || e->tokens == 1 || (e->variant == 0 && linear_w8_gemv_supported(e->tokens, e->icp, e->bs))) {
+    if (e->variant == 4 || e->tokens == 1 || (e->variant == 0 && linear_w8_gemv_supported(e->tokens, e->icp, e->bs, e->w4))) {
         GemvW8Params g;
         g.x = x; g.w = e->d_w; g.y = y; g.alpha = e->d_alpha; g.bias = e->has_bias ? static_cast<float*>(e->d_bias) : nullptr; g.wsumf = e->d_wsumf;
         g.wzero = e->has_zero ? static_cast<float*>(e->d_wzero) : nullptr; g.wsum128 = e->d_wsum128;
         g.tokens = e->tokens; g.ic = e->ic; g.oc = e->oc; g.ocp = e->ocp; g.icp = e->icp; g.ldy = e->oc; g.relu = e->relu; g.relu6 = e->relu6;
-        g.bs = e->bs; g.balpha = e->d_balpha; g.bwzero = e->d_bwzero;
+        g.bs = e->bs; g.balpha = e->d_balpha; g.bwzero = e->d_bwzero; g.w4 = e->w4;
         CK(launch_linear_w8_gemv(g, e->rt->stream, e->rt->prop.multiProcessorCount));
         return MNNB200_OK;
     }
@@ -1346,6 +1428,7 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
     g.relu = e->relu; g.relu6 = e->relu6;
     g.bs = e->bs; g.blocks = e->blocks; g.balpha = e->d_talpha; g.bwzero = e->d_twzero; g.bws = e->d_tws; g.bw128 = e->d_tw128;
     g.xsb = e->d_xsb;
+    g.w4 = e->w4;
     if (e->variant == 3 || (e->variant == 0 && e->bn2)) {
         CK(launch_gemm_i8_2cta(g, &e->tmap_a, &e->tmap_b_half, e->bn2, e->rt->stream, e->rt->prop.multiProcessorCount));
         return MNNB200_OK;

@@ -10,6 +10,8 @@
 //   * epilogue: straight from the accumulator registers: the CPU backend's dynamic-quant linear or Winograd position fp32
 //               forms, bit for bit
 //   * persistent: grid = #SMs, static round-robin over (batch, m_tile, n_chunk) work items
+//   * 4-bit weights (EPI 1, single CTA): TMA brings the packed nibbles (half the bytes of B), the consumer warpgroups expand
+//               them into the int8 B tile of the stage (or the resident B once) before the wgmmas read it
 //   * pair mode (launch_gemm_i8_2cta): a 2-CTA cluster computes 256 x bn; each CTA loads its own 128 rows of A and HALF of
 //     the B tile, multicast into both CTAs' shared memory, so each SM ingests 3/4 of the operand bytes of a lone CTA
 #include <cuda.h>
@@ -33,18 +35,21 @@ constexpr int kSmemBudget = 227 * 1024 - 1024;   // minus the 1024B alignment sl
 
 struct SmemPlan {
     int stages, stage_bytes, resident_b;   // resident_b: B (weights) loaded once per CTA
-    int off_resb, off_consts, off_bars, total;
+    int off_resb, off_resp, off_consts, off_bars, total;   // off_resp: the packed resident B of 4-bit weights
 };
-__host__ __device__ inline SmemPlan make_plan(int bn, int n_chunks, int num_kb, bool pair) {
+// w4: B arrives as packed nibbles (bn * kBK / 2 bytes per K block) next to the int8 tile they are expanded into
+__host__ __device__ inline SmemPlan make_plan(int bn, int n_chunks, int num_kb, bool pair, int w4 = 0) {
     SmemPlan pl;
     const int resb_bytes = bn * kBK * num_kb;
+    const int packed = w4 ? bn * kBK / 2 : 0;
     pl.resident_b = (!pair && n_chunks == 1 && resb_bytes <= 72 * 1024) ? 1 : 0;
-    pl.stage_bytes = kStageBytesA + (pl.resident_b ? 0 : bn * kBK);
-    const int fixed = (pl.resident_b ? resb_bytes : 0) + kConstBytes + 256;
+    pl.stage_bytes = kStageBytesA + (pl.resident_b ? 0 : bn * kBK + packed);
+    const int fixed = (pl.resident_b ? resb_bytes + packed * num_kb : 0) + kConstBytes + 256;
     const int st = (kSmemBudget - fixed) / pl.stage_bytes;
     pl.stages = st > kMaxStages ? kMaxStages : (st < 2 ? 2 : st);
     pl.off_resb = pl.stages * pl.stage_bytes;
-    pl.off_consts = pl.off_resb + (pl.resident_b ? resb_bytes : 0);
+    pl.off_resp = pl.off_resb + (pl.resident_b ? resb_bytes : 0);
+    pl.off_consts = pl.off_resp + (pl.resident_b ? packed * num_kb : 0);
     pl.off_bars = pl.off_consts + kConstBytes;
     pl.total = pl.off_bars + 256;
     return pl;
@@ -72,6 +77,7 @@ struct KParams {
     // batched mode (Winograd: one GEMM per transform position): work item = (batch, m_tile, n_chunk)
     int batch, a_batch_rows, b_batch_rows, c_batch_stride;
     int one_tile;   // grid == number of work items: every CTA owns exactly one (batch, m tile, n chunk)
+    int w4;         // B holds 4-bit weights, packed as GemmI8Params::w4 describes
 };
 
 // EPI 1: fp32 dynamic-quant linear, 2: fp32 Winograd position GEMM.  PAIR: 2-CTA cluster (EPI 1).
@@ -91,7 +97,8 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
     // "fixed tile": the CTA's n chunk (and batch) never changes, so its weights can stay resident and its per-column
     // constants are loaded once -- and, since neither depends on the previous layer, BEFORE griddepcontrol.wait.
     const bool fixed_tile = !PAIR && (p.one_tile || p.n_chunks * p.batch == 1);
-    const SmemPlan pl = make_plan(p.bn, fixed_tile ? 1 : p.n_chunks * p.batch, num_kb, PAIR);
+    const int w4 = (EPI == 1 && !PAIR && p.w4) ? 1 : 0;
+    const SmemPlan pl = make_plan(p.bn, fixed_tile ? 1 : p.n_chunks * p.batch, num_kb, PAIR, w4);
     int nc0 = 0, bt0 = 0;
     if (p.one_tile) { nc0 = blockIdx.x % p.n_chunks; bt0 = (blockIdx.x / p.n_chunks) / p.m_tiles; }
     const int S = pl.stages;
@@ -120,10 +127,11 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
 
     if (warp == 8) {
         // ================= TMA producer =================
-        if (lane == 0 && pl.resident_b) {    // weights: once per CTA, all K blocks
-            mbar_expect_tx(bres_bar, (uint32_t)(p.bn * kBK * num_kb));
+        if (lane == 0 && pl.resident_b) {    // weights: once per CTA, all K blocks (4-bit: packed, expanded by the consumers)
+            mbar_expect_tx(bres_bar, (uint32_t)((p.bn * kBK * num_kb) >> w4));
             for (int kb = 0; kb < num_kb; ++kb)
-                tma_load_2d(base + pl.off_resb + kb * p.bn * kBK, &tmap_b, bres_bar, kb * kBK, bt0 * p.b_batch_rows + nc0 * p.bn);
+                tma_load_2d(base + (w4 ? pl.off_resp : pl.off_resb) + ((kb * p.bn * kBK) >> w4), &tmap_b, bres_bar, kb * (kBK >> w4),
+                            bt0 * p.b_batch_rows + nc0 * p.bn);
         }
         pdl_wait();
         if (lane == 0) {
@@ -135,14 +143,14 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
                 const int a_row = bt * p.a_batch_rows + mt * tile_rows + (int)rank * kBM, b_row = bt * p.b_batch_rows + nc * p.bn;
                 for (int kb = 0; kb < num_kb; ++kb) {
                     mbar_wait(empty_bar(stage), phase ^ 1);
-                    mbar_expect_tx(full_bar(stage), (uint32_t)(PAIR ? kStageBytesA + p.bn * kBK : pl.stage_bytes));
+                    mbar_expect_tx(full_bar(stage), (uint32_t)(kStageBytesA + (PAIR || !pl.resident_b ? (p.bn * kBK) >> w4 : 0)));
                     const uint32_t a_dst = base + stage * pl.stage_bytes;
                     tma_load_2d(a_dst, &tmap_a, full_bar(stage), kb * kBK, a_row);
                     if (PAIR)
                         tma_load_2d_multicast(a_dst + kStageBytesA + rank * half_bn * kBK, &tmap_b, full_bar(stage), kb * kBK,
                                               b_row + (int)rank * half_bn, (uint16_t)3);
                     else if (!pl.resident_b)
-                        tma_load_2d(a_dst + kStageBytesA, &tmap_b, full_bar(stage), kb * kBK, b_row);
+                        tma_load_2d(a_dst + kStageBytesA + (w4 ? p.bn * kBK : 0), &tmap_b, full_bar(stage), kb * (kBK >> w4), b_row);
                     if (++stage == S) { stage = 0; phase ^= 1; }
                 }
             }
@@ -178,8 +186,29 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
             load_consts(nc0 * p.bn, bt0 * p.c_batch_stride);
             named_sync(1, kConsumerThreads);
         }
+        // 4-bit weights: rows of 64 packed bytes (K block of 128), 16-byte group g holding K 32 g + j in its low nibbles and
+        // K 32 g + 16 + j in its high ones, become rows of the 128B-swizzled int8 tile the TMA would have written (u = q + 8 in
+        // 0..15; the epilogue's wsum128 / wsumf / wzero carry the offset).  Written through the generic proxy, so fenced for
+        // the wgmmas' async proxy; both warpgroups read every row, so both expand and meet at named barrier 2.
+        auto expand_w4 = [&](uint32_t pk, uint32_t dst, int rows) {     // shared-memory addresses
+#pragma unroll 1
+            for (int i = ct; i < rows * 4; i += kConsumerThreads) {
+                const uint32_t r = (uint32_t)i >> 2, g = (uint32_t)i & 3u, m = 0x0F0F0F0Fu;
+                uint32_t v0, v1, v2, v3;
+                asm volatile("ld.shared.v4.u32 {%0, %1, %2, %3}, [%4];\n" : "=r"(v0), "=r"(v1), "=r"(v2), "=r"(v3)
+                             : "r"(pk + r * (kBK / 2) + g * 16));
+                const uint32_t row = dst + r * kBK;
+                asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};\n" ::"r"(row + (((2 * g) ^ (r & 7)) << 4)),
+                             "r"(v0 & m), "r"(v1 & m), "r"(v2 & m), "r"(v3 & m) : "memory");
+                asm volatile("st.shared.v4.u32 [%0], {%1, %2, %3, %4};\n" ::"r"(row + (((2 * g + 1) ^ (r & 7)) << 4)),
+                             "r"((v0 >> 4) & m), "r"((v1 >> 4) & m), "r"((v2 >> 4) & m), "r"((v3 >> 4) & m) : "memory");
+            }
+            asm volatile("fence.proxy.async.shared::cta;\n" ::: "memory");
+            named_sync(2, kConsumerThreads);
+        };
         pdl_wait();
         if (pl.resident_b) mbar_wait(bres_bar, 0);
+        if (w4 && pl.resident_b) expand_w4(base + pl.off_resp, base + pl.off_resb, p.bn * num_kb);
         auto release = [&](int s) {                  // this warp's MMAs on stage s have completed
             __syncwarp();
             if (lane == 0) {
@@ -248,6 +277,8 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
             }
             for (int kb = 0; kb < num_kb; ++kb) {
                 mbar_wait(full_bar(stage), phase);  // TMA bytes have landed
+                if (w4 && !pl.resident_b)
+                    expand_w4(base + stage * pl.stage_bytes + kStageBytesA + p.bn * kBK, base + stage * pl.stage_bytes + kStageBytesA, p.bn);
                 const uint32_t a_addr = base + stage * pl.stage_bytes + wg * 64 * kBK;
                 const uint32_t b_addr = pl.resident_b ? base + pl.off_resb + kb * p.bn * kBK : base + stage * pl.stage_bytes + kStageBytesA;
                 const int kleft = p.K - kb * kBK;
@@ -379,6 +410,7 @@ KParams make_params(const GemmI8Params& g, int bn) {
     p.batch = g.batch > 0 ? g.batch : 1;
     p.a_batch_rows = g.a_batch_rows; p.b_batch_rows = g.b_batch_rows; p.c_batch_stride = g.c_batch_stride;
     p.one_tile = 0;
+    p.w4 = g.w4;
     return p;
 }
 
@@ -392,7 +424,7 @@ GemmI8Launch gemm_i8_wgmma_launch(const GemmI8Params& g, int bn, int sm_count) {
     l.grid = l.items < sm_count ? l.items : sm_count;
     l.one_tile = l.grid == l.items ? 1 : 0;
     const bool fixed_tile = l.one_tile || p.n_chunks * p.batch == 1;
-    const SmemPlan pl = make_plan(bn, fixed_tile ? 1 : p.n_chunks * p.batch, l.num_kb, false);
+    const SmemPlan pl = make_plan(bn, fixed_tile ? 1 : p.n_chunks * p.batch, l.num_kb, false, g.w4);
     l.resident_b = pl.resident_b;
     l.stages = pl.stages;
     l.smem = pl.total + 1024;
@@ -403,6 +435,7 @@ cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& g, const void* tmap_a, cons
                                  int sm_count) {
     if (bn < 16 || bn > kMaxBN || (bn & 15) || g.y_f32 == nullptr) return cudaErrorInvalidValue;
     if (g.bs && (g.wino || bn > kMaxBN / 2 || g.bs % 32 || g.K % g.bs || g.blocks != g.K / g.bs)) return cudaErrorInvalidValue;
+    if (g.w4 && (g.wino || g.K % 32)) return cudaErrorInvalidValue;
     KParams p = make_params(g, bn);
     const GemmI8Launch l = gemm_i8_wgmma_launch(g, bn, sm_count);
     p.one_tile = l.one_tile;
@@ -414,7 +447,7 @@ cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& g, const void* tmap_a, cons
 
 cudaError_t launch_gemm_i8_2cta(const GemmI8Params& g, const void* tmap_a, const void* tmap_b_half, int bn, cudaStream_t stream,
                                 int sm_count) {
-    if (bn < 32 || bn > kMaxBN || (bn & 31) || g.y_f32 == nullptr || g.wino || g.bs) return cudaErrorInvalidValue;
+    if (bn < 32 || bn > kMaxBN || (bn & 31) || g.y_f32 == nullptr || g.wino || g.bs || g.w4) return cudaErrorInvalidValue;
     KParams p = make_params(g, bn);
     p.batch = 1;
     p.m_tiles = (g.M + 2 * kBM - 1) / (2 * kBM);

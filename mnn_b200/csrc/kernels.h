@@ -61,6 +61,10 @@ struct GemmI8Params {
     // B = [batch][b_batch_rows][K], per-column constants [batch][c_batch_stride], fp32 out [batch][a_batch_rows][ldy]:
     //   y = float(acc + wsum128[a][n]) * wscale[a][n] + bias[a][n]        (wino = 1)
     int batch, a_batch_rows, b_batch_rows, c_batch_stride, wino;
+    // 4-bit weights (linear only, K % 32 == 0): b = [Nw][K / 2] bytes of unsigned nibbles u = q + 8, K group of 32 g in bytes
+    // [16 g, 16 g + 16), the first 16 weights in the low nibbles; the int32 accumulators are sum (xq + 128) * u once the
+    // per-column tables (wsum128 / bw128 = 128 sum u) are added
+    int w4;
 };
 cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& p, const void* tmap_a, const void* tmap_b, int bn, cudaStream_t stream,
                                  int sm_count);
@@ -283,8 +287,11 @@ struct GemvW8Params {
     // alpha / wsumf / wzero / wsum128 are not read.
     int bs;
     const float *balpha, *bwzero;
+    // 4-bit weights (icp % 32 == 0): w = [ocp][icp / 2] packed as GemmI8Params::w4; blocked, the single weightKernelSum is wsumf
+    // and enters with the first block (ws_b is not derived from the weights)
+    int w4;
 };
-bool linear_w8_gemv_supported(int tokens, int icp, int bs = 0);
+bool linear_w8_gemv_supported(int tokens, int icp, int bs = 0, int w4 = 0);
 cudaError_t launch_linear_w8_gemv(const GemvW8Params& p, cudaStream_t s, int sm_count);
 
 // dynamic per-token quantisation (MNNAbsMax + MNNQuantScale + MNNDynamicQuant fused); bs > 0 also writes

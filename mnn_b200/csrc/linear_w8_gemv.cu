@@ -10,10 +10,16 @@
 //     order-independent, so the result is bit-identical to the tensor-core path;
 //   * K-blocked weight scales (p.bs != 0, MNN-LLM's quant_block export) take a run-time branch of the same kernel: exact int32
 //     sums per block, finished in block order as gemm_i8_wgmma's blocked EPI 1 does, so again bit-identical to it;
+//   * 4-bit weights (p.w4) take another run-time branch: a 16-byte load brings 32 packed weights (K 2kb..2kb+31 for byte
+//     offset kb, the first 16 in the low nibbles), a mask and a shift per dword expand them to bytes u = q + 8, and everything
+//     after the dp4a is the 8-bit code with the tables of mnnb200_linear_w4_create_blocked.  Only in the instantiations with
+//     two or more tokens and at most two rows per warp (see stream_rows);
 //   * programmatic dependent launch: the first weight chunk is requested before griddepcontrol.wait, so the next layer's blocks
 //     are resident and loading while this layer drains (a decode step is ~120 dependent launches of 2-10 us each).
 #include "common.cuh"
 #include "kernels.h"
+
+#include <type_traits>
 
 namespace mnnb200 {
 namespace {
@@ -28,7 +34,18 @@ __global__ void __launch_bounds__(256, 2) linear_w8_gemv_kernel(GemvW8Params p) 
     __shared__ float s_dq[T], s_ss[T];
     __shared__ float s_min[8], s_izf;      // single-token (decode) branch: row minimum per warp, folded input zero
     asm volatile("griddepcontrol.launch_dependents;\n" ::: "memory");
+    auto dot16 = [](const int4& xv, const int4& w, int a) {
+        a = __dp4a(xv.x, w.x, a);
+        a = __dp4a(xv.y, w.y, a);
+        a = __dp4a(xv.z, w.z, a);
+        return __dp4a(xv.w, w.w, a);
+    };
+    auto lo4 = [](const int4& v) { return make_int4(v.x & 0x0F0F0F0F, v.y & 0x0F0F0F0F, v.z & 0x0F0F0F0F, v.w & 0x0F0F0F0F); };
+    auto hi4 = [](const int4& v) {
+        return make_int4((v.x >> 4) & 0x0F0F0F0F, (v.y >> 4) & 0x0F0F0F0F, (v.z >> 4) & 0x0F0F0F0F, (v.w >> 4) & 0x0F0F0F0F);
+    };
     const int icp = p.icp, ic = p.ic;
+    const int w4 = T > 1 && R < 4 ? p.w4 : 0, rowb = icp >> w4;       // weight bytes per row
     const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
     const int warps = blockDim.x >> 5;
     int n0 = (blockIdx.x * warps + warp) * R;
@@ -38,11 +55,11 @@ __global__ void __launch_bounds__(256, 2) linear_w8_gemv_kernel(GemvW8Params p) 
     int4 wv[R][U];
 #pragma unroll
     for (int r = 0; r < R; ++r) {
-        wrow[r] = p.w + (size_t)min(n0 + r, p.ocp - 1) * icp;
+        wrow[r] = p.w + (size_t)min(n0 + r, p.ocp - 1) * rowb;
 #pragma unroll
         for (int u = 0; u < U; ++u) {
             const int k = lane * 16 + u * 512;
-            wv[r][u] = (n0 < p.oc && k < icp) ? ld_nc_16(wrow[r] + k) : make_int4(0, 0, 0, 0);
+            wv[r][u] = (n0 < p.oc && k < rowb) ? ld_nc_16(wrow[r] + k) : make_int4(0, 0, 0, 0);
         }
     }
     // ... and so are the epilogue constants of the output this lane will finish (lane = token * R + row)
@@ -219,198 +236,220 @@ __global__ void __launch_bounds__(256, 2) linear_w8_gemv_kernel(GemvW8Params p) 
     }
     __syncthreads();
 
-    bool first = true;
-    if (p.bs) {
-        // ---- K-blocked weight scales (mnn_oracle_linear_w8_dynamic_blocks): every output sums, block after block, the fp32
-        //      finish of its exact int32 block accumulator.  The quantisation above is unchanged; the per-block input sums
-        //      xsum_b * scale come from the quantised rows in shared memory.  In a 512-byte window of K the G = bs / 16 lanes of a
-        //      block reduce its int32 sums with a butterfly, the group's first lane finishes the block (sum_b w is dp4a'd from the
-        //      streamed weights, not stored) into shared memory, and the lane owning the output adds the parts in block order.
-        const int bs = p.bs, G = bs >> 4, nb = ic / bs;
-        float* s_xs = reinterpret_cast<float*>(smem_x + T * icp);                 // [T][nb]
-        float* s_part = s_xs + T * nb + warp * (T * R + R) * 16;                 // [T * R][16] parts, then [R][16] ws_b
-        float* s_wsb = s_part + T * R * 16;
-        for (int i = threadIdx.x; i < T * nb; i += blockDim.x) {
-            const int t = i / nb, b = i - t * nb;
-            float v = 0.f;
-            if (t < p.tokens) {
-                const int4* q4 = reinterpret_cast<const int4*>(smem_x + t * icp + b * bs);
-                int sum = 0;
-                for (int j = 0; j < (bs >> 4); ++j) {
-                    const int4 q = q4[j];
-                    sum = __dp4a(q.x, 0x01010101, sum); sum = __dp4a(q.y, 0x01010101, sum);
-                    sum = __dp4a(q.z, 0x01010101, sum); sum = __dp4a(q.w, 0x01010101, sum);
+    // everything after the quantisation once per weight format, W4 a constant in each.  The 4-bit branch is not in the
+    // one-token and the four-row instantiations at all: next to it the 8-bit decode step of Qwen-1.8B took 0.924 ms instead of
+    // 0.882 (H100 80GB HBM3, 700 W), so 4-bit layers run one token on the two-token kernel and at most two rows per warp
+    auto stream_rows = [&](auto w4c) {
+        constexpr int W4 = decltype(w4c)::value;
+        const int row_bytes = icp >> W4;
+        bool first = true;
+        if (p.bs) {
+            // ---- K-blocked weight scales (mnn_oracle_linear_w8_dynamic_blocks): every output sums, block after block, the fp32
+            //      finish of its exact int32 block accumulator.  The quantisation above is unchanged; the per-block input sums
+            //      xsum_b * scale come from the quantised rows in shared memory.  In a 512-byte window of K the G = bs / 16 lanes of a
+            //      block reduce its int32 sums with a butterfly, the group's first lane finishes the block (sum_b w is dp4a'd from the
+            //      streamed weights, not stored) into shared memory, and the lane owning the output adds the parts in block order.
+            //      4-bit: a lane covers 32 channels, so G = bs / 32 and a 1024-channel window holds up to 32 blocks (SL slots); ws_b
+            //      is the layer's weightKernelSum for the first block and 0 after it (the reference's 4-bit kernel adds it once).
+            const int bs = p.bs, G = bs >> (4 + W4), nb = ic / bs, SL = 16 << W4;
+            float* s_xs = reinterpret_cast<float*>(smem_x + T * icp);                 // [T][nb]
+            float* s_part = s_xs + T * nb + warp * (T * R + R) * SL;                 // [T * R][SL] parts, then [R][SL] ws_b
+            float* s_wsb = s_part + T * R * SL;
+            for (int i = threadIdx.x; i < T * nb; i += blockDim.x) {
+                const int t = i / nb, b = i - t * nb;
+                float v = 0.f;
+                if (t < p.tokens) {
+                    const int4* q4 = reinterpret_cast<const int4*>(smem_x + t * icp + b * bs);
+                    int sum = 0;
+                    for (int j = 0; j < (bs >> 4); ++j) {
+                        const int4 q = q4[j];
+                        sum = __dp4a(q.x, 0x01010101, sum); sum = __dp4a(q.y, 0x01010101, sum);
+                        sum = __dp4a(q.z, 0x01010101, sum); sum = __dp4a(q.w, 0x01010101, sum);
+                    }
+                    v = __fmul_rn(__int2float_rn(sum + 128 * bs), s_dq[t]);
                 }
-                v = __fmul_rn(__int2float_rn(sum + 128 * bs), s_dq[t]);
+                s_xs[i] = v;
             }
-            s_xs[i] = v;
-        }
-        __syncthreads();
-        for (; n0 < p.oc; n0 += gridDim.x * warps * R) {
-            if (!first) {
+            __syncthreads();
+            for (; n0 < p.oc; n0 += gridDim.x * warps * R) {
+                if (!first) {
 #pragma unroll
-                for (int r = 0; r < R; ++r) wrow[r] = p.w + (size_t)min(n0 + r, p.ocp - 1) * icp;
-            }
-            float f = 0.f, wtot = 0.f;
-            for (int kbase = 0; kbase < icp; kbase += 512 * U) {
-                if (!(first && kbase == 0)) {
-#pragma unroll
-                    for (int r = 0; r < R; ++r)
-#pragma unroll
-                        for (int u = 0; u < U; ++u) {
-                            const int k = kbase + lane * 16 + u * 512;
-                            wv[r][u] = k < icp ? ld_nc_16(wrow[r] + k) : make_int4(0, 0, 0, 0);
-                        }
+                    for (int r = 0; r < R; ++r) wrow[r] = p.w + (size_t)min(n0 + r, p.ocp - 1) * row_bytes;
                 }
+                float f = 0.f, wtot = 0.f;
+                for (int kbase = 0; kbase < row_bytes; kbase += 512 * U) {
+                    if (!(first && kbase == 0)) {
 #pragma unroll
-                for (int u = 0; u < U; ++u) {
-                    const int kw = kbase + u * 512, k = kw + lane * 16;
-                    if (kw >= icp) break;
-                    // one weight row at a time: its T block sums and sum_b w are the only new values live next to the weights
+                        for (int r = 0; r < R; ++r)
 #pragma unroll
-                    for (int r = 0; r < R; ++r) {
-                        const int4 w = wv[r][u];
-                        int sw = __dp4a(w.x, 0x01010101, 0);
-                        sw = __dp4a(w.y, 0x01010101, sw);
-                        sw = __dp4a(w.z, 0x01010101, sw);
-                        sw = __dp4a(w.w, 0x01010101, sw);
-                        int a[T];
-#pragma unroll
-                        for (int t = 0; t < T; ++t) {
-                            const int4 xv = k < icp ? *reinterpret_cast<const int4*>(smem_x + t * icp + k) : make_int4(0, 0, 0, 0);
-                            int v = __dp4a(xv.x, w.x, 0);
-                            v = __dp4a(xv.y, w.y, v);
-                            v = __dp4a(xv.z, w.z, v);
-                            a[t] = __dp4a(xv.w, w.w, v);
-                        }
-                        for (int o = 1; o < G; o <<= 1) {
-                            sw += __shfl_xor_sync(0xffffffffu, sw, o);
-#pragma unroll
-                            for (int t = 0; t < T; ++t) a[t] += __shfl_xor_sync(0xffffffffu, a[t], o);
-                        }
-                        if ((lane & (G - 1)) == 0 && k < icp) {
-                            const int g = lane / G, b = k / bs;
-                            const size_t ci = (size_t)min(n0 + r, p.ocp - 1) * nb + b;   // alpha_b / wzero_b (zero past oc)
-                            const float c_al = __ldg(p.balpha + ci), c_wz = __ldg(p.bwzero + ci);
-                            // ws_b = float(sum_b w) * alpha_b + bs * wzero_b;  the block's accumulator includes the +128 offset
-                            const float ws = __fadd_rn(__fmul_rn(__int2float_rn(sw), c_al), __fmul_rn((float)bs, c_wz));
-                            s_wsb[r * 16 + g] = ws;
-#pragma unroll
-                            for (int t = 0; t < T; ++t) {
-                                const float sc = s_dq[t];
-                                float part = __fmul_rn(__int2float_rn(a[t] + 128 * sw), c_al);
-                                part = __fmul_rn(part, sc);
-                                part = __fadd_rn(part, __fmul_rn(__fmul_rn(sc, -128.f), ws));
-                                part = __fadd_rn(__fmul_rn(s_xs[t * nb + b], c_wz), part);
-                                s_part[(t * R + r) * 16 + g] = part;
+                            for (int u = 0; u < U; ++u) {
+                                const int k = kbase + lane * 16 + u * 512;
+                                wv[r][u] = k < row_bytes ? ld_nc_16(wrow[r] + k) : make_int4(0, 0, 0, 0);
                             }
-                        }
                     }
-                    __syncwarp();
-                    if (lane < T * R) {
-                        const int nbw = min(32 / G, nb - kw / bs);     // blocks in this window, in order
-                        for (int g = 0; g < nbw; ++g) {
-                            f = __fadd_rn(f, s_part[lane * 16 + g]);
-                            wtot = __fadd_rn(wtot, s_wsb[(lane % R) * 16 + g]);
-                        }
-                    }
-                    __syncwarp();
-                }
-            }
-            first = false;
-            if (lane < T * R) {
-                const int n = n0 + lane % R, m = lane / R;
-                if (n < p.oc && m < p.tokens) {
-                    const float bias = p.bias ? __ldg(p.bias + n) : 0.f;
-                    if (p.tokens == 1) f = __fadd_rn(f, __fadd_rn(bias, __fmul_rn(wtot, s_izf)));   // bias' = bias + sum_b ws_b * izf
-                    else if (p.bias) f = __fadd_rn(f, bias);
-                    if (p.relu | p.relu6) { f = fminf(f, p.relu6 ? 6.0f : 3.4028234663852886e38f); f = fmaxf(f, 0.f); }
-                    p.y[(size_t)m * p.ldy + n] = f;
-                }
-            }
-        }
-        return;
-    }
-    for (; n0 < p.oc; n0 += gridDim.x * warps * R) {
-        int acc[T][R];
-#pragma unroll
-        for (int t = 0; t < T; ++t)
-#pragma unroll
-            for (int r = 0; r < R; ++r) acc[t][r] = 0;
-        if (!first) {
-#pragma unroll
-            for (int r = 0; r < R; ++r) wrow[r] = p.w + (size_t)min(n0 + r, p.ocp - 1) * icp;
-        }
-        for (int k0 = lane * 16; k0 < icp; k0 += 512 * U) {
-            if (!(first && k0 == lane * 16)) {
-#pragma unroll
-                for (int r = 0; r < R; ++r)
 #pragma unroll
                     for (int u = 0; u < U; ++u) {
-                        const int k = k0 + u * 512;
-                        wv[r][u] = k < icp ? ld_nc_16(wrow[r] + k) : make_int4(0, 0, 0, 0);
-                    }
-            }
-#pragma unroll
-            for (int u = 0; u < U; ++u) {
-                const int k = k0 + u * 512;
-                if (k < icp) {
-#pragma unroll
-                    for (int t = 0; t < T; ++t) {
-                        const int4 xv = *reinterpret_cast<const int4*>(smem_x + t * icp + k);
+                        const int kw = kbase + u * 512, k = kw + lane * 16;     // bytes of the weight row
+                        if (kw >= row_bytes) break;
+                        // one weight row at a time: its T block sums and sum_b w are the only new values live next to the weights
 #pragma unroll
                         for (int r = 0; r < R; ++r) {
-                            int a = acc[t][r];
-                            a = __dp4a(xv.x, wv[r][u].x, a);
-                            a = __dp4a(xv.y, wv[r][u].y, a);
-                            a = __dp4a(xv.z, wv[r][u].z, a);
-                            a = __dp4a(xv.w, wv[r][u].w, a);
-                            acc[t][r] = a;
+                            const int4 ones = make_int4(0x01010101, 0x01010101, 0x01010101, 0x01010101);
+                            const int4 w = W4 ? lo4(wv[r][u]) : wv[r][u], wh = hi4(wv[r][u]);
+                            int sw = dot16(ones, w, 0);
+                            if (W4) sw = dot16(ones, wh, sw);
+                            int a[T];
+#pragma unroll
+                            for (int t = 0; t < T; ++t) {
+                                const uint8_t* xr = smem_x + t * icp + (k << W4);
+                                a[t] = k < row_bytes ? dot16(*reinterpret_cast<const int4*>(xr), w, 0) : 0;
+                                if (W4 && k < row_bytes) a[t] = dot16(*reinterpret_cast<const int4*>(xr + 16), wh, a[t]);
+                            }
+                            for (int o = 1; o < G; o <<= 1) {
+                                sw += __shfl_xor_sync(0xffffffffu, sw, o);
+#pragma unroll
+                                for (int t = 0; t < T; ++t) a[t] += __shfl_xor_sync(0xffffffffu, a[t], o);
+                            }
+                            if ((lane & (G - 1)) == 0 && k < row_bytes) {
+                                const int g = lane / G, b = (k << W4) / bs;
+                                const size_t ci = (size_t)min(n0 + r, p.ocp - 1) * nb + b;   // alpha_b / wzero_b (zero past oc)
+                                const float c_al = __ldg(p.balpha + ci), c_wz = __ldg(p.bwzero + ci);
+                                // ws_b = float(sum_b w) * alpha_b + bs * wzero_b;  the block's accumulator includes the +128 offset
+                                const float ws = W4 ? (b == 0 ? __ldg(p.wsumf + min(n0 + r, p.ocp - 1)) : 0.f)
+                                                    : __fadd_rn(__fmul_rn(__int2float_rn(sw), c_al), __fmul_rn((float)bs, c_wz));
+                                s_wsb[r * SL + g] = ws;
+#pragma unroll
+                                for (int t = 0; t < T; ++t) {
+                                    const float sc = s_dq[t];
+                                    float part = __fmul_rn(__int2float_rn(a[t] + 128 * sw), c_al);
+                                    part = __fmul_rn(part, sc);
+                                    part = __fadd_rn(part, __fmul_rn(__fmul_rn(sc, -128.f), ws));
+                                    part = __fadd_rn(__fmul_rn(s_xs[t * nb + b], c_wz), part);
+                                    s_part[(t * R + r) * SL + g] = part;
+                                }
+                            }
                         }
+                        __syncwarp();
+                        if (lane < T * R) {
+                            const int nbw = min(32 / G, nb - (kw << W4) / bs);     // blocks in this window, in order
+                            for (int g = 0; g < nbw; ++g) {
+                                f = __fadd_rn(f, s_part[lane * SL + g]);
+                                wtot = __fadd_rn(wtot, s_wsb[(lane % R) * SL + g]);
+                            }
+                        }
+                        __syncwarp();
                     }
                 }
-            }
-        }
-        if (!first) {
-            const int n = n0 + lane % R;
-            if (lane < T * R && n < p.oc) {
-                c_alpha = __ldg(p.alpha + n); c_wsumf = __ldg(p.wsumf + n); c_wsum128 = __ldg(p.wsum128 + n);
-                c_wzero = p.wzero ? __ldg(p.wzero + n) : 0.f;
-                c_bias = p.bias ? __ldg(p.bias + n) : 0.f;
-            }
-        }
-        first = false;
-#pragma unroll
-        for (int t = 0; t < T; ++t)
-#pragma unroll
-            for (int r = 0; r < R; ++r) {
-                int a = acc[t][r];
-#pragma unroll
-                for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
-                // lane (t * R + r) finishes output (token t, row n0 + r): gemm_i8_wgmma.cu EPI 1, operation for operation
-                if (lane == t * R + r) {
-                    const int n = n0 + r, m = t;
+                first = false;
+                if (lane < T * R) {
+                    const int n = n0 + lane % R, m = lane / R;
                     if (n < p.oc && m < p.tokens) {
-                        const float dqm = s_dq[m], ss = s_ss[m];
-                        const float corr = __fmul_rn(dqm, -128.f);
-                        float f = __fmul_rn(__int2float_rn(a + c_wsum128), c_alpha);
-                        f = __fmul_rn(f, dqm);
-                        f = __fadd_rn(f, __fmul_rn(corr, c_wsumf));
-                        f = __fadd_rn(__fmul_rn(ss, c_wzero), f);
-                        if (p.tokens == 1) f = __fadd_rn(f, __fadd_rn(c_bias, __fmul_rn(c_wsumf, s_izf)));   // bias' = bias + weightKernelSum * (-qbias * scale)
-                        else if (p.bias) f = __fadd_rn(f, c_bias);
+                        const float bias = p.bias ? __ldg(p.bias + n) : 0.f;
+                        if (p.tokens == 1) f = __fadd_rn(f, __fadd_rn(bias, __fmul_rn(wtot, s_izf)));   // bias' = bias + sum_b ws_b * izf
+                        else if (p.bias) f = __fadd_rn(f, bias);
                         if (p.relu | p.relu6) { f = fminf(f, p.relu6 ? 6.0f : 3.4028234663852886e38f); f = fmaxf(f, 0.f); }
                         p.y[(size_t)m * p.ldy + n] = f;
                     }
                 }
             }
+            return;
+        }
+        for (; n0 < p.oc; n0 += gridDim.x * warps * R) {
+            int acc[T][R];
+#pragma unroll
+            for (int t = 0; t < T; ++t)
+#pragma unroll
+                for (int r = 0; r < R; ++r) acc[t][r] = 0;
+            if (!first) {
+#pragma unroll
+                for (int r = 0; r < R; ++r) wrow[r] = p.w + (size_t)min(n0 + r, p.ocp - 1) * row_bytes;
+            }
+            for (int k0 = lane * 16; k0 < row_bytes; k0 += 512 * U) {
+                if (!(first && k0 == lane * 16)) {
+#pragma unroll
+                    for (int r = 0; r < R; ++r)
+#pragma unroll
+                        for (int u = 0; u < U; ++u) {
+                            const int k = k0 + u * 512;
+                            wv[r][u] = k < row_bytes ? ld_nc_16(wrow[r] + k) : make_int4(0, 0, 0, 0);
+                        }
+                }
+#pragma unroll
+                for (int u = 0; u < U; ++u) {
+                    const int k = k0 + u * 512;
+                    if (W4 && k < row_bytes) {
+                        // one row at a time, so that only one row's expanded weights are live next to the packed ones
+#pragma unroll
+                        for (int r = 0; r < R; ++r) {
+                            const int4 lo = lo4(wv[r][u]), hi = hi4(wv[r][u]);
+#pragma unroll
+                            for (int t = 0; t < T; ++t) {
+                                const uint8_t* xr = smem_x + t * icp + 2 * k;
+                                acc[t][r] = dot16(*reinterpret_cast<const int4*>(xr + 16), hi, dot16(*reinterpret_cast<const int4*>(xr), lo, acc[t][r]));
+                            }
+                        }
+                    } else if (k < row_bytes) {
+#pragma unroll
+                        for (int t = 0; t < T; ++t) {
+                            const int4 xv = *reinterpret_cast<const int4*>(smem_x + t * icp + k);
+#pragma unroll
+                            for (int r = 0; r < R; ++r) {
+                                int a = acc[t][r];
+                                a = __dp4a(xv.x, wv[r][u].x, a);
+                                a = __dp4a(xv.y, wv[r][u].y, a);
+                                a = __dp4a(xv.z, wv[r][u].z, a);
+                                a = __dp4a(xv.w, wv[r][u].w, a);
+                                acc[t][r] = a;
+                            }
+                        }
+                    }
+                }
+            }
+            if (!first) {
+                const int n = n0 + lane % R;
+                if (lane < T * R && n < p.oc) {
+                    c_alpha = __ldg(p.alpha + n); c_wsumf = __ldg(p.wsumf + n); c_wsum128 = __ldg(p.wsum128 + n);
+                    c_wzero = p.wzero ? __ldg(p.wzero + n) : 0.f;
+                    c_bias = p.bias ? __ldg(p.bias + n) : 0.f;
+                }
+            }
+            first = false;
+#pragma unroll
+            for (int t = 0; t < T; ++t)
+#pragma unroll
+                for (int r = 0; r < R; ++r) {
+                    int a = acc[t][r];
+#pragma unroll
+                    for (int o = 16; o > 0; o >>= 1) a += __shfl_xor_sync(0xffffffffu, a, o);
+                    // lane (t * R + r) finishes output (token t, row n0 + r): gemm_i8_wgmma.cu EPI 1, operation for operation
+                    if (lane == t * R + r) {
+                        const int n = n0 + r, m = t;
+                        if (n < p.oc && m < p.tokens) {
+                            const float dqm = s_dq[m], ss = s_ss[m];
+                            const float corr = __fmul_rn(dqm, -128.f);
+                            float f = __fmul_rn(__int2float_rn(a + c_wsum128), c_alpha);
+                            f = __fmul_rn(f, dqm);
+                            f = __fadd_rn(f, __fmul_rn(corr, c_wsumf));
+                            f = __fadd_rn(__fmul_rn(ss, c_wzero), f);
+                            if (p.tokens == 1) f = __fadd_rn(f, __fadd_rn(c_bias, __fmul_rn(c_wsumf, s_izf)));   // bias' = bias + weightKernelSum * (-qbias * scale)
+                            else if (p.bias) f = __fadd_rn(f, c_bias);
+                            if (p.relu | p.relu6) { f = fminf(f, p.relu6 ? 6.0f : 3.4028234663852886e38f); f = fmaxf(f, 0.f); }
+                            p.y[(size_t)m * p.ldy + n] = f;
+                        }
+                    }
+                }
+        }
+    };
+    if constexpr (T > 1 && R < 4) {
+        if (w4) return stream_rows(std::integral_constant<int, 1>{});
     }
+    stream_rows(std::integral_constant<int, 0>{});
 }
 
 template <int T, int R, int U>
 cudaError_t launch_t(const GemvW8Params& p, cudaStream_t stream, int sms) {
     // blocked: + the per-block input sums [T][ic / bs] and each warp's block parts
-    const size_t smem = (size_t)T * p.icp + (p.bs ? ((size_t)T * (p.ic / p.bs) + 8 * (T * R + R) * 16) * sizeof(float) : 0);
+    const size_t smem = (size_t)T * p.icp + (p.bs ? ((size_t)T * (p.ic / p.bs) + 8 * (T * R + R) * (16 << p.w4)) * sizeof(float) : 0);
     if (smem > 40 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(linear_w8_gemv_kernel<T, R, U>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return e;
@@ -438,7 +477,7 @@ cudaError_t launch_t(const GemvW8Params& p, cudaStream_t stream, int sms) {
 template <int T>
 cudaError_t launch_r(const GemvW8Params& p, cudaStream_t stream, int sms) {
     if constexpr (T <= 2) {
-        if (p.oc >= sms * 2 * 8 * 4) return launch_t<T, 4, 4>(p, stream, sms);
+        if (p.oc >= sms * 2 * 8 * 4 && !p.w4) return launch_t<T, 4, 4>(p, stream, sms);
     }
     if (p.oc >= sms * 2 * 8 * 2) return launch_t<T, 2, 4>(p, stream, sms);
     return launch_t<T, 1, 4>(p, stream, sms);
@@ -447,13 +486,13 @@ cudaError_t launch_r(const GemvW8Params& p, cudaStream_t stream, int sms) {
 }  // namespace
 
 // blocked (bs > 0): the shared memory also holds the per-block input sums and every warp's block parts (launch_t)
-bool linear_w8_gemv_supported(int tokens, int icp, int bs) {
-    const size_t extra = bs ? ((size_t)8 * (icp / bs) + 8 * 18 * 16) * sizeof(float) : 0;
+bool linear_w8_gemv_supported(int tokens, int icp, int bs, int w4) {
+    const size_t extra = bs ? ((size_t)8 * (icp / bs) + 8 * 18 * (16 << w4)) * sizeof(float) : 0;
     return tokens >= 1 && tokens <= 8 && (size_t)8 * icp + extra <= 200 * 1024;
 }
 
 cudaError_t launch_linear_w8_gemv(const GemvW8Params& p, cudaStream_t stream, int sms) {
-    if (p.tokens <= 1) return launch_r<1>(p, stream, sms);
+    if (p.tokens <= 1 && !p.w4) return launch_r<1>(p, stream, sms);
     if (p.tokens <= 2) return launch_r<2>(p, stream, sms);
     if (p.tokens <= 4) return launch_r<4>(p, stream, sms);
     return launch_r<8>(p, stream, sms);

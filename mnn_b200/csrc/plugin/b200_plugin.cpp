@@ -622,9 +622,12 @@ public:
             return nullptr;
         auto q = ConvolutionCommon::load(op, bn, false, true);     // reference's own IDST decoder, int8 weights kept
         if (!q || q->weight.get() == nullptr) return nullptr;
-        const int oc = cm->outputCount();
-        const int ic = (int)(q->weight.size() / oc);
-        if (ic <= 0 || q->weight.size() != (size_t)oc * ic) return nullptr;
+        // 4-bit layers come back packed, two weights per byte (canUseInt4, ConvolutionCommon.cpp:279-307, :357-371), so the input
+        // width is the op's inputCount, never weight.size() / oc; 2- and 3-bit layers stay on the CPU
+        if (q->canUseInt2 || q->canUseInt3) return nullptr;
+        const int oc = cm->outputCount(), ic = cm->inputCount();
+        const size_t wbytes = q->canUseInt4 ? (size_t)oc * ic / 2 : (size_t)oc * ic;
+        if (oc <= 0 || ic <= 0 || q->weight.size() != wbytes) return nullptr;
         const float* al = q->getAlphaFloat();
         const int per = q->asymmetric ? 2 : 1;
         // per-channel scales, or K-blocked ones (quant_block): [oc][blocks], blocks = alphaSize / (per * oc)
@@ -644,9 +647,14 @@ public:
         const bool hasBias = conv->bias() && (int)conv->bias()->size() == oc;
         if (hasBias) ::memcpy(bias.data(), conv->bias()->data(), sizeof(float) * oc);
         mnnb200_exec* h = nullptr;
-        if (mnnb200_linear_w8_create_blocked(bn->handle(), ic, oc, blocks, q->weight.get(), alpha.data(),
-                                             q->asymmetric ? wzero.data() : nullptr, hasBias ? bias.data() : nullptr,
-                                             cm->relu() ? 1 : 0, cm->relu6() ? 1 : 0, &h) != MNNB200_OK) {
+        const mnnb200_status st =
+            q->canUseInt4 ? mnnb200_linear_w4_create_blocked(bn->handle(), ic, oc, blocks, (const uint8_t*)q->weight.get(), alpha.data(),
+                                                             q->asymmetric ? wzero.data() : nullptr, hasBias ? bias.data() : nullptr,
+                                                             cm->relu() ? 1 : 0, cm->relu6() ? 1 : 0, &h)
+                          : mnnb200_linear_w8_create_blocked(bn->handle(), ic, oc, blocks, q->weight.get(), alpha.data(),
+                                                             q->asymmetric ? wzero.data() : nullptr, hasBias ? bias.data() : nullptr,
+                                                             cm->relu() ? 1 : 0, cm->relu6() ? 1 : 0, &h);
+        if (st != MNNB200_OK) {
             MNN_ERROR("mnn_b200 linear create: %s\n", mnnb200_last_error());
             return nullptr;
         }
@@ -654,6 +662,7 @@ public:
     }
     ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>&) override {
         auto d = dims4(inputs[0]);
+        if (d.c != mIc) return COMPUTE_SIZE_ERROR;      // the weights were made for mIc input channels
         mN = d.n; mArea = d.h * d.w;
         const int tokens = mN * mArea;
         if (mArea > 1 && (!mX.get((size_t)tokens * mIc * 4) || !mY.get((size_t)tokens * mOc * 4))) return OUT_OF_MEMORY;
