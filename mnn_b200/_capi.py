@@ -97,6 +97,7 @@ SIGNATURES = {
     "mnnb200_linear_w4_create_blocked": (C.c_int, [P, C.c_int, C.c_int, C.c_int, P, P, P, P, C.c_int, C.c_int, C.POINTER(P)]),
     "mnnb200_linear_w8_resize": (C.c_int, [P, C.c_int]),
     "mnnb200_linear_w8_execute": (C.c_int, [P, P, P]),
+    "mnnb200_linear_w8_plan": (C.c_int, [P, C.POINTER(C.c_int), C.c_int]),
     "mnnb200_matmul_create": (C.c_int, [P] + [C.c_int] * 7 + [C.POINTER(P)]),
     "mnnb200_matmul_execute": (C.c_int, [P, P, P, P, P]),
     "mnnb200_conv_f32_create": (C.c_int, [P, C.POINTER(ConvDesc), P, P, C.c_int, C.POINTER(P)]),

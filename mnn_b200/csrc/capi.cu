@@ -1236,6 +1236,42 @@ struct LinearW8Exec : Tagged<kLinearW8> {
     int w4 = 0;     // 4-bit weights (mnnb200_linear_w4_create_blocked): d_w holds [ocp][icp / 2] packed nibbles, icp % 32 == 0
 };
 
+enum class LinearPath { Gemv = 0, Gemm = 1, Pair = 2, Refused = -1 };
+// The kernel mnnb200_linear_w8_execute runs for the resized execution at its variant (0 auto, 2 GEMM, 3 CTA pair, 4 GEMV);
+// *why says why a combination is refused.
+static LinearPath linear_path(const LinearW8Exec* e, const char** why) {
+    const bool gemv = linear_w8_gemv_supported(e->tokens, e->icp, e->bs, e->w4);
+    *why = nullptr;
+    if (e->bs && e->variant == 3) *why = "the CTA-pair variant takes per-channel weight scales only";
+    else if (e->w4 && e->variant == 3) *why = "the CTA-pair variant takes 8-bit weights only";
+    // decode (<= 8 tokens): weight-streaming GEMV, bit-identical to the tensor-core kernels (variant 4 forces it)
+    else if (e->variant == 4 && !gemv) *why = "the GEMV variant takes 1..8 tokens";
+    // ONE token is a different ARITHMETIC in the reference (asymmetric single-quant, input zero folded into the bias: see
+    // linear_w8_gemv.cu), which only the GEMV kernel implements: the tensor-core kernels would silently compute the multi-token form
+    else if (e->tokens == 1 && (e->variant == 2 || e->variant == 3 || !gemv))
+        *why = "a single token runs the reference's decode arithmetic: GEMV kernel only (variant 0 or 4, ic <= 25600)";
+    else if (e->variant == 3 && !e->bn2) *why = "the CTA-pair variant needs >= 256 tokens and >= 64 output channels";
+    if (*why) return LinearPath::Refused;
+    if (e->variant == 4 || e->tokens == 1 || (e->variant == 0 && gemv)) return LinearPath::Gemv;
+    if (e->variant == 3 || (e->variant == 0 && e->bn2)) return LinearPath::Pair;
+    return LinearPath::Gemm;
+}
+// the tensor-core GEMMs' parameters for the resized execution writing y (nullptr for a plan query, which launches nothing)
+static GemmI8Params linear_gemm_params(const LinearW8Exec* e, float* y) {
+    GemmI8Params g;
+    memset(&g, 0, sizeof(g));
+    g.a = e->d_xq; g.b = e->d_w; g.M = e->tokens; g.N = e->ocp; g.K = e->icp;
+    g.y_f32 = y; g.ldy = e->oc; g.wscale = e->d_alpha; g.bias = e->has_bias ? static_cast<const float*>(e->d_bias) : nullptr;
+    g.wsum128 = e->d_wsum128;
+    g.OC = e->oc; g.dq = e->d_dq; g.srcsum = e->d_srcsum; g.wsumf = e->d_wsumf;
+    g.wzero = e->has_zero ? static_cast<const float*>(e->d_wzero) : nullptr;
+    g.relu = e->relu; g.relu6 = e->relu6;
+    g.bs = e->bs; g.blocks = e->blocks; g.balpha = e->d_talpha; g.bwzero = e->d_twzero; g.bws = e->d_tws; g.bw128 = e->d_tw128;
+    g.xsb = e->d_xsb;
+    g.w4 = e->w4;
+    return g;
+}
+
 extern "C" {
 mnnb200_status mnnb200_linear_w8_create(mnnb200_runtime* rt, int ic, int oc, const int8_t* wq, const float* alpha,
                                         const float* wzero, const float* bias, int relu, int relu6, mnnb200_exec** out) {
@@ -1401,15 +1437,10 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
     auto* e = exec_as<LinearW8Exec>(ex);
     if (!e) return fail(MNNB200_INVALID_VALUE, "linear_w8_execute: not a linear execution");
     if (e->tokens <= 0) return fail(MNNB200_NO_EXECUTION, "linear_w8_execute before resize");
-    if (e->bs && e->variant == 3) return fail(MNNB200_NOT_SUPPORT, "the CTA-pair variant takes per-channel weight scales only");
-    if (e->w4 && e->variant == 3) return fail(MNNB200_NOT_SUPPORT, "the CTA-pair variant takes 8-bit weights only");
-    // decode (<= 8 tokens): weight-streaming GEMV, bit-identical to the tensor-core kernels (variant 4 forces it)
-    if (e->variant == 4 && !linear_w8_gemv_supported(e->tokens, e->icp, e->bs, e->w4)) return fail(MNNB200_NOT_SUPPORT, "the GEMV variant takes 1..8 tokens");
-    // ONE token is a different ARITHMETIC in the reference (asymmetric single-quant, input zero folded into the bias: see
-    // linear_w8_gemv.cu), which only the GEMV kernel implements: the tensor-core kernels would silently compute the multi-token form
-    if (e->tokens == 1 && (e->variant == 2 || e->variant == 3 || !linear_w8_gemv_supported(1, e->icp, e->bs, e->w4)))
-        return fail(MNNB200_NOT_SUPPORT, "a single token runs the reference's decode arithmetic: GEMV kernel only (variant 0 or 4, ic <= 25600)");
-    if (e->variant == 4 || e->tokens == 1 || (e->variant == 0 && linear_w8_gemv_supported(e->tokens, e->icp, e->bs, e->w4))) {
+    const char* why;
+    const LinearPath path = linear_path(e, &why);
+    if (path == LinearPath::Refused) return fail(MNNB200_NOT_SUPPORT, why);
+    if (path == LinearPath::Gemv) {
         GemvW8Params g;
         g.x = x; g.w = e->d_w; g.y = y; g.alpha = e->d_alpha; g.bias = e->has_bias ? static_cast<float*>(e->d_bias) : nullptr; g.wsumf = e->d_wsumf;
         g.wzero = e->has_zero ? static_cast<float*>(e->d_wzero) : nullptr; g.wsum128 = e->d_wsum128;
@@ -1419,22 +1450,29 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
         return MNNB200_OK;
     }
     CK(launch_dynamic_quant(x, e->tokens, e->ic, e->icp, e->d_xq, e->d_dq, e->d_srcsum, e->rt->stream, e->bs, e->d_xsb));
-    if (e->variant == 3 && !e->bn2) return fail(MNNB200_NOT_SUPPORT, "the CTA-pair variant needs >= 256 tokens and >= 64 output channels");
-    GemmI8Params g;
-    memset(&g, 0, sizeof(g));
-    g.a = e->d_xq; g.b = e->d_w; g.M = e->tokens; g.N = e->ocp; g.K = e->icp;
-    g.y_f32 = y; g.ldy = e->oc; g.wscale = e->d_alpha; g.bias = e->has_bias ? static_cast<float*>(e->d_bias) : nullptr; g.wsum128 = e->d_wsum128;
-    g.OC = e->oc; g.dq = e->d_dq; g.srcsum = e->d_srcsum; g.wsumf = e->d_wsumf; g.wzero = e->has_zero ? static_cast<float*>(e->d_wzero) : nullptr;
-    g.relu = e->relu; g.relu6 = e->relu6;
-    g.bs = e->bs; g.blocks = e->blocks; g.balpha = e->d_talpha; g.bwzero = e->d_twzero; g.bws = e->d_tws; g.bw128 = e->d_tw128;
-    g.xsb = e->d_xsb;
-    g.w4 = e->w4;
-    if (e->variant == 3 || (e->variant == 0 && e->bn2)) {
+    const GemmI8Params g = linear_gemm_params(e, y);
+    if (path == LinearPath::Pair) {
         CK(launch_gemm_i8_2cta(g, &e->tmap_a, &e->tmap_b_half, e->bn2, e->rt->stream, e->rt->prop.multiProcessorCount));
         return MNNB200_OK;
     }
     CK(launch_gemm_i8_wgmma(g, &e->tmap_a, &e->tmap_b, e->bn, e->rt->stream, e->rt->prop.multiProcessorCount));
     return MNNB200_OK;
+}
+
+mnnb200_status mnnb200_linear_w8_plan(mnnb200_exec* ex, int* fields, int count) {
+    auto* e = exec_as<LinearW8Exec>(ex);
+    if (!e || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "linear_w8_plan: bad argument");
+    if (e->tokens <= 0) return fail(MNNB200_NO_EXECUTION, "linear_w8_plan before resize");
+    const char* why;
+    const LinearPath path = linear_path(e, &why);
+    const int sm = e->rt->prop.multiProcessorCount;
+    int bn = 0;
+    GemmI8Launch l;
+    memset(&l, 0, sizeof(l));
+    if (path == LinearPath::Gemm) { bn = e->bn; l = gemm_i8_wgmma_launch(linear_gemm_params(e, nullptr), bn, sm); }
+    if (path == LinearPath::Pair) { bn = e->bn2; l = gemm_i8_2cta_launch(linear_gemm_params(e, nullptr), bn, sm); }
+    const int v[] = {(int)path, bn, l.n_chunks, l.m_tiles, l.items, l.grid, l.one_tile, l.resident_b, l.stages, l.num_kb, l.smem};
+    return copy_fields(v, fields, count);
 }
 }  // extern "C"
 

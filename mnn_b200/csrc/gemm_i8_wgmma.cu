@@ -325,7 +325,8 @@ gemm_i8_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_co
                 float dqm = 0.f, ss = 0.f, corr = 0.f;
                 if (EPI == 1 && !blocked) { dqm = p.dq[m]; ss = p.srcsum[m]; corr = __fmul_rn(dqm, -128.f); }
                 float* yrow = p.y_f32 + ((size_t)bt * p.a_batch_rows + m) * p.ldy;
-                const bool vec_ok = (p.ldy & 1) == 0;
+                // float2 stores need an 8-byte aligned row: an even ldy and y itself 8-byte aligned (y need only be 4-byte aligned)
+                const bool vec_ok = (p.ldy & 1) == 0 && ((uintptr_t)p.y_f32 & 7) == 0;
 #pragma unroll
                 for (int j = 0; j < MAXBN / 8; ++j) {
                     if (j < nblk) {
@@ -419,6 +420,8 @@ KParams make_params(const GemmI8Params& g, int bn) {
 GemmI8Launch gemm_i8_wgmma_launch(const GemmI8Params& g, int bn, int sm_count) {
     const KParams p = make_params(g, bn);
     GemmI8Launch l;
+    l.n_chunks = p.n_chunks;
+    l.m_tiles = p.m_tiles;
     l.num_kb = (g.K + kBK - 1) / kBK;
     l.items = p.batch * p.m_tiles * p.n_chunks;
     l.grid = l.items < sm_count ? l.items : sm_count;
@@ -449,15 +452,27 @@ cudaError_t launch_gemm_i8_2cta(const GemmI8Params& g, const void* tmap_a, const
                                 int sm_count) {
     if (bn < 32 || bn > kMaxBN || (bn & 31) || g.y_f32 == nullptr || g.wino || g.bs || g.w4) return cudaErrorInvalidValue;
     KParams p = make_params(g, bn);
+    const GemmI8Launch l = gemm_i8_2cta_launch(g, bn, sm_count);
     p.batch = 1;
-    p.m_tiles = (g.M + 2 * kBM - 1) / (2 * kBM);
-    const int num_kb = (g.K + kBK - 1) / kBK;
-    const int smem = make_plan(bn, p.n_chunks, num_kb, true).total + 1024;
-    const int work = p.m_tiles * p.n_chunks;
-    int pairs = sm_count / 2;
-    if (work < pairs) pairs = work;
+    p.m_tiles = l.m_tiles;
     return launch(gemm_i8_wgmma_kernel<1, true, 256>, reinterpret_cast<const CUtensorMap*>(tmap_a),
-                  reinterpret_cast<const CUtensorMap*>(tmap_b_half), p, 2 * pairs, smem, 227 * 1024, true, stream);
+                  reinterpret_cast<const CUtensorMap*>(tmap_b_half), p, l.grid, l.smem, 227 * 1024, true, stream);
+}
+
+GemmI8Launch gemm_i8_2cta_launch(const GemmI8Params& g, int bn, int sm_count) {
+    GemmI8Launch l;
+    l.n_chunks = (g.N + bn - 1) / bn;
+    l.m_tiles = (g.M + 2 * kBM - 1) / (2 * kBM);
+    l.num_kb = (g.K + kBK - 1) / kBK;
+    l.items = l.m_tiles * l.n_chunks;
+    const int pairs = l.items < sm_count / 2 ? l.items : sm_count / 2;
+    l.grid = 2 * pairs;
+    l.one_tile = 0;
+    const SmemPlan pl = make_plan(bn, l.n_chunks, l.num_kb, true);
+    l.resident_b = pl.resident_b;
+    l.stages = pl.stages;
+    l.smem = pl.total + 1024;
+    return l;
 }
 
 }  // namespace mnnb200

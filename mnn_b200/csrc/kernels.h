@@ -68,11 +68,11 @@ struct GemmI8Params {
 };
 cudaError_t launch_gemm_i8_wgmma(const GemmI8Params& p, const void* tmap_a, const void* tmap_b, int bn, cudaStream_t stream,
                                  int sm_count);
-// the launch launch_gemm_i8_wgmma makes for (p, bn) on sm_count SMs: work items (batch, m tile, n chunk), persistent grid,
-// one_tile (every CTA owns exactly one item), resident_b (the weights stay in shared memory for the whole launch), the
-// operand ring's stages, 128-byte K blocks per item and the dynamic shared memory
+// the launch launch_gemm_i8_wgmma makes for (p, bn) on sm_count SMs: n chunks and 128-row m tiles, work items (batch, m tile,
+// n chunk), persistent grid, one_tile (every CTA owns exactly one item), resident_b (the weights stay in shared memory for the
+// whole launch), the operand ring's stages, 128-byte K blocks per item and the dynamic shared memory
 struct GemmI8Launch {
-    int items, grid, one_tile, resident_b, stages, num_kb, smem;
+    int n_chunks, m_tiles, items, grid, one_tile, resident_b, stages, num_kb, smem;
 };
 GemmI8Launch gemm_i8_wgmma_launch(const GemmI8Params& p, int bn, int sm_count);
 // ---- one persistent launch over a LIST of int8 convolutions (conv_group_wgmma.cu); a lone conv runs as a one-layer list.
@@ -139,6 +139,9 @@ cudaError_t launch_conv_group(const GroupMapsParam* maps_host, const GroupLayerP
 // bn % 32 == 0.
 cudaError_t launch_gemm_i8_2cta(const GemmI8Params& p, const void* tmap_a, const void* tmap_b_half, int bn, cudaStream_t stream,
                                 int sm_count);
+// the launch launch_gemm_i8_2cta makes: m_tiles counts 256-row pair tiles, items = m_tiles * n_chunks, grid = 2 CTAs per pair
+// (at most sm_count / 2 pairs); one_tile and resident_b are 0, the pair kernel has neither mode
+GemmI8Launch gemm_i8_2cta_launch(const GemmI8Params& p, int bn, int sm_count);
 
 // float (batched) MatMul on wgmma f16 / tf32 (gemm_f16_wgmma.cu): an operand that is not K-major already is packed first, in its
 // own type (fp16 or fp32)

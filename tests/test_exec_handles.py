@@ -97,7 +97,7 @@ TAKES = {
     "conv": {"mnnb200_conv_int8_resize", "mnnb200_conv_int8_execute", "mnnb200_conv_int8_groupable",
              "mnnb200_conv_int8_group_plan", "mnnb200_conv_int8_set_pad", "mnnb200_conv_int8_set_variant"},
     "dwconv": {"mnnb200_dwconv_int8_resize", "mnnb200_dwconv_int8_execute", "mnnb200_conv_int8_set_pad"},
-    "linear": {"mnnb200_linear_w8_resize", "mnnb200_linear_w8_execute", "mnnb200_conv_int8_set_variant"},
+    "linear": {"mnnb200_linear_w8_resize", "mnnb200_linear_w8_execute", "mnnb200_linear_w8_plan", "mnnb200_conv_int8_set_variant"},
     "wino": {"mnnb200_conv_int8_wino_resize", "mnnb200_conv_int8_wino_execute", "mnnb200_conv_int8_wino_execute_phases",
              "mnnb200_conv_int8_wino_plan", "mnnb200_conv_int8_set_pad"},
     "matmul": {"mnnb200_matmul_execute"},
@@ -111,7 +111,7 @@ EVERY_TYPE = {"mnnb200_exec_cost", "mnnb200_exec_destroy"}
 # execute and plan of a type before its resize (the group: before bind); matmul has no resize
 BEFORE_RESIZE = {
     "conv": ["mnnb200_conv_int8_execute", "mnnb200_conv_int8_group_plan"], "dwconv": ["mnnb200_dwconv_int8_execute"],
-    "linear": ["mnnb200_linear_w8_execute"],
+    "linear": ["mnnb200_linear_w8_execute", "mnnb200_linear_w8_plan"],
     "wino": ["mnnb200_conv_int8_wino_execute", "mnnb200_conv_int8_wino_execute_phases", "mnnb200_conv_int8_wino_plan"],
     "group": ["mnnb200_conv_group_execute"], "scale_int8": ["mnnb200_scale_int8_execute"],
     "conv_f32": ["mnnb200_conv_f32_execute", "mnnb200_conv_f32_plan"], "dwconv_f32": ["mnnb200_dwconv_f32_execute"],
@@ -120,7 +120,7 @@ BEFORE_RESIZE = {
 
 
 @pytest.mark.gpu
-def test_wrong_type_refused_and_execute_before_resize(backend):
+def test_exec_entry_points_refuse_wrong_type_and_before_resize(backend):
     L = _capi.lib()
     names = handle_entry_points("exec")
     assert set().union(*TAKES.values()) | EVERY_TYPE == set(names)
