@@ -19,6 +19,10 @@ class ConvDesc(C.Structure):
                                          "dilate_h", "dilate_w", "group", "relu")]
 
 
+class RopeNorm(C.Structure):
+    _fields_ = [("gamma", C.c_void_p), ("beta", C.c_void_p), ("size", C.c_int32), ("eps", C.c_float), ("rms", C.c_int32)]
+
+
 _lib = None
 
 # name -> (restype, argtypes); every symbol include/mnn_b200.h declares
@@ -118,6 +122,36 @@ SIGNATURES = {
     "mnnb200_argmax_f32": (C.c_int, [P, P, C.c_int, C.c_int, C.c_int, C.c_int, P]),
     "mnnb200_exec_destroy": (None, [P]),
 }
+
+
+# libmnn_b200_llm.so (include/mnn_b200_llm.h): MNN-LLM's LayerNorm / RoPE executions, on the runtime and execution handles above
+LLM_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_llm.so")
+LLM_SIGNATURES = {
+    "mnnb200_layernorm_f32_create": (C.c_int, [P, C.c_int, C.c_float, C.c_int, P, P, C.c_int, C.POINTER(P)]),
+    "mnnb200_layernorm_f32_resize": (C.c_int, [P, C.c_int]),
+    "mnnb200_layernorm_f32_execute": (C.c_int, [P, P, P, P, P]),
+    "mnnb200_rope_f32_create": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(RopeNorm), C.POINTER(RopeNorm),
+                                          C.POINTER(P)]),
+    "mnnb200_rope_f32_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int]),
+    "mnnb200_rope_f32_execute": (C.c_int, [P, P, P, P, P, P, P]),
+}
+_llm_lib = None
+
+
+def llm_lib():
+    """libmnn_b200_llm.so with every LLM_SIGNATURES symbol resolved (after libmnn_b200.so, whose handles it shares)"""
+    global _llm_lib
+    if _llm_lib is None:
+        lib()
+        if not os.path.exists(LLM_LIB_PATH):
+            raise MnnB200Error(f"{LLM_LIB_PATH} is missing: run `python -m mnn_b200.build` (there is no CPU fallback)")
+        L = C.CDLL(LLM_LIB_PATH)
+        for name, (res, args) in LLM_SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype = res
+            fn.argtypes = args
+        _llm_lib = L
+    return _llm_lib
 
 
 def lib():

@@ -20,114 +20,31 @@
 
 #include "../../include/mnn_b200.h"
 #include "common.cuh"
+#include "exec.h"
 #include "kernels.h"
 
 namespace mnnb200 {
-std::atomic<unsigned long long> g_launch_count{0};
+MNNB200_INTERNAL std::atomic<unsigned long long> g_launch_count{0};
 }
 using namespace mnnb200;
 
 static thread_local std::string g_err;
-static mnnb200_status fail(mnnb200_status s, const std::string& m) {
+namespace mnnb200 {
+MNNB200_INTERNAL mnnb200_status fail(mnnb200_status s, const std::string& m) {
     g_err = m;
     return s;
 }
-#define CK(call)                                                                                   \
-    do {                                                                                           \
-        cudaError_t _e = (call);                                                                   \
-        if (_e != cudaSuccess) {                                                                   \
-            cudaGetLastError(); /* do not leave it for an unrelated cudaGetLastError() to report */ \
-            return fail(MNNB200_CUDA_ERROR, std::string(#call) + ": " + cudaGetErrorString(_e));   \
-        }                                                                                          \
-    } while (0)
+}  // namespace mnnb200
 
-struct mnnb200_runtime {
-    int device = 0;
-    cudaStream_t stream = nullptr;
-    bool own_stream = false;
-    cudaDeviceProp prop;
-    cudaEvent_t ev_begin = nullptr, ev_end = nullptr;   // onGetLastGpuTimeMs
-    bool ev_valid = false;
-};
 struct mnnb200_graph {
     cudaGraph_t graph = nullptr;
     cudaGraphExec_t exec = nullptr;
 };
 
-// One device allocation, owned by the execution (or conv group) that holds it and freed with it.  Zero elements allocate 16
-// bytes, so every buffer has an address.  It converts to T* where a kernel's parameter block takes the pointer.
-template <class T>
-class DevBuf {
-  public:
-    DevBuf() = default;
-    DevBuf(const DevBuf&) = delete;
-    DevBuf& operator=(const DevBuf&) = delete;
-    ~DevBuf() { reset(); }
-    operator T*() const { return p_; }
-    // grow-only: a new allocation only when n elements do not fit.  The old one is released then (cudaFree waits for the
-    // device, so kernels still reading it have finished): repeated resizes do not accumulate device memory.
-    mnnb200_status reserve(size_t n) {
-        if (p_ && n <= cap_) return MNNB200_OK;
-        void* q = nullptr;
-        CK(cudaMalloc(&q, n ? n * sizeof(T) : 16));
-        reset();
-        p_ = static_cast<T*>(q);
-        cap_ = n;
-        return MNNB200_OK;
-    }
-    // reserve(h.size()), then copy h to the front of the buffer and wait for the copy: h may be a temporary
-    mnnb200_status upload(const std::vector<T>& h, cudaStream_t s) {
-        if (mnnb200_status st = reserve(h.size())) return st;
-        if (!h.empty()) CK(cudaMemcpyAsync(p_, h.data(), h.size() * sizeof(T), cudaMemcpyHostToDevice, s));
-        CK(cudaStreamSynchronize(s));
-        return MNNB200_OK;
-    }
-    void reset() {
-        if (p_) cudaFree(p_);
-        p_ = nullptr;
-        cap_ = 0;
-    }
-
-  private:
-    T* p_ = nullptr;
-    size_t cap_ = 0;
-};
-
-// The execution types, one bit each: a handle is tested against the types an entry point takes before it is cast (exec_as).
-enum ExecType : unsigned {
-    kConvInt8 = 1u << 0, kDwConvInt8 = 1u << 1, kLinearW8 = 1u << 2, kWinoInt8 = 1u << 3, kMatMul = 1u << 4,
-    kConvGroup = 1u << 5, kScaleInt8 = 1u << 6, kConvF32 = 1u << 7, kDwConvF32 = 1u << 8, kScaleF32 = 1u << 9,
-};
-struct mnnb200_exec {
-    unsigned type = 0;  // the ExecType of the struct new_exec made
-    mnnb200_runtime* rt = nullptr;
-    int variant = 0;  // mnnb200_conv_int8_set_variant: 0 auto, 1 mma.sync implicit GEMM (conv), 2 wgmma, 3 CTA pair, 4 GEMV (linear)
-    bool resized = false;
-    double cost_bytes = 0, cost_macs = 0;
-    virtual ~mnnb200_exec() = default;
-};
 // The five convolutions: the descriptor that set_pad edits.
 struct ConvExec : mnnb200_exec {
     mnnb200_conv_desc d;
 };
-// An execution struct derives from Tagged<its ExecType, its base>.
-template <unsigned Type, class Base = mnnb200_exec>
-struct Tagged : Base {
-    static constexpr unsigned kTypes = Type;
-};
-template <class T>
-static std::unique_ptr<T> new_exec(mnnb200_runtime* rt) {
-    auto e = std::make_unique<T>();
-    e->type = T::kTypes;
-    e->rt = rt;
-    return e;
-}
-// The handle as a T, or null for a NULL handle or a handle of a type outside `types`.  A tag compare rather than
-// dynamic_cast: nothing depends on RTTI across the library's hidden symbols.
-template <class T>
-static T* exec_as(mnnb200_exec* ex, unsigned types = T::kTypes) {
-    return ex && (ex->type & types) ? static_cast<T*>(ex) : nullptr;
-}
 // a plan query: the first `count` (at most N) of the plan's fields go to `fields`
 template <size_t N>
 static mnnb200_status copy_fields(const int (&v)[N], int* fields, int count) {
@@ -2038,3 +1955,4 @@ mnnb200_status mnnb200_softmax_f32(mnnb200_runtime* rt, const float* x, int outs
     return MNNB200_OK;
 }
 }  // extern "C"
+

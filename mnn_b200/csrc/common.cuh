@@ -84,6 +84,6 @@ __device__ __forceinline__ int4 ld_nc_16(const void* p) {
     return r;
 }
 
-extern std::atomic<unsigned long long> g_launch_count;  // host-side counter (capi.cu); any thread may launch
+extern __attribute__((visibility("default"))) std::atomic<unsigned long long> g_launch_count;  // host-side counter (capi.cu); any thread may launch
 
 }  // namespace mnnb200

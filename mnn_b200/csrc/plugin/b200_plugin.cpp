@@ -38,7 +38,7 @@
 #include "core/OpCommonUtils.hpp"
 #include "core/TensorUtils.hpp"
 
-#include "../../../include/mnn_b200.h"
+#include "../../../include/mnn_b200_llm.h"
 
 namespace MNN {
 namespace {
@@ -1077,6 +1077,144 @@ private:
     int mAxis;
 };
 
+// LayerNorm / RMSNorm fp32 (CPULayerNorm.cpp).  The [rows][inner] view comes from the input's shape, so the C ABI execution is made
+// at the first resize and again when inner changes; gamma / beta are read from the op as CPULayerNorm::makeResource reads them.
+class LayerNormF32Exec : public ClonedFromOp<LayerNormF32Exec> {
+public:
+    LayerNormF32Exec(Backend* bn, const Op* op) : ClonedFromOp(bn), mOp(op) {}
+    static Execution* create(B200Backend* bn, const Op* op) {
+        auto ln = op->main_as_LayerNorm();
+        if (!ln) return nullptr;
+        // gamma / beta held outside the op (LayerNorm.external, the useCachedMmap path) are not read here
+        const bool external = ln->external() && ln->external()->size() > 1 && ln->external()->data()[1] > 0;
+        if ((external && !(ln->gamma() && ln->beta())) || bn->getRuntime()->hint().useCachedMmap > 1) return nullptr;
+        return new LayerNormF32Exec(bn, op);
+    }
+    // rows x inner of the CPU's onResize (CPULayerNorm.cpp:228-256): the NC4HW4 forms normalise channels of [tokens, C, 1, 1];
+    // group > 1: length(0) * group rows; otherwise the last axis().size() dims.  false: a shape the execution does not take
+    static bool view(const Op* op, const Tensor* x, int* rows, int* inner) {
+        auto ln = op->main_as_LayerNorm();
+        const int rank = x->dimensions();
+        long long r = 1, n = 1;
+        if (TensorUtils::getDescribe(x)->dimensionFormat == MNN_DATA_FORMAT_NC4HW4) {
+            if (rank < 2) return false;
+            r = x->length(0); n = x->length(1);
+            if ((long long)elemCount(x) != r * n) return false;   // H * W > 1: the CPU's NC4HW4 branch ignores the spatial dims
+        } else if (ln->group() > 1) {
+            if (rank < 1) return false;
+            r = (long long)x->length(0) * ln->group();
+            for (int i = 1; i < rank; ++i) n *= x->length(i);
+            if (n % ln->group()) return false;
+            n /= ln->group();
+        } else {
+            const int axis = ln->axis() ? (int)ln->axis()->size() : 0;
+            if (axis > rank) return false;
+            for (int i = 0; i < rank - axis; ++i) r *= x->length(i);
+            for (int i = rank - axis; i < rank; ++i) n *= x->length(i);
+        }
+        if (r <= 0 || n <= 0 || r > 0x7fffffffLL || n > 0x7fffffffLL) return false;
+        *rows = (int)r; *inner = (int)n;
+        return true;
+    }
+    // the 1-in / 1-out form, or the NC4HW4 residual form (2-in / 2-out, CPULayerNorm.cpp:93-153); fp32 tensors only
+    static bool takes(const Op* op, const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) {
+        if (inputs.empty() || inputs.size() != outputs.size() || inputs.size() > 2) return false;
+        for (auto t : inputs) if (!isF32(t) || isInt8(t) || elemCount(t) != elemCount(inputs[0])) return false;
+        for (auto t : outputs) if (!isF32(t) || isInt8(t) || elemCount(t) != elemCount(inputs[0])) return false;
+        if (inputs.size() == 2) {
+            for (auto t : inputs) if (TensorUtils::getDescribe(t)->dimensionFormat != MNN_DATA_FORMAT_NC4HW4) return false;
+        }
+        int rows, inner;
+        if (!view(op, inputs[0], &rows, &inner)) return false;
+        auto ln = op->main_as_LayerNorm();
+        if (ln->gamma() && ln->beta() && ((int)ln->gamma()->size() != inner || (int)ln->beta()->size() != inner)) return false;
+        return true;
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        int rows, inner;
+        if (!takes(mOp, inputs, outputs) || !view(mOp, inputs[0], &rows, &inner)) return NOT_SUPPORT;
+        if (!mH || inner != mInner) {
+            auto ln = mOp->main_as_LayerNorm();
+            const bool affine = ln->gamma() && ln->beta();
+            mnnb200_exec* h = nullptr;
+            ErrorCode ec = toErr(mnnb200_layernorm_f32_create(rt(), inner, ln->epsilon(), ln->useRMSNorm() ? 1 : 0,
+                                                              affine ? ln->gamma()->data() : nullptr,
+                                                              affine ? ln->beta()->data() : nullptr, affine ? inner : 0, &h),
+                                 "LayerNorm fp32 create");
+            if (ec != NO_ERROR) return ec;
+            mH.reset(h);
+            mInner = inner;
+        }
+        return toErr(mnnb200_layernorm_f32_resize(mH.get(), rows), "LayerNorm fp32 resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        if (inputs.size() == 2)   // outputs: the sum x + r, then its norm
+            return toErr(mnnb200_layernorm_f32_execute(mH.get(), (const float*)dev(inputs[0]), (const float*)dev(inputs[1]),
+                                                       (float*)dev(outputs[0]), (float*)dev(outputs[1])), "LayerNorm fp32");
+        return toErr(mnnb200_layernorm_f32_execute(mH.get(), (const float*)dev(inputs[0]), nullptr, nullptr, (float*)dev(outputs[0])),
+                     "LayerNorm fp32");
+    }
+private:
+    const Op* mOp;
+    ExecHandle mH;
+    int mInner = 0;
+};
+// Fused RoPE fp32 (CPURoPE.cpp): q / k NC4HW4 [seq, C, 1, 1] (stored [seq][C] here), cos / sin [seq][ropeDim], outputs NHWC
+// [1, seq, heads, head_dim]; the q / k norm tables read from RoPEParam as makeRopeNormResource reads them (CPURoPE.cpp:20-49)
+class RoPEF32Exec : public ClonedFromOp<RoPEF32Exec> {
+public:
+    RoPEF32Exec(Backend* bn, mnnb200_exec* h) : ClonedFromOp(bn), mH(h) {}
+    static Execution* create(B200Backend* bn, const Op* op) {
+        auto rp = op->main_as_RoPEParam();
+        if (!rp) return nullptr;
+        mnnb200_rope_norm qn, kn;
+        auto table = [](const LayerNorm* ln, mnnb200_rope_norm* t) -> const mnnb200_rope_norm* {
+            if (!ln || !ln->gamma() || ln->gamma()->size() == 0) return nullptr;
+            const int size = (int)ln->gamma()->size();
+            *t = mnnb200_rope_norm{ln->gamma()->data(), (ln->beta() && (int)ln->beta()->size() == size) ? ln->beta()->data() : nullptr,
+                                   size, ln->epsilon(), ln->useRMSNorm() ? 1 : 0};
+            return t;
+        };
+        mnnb200_exec* h = nullptr;
+        if (mnnb200_rope_f32_create(bn->handle(), rp->num_head(), rp->kv_num_head(), rp->head_dim(), rp->rope_cut_head_dim(),
+                                    table(rp->q_norm(), &qn), table(rp->k_norm(), &kn), &h) != MNNB200_OK)
+            return nullptr;
+        return new RoPEF32Exec(bn, h);
+    }
+    // validRopeC4Input (CPURoPE.cpp:71-84), fp32 everywhere, cos / sin linear with a ropeDim row per token
+    static bool takes(const Op* op, const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) {
+        auto rp = op->main_as_RoPEParam();
+        if (!rp || inputs.size() != 4 || outputs.size() != 2) return false;
+        const int heads = rp->num_head(), kvh = rp->kv_num_head(), hd = rp->head_dim();
+        if (heads <= 0 || kvh <= 0 || hd <= 0) return false;
+        for (auto t : inputs) if (!isF32(t) || isInt8(t)) return false;
+        for (auto t : outputs) if (!isF32(t) || isInt8(t)) return false;
+        auto q = inputs[0], k = inputs[1];
+        for (auto t : {q, k})
+            if (TensorUtils::getDescribe(t)->dimensionFormat != MNN_DATA_FORMAT_NC4HW4 || t->dimensions() != 4 || t->length(2) != 1 ||
+                t->length(3) != 1)
+                return false;
+        if (q->length(0) != k->length(0) || q->length(1) != heads * hd || k->length(1) != kvh * hd) return false;
+        const int cut = rp->rope_cut_head_dim();
+        const size_t ropeDim = (size_t)((cut <= 0 || cut > hd ? hd : cut) / 2 * 2);
+        for (int i = 2; i < 4; ++i)
+            if (TensorUtils::getDescribe(inputs[i])->dimensionFormat == MNN_DATA_FORMAT_NC4HW4 ||
+                elemCount(inputs[i]) < (size_t)q->length(0) * ropeDim)
+                return false;
+        return elemCount(outputs[0]) == elemCount(q) && elemCount(outputs[1]) == elemCount(k);
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>&) override {
+        return toErr(mnnb200_rope_f32_resize(mH.get(), inputs[0]->length(0), inputs[0]->length(1), inputs[1]->length(1)), "RoPE fp32 resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        return toErr(mnnb200_rope_f32_execute(mH.get(), (const float*)dev(inputs[0]), (const float*)dev(inputs[1]),
+                                              (const float*)dev(inputs[2]), (const float*)dev(inputs[3]), (float*)dev(outputs[0]),
+                                              (float*)dev(outputs[1])), "RoPE fp32");
+    }
+private:
+    ExecHandle mH;
+};
+
 Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs, const MNN::Op* op) {
     Execution* e = nullptr;
     const bool quantOut = !outputs.empty() && TensorUtils::getDescribe(outputs[0])->quantAttr.get() != nullptr &&
@@ -1209,6 +1347,12 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
             if (ok) e = new RasterExec(this);
             break;
         }
+        case OpType_LayerNorm:
+            if (!quantOut && LayerNormF32Exec::takes(op, inputs, outputs)) e = LayerNormF32Exec::create(this, op);
+            break;
+        case OpType_RoPE:
+            if (!quantOut && RoPEF32Exec::takes(op, inputs, outputs)) e = RoPEF32Exec::create(this, op);
+            break;
         default:
             break;
     }
