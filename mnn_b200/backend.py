@@ -374,27 +374,21 @@ class LinearW8Execution(Execution):
         wz = None if op.wzero is None else np.ascontiguousarray(op.wzero, np.float32)
         b = None if op.bias is None else np.ascontiguousarray(op.bias, np.float32)
         relu = int(bool(op.conv.get("relu", False)))
-        self.oc = op.conv["oc"]
-        if op.bits == 4:        # alpha [oc] or [oc, blocks], wzero of the same shape or None
-            wp = np.ascontiguousarray(op.weight, np.uint8).reshape(-1)
-            if wp.size * 2 != op.conv["oc"] * op.conv["ic"]:
-                raise MnnB200Error(f"LinearW8 bits=4: {wp.size} packed bytes for oc {op.conv['oc']} x ic {op.conv['ic']}")
-            check(_capi.lib().mnnb200_linear_w4_create_blocked(backend.runtime._h, op.conv["ic"], op.conv["oc"],
-                                                               al.shape[1] if al.ndim == 2 else 1, _np_ptr(wp), _np_ptr(al),
-                                                               _np_ptr(wz), _np_ptr(b), relu, int(op.relu6), C.byref(self._h)),
-                  "linear_w4_create_blocked")
-            return
-        if op.bits != 8:
-            raise MnnB200Error(f"LinearW8: {op.bits}-bit weights are not supported")
-        wq = np.ascontiguousarray(op.weight, np.int8).reshape(op.conv["oc"], op.conv["ic"])
-        if al.ndim == 2:        # [oc, blocks]: K-blocked weight scales (quant_block), wzero of the same shape or None
-            check(_capi.lib().mnnb200_linear_w8_create_blocked(backend.runtime._h, op.conv["ic"], op.conv["oc"], al.shape[1],
-                                                               _np_ptr(wq), _np_ptr(al), _np_ptr(wz), _np_ptr(b), relu,
-                                                               int(op.relu6), C.byref(self._h)), "linear_w8_create_blocked")
+        ic, self.oc = op.conv["ic"], op.conv["oc"]
+        # alpha [oc] (per channel) or [oc, blocks] (K-blocked weight scales, quant_block), wzero of the same shape or None
+        blocks = al.shape[1] if al.ndim == 2 else 1
+        if op.bits == 4:
+            w = np.ascontiguousarray(op.weight, np.uint8).reshape(-1)
+            if w.size * 2 != self.oc * ic:
+                raise MnnB200Error(f"LinearW8 bits=4: {w.size} packed bytes for oc {self.oc} x ic {ic}")
+            create = _capi.lib().mnnb200_linear_w4_create_blocked
+        elif op.bits == 8:
+            w = np.ascontiguousarray(op.weight, np.int8).reshape(self.oc, ic)
+            create = _capi.lib().mnnb200_linear_w8_create_blocked
         else:
-            check(_capi.lib().mnnb200_linear_w8_create(backend.runtime._h, op.conv["ic"], op.conv["oc"], _np_ptr(wq),
-                                                       _np_ptr(al), _np_ptr(wz), _np_ptr(b), relu, int(op.relu6),
-                                                       C.byref(self._h)), "linear_w8_create")
+            raise MnnB200Error(f"LinearW8: {op.bits}-bit weights are not supported")
+        check(create(backend.runtime._h, ic, self.oc, blocks, _np_ptr(w), _np_ptr(al), _np_ptr(wz), _np_ptr(b), relu,
+                     int(op.relu6), C.byref(self._h)), f"LinearW8 bits={op.bits}")
 
     def onResize(self, inputs, outputs):
         tokens = inputs[0].shape[0]

@@ -251,21 +251,39 @@ def ref_conv(mode, x, w, bias, scale, stride=(1, 1), pad=(0, 0), dilate=(1, 1), 
     return np.frombuffer(raw[16:], np.int8).reshape(dims).copy()
 
 
-def ref_linear(x, wq, alpha, asym=False, bias=None, relu=False, relu6=False, threads=1, blocks=1):
-    """alpha: [oc * blocks] scales (or {min, scale} pairs when asym), K split into `blocks` equal runs per output channel."""
+def linear_request(x, q, alpha, asym=False, bias=None, blocks=1, relu=False, relu6=False):
+    """the request file of `refdump linear` and `refdump_w4 linear`: x [tokens][ic] fp32, q [oc][ic] int8 (in [-8, 7] for
+    refdump_w4), alpha [oc * blocks] scales or {min, scale} pairs when asym, K split into `blocks` equal runs per output channel"""
     x = np.ascontiguousarray(x, np.float32)
-    wq = np.ascontiguousarray(wq, np.int8)
+    q = np.ascontiguousarray(q, np.int8)
     tokens, ic = x.shape
-    oc = wq.shape[0]
-    hdr = struct.pack("<8i", tokens, ic, oc, int(asym), int(relu), int(relu6), int(bias is not None), int(blocks) if blocks > 1 else 0)
-    payload = hdr + x.tobytes() + wq.tobytes() + np.ascontiguousarray(alpha, np.float32).tobytes()
+    hdr = struct.pack("<8i", tokens, ic, q.shape[0], int(asym), int(relu), int(relu6), int(bias is not None),
+                      int(blocks) if blocks > 1 else 0)
+    payload = hdr + x.tobytes() + q.tobytes() + np.ascontiguousarray(alpha, np.float32).tobytes()
     if bias is not None:
         payload += np.ascontiguousarray(bias, np.float32).tobytes()
+    return payload
+
+
+def run_linear_request(payload, tokens, oc, harness=REFDUMP, env=None, threads=1):
+    """`harness linear` (REFDUMP, or w4_oracle.REFDUMP_W4) on a linear_request: (y [tokens][oc], the finished process).
+    env: the harness's environment, by default this one with oracle/_ref on the library path."""
+    if env is None:
+        env = dict(os.environ)
+        env["LD_LIBRARY_PATH"] = REF_DIR + ":" + env.get("LD_LIBRARY_PATH", "")
     with tempfile.TemporaryDirectory() as d:
         req, out = os.path.join(d, "req.bin"), os.path.join(d, "out.bin")
         open(req, "wb").write(payload)
-        _run_refdump(["linear", req, out, threads])
-        return np.fromfile(out, np.float32).reshape(tokens, oc)
+        r = subprocess.run([harness, "linear", req, out, str(threads)], env=env, capture_output=True, text=True, timeout=600)
+        assert r.returncode == 0, r.stderr[-1500:]
+        return np.fromfile(out, np.float32).reshape(tokens, oc), r
+
+
+def ref_linear(x, wq, alpha, asym=False, bias=None, relu=False, relu6=False, threads=1, blocks=1):
+    """the reference CPU backend's linear layer: alpha [oc * blocks] scales (or {min, scale} pairs when asym), K split into
+    `blocks` equal runs per output channel."""
+    payload = linear_request(x, wq, alpha, asym, bias, blocks, relu, relu6)
+    return run_linear_request(payload, np.shape(x)[0], np.shape(wq)[0], threads=threads)[0]
 
 
 def ref_run_model(model, batch, seed, outdir, threads=1):

@@ -4,9 +4,7 @@ TEST INFRASTRUCTURE ONLY, like oracle/oracle.py: mnn_b200 (the product) never im
 """
 import ctypes as C
 import os
-import struct
 import subprocess
-import tempfile
 
 import numpy as np
 
@@ -89,29 +87,7 @@ def linear_w4_dynamic_blocks(x, wpacked, oc, alpha, wzero=None, bias=None, block
     return y
 
 
-def linear_request(x, q, alpha, asym=False, bias=None, blocks=1):
-    """the request file of `refdump linear` / `refdump_w4 linear`: q [oc][ic] int8, alpha [oc * blocks] scales or {min, scale}"""
-    x = np.ascontiguousarray(x, np.float32)
-    q = np.ascontiguousarray(q, np.int8)
-    tokens, ic = x.shape
-    hdr = struct.pack("<8i", tokens, ic, q.shape[0], int(asym), 0, 0, int(bias is not None), int(blocks) if blocks > 1 else 0)
-    return hdr + x.tobytes() + q.tobytes() + np.ascontiguousarray(alpha, np.float32).tobytes() + \
-        (np.ascontiguousarray(bias, np.float32).tobytes() if bias is not None else b"")
-
-
-def run_refdump(payload, tokens, oc, env=None, threads=1):
-    """refdump_w4 linear on a request: (y [tokens][oc], stdout)"""
-    if env is None:
-        env = dict(os.environ)
-        env["LD_LIBRARY_PATH"] = O.REF_DIR + ":" + env.get("LD_LIBRARY_PATH", "")
-    with tempfile.TemporaryDirectory() as d:
-        req, out = os.path.join(d, "req.bin"), os.path.join(d, "out.bin")
-        open(req, "wb").write(payload)
-        r = subprocess.run([REFDUMP_W4, "linear", req, out, str(threads)], env=env, capture_output=True, text=True, timeout=300)
-        assert r.returncode == 0, r.stderr[-1500:]
-        return np.fromfile(out, np.float32).reshape(tokens, oc), r.stdout
-
-
 def ref_linear(x, q, alpha, asym=False, bias=None, blocks=1, threads=1):
     """the reference CPU backend's 4-bit linear layer: q [oc][ic] in [-8, 7], alpha as the wire holds it"""
-    return run_refdump(linear_request(x, q, alpha, asym, bias, blocks), x.shape[0], q.shape[0], threads=threads)[0]
+    payload = O.linear_request(x, q, alpha, asym, bias, blocks)
+    return O.run_linear_request(payload, np.shape(x)[0], np.shape(q)[0], REFDUMP_W4, threads=threads)[0]

@@ -5,19 +5,15 @@ tokens.  The plugin cases drive the reference's own Executor through libmnn_b200
 import ctypes as C
 import json
 import os
-import struct
-import subprocess
-import sys
-import tempfile
 
 import numpy as np
 import pytest
 
 from oracle import oracle as O
-from tests.test_gpu_dispatch import KERNEL_TESTS, WGMMA_KEY, expect, launched, ok
+from oracle import w4_oracle as W
+from tests.test_gpu_dispatch import (ROOT, check_linear, create_linear, golden_cases, golden_check, golden_check_profiled_in_child,
+                                     linear_data, profile_golden_cases, run_linear)
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-GOLD = os.path.join(ROOT, "tests", "golden", "block_linear_golden.npz")
 PLUGIN = os.path.join(ROOT, "mnn_b200", "libmnn_b200_plugin.so")
 
 
@@ -28,94 +24,23 @@ def status_codes():
     return tuple(int(re.search(rf"MNNB200_{n}\s*=\s*(-?\d+)", h).group(1)) for n in ("INVALID_VALUE", "NOT_SUPPORT"))
 
 
-def golden_cases():
-    g = np.load(GOLD)
-    out = []
-    for j in range(int(g["n"])):
-        alpha, wmin, bias = g[f"b{j}_alpha"], g[f"b{j}_wmin"], g[f"b{j}_bias"]
-        wz = (wmin - np.float32(-128) * alpha).astype(np.float32) if wmin.size else None
-        out.append((g[f"b{j}_x"], g[f"b{j}_wq"], alpha, wz, wmin if wmin.size else None, bias if bias.size else None, g[f"b{j}_y"]))
-    return out
-
-
-def block_data(rng, tokens, ic, oc, bs, asym, has_bias):
-    blocks = ic // bs
-    x = rng.uniform(-1, 1, (tokens, ic)).astype(np.float32)
-    wq = rng.integers(-128, 128, (oc, ic), dtype=np.int8)
-    alpha = rng.uniform(0.001, 0.01, (oc, blocks)).astype(np.float32)
-    wzero = rng.uniform(-0.05, 0.05, (oc, blocks)).astype(np.float32) if asym else None
-    bias = rng.uniform(-1, 1, oc).astype(np.float32) if has_bias else None
-    return x, wq, alpha, wzero, bias
-
-
-def run_blocked(backend, x, wq, alpha, wzero, bias, variants, relu6=False, misalign=False, profile=False):
-    """the layer at each variant (0 auto, 2 GEMM, 4 GEMV) on one execution, outputs NaN-poisoned first: {variant: (y, keys)}.
-    profile: run each under torch.profiler (test_gpu_dispatch.launched) and return the launched kernel keys, else keys = None."""
-    import torch
-    from mnn_b200 import _capi
-    from mnn_b200.backend import Op, Tensor
-    tokens, ic = x.shape
-    oc = wq.shape[0]
-    op = Op(type="LinearW8", conv=dict(ic=ic, oc=oc, kernel=(1, 1)), weight=wq, wscale=alpha, wzero=wzero, bias=bias,
-            relu6=relu6)
-    if misalign:        # a view 4 bytes into a buffer: x is 4 bytes past 16-byte alignment
-        buf = torch.zeros(tokens * ic + 8, dtype=torch.float32, device="cuda")
-        xd = buf[1:1 + tokens * ic].view(tokens, ic)
-        xd.copy_(torch.from_numpy(x))
-        assert xd.data_ptr() % 16 == 4
-    else:
-        xd = torch.from_numpy(x).cuda()
-    xin = Tensor((tokens, ic), "float", data=xd)
-    yout = Tensor((tokens, oc), "float")
-    ex = backend.onCreate([xin], [yout], op)
-    assert ex is not None and ex.onResize([xin], [yout]) == 0
-    yout.data = torch.empty((tokens, oc), dtype=torch.float32, device="cuda")
-    res = {}
-    for v in variants:
-        _capi.check(_capi.lib().mnnb200_conv_int8_set_variant(ex._h, v))
-        keys = None
-        if profile:
-            keys = launched(backend, lambda: ok(ex.onExecute([xin], [yout])), lambda: yout.data.fill_(float("nan")))
-        else:
-            yout.data.fill_(float("nan"))
-            ok(ex.onExecute([xin], [yout]))
-            backend.onSync()
-        y = yout.data.cpu().numpy()
-        assert not np.isnan(y).any(), f"variant {v}: outputs left unwritten"
-        res[v] = (y, keys)
-    return res
-
-
-def variants_for(tokens):
-    return (0,) if tokens == 1 else (0, 2, 4) if tokens <= 8 else (0, 2)
-
-
-def check_blocked(backend, x, wq, alpha, wzero, bias, relu6=False, misalign=False, profile=False):
-    """auto (and the forced GEMM / GEMV where they apply) against the oracle, bit for bit; returns the output.  profile: also
-    every launched kernel is one of the instantiations KERNEL_TESTS lists (blocked layers add no entry point)"""
-    tokens = x.shape[0]
-    ref = O.linear_w8_dynamic_blocks(x, wq, alpha, wzero, bias, alpha.shape[1], relu6=relu6)
-    res = run_blocked(backend, x, wq, alpha, wzero, bias, variants_for(tokens), relu6=relu6, misalign=misalign, profile=profile)
-    for v, (y, keys) in res.items():
-        assert np.array_equal(y, ref), f"variant {v}: {np.count_nonzero(y != ref)} outputs differ, max {np.abs(y - ref).max()}"
-        if profile:
-            assert set(keys) <= set(KERNEL_TESTS), f"variant {v} launched kernels outside KERNEL_TESTS: {sorted(keys)}"
-            if v == 2 or (v == 0 and tokens > 8):
-                expect(keys, WGMMA_KEY)
-            if v == 4 or (v == 0 and tokens <= 8):
-                assert {k[0] for k in keys} == {"linear_w8_gemv_kernel"}, sorted(keys)
-    return ref
-
-
-def golden_check(backend, profile):
-    for j, (x, wq, alpha, wz, _, bias, gold) in enumerate(golden_cases()):
-        y = check_blocked(backend, x, wq, alpha, wz, bias, profile=profile)
-        assert np.abs(y - gold).max() <= 4e-6 * np.abs(gold).max(), f"golden {j}: {np.abs(y - gold).max() / np.abs(gold).max()}"
+def run_on_plugin(x, w, alpha, wmin, bias, blocks, bits=8):
+    """one linear layer (wmin: the wire min or None) through the reference's Executor on MNN_FORWARD_CUDA, the plugin loaded
+    into refdump (4-bit: refdump_w4): (y, the plugin's last stats line or None, the finished process)"""
+    env = dict(os.environ, REFDUMP_PLUGIN=PLUGIN)
+    env["LD_LIBRARY_PATH"] = O.REF_DIR + ":" + os.path.join(ROOT, "mnn_b200") + ":" + env.get("LD_LIBRARY_PATH", "")
+    oc = alpha.shape[0]
+    q = W.unpack_w4(w, oc) if bits == 4 else w
+    al = np.stack([wmin, alpha], 2) if wmin is not None else alpha         # {min, scale} pairs when asymmetric
+    payload = O.linear_request(x, q, al.ravel(), wmin is not None, bias, blocks)
+    y, r = O.run_linear_request(payload, x.shape[0], oc, W.REFDUMP_W4 if bits == 4 else O.REFDUMP, env=env)
+    stats = [json.loads(l) for l in r.stdout.splitlines() if l.startswith("{\"plugin_")]
+    return y, (stats[-1] if stats else None), r
 
 
 @pytest.mark.gpu
 def test_block_linear_golden_cases(backend):
-    golden_check(backend, profile=False)
+    golden_check(backend, 8)
 
 
 @pytest.mark.gpu
@@ -124,9 +49,7 @@ def test_block_linear_launches_listed_kernels():
     the GEMM for the forced tensor-core variant, the GEMV alone for <= 8 tokens.  In a child process: a profiler that this
     module starts early in the GPU suite leaves CUPTI subscribed (test_gpu_dispatch keeps it so), and the windows
     test_gpu_dispatch opens later in the same process then recorded no kernel launches."""
-    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-m", "tests.test_gpu_block_linear"]
-    r = subprocess.run(cmd, cwd=ROOT, capture_output=True, text=True, timeout=600)
-    assert r.returncode == 0 and "golden cases profiled" in r.stdout, r.stdout[-1500:] + r.stderr[-3000:]
+    golden_check_profiled_in_child("tests.test_gpu_block_linear")
 
 
 SWEEP = [  # (tokens, ic, oc, bs, asym, bias, relu6)
@@ -144,40 +67,21 @@ SWEEP = [  # (tokens, ic, oc, bs, asym, bias, relu6)
 @pytest.mark.parametrize("tokens,ic,oc,bs,asym,has_bias,relu6", SWEEP)
 def test_block_linear_sweep(backend, tokens, ic, oc, bs, asym, has_bias, relu6):
     rng = np.random.default_rng(tokens * 7919 + ic * 31 + oc + bs)
-    x, wq, alpha, wzero, bias = block_data(rng, tokens, ic, oc, bs, asym, has_bias)
-    check_blocked(backend, x, wq, alpha, wzero, bias, relu6=relu6)
+    x, wq, alpha, wzero, bias = linear_data(rng, tokens, ic, oc, asym, has_bias, bs=bs)
+    check_linear(backend, x, wq, alpha, wzero, bias, relu6=relu6)
 
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("tokens", [1, 3, 20])
 def test_block_linear_relu_zero_row_misaligned(backend, tokens):
     """relu (conv flag), an all-zero token row (the amax < 1e-7 / range <= 1e-7 branches) and x 4 bytes past alignment"""
-    import torch
-    from mnn_b200 import _capi
-    from mnn_b200.backend import Op, Tensor
     rng = np.random.default_rng(5 + tokens)
-    x, wq, alpha, wzero, bias = block_data(rng, tokens, 1024, 72, 64, True, True)
+    x, wq, alpha, wzero, bias = linear_data(rng, tokens, 1024, 72, True, True, bs=64)
     x[tokens // 2] = 0
-    check_blocked(backend, x, wq, alpha, wzero, bias, misalign=True)
+    check_linear(backend, x, wq, alpha, wzero, bias, misalign=True)
     ref = O.linear_w8_dynamic_blocks(x, wq, alpha, wzero, bias, alpha.shape[1], relu=True)
-    op = Op(type="LinearW8", conv=dict(ic=1024, oc=72, kernel=(1, 1), relu=True), weight=wq, wscale=alpha, wzero=wzero, bias=bias)
-    xin = Tensor((tokens, 1024), "float", data=torch.from_numpy(x).cuda())
-    yout = Tensor((tokens, 72), "float")
-    ex = backend.onCreate([xin], [yout], op)
-    assert ex is not None and ex.onResize([xin], [yout]) == 0
-    yout.data = torch.full((tokens, 72), float("nan"), dtype=torch.float32, device="cuda")
-    _capi.check(ex.onExecute([xin], [yout]))
-    backend.onSync()
-    assert np.array_equal(yout.data.cpu().numpy(), ref)
-
-
-def _create(backend, ic, oc, blocks, wq, alpha, wzero=None, bias=None):
-    from mnn_b200 import _capi
-    h = C.c_void_p()
-    ptr = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-    st = _capi.lib().mnnb200_linear_w8_create_blocked(backend.runtime._h, ic, oc, blocks, ptr(wq), ptr(alpha), ptr(wzero),
-                                                      ptr(bias), 0, 0, C.byref(h))
-    return st, h
+    y = run_linear(backend, x, wq, alpha, wzero, bias, (0,), relu=True)[0][0]
+    assert np.array_equal(y, ref)
 
 
 @pytest.mark.gpu
@@ -189,11 +93,11 @@ def test_block_linear_variants_and_validation(backend):
     rng = np.random.default_rng(3)
     ic, oc = 512, 96
     for tokens in (2, 5, 8):        # GEMV (variant 4) and GEMM (variant 2): identical bits
-        x, wq, alpha, wzero, bias = block_data(rng, tokens, ic, oc, 64, True, True)
-        res = run_blocked(backend, x, wq, alpha, wzero, bias, (4, 2))
+        x, wq, alpha, wzero, bias = linear_data(rng, tokens, ic, oc, True, True, bs=64)
+        res = run_linear(backend, x, wq, alpha, wzero, bias, (4, 2))
         assert np.array_equal(res[4][0], res[2][0]), f"{tokens} tokens: GEMV and GEMM differ"
-    x, wq, alpha, wzero, bias = block_data(rng, 300, ic, oc, 64, True, True)
-    st, h = _create(backend, ic, oc, ic // 64, wq, alpha, wzero, bias)
+    x, wq, alpha, wzero, bias = linear_data(rng, 300, ic, oc, True, True, bs=64)
+    st, h = create_linear(backend, ic, oc, wq, alpha, wzero, bias)
     assert st == 0
     try:
         xd = torch.from_numpy(x).cuda()
@@ -206,16 +110,25 @@ def test_block_linear_variants_and_validation(backend):
         assert lib.mnnb200_linear_w8_execute(h, C.c_void_p(xd.data_ptr()), C.c_void_p(yd.data_ptr())) == nsup
     finally:
         lib.mnnb200_exec_destroy(h)
-    # blocks == 1 through the blocked entry is the per-channel layer, bit for bit
+    # blocks == 1 through the blocked entry (the layer's Op) is the per-channel layer (mnnb200_linear_w8_create), bit for bit
     for tokens in (1, 4, 40):
-        x, wq, alpha, wzero, bias = block_data(rng, tokens, ic, oc, ic, True, True)
-        yb = run_blocked(backend, x, wq, alpha, wzero, bias, (0,))[0][0]
-        yc = run_blocked(backend, x, wq, alpha[:, 0].copy(), wzero[:, 0].copy(), bias, (0,))[0][0]
-        assert np.array_equal(yb, yc)
+        x, wq, alpha, wzero, bias = linear_data(rng, tokens, ic, oc, True, True, bs=ic)
+        yb = run_linear(backend, x, wq, alpha, wzero, bias, (0,))[0][0]
+        st, h = create_linear(backend, ic, oc, wq, alpha[:, 0].copy(), wzero[:, 0].copy(), bias)
+        assert st == 0
+        try:
+            xd = torch.from_numpy(x).cuda()
+            yd = torch.full((tokens, oc), float("nan"), dtype=torch.float32, device="cuda")
+            assert lib.mnnb200_linear_w8_resize(h, tokens) == 0
+            assert lib.mnnb200_linear_w8_execute(h, C.c_void_p(xd.data_ptr()), C.c_void_p(yd.data_ptr())) == 0
+            backend.onSync()
+        finally:
+            lib.mnnb200_exec_destroy(h)
+        assert np.array_equal(yb, yd.cpu().numpy())
     wq = np.zeros((oc, ic), np.int8)
     for blocks, want in ((0, inval), (-1, inval), (3, inval), (ic // 16, nsup), (5, inval)):
         al = np.ones((oc, max(blocks, 1)), np.float32)
-        st, h = _create(backend, ic, oc, blocks, wq, al)
+        st, h = create_linear(backend, ic, oc, wq, al, blocks=blocks)
         if st == 0:
             lib.mnnb200_exec_destroy(h)
         assert st == want, (blocks, st)
@@ -229,40 +142,19 @@ def test_block_linear_through_reference_executor_on_plugin():
         pytest.skip("the reference core (oracle/_ref) is not in this snapshot")
     if not os.path.exists(PLUGIN):
         pytest.fail("mnn_b200/libmnn_b200_plugin.so is missing although the reference core is present")
-    env = dict(os.environ, REFDUMP_PLUGIN=PLUGIN)
-    env["LD_LIBRARY_PATH"] = O.REF_DIR + ":" + os.path.join(ROOT, "mnn_b200") + ":" + env.get("LD_LIBRARY_PATH", "")
-
-    def run(x, wq, alpha, wmin, bias, blocks):
-        tokens, ic = x.shape
-        oc = wq.shape[0]
-        al = np.stack([wmin, alpha], 2).astype(np.float32).ravel() if wmin is not None else alpha.astype(np.float32).ravel()
-        payload = struct.pack("<8i", tokens, ic, oc, int(wmin is not None), 0, 0, int(bias is not None), blocks)
-        payload += x.tobytes() + wq.tobytes() + al.tobytes() + (bias.astype(np.float32).tobytes() if bias is not None else b"")
-        with tempfile.TemporaryDirectory() as d:
-            req, out = os.path.join(d, "req.bin"), os.path.join(d, "out.bin")
-            open(req, "wb").write(payload)
-            r = subprocess.run([O.REFDUMP, "linear", req, out, "1"], env=env, capture_output=True, text=True, timeout=300)
-            assert r.returncode == 0, r.stderr[-1500:]
-            stats = [json.loads(l) for l in r.stdout.splitlines() if l.startswith("{\"plugin_")]
-            return np.fromfile(out, np.float32).reshape(tokens, oc), (stats[-1] if stats else None), r
-
-    for j, (x, wq, alpha, _, wmin, bias, gold) in enumerate(golden_cases()):
-        y, stats, r = run(x, wq, alpha, wmin, bias, alpha.shape[1])
+    for j, (x, wq, alpha, _, wmin, bias, gold) in enumerate(golden_cases(8)):
+        y, stats, r = run_on_plugin(x, wq, alpha, wmin, bias, alpha.shape[1])
         assert stats, r.stdout[-500:]
         assert stats["plugin_created"] >= 1 and stats["plugin_declined"] == 0, f"golden {j}: {stats} {r.stderr[-800:]}"
         assert np.abs(y - gold).max() <= 4e-6 * np.abs(gold).max(), f"golden {j}: {np.abs(y - gold).max() / np.abs(gold).max()}"
     rng = np.random.default_rng(16)
-    x, wq, alpha, wzero, bias = block_data(rng, 3, 256, 48, 16, False, True)
-    y, stats, r = run(x, wq, alpha, None, bias, 16)
+    x, wq, alpha, wzero, bias = linear_data(rng, 3, 256, 48, False, True, bs=16)
+    y, stats, r = run_on_plugin(x, wq, alpha, None, bias, 16)
     assert stats and stats["plugin_declined"] >= 1, f"a 16-channel-block layer was not declined: {stats} {r.stdout[-500:]}"
     # the backup backend runs it in its own float arithmetic, not the W8A8 one of the oracle: close, not equal
     ref = O.linear_w8_dynamic_blocks(x, wq, alpha, None, bias, 16)
     assert np.abs(y - ref).max() <= 1e-2 * np.abs(ref).max(), f"declined layer: {np.abs(y - ref).max() / np.abs(ref).max()}"
 
 
-if __name__ == "__main__":       # test_block_linear_launches_listed_kernels' child: the session backend of tests/conftest.py
-    import torch
-    from mnn_b200.backend import Runtime
-    torch.cuda.set_stream(torch.cuda.Stream())
-    golden_check(Runtime(0).onCreate(), profile=True)
-    print("golden cases profiled")
+if __name__ == "__main__":       # test_block_linear_launches_listed_kernels' child
+    profile_golden_cases(8)

@@ -7,18 +7,22 @@ tile (capi.cu: pick_tile), the stem's output-channel width (conv_int8_stem.cu) a
 (elementwise.cu: launch_dwconv_int8).  Every case below derives its shape from the SM count with the launcher's own rule,
 runs under torch.profiler and asserts that the intended instantiation ran, so a case that dispatch moves off its branch fails
 instead of silently losing coverage.  int8 outputs are poisoned before the run and must equal the oracle bit for bit with
-zero NHWC16 channel padding; linear outputs are NaN-poisoned and must equal O.linear_w8_dynamic bit for bit and, for 2..8
-tokens, the tensor-core path (variant 2)."""
+zero NHWC16 channel padding; linear outputs are NaN-poisoned and must equal O.linear_w8_dynamic bit for bit on auto and, where
+they apply, the forced tensor-core (2) and GEMV (4) variants.  The linear harness (check_linear) serves every weight form: the
+K-blocked and 4-bit modules run their cases through it."""
+import ctypes as C
 import os
 import re
 import shutil
 import subprocess
+import sys
 from collections import Counter
 
 import numpy as np
 import pytest
 
 from oracle import oracle as O
+from oracle import w4_oracle as W
 from tests.cases import random_modern_case
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -249,9 +253,9 @@ def gemv_key(tokens, oc, sms):
     return ("linear_w8_gemv_kernel", (gemv_template(tokens), gemv_rows(tokens, oc, sms), 4))
 
 
-def quant_key(ic, aligned=True):
-    """elementwise.cu launch_dynamic_quant"""
-    icp = (ic + 15) // 16 * 16
+def quant_key(ic, aligned=True, pad=16):
+    """elementwise.cu launch_dynamic_quant (icp: ic padded to 16, to 32 for 4-bit weights)"""
+    icp = (ic + pad - 1) // pad * pad
     if ic % 4 == 0 and aligned:
         for nv in (2, 4, 8):
             if icp <= 1024 * nv:
@@ -262,26 +266,57 @@ def quant_key(ic, aligned=True):
 WGMMA_KEY = ("gemm_i8_wgmma_kernel", (1, 0, 256))
 
 
-def linear_data(rng, tokens, ic, oc, asym, has_bias, zero_token=None):
+def linear_data(rng, tokens, ic, oc, asym, has_bias, zero_token=None, bits=8, bs=None):
+    """x, weights, alpha, wzero, bias of a linear layer: wq [oc][ic] int8, or for bits 4 the packed nibbles load() returns
+    (W.pack_w4); alpha / wzero [oc] for bs None, else [oc][ic / bs] (bs 0: one block)"""
     x = rng.uniform(-1, 1, (tokens, ic)).astype(np.float32)
     if zero_token is not None:
         x[zero_token, :] = 0                      # amax < 1e-7 branch
-    wq = rng.integers(-128, 128, (oc, ic), dtype=np.int8)
-    alpha = rng.uniform(0.001, 0.01, oc).astype(np.float32)
-    wzero = rng.uniform(-0.05, 0.05, oc).astype(np.float32) if asym else None
+    w = W.pack_w4(rng.integers(-8, 8, (oc, ic))) if bits == 4 else rng.integers(-128, 128, (oc, ic), dtype=np.int8)
+    shape = oc if bs is None else (oc, ic // bs if bs else 1)
+    alpha = rng.uniform(0.001, 0.01, shape).astype(np.float32)
+    wzero = None
+    if asym:
+        wzero = (rng.uniform(-0.01, 0.09, shape) if bits == 4 else rng.uniform(-0.05, 0.05, shape)).astype(np.float32)
     bias = rng.uniform(-1, 1, oc).astype(np.float32) if has_bias else None
-    return x, wq, alpha, wzero, bias
+    return x, w, alpha, wzero, bias
 
 
-def run_linear(backend, x, wq, alpha, wzero, bias, variants, relu6=False, misalign=False):
-    """the layer at each variant (0 auto, 2 tensor core, 4 GEMV) on one execution: {variant: (y, launched keys)}"""
+# A linear layer's weight form is its bits and the shape of alpha (wzero alike): 8-bit per channel takes alpha [oc], the K-blocked
+# and the 4-bit forms alpha [oc][blocks].
+def linear_oracle(x, w, alpha, wzero, bias, bits=8, relu=False, relu6=False):
+    if bits == 4:
+        return W.linear_w4_dynamic_blocks(x, w, alpha.shape[0], alpha, wzero, bias, alpha.shape[1], relu=relu, relu6=relu6)
+    if alpha.ndim == 2:
+        return O.linear_w8_dynamic_blocks(x, w, alpha, wzero, bias, alpha.shape[1], relu=relu, relu6=relu6)
+    return O.linear_w8_dynamic(x, w, alpha, wzero, bias, relu=relu, relu6=relu6)
+
+
+def create_linear(backend, ic, oc, w, alpha, wzero=None, bias=None, bits=8, blocks=None):
+    """(status, handle) of the C entry of the weight form: mnnb200_linear_w8_create, or the blocked entry of `bits` with
+    `blocks` (default alpha's)"""
+    from mnn_b200 import _capi
+    lib = _capi.lib()
+    h = C.c_void_p()
+    ptr = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
+    args = (ptr(w), ptr(alpha), ptr(wzero), ptr(bias), 0, 0, C.byref(h))
+    if bits == 8 and alpha.ndim == 1:
+        return lib.mnnb200_linear_w8_create(backend.runtime._h, ic, oc, *args), h
+    fn = lib.mnnb200_linear_w4_create_blocked if bits == 4 else lib.mnnb200_linear_w8_create_blocked
+    return fn(backend.runtime._h, ic, oc, alpha.shape[1] if blocks is None else blocks, *args), h
+
+
+def run_linear(backend, x, w, alpha, wzero, bias, variants, bits=8, relu=False, relu6=False, misalign=False, profile=False):
+    """the layer (Op(type="LinearW8")) at each variant (0 auto, 2 tensor core, 4 GEMV) on one execution, the output NaN-poisoned
+    before each run: {variant: (y, launched keys)}.  The keys come from torch.profiler (launched) when profile is set, else
+    they are None."""
     import torch
     from mnn_b200 import _capi
     from mnn_b200.backend import Op, Tensor
     tokens, ic = x.shape
-    oc = wq.shape[0]
-    op = Op(type="LinearW8", conv=dict(ic=ic, oc=oc, kernel=(1, 1)), weight=wq, wscale=alpha, wzero=wzero, bias=bias,
-            relu6=relu6)
+    oc = alpha.shape[0]
+    op = Op(type="LinearW8", conv=dict(ic=ic, oc=oc, kernel=(1, 1), relu=relu), weight=w, wscale=alpha, wzero=wzero, bias=bias,
+            relu6=relu6, bits=bits)
     if misalign:        # a view 4 bytes into a buffer: x is 4 bytes past 16-byte alignment
         buf = torch.zeros(tokens * ic + 8, dtype=torch.float32, device="cuda")
         xd = buf[1:1 + tokens * ic].view(tokens, ic)
@@ -297,26 +332,88 @@ def run_linear(backend, x, wq, alpha, wzero, bias, variants, relu6=False, misali
     res = {}
     for v in variants:
         _capi.check(_capi.lib().mnnb200_conv_int8_set_variant(ex._h, v))
-        keys = launched(backend, lambda: ok(ex.onExecute([xin], [yout])), lambda: yout.data.fill_(float("nan")))
+        keys = None
+        if profile:
+            keys = launched(backend, lambda: ok(ex.onExecute([xin], [yout])), lambda: yout.data.fill_(float("nan")))
+        else:
+            yout.data.fill_(float("nan"))
+            ok(ex.onExecute([xin], [yout]))
+            backend.onSync()
         y = yout.data.cpu().numpy()
         assert not np.isnan(y).any(), f"variant {v}: outputs left unwritten"
         res[v] = (y, keys)
     return res
 
 
-def check_linear(backend, x, wq, alpha, wzero, bias, gemv_expected, relu6=False, misalign=False):
-    """auto (GEMV for <= 8 tokens) against the oracle; for 2..8 tokens also the tensor-core variant, bit for bit"""
+def variants_for(tokens):
+    return (0,) if tokens == 1 else (0, 2, 4) if tokens <= 8 else (0, 2)
+
+
+def check_linear(backend, x, w, alpha, wzero, bias, bits=8, relu=False, relu6=False, misalign=False, profile=False,
+                 gemv_expected=None):
+    """auto and the forced GEMM / GEMV where they apply against the oracle of the weight form, bit for bit; returns the
+    oracle's output.  profile: every launched kernel is one KERNEL_TESTS lists, the GEMV alone (gemv_expected among them) for
+    <= 8 tokens on auto and variant 4, the quantisation kernel and the single-CTA GEMM otherwise (auto on the CTA pair, 8-bit
+    per channel from 256 tokens, is not profiled here)"""
     tokens, ic = x.shape
-    ref = O.linear_w8_dynamic(x, wq, alpha, wzero, bias, relu6=relu6)
-    res = run_linear(backend, x, wq, alpha, wzero, bias, (0,) if tokens == 1 else (0, 2), relu6=relu6, misalign=misalign)
-    y, keys = res[0]
-    expect(keys, gemv_expected)
-    assert np.array_equal(y, ref), f"GEMV vs oracle: {np.count_nonzero(y != ref)} outputs differ, max {np.abs(y - ref).max()}"
-    if tokens > 1:
-        y2, keys2 = res[2]
-        expect(keys2, quant_key(ic, not misalign), WGMMA_KEY)
-        assert np.array_equal(y, y2), f"GEMV vs tensor core: {np.count_nonzero(y != y2)} outputs differ"
+    ref = linear_oracle(x, w, alpha, wzero, bias, bits, relu=relu, relu6=relu6)
+    res = run_linear(backend, x, w, alpha, wzero, bias, variants_for(tokens), bits, relu, relu6, misalign, profile)
+    for v, (y, keys) in res.items():
+        assert np.array_equal(y, ref), f"variant {v}: {np.count_nonzero(y != ref)} outputs differ, max {np.abs(y - ref).max()}"
+        if profile:
+            assert set(keys) <= set(KERNEL_TESTS), f"variant {v} launched kernels outside KERNEL_TESTS: {sorted(keys)}"
+            if v == 4 or (v == 0 and tokens <= 8):
+                assert {k[0] for k in keys} == {"linear_w8_gemv_kernel"}, sorted(keys)
+                if gemv_expected:
+                    expect(keys, gemv_expected)
+            else:
+                expect(keys, quant_key(ic, not misalign, 32 if bits == 4 else 16), WGMMA_KEY)
     return ref
+
+
+# the recorded reference cases of each weight width: file under tests/golden, key prefix, the wire's clamp minimum (load()
+# hands a backend wzero = wire min - clamp minimum * alpha)
+GOLDEN = {8: ("block_linear_golden.npz", "b", -128), 4: ("w4_linear_golden.npz", "c", -8)}
+GOLDEN_TOL = 4e-6       # of max|y|: the oracle against the recorded reference (tests/test_oracle.py, tests/test_w4_linear_cpu.py)
+
+
+def golden_cases(bits):
+    """(x, weights, alpha, wzero, wire min or None, bias or None, recorded y) of every recorded case"""
+    name, p, clamp_min = GOLDEN[bits]
+    g = np.load(os.path.join(ROOT, "tests", "golden", name))
+    out = []
+    for j in range(int(g["n"])):
+        k = f"{p}{j}_"
+        alpha, wmin, bias = g[k + "alpha"], g[k + "wmin"], g[k + "bias"]
+        wz = (wmin - np.float32(clamp_min) * alpha).astype(np.float32) if wmin.size else None
+        w = g[k + ("wq" if bits == 8 else "w")]
+        out.append((g[k + "x"], w, alpha, wz, wmin if wmin.size else None, bias if bias.size else None, g[k + "y"]))
+    return out
+
+
+def golden_check(backend, bits, profile=False):
+    for j, (x, w, alpha, wz, _, bias, gold) in enumerate(golden_cases(bits)):
+        y = check_linear(backend, x, w, alpha, wz, bias, bits, profile=profile)
+        err = np.abs(y - gold).max() / np.abs(gold).max()
+        assert err <= GOLDEN_TOL, f"golden {j}: {err}"
+
+
+def golden_check_profiled_in_child(module):
+    """golden_check with profile set, in `python -m module` (its __main__: profile_golden_cases): a profiler started in this
+    process early in the GPU suite leaves CUPTI subscribed (this module keeps it so), and the windows this module opens later
+    in the same process then recorded no kernel launches"""
+    cmd = [sys.executable] + (["-s"] if sys.flags.no_user_site else []) + ["-m", module]
+    r = subprocess.run(cmd, cwd=ROOT, capture_output=True, text=True, timeout=600)
+    assert r.returncode == 0 and "golden cases profiled" in r.stdout, r.stdout[-1500:] + r.stderr[-3000:]
+
+
+def profile_golden_cases(bits):
+    """the child's side of golden_check_profiled_in_child, on a backend made as tests/conftest.py makes the session's"""
+    import torch
+    from mnn_b200.backend import Runtime
+    torch.cuda.set_stream(torch.cuda.Stream())
+    golden_check(Runtime(0).onCreate(), bits, profile=True)
+    print("golden cases profiled")
 
 
 def gemv_cases():
@@ -352,7 +449,7 @@ def test_gemv_dispatch(backend, tokens, r, passes):
     rng = np.random.default_rng(tokens * 1009 + r * 31 + passes)
     data = linear_data(rng, tokens, ic, oc, asym=tokens % 2 == 1 or passes > 1, has_bias=passes > 1 or tokens in (2, 5),
                        zero_token=1 if tokens > 1 else None)
-    check_linear(backend, *data, gemv_expected=("linear_w8_gemv_kernel", (gemv_template(tokens), r, 4)))
+    check_linear(backend, *data, profile=True, gemv_expected=("linear_w8_gemv_kernel", (gemv_template(tokens), r, 4)))
 
 
 @pytest.mark.gpu
@@ -362,7 +459,7 @@ def test_gemv_lm_head(backend, tokens):
     sms = sm_count()
     rng = np.random.default_rng(151936 + tokens)
     data = linear_data(rng, tokens, 2048, 151936, asym=False, has_bias=False)
-    check_linear(backend, *data, gemv_expected=gemv_key(tokens, 151936, sms))
+    check_linear(backend, *data, profile=True, gemv_expected=gemv_key(tokens, 151936, sms))
 
 
 GEMV_EDGES = {   # name: tokens, ic, oc, asym, bias, relu6, misaligned x
@@ -384,7 +481,8 @@ def test_gemv_edges(backend, name):
     x, wq, alpha, wzero, bias = linear_data(rng, tokens, ic, oc, asym, has_bias)
     if relu6:
         alpha = alpha * 3                              # outputs well beyond 6 and below 0: both clamps bite
-    ref = check_linear(backend, x, wq, alpha, wzero, bias, gemv_key(tokens, oc, sm_count()), relu6=relu6, misalign=mis)
+    ref = check_linear(backend, x, wq, alpha, wzero, bias, relu6=relu6, misalign=mis, profile=True,
+                       gemv_expected=gemv_key(tokens, oc, sm_count()))
     if relu6:
         assert (ref == 6).any() and (ref == 0).any()
 
@@ -412,11 +510,7 @@ def test_prefill_dynamic_quant(backend, name):
     x, wq, alpha, wzero, bias = linear_data(rng, tokens, ic, oc, asym, has_bias, zero_token=zero)
     if relu6:
         alpha = alpha * 3
-    ref = O.linear_w8_dynamic(x, wq, alpha, wzero, bias, relu6=relu6)
-    res = run_linear(backend, x, wq, alpha, wzero, bias, (0, 2), relu6=relu6, misalign=mis)
-    for v, (y, keys) in res.items():
-        expect(keys, quant_key(ic, not mis), WGMMA_KEY)
-        assert np.array_equal(y, ref), f"variant {v}: {np.count_nonzero(y != ref)} outputs differ, max {np.abs(y - ref).max()}"
+    ref = check_linear(backend, x, wq, alpha, wzero, bias, relu6=relu6, misalign=mis, profile=True)
     if relu6:
         assert (ref == 6).any() and (ref == 0).any()
 

@@ -13,8 +13,8 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from oracle import oracle as O
 from oracle import w4_oracle as W
+from tests.test_gpu_dispatch import create_linear, linear_oracle
 
 pytestmark = pytest.mark.gpu
 
@@ -58,24 +58,19 @@ class Layer:
         assert ic % self.blocks == 0
         rng = np.random.default_rng(seed)
         w4 = form.startswith("w4")
+        self.bits = 4 if w4 else 8
         self.alpha = rng.uniform(0.001, 0.01, (oc, self.blocks)).astype(np.float32)
         self.wzero = (rng.uniform(-0.01, 0.09, (oc, self.blocks)) if w4 else rng.uniform(-0.05, 0.05, (oc, self.blocks))).astype(np.float32)
         self.bias = rng.uniform(-1, 1, oc).astype(np.float32)
         self.w = W.pack_w4(rng.integers(-8, 8, (oc, ic))) if w4 else rng.integers(-128, 128, (oc, ic), dtype=np.int8)
+        if form == "w8":        # the 8-bit per-channel form takes alpha / wzero [oc]
+            self.alpha, self.wzero = self.alpha[:, 0].copy(), self.wzero[:, 0].copy()
         self.h = self.create()
         self.tokens = 0
 
     def create(self):
         """a new execution of this layer"""
-        h = C.c_void_p()
-        p = lambda a: a.ctypes.data_as(C.c_void_p)
-        rt = self.backend.runtime._h
-        if self.form == "w8":
-            st = lib().mnnb200_linear_w8_create(rt, self.ic, self.oc, p(self.w), p(self.alpha[:, 0].copy()),
-                                                p(self.wzero[:, 0].copy()), p(self.bias), 0, 0, C.byref(h))
-        else:
-            fn = lib().mnnb200_linear_w4_create_blocked if self.form.startswith("w4") else lib().mnnb200_linear_w8_create_blocked
-            st = fn(rt, self.ic, self.oc, self.blocks, p(self.w), p(self.alpha), p(self.wzero), p(self.bias), 0, 0, C.byref(h))
+        st, h = create_linear(self.backend, self.ic, self.oc, self.w, self.alpha, self.wzero, self.bias, self.bits)
         assert st == 0, lib().mnnb200_last_error()
         return h
 
@@ -115,11 +110,7 @@ class Layer:
         return y.view(self.tokens, self.oc)
 
     def oracle(self, x):
-        if self.form.startswith("w4"):
-            return W.linear_w4_dynamic_blocks(x, self.w, self.oc, self.alpha, self.wzero, self.bias, self.blocks)
-        if self.form == "w8":
-            return O.linear_w8_dynamic(x, self.w, self.alpha[:, 0].copy(), self.wzero[:, 0].copy(), self.bias)
-        return O.linear_w8_dynamic_blocks(x, self.w, self.alpha, self.wzero, self.bias, self.blocks)
+        return linear_oracle(x, self.w, self.alpha, self.wzero, self.bias, self.bits)
 
     def check(self, x, y, what):
         """the sampled rows of y equal the oracle's bit for bit"""
