@@ -275,6 +275,8 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin, const std::vector<floa
     plan.stem = conv_int8_stem_supported(p, d.ic);
     plan.group = false;
     if (!plan.gemm && (p.sw > 2 || p.KH > 32 || p.KW > 32 || (p.sw == 2 && p.IW < 2))) return MNNB200_OK;
+    // the kernel clamps its outputs after packing them to s16 with saturation, which changes no result for bounds in that range
+    if (p.minv < -32768.f || p.minv > 32767.f || p.maxv < -32768.f || p.maxv > 32767.f) return MNNB200_OK;
     GroupLayerParams& q = plan.q;
     GroupConvGeom& g = plan.g;
     memset(&q, 0, sizeof(q));
@@ -285,7 +287,7 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin, const std::vector<floa
     auto channel = [&](int nc, int c) { return nc * q.bn + group_column_channel(c, q.bn); };
     const int ncol = q.n_chunks * q.bn;
     q.M = p.M; q.N = e->OCp; q.OC = d.oc;
-    q.ldy = e->OCp; q.scale_x = p.scale_x; q.minv = p.minv; q.maxv = p.maxv;
+    q.ldy = e->OCp; q.scale_x = p.scale_x; q.minv = (int)p.minv; q.maxv = (int)p.maxv;
     q.mode = plan.gemm ? 0 : 1;
     const int taps = p.KH * p.KW;
     if (plan.gemm) {
@@ -322,7 +324,7 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin, const std::vector<floa
         cuuint32_t box[2] = {(cuuint32_t)q.cb, (cuuint32_t)q.bn};
         if ((st = make_tmap_u8(&plan.tmap_b, e->d_wg, 2, dims, strides, box))) return st;
     }
-    {   // epilogue table [n_chunks][3][bn]: wscale, biasFloat, preset = 128 sum w (+ 0x4B400000 for requant_fast_small)
+    {   // epilogue table [n_chunks][3][bn]: wscale, biasFloat, preset = 128 sum w (+ 0x4B400000 for requant_round_small)
         const int32_t magic = q.K <= 128 ? 0x4B400000 : 0;
         std::vector<float> ep((size_t)3 * ncol, 0.f);
         for (int nc = 0; nc < q.n_chunks; ++nc)

@@ -73,27 +73,32 @@ constexpr int kCgThreads = kConsumerThreads + 128;
 constexpr int kProducerRegs = 88, kConsumerRegs = 208;
 static_assert(kProducerRegs + 2 * kConsumerRegs <= 512, "conv group kernel: register split does not fit");
 
-// requant_cpu_exact (common.cuh) with the +-0.5 select done as copysign(0.5, f): one LOP3, identical result
-__device__ __forceinline__ int requant_fast(int acc_u, float wscale, float scale_x, float bias_float, float minv, float maxv) {
+// requant_cpu_exact (common.cuh) WITHOUT its clamp, which the epilogue applies to the rounded integers (see consume_run's
+// column run for why that is exact).  The +-0.5 is copysign(0.5, f) = (f & sign) | 0.5 in one LOP3 with 0.5 in a register:
+// written as an and and an or of two immediates, ptxas emits two LOP3s.
+__device__ __forceinline__ int round_half_away(float f) {
+    uint32_t h;
+    asm("lop3.b32 %0, %1, 0x80000000, 0x3f000000, 0xEA;" : "=r"(h) : "r"(__float_as_uint(f)));   // 0xEA: (a & b) | c
+    return __float2int_rz(__fadd_rn(f, __uint_as_float(h)));
+}
+__device__ __forceinline__ int requant_round(int acc_u, float wscale, float scale_x, float bias_float) {
     float f = __fmul_rn(__int2float_rn(acc_u), wscale);
     f = __fmul_rn(f, scale_x);
-    f = __fadd_rn(f, bias_float);
-    f = fminf(f, maxv);
-    f = fmaxf(f, minv);
-    float h = __int_as_float((__float_as_int(f) & 0x80000000) | 0x3f000000);
-    return __float2int_rz(__fadd_rn(f, h));
+    return round_half_away(__fadd_rn(f, bias_float));
 }
 // the same sequence for accumulators with |acc_u| < 2^22: float(acc_u) = as_float(0x4B400000 + acc_u) - 1.5 * 2^23 is exact (the
 // integer lands in the mantissa of a float in [2^23, 2^24)): one IADD + one FADD instead of an I2F on the conversion unit
 // (the conv-group kernel's accumulators start at 0x4B400000 + 128 sum w, so acc_m here is already 0x4B400000 + acc_u)
-__device__ __forceinline__ int requant_fast_small(int acc_m, float wscale, float scale_x, float bias_float, float minv, float maxv) {
+__device__ __forceinline__ int requant_round_small(int acc_m, float wscale, float scale_x, float bias_float) {
     float f = __fmul_rn(__fsub_rn(__int_as_float(acc_m), 12582912.0f), wscale);
     f = __fmul_rn(f, scale_x);
-    f = __fadd_rn(f, bias_float);
-    f = fminf(f, maxv);
-    f = fmaxf(f, minv);
-    float h = __int_as_float((__float_as_int(f) & 0x80000000) | 0x3f000000);
-    return __float2int_rz(__fadd_rn(f, h));
+    return round_half_away(__fadd_rn(f, bias_float));
+}
+// two int32 -> one s16 pair, each saturated to [-32768, 32767] (one I2IP): lo in bits 0-15, hi in bits 16-31
+__device__ __forceinline__ uint32_t pack_sat_s16x2(int lo, int hi) {
+    uint32_t d;
+    asm("cvt.pack.sat.s16.s32 %0, %1, %2;" : "=r"(d) : "r"(hi), "r"(lo));
+    return d;
 }
 
 // work item = `cnt` consecutive M tiles of one (layer, n chunk), encoded as kernels.h describes.
@@ -141,6 +146,9 @@ __device__ __forceinline__ bool stage_landed(uint32_t bar, uint32_t parity, int 
 // layers have few tiles per CTA, so there is little to overlap.
 constexpr int kOverlapMaxBN = 64;
 
+// widths up to this one keep a run's epilogue constants in registers (consume_run)
+constexpr int kConstRegsMaxBN = 64;
+
 // One RUN on one consumer warpgroup: the consecutive items my[i], my[i + 1], ... of the CTA's schedule row with the same
 // (layer, n chunk), each `cnt` M tiles of rows [64 wg, 64 wg + 64) x BN columns; on return i is the run's last item.  BN is a
 // compile-time constant so the accumulator arrays, the wgmma_span chain and the epilogue's column loop are fixed: a run-time
@@ -168,7 +176,42 @@ __device__ __forceinline__ void consume_run(const GroupLayerParams& lp, const Gr
     // the next tile's first K block while acc's epilogue runs.  Only wgmmas write it: a register write to an accumulator
     // while a wgmma pipeline is open makes ptxas serialise every wgmma of the kernel
     int nxt[kTwoSets ? BN / 2 : 1];
-    const float scale_x = lp.scale_x, minv = lp.minv, maxv = lp.maxv;
+    const float scale_x = lp.scale_x;
+    // The clamp runs on the rounded integers.  The reference's rounding round(f) = trunc(fadd_rn(f, copysign(0.5, f))) is
+    // monotone non-decreasing and maps every integer bound to itself (|bound| < 2^23), and a monotone function commutes with
+    // min and max, so max(min(round(f), maxv), minv) = round(max(min(f, maxv), minv)) bit for bit, also when minv > maxv.  The
+    // saturations on the way are monotone and the identity on the bounds' range, so they change nothing: F2I.TRUNC at the
+    // int32 range, the pack at the s16 range (conv_plan gives the kernel no bounds outside it).  (Only a NaN f, which needs a
+    // non-finite table constant, would differ: fminf sends it to maxv, F2I to 0.)  Per 4 outputs that is two saturating packs
+    // to s16 pairs, one s16x2 min and one max per pair, and one PRMT to the low bytes, instead of 8 FMNMX and 3 PRMTs.
+    const int minv = lp.minv, maxv = lp.maxv;
+    const uint32_t min2 = (uint32_t)(minv & 0xffff) * 0x10001u, max2 = (uint32_t)(maxv & 0xffff) * 0x10001u;
+    // the chunk's pad channels (>= OC) are stored and must stay zero.  Their table constants are zero, so they requantise to
+    // clamp(0): only a clamp without 0 needs their bytes cleared, and only in the chunk that holds them (all ones elsewhere).
+    // The byte masks of the thread's 32-column groups are set here, once per run: one AND per 4 outputs in the column run, no
+    // instruction to build them per tile and no second instantiation of the column run.
+    const bool pad = lp.OC - n0 < ncols && (minv > 0 || maxv < 0);
+    constexpr int kGroups = (BN + 31) / 32;
+    uint32_t mlo[kGroups], mhi[kGroups];
+#pragma unroll
+    for (int G = 0; G < kGroups; ++G) {
+        const int nv = pad ? lp.OC - n0 - (32 * G + 2 * (BN - 32 * G >= 32 ? 4 : 2) * q4) : 8;   // the group's valid channels
+        mlo[G] = nv >= 4 ? 0xffffffffu : (nv <= 0 ? 0u : (1u << (8 * nv)) - 1u);
+        mhi[G] = nv >= 8 ? 0xffffffffu : (nv <= 4 ? 0u : (1u << (8 * (nv - 4))) - 1u);
+    }
+    // the thread's wscale and biasFloat pairs, the same for every tile of the run: pair j = 4 G + s of the column run below.
+    // Up to kConstRegsMaxBN they are read once, here; wider tiles read them from shared memory per tile, as their 4 BN / 8
+    // registers next to BN / 2 accumulators do not fit.
+    constexpr bool kRegConsts = BN <= kConstRegsMaxBN;
+    float2 ws[kRegConsts ? BN / 8 : 1], bs[kRegConsts ? BN / 8 : 1];
+    auto load_consts = [&](int j, float2& w, float2& b) {
+        w = *reinterpret_cast<const float2*>(wscale + 8 * j + 2 * q4);
+        b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4);
+    };
+    if constexpr (kRegConsts) {
+#pragma unroll
+        for (int j = 0; j < BN / 8; ++j) load_consts(j, ws[j], bs[j]);
+    }
     // |sum (x + 128) w| <= 128 * 255 * 128 < 2^22.  Broadcast like cb: the epilogue branches on it and on mode while the next
     // tile's wgmmas run, and a branch ptxas cannot prove uniform there makes it serialise the wgmmas
     const bool small_acc = __shfl_sync(0xffffffffu, lp.K, 0) <= 128;
@@ -176,7 +219,7 @@ __device__ __forceinline__ void consume_run(const GroupLayerParams& lp, const Gr
     const int OC = lp.OC, M = lp.M, ldy = lp.ldy, mode = __shfl_sync(0xffffffffu, lp.mode, 0);
     int8_t* const y = lp.y;
 
-    // the accumulators start at their column's preset (128 sum w, + 0x4B400000 for requant_fast_small), so every wgmma
+    // the accumulators start at their column's preset (128 sum w, + 0x4B400000 for requant_round_small), so every wgmma
     // accumulates and the epilogue adds no per-column integer
     auto init = [&](int (&a)[BN / 2]) {
 #pragma unroll
@@ -330,24 +373,25 @@ __device__ __forceinline__ void consume_run(const GroupLayerParams& lp, const Gr
         // whole: valid columns come in multiples of 16).  With no control flow inside, ptxas overlaps the requant chains.  The
         // requant path and the border correction are chosen once per run.
         auto columns = [&](auto small, auto with_corr) {
+            // 4 rounded outputs -> their 4 clamped bytes, q[0] in byte 0 (see clamp above)
+            auto clamp4 = [&](const int* q) -> uint32_t {
+                const uint32_t p0 = __vmaxs2(__vmins2(pack_sat_s16x2(q[0], q[1]), max2), min2);
+                const uint32_t p1 = __vmaxs2(__vmins2(pack_sat_s16x2(q[2], q[3]), max2), min2);
+                return __byte_perm(p0, p1, 0x6420);
+            };
 #pragma unroll
             for (int G = 0; G < (BN + 31) / 32; ++G) {
                 constexpr int kFull = 4;
                 const int S = BN - 32 * G >= 32 ? kFull : 2;      // column pairs of the thread per row in this group
                 const int ch = 32 * G + 2 * S * q4;              // its first channel
-                // NHWC16 pad channels (>= OC) stay zero: the clamp would give them minv, which is the output zero point with ReLU
-                const int nv = OC - n0 - ch;
-                const uint32_t mlo = nv >= 4 ? 0xffffffffu : (nv <= 0 ? 0u : (1u << (8 * nv)) - 1u);
-                const uint32_t mhi = nv >= 8 ? 0xffffffffu : (nv <= 4 ? 0u : (1u << (8 * (nv - 4))) - 1u);
-                float2 ws[kFull], bs[kFull];
+                float2 wg[kFull], bg[kFull];         // the group's constants serve both rows
 #pragma unroll
                 for (int s = 0; s < S; ++s) {
-                    const int c = 8 * (4 * G + s) + 2 * q4;
-                    ws[s] = *reinterpret_cast<const float2*>(wscale + c);
-                    bs[s] = *reinterpret_cast<const float2*>(bias + c);
+                    if constexpr (kRegConsts) { wg[s] = ws[4 * G + s]; bg[s] = bs[4 * G + s]; }
+                    else load_consts(4 * G + s, wg[s], bg[s]);
                 }
 #pragma unroll
-                for (int h = 0; h < 2; ++h) {        // rows inside: a group's constants serve both rows, then die
+                for (int h = 0; h < 2; ++h) {
                     int q[2 * kFull];
 #pragma unroll
                     for (int s = 0; s < S; ++s) {
@@ -359,16 +403,16 @@ __device__ __forceinline__ void consume_run(const GroupLayerParams& lp, const Gr
                             a1 += k.y;
                         }
                         if constexpr (decltype(small)::value) {   // |acc_u| < 2^22: int -> float on the FP32 pipe (exact)
-                            q[2 * s] = requant_fast_small(a0, ws[s].x, scale_x, bs[s].x, minv, maxv);
-                            q[2 * s + 1] = requant_fast_small(a1, ws[s].y, scale_x, bs[s].y, minv, maxv);
+                            q[2 * s] = requant_round_small(a0, wg[s].x, scale_x, bg[s].x);
+                            q[2 * s + 1] = requant_round_small(a1, wg[s].y, scale_x, bg[s].y);
                         } else {
-                            q[2 * s] = requant_fast(a0, ws[s].x, scale_x, bs[s].x, minv, maxv);
-                            q[2 * s + 1] = requant_fast(a1, ws[s].y, scale_x, bs[s].y, minv, maxv);
+                            q[2 * s] = requant_round(a0, wg[s].x, scale_x, bg[s].x);
+                            q[2 * s + 1] = requant_round(a1, wg[s].y, scale_x, bg[s].y);
                         }
                     }
-                    const uint32_t lo = __byte_perm(__byte_perm(q[0], q[1], 0x0040), __byte_perm(q[2], q[3], 0x0040), 0x5410) & mlo;
+                    const uint32_t lo = clamp4(q) & mlo[G];
                     if (S == kFull) {
-                        const uint32_t hi = __byte_perm(__byte_perm(q[4], q[5], 0x0040), __byte_perm(q[6], q[7], 0x0040), 0x5410) & mhi;
+                        const uint32_t hi = clamp4(q + 4) & mhi[G];
                         st_global_v2_if(yrow[h] + ch, lo, hi, ch, lim[h]);
                     } else {
                         st_global_b32_if(yrow[h] + ch, lo, ch, lim[h]);

@@ -109,7 +109,8 @@ struct GroupLayerParams {            // copied to shared memory by every CTA
     int M, N, K, bn;                 // mode 0: M rows, K = Cp.  mode 1: M = N*OH*OW, K = taps*Cp
     int n_chunks, m_tiles, num_kb, OC;
     int ldy;
-    float scale_x, minv, maxv;
+    float scale_x;
+    int minv, maxv;                  // the clamp, in the s16 range (conv_plan)
     int mode, cb, TWp, R;            // cb: bytes of K per TMA chunk (128 / 64 / 16, mode 0 also 32); mode 1: R boxes of BH rows x TWp pixels per M tile
 };
 struct GroupConvGeom {               // mode 1 only; stays in global memory (read once per tile)
