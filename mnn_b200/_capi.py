@@ -124,6 +124,20 @@ SIGNATURES = {
 }
 
 
+# libmnn_b200_deconv.so (include/mnn_b200_deconv.h): the float Deconvolution executions, on the runtime and execution handles above
+DECONV_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_deconv.so")
+DECONV_SIGNATURES = {
+    "mnnb200_deconv_f32_create": (C.c_int, [P, C.POINTER(ConvDesc), P, P, C.c_int, C.POINTER(P)]),
+    "mnnb200_deconv_f32_set_pad": (C.c_int, [P, C.c_int, C.c_int]),
+    "mnnb200_deconv_f32_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "mnnb200_deconv_f32_execute": (C.c_int, [P, P, P]),
+    "mnnb200_deconv_f32_plan": (C.c_int, [P, C.POINTER(C.c_int), C.c_int]),
+    "mnnb200_dwdeconv_f32_create": (C.c_int, [P, C.POINTER(ConvDesc), P, P, C.c_int, C.POINTER(P)]),
+    "mnnb200_dwdeconv_f32_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
+    "mnnb200_dwdeconv_f32_execute": (C.c_int, [P, P, P]),
+}
+_deconv_lib = None
+
 # libmnn_b200_llm.so (include/mnn_b200_llm.h): MNN-LLM's LayerNorm / RoPE executions, on the runtime and execution handles above
 LLM_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_llm.so")
 LLM_SIGNATURES = {
@@ -153,6 +167,21 @@ def llm_lib():
         _llm_lib = L
     return _llm_lib
 
+
+def deconv_lib():
+    """libmnn_b200_deconv.so with every DECONV_SIGNATURES symbol resolved (after libmnn_b200.so, whose handles it shares)"""
+    global _deconv_lib
+    if _deconv_lib is None:
+        lib()
+        if not os.path.exists(DECONV_LIB_PATH):
+            raise MnnB200Error(f"{DECONV_LIB_PATH} is missing: run `python -m mnn_b200.build` (there is no CPU fallback)")
+        L = C.CDLL(DECONV_LIB_PATH)
+        for name, (res, args) in DECONV_SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype = res
+            fn.argtypes = args
+        _deconv_lib = L
+    return _deconv_lib
 
 def lib():
     global _lib

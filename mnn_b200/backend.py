@@ -460,6 +460,35 @@ class ConvF32Execution(Execution):
         return f(self._h, inputs[0].ptr(), outputs[0].ptr())
 
 
+class DeconvF32Execution(Execution):
+    """Float Deconvolution (group 1, split-TF32 wgmma over the stride phases) or DeconvolutionDepthwise on NCHW fp32 tensors: the
+    CPU backend's CPUDeconvolution / CPUDeconvolutionDepthwise.  op.weight fp32 [ic][oc][kh][kw] ([c][1][kh][kw] depthwise),
+    op.bias fp32 [oc] or None; op.conv['pad'] the begin pads, op.conv['out_hw'] an explicit output size (else the natural one)."""
+
+    def __init__(self, backend, op: Op, depthwise=False):
+        super().__init__(backend)
+        self.op, self.depthwise = op, depthwise
+        d = _desc(op.conv)
+        w = np.ascontiguousarray(op.weight, np.float32)
+        b = None if op.bias is None else np.ascontiguousarray(op.bias, np.float32)
+        f = _capi.deconv_lib().mnnb200_dwdeconv_f32_create if depthwise else _capi.deconv_lib().mnnb200_deconv_f32_create
+        check(f(backend.runtime._h, C.byref(d), _np_ptr(w), _np_ptr(b), int(op.relu6), C.byref(self._h)),
+              "dwdeconv_f32_create" if depthwise else "deconv_f32_create")
+
+    def onResize(self, inputs, outputs):
+        n, _, ih, iw = inputs[0].shape
+        oh, ow = (C.c_int(v) for v in self.op.conv.get("out_hw", (0, 0)))
+        f = _capi.deconv_lib().mnnb200_dwdeconv_f32_resize if self.depthwise else _capi.deconv_lib().mnnb200_deconv_f32_resize
+        st = f(self._h, n, ih, iw, C.byref(oh), C.byref(ow))
+        if st == 0:
+            outputs[0].shape = (n, self.op.conv["oc"], oh.value, ow.value)
+        return st
+
+    def onExecute(self, inputs, outputs):
+        f = _capi.deconv_lib().mnnb200_dwdeconv_f32_execute if self.depthwise else _capi.deconv_lib().mnnb200_deconv_f32_execute
+        return f(self._h, inputs[0].ptr(), outputs[0].ptr())
+
+
 class Backend:
     """CUDABackend's role: creator map, buffer acquisition, host<->device copies with layout + quant casts."""
 
@@ -548,3 +577,13 @@ def _create_conv_f32(b, i, o, op):
 
 Backend.addCreator("Convolution", _create_conv_f32)
 Backend.addCreator("ConvolutionDepthwise", lambda b, i, o, op: ConvF32Execution(b, op, depthwise=True))
+
+
+def _create_deconv_f32(b, i, o, op):
+    if op.conv.get("group", 1) != 1:      # CPUDeconvolution ignores group; a grouped deconvolution is not taken
+        return None
+    return DeconvF32Execution(b, op)
+
+
+Backend.addCreator("DeconvF32", _create_deconv_f32)
+Backend.addCreator("DwDeconvF32", lambda b, i, o, op: DeconvF32Execution(b, op, depthwise=True))

@@ -1,5 +1,6 @@
-"""Builds libmnn_b200.so (CUDA kernels + C ABI) and libmnn_b200_llm.so (the MNN-LLM LayerNorm / RoPE ops, include/mnn_b200_llm.h,
-linked against libmnn_b200.so) in-tree for sm_90a (H100) with nvcc.  No torch involvement."""
+"""Builds libmnn_b200.so (CUDA kernels + C ABI), libmnn_b200_llm.so (the MNN-LLM LayerNorm / RoPE ops, include/mnn_b200_llm.h)
+and libmnn_b200_deconv.so (the float Deconvolution, include/mnn_b200_deconv.h), the last two linked against libmnn_b200.so,
+in-tree for sm_90a (H100) with nvcc.  No torch involvement."""
 import os
 import subprocess
 import sys
@@ -8,8 +9,10 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 CSRC = os.path.join(HERE, "csrc")
 LIB = os.path.join(HERE, "libmnn_b200.so")
 LLM_LIB = os.path.join(HERE, "libmnn_b200_llm.so")
+DECONV_LIB = os.path.join(HERE, "libmnn_b200_deconv.so")
 SOURCES = ["capi.cu", "conv_int8_mma.cu", "elementwise.cu", "gemm_i8_wgmma.cu", "winograd_int8.cu", "gemm_f16_wgmma.cu", "conv_int8_stem.cu", "conv_group_wgmma.cu", "linear_w8_gemv.cu", "conv_f32_wgmma.cu"]
 LLM_SOURCES = ["llm_ops.cu", "llm_capi.cu"]
+DECONV_SOURCES = ["deconv_f32_wgmma.cu", "deconv_capi.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-ffp-contract=off,-fvisibility=hidden", "--expt-relaxed-constexpr"]
@@ -37,19 +40,24 @@ def _compile(srcs, nvcc, verbose):
 
 
 def build(force=False, verbose=False):
-    """both libraries; returns the path of libmnn_b200.so"""
+    """the three libraries; returns the path of libmnn_b200.so"""
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
     llm_srcs = [os.path.join(CSRC, s) for s in LLM_SOURCES]
     inc = os.path.join(HERE, "..", "include")
     deps = srcs + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))] + \
            [os.path.join(inc, "mnn_b200.h")]
     llm_deps = deps + llm_srcs + [os.path.join(inc, "mnn_b200_llm.h")]
+    deconv_srcs = [os.path.join(CSRC, s) for s in DECONV_SOURCES]
+    deconv_deps = deps + deconv_srcs + [os.path.join(inc, "mnn_b200_deconv.h")]
     fresh = lambda lib, ds: os.path.exists(lib) and all(os.path.getmtime(lib) > os.path.getmtime(d) for d in ds)
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     if force or not fresh(LIB, deps):
         subprocess.check_call([nvcc, "-shared", "-o", LIB] + _compile(srcs, nvcc, verbose) + ARCH + ["-lcudart"])
     if force or not fresh(LLM_LIB, llm_deps + [LIB]):
         subprocess.check_call([nvcc, "-shared", "-o", LLM_LIB] + _compile(llm_srcs, nvcc, verbose) + ARCH +
+                              ["-L" + HERE, "-lmnn_b200", "-Xlinker", "-rpath,$ORIGIN", "-lcudart"])
+    if force or not fresh(DECONV_LIB, deconv_deps + [LIB]):
+        subprocess.check_call([nvcc, "-shared", "-o", DECONV_LIB] + _compile(deconv_srcs, nvcc, verbose) + ARCH +
                               ["-L" + HERE, "-lmnn_b200", "-Xlinker", "-rpath,$ORIGIN", "-lcudart"])
     return LIB
 

@@ -41,17 +41,6 @@ struct mnnb200_graph {
     cudaGraphExec_t exec = nullptr;
 };
 
-// The five convolutions: the descriptor that set_pad edits.
-struct ConvExec : mnnb200_exec {
-    mnnb200_conv_desc d;
-};
-// a plan query: the first `count` (at most N) of the plan's fields go to `fields`
-template <size_t N>
-static mnnb200_status copy_fields(const int (&v)[N], int* fields, int count) {
-    for (int i = 0; i < count && i < (int)N; ++i) fields[i] = v[i];
-    return MNNB200_OK;
-}
-
 // ---- TMA descriptors (driver entry point fetched through the runtime: no link-time libcuda dependency)
 typedef CUresult (*PFN_encodeTiled)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*, const cuuint64_t*,
                                     const cuuint32_t*, const cuuint32_t*, CUtensorMapInterleave, CUtensorMapSwizzle,
@@ -67,8 +56,8 @@ static PFN_encodeTiled get_encode() {
     });
     return fn;
 }
-// row-major int8 matrix [rows][k] -> 2D tensor map with a {128 bytes, box_rows} box, 128B swizzle, zero OOB fill
-static mnnb200_status make_tmap_i8(CUtensorMap* m, const void* ptr, int rows, int k, int box_rows) {
+namespace mnnb200 {
+MNNB200_INTERNAL mnnb200_status make_tmap_i8(CUtensorMap* m, const void* ptr, int rows, int k, int box_rows) {
     PFN_encodeTiled enc = get_encode();
     if (!enc) return fail(MNNB200_CUDA_ERROR, "cuTensorMapEncodeTiled entry point not available");
     cuuint64_t dims[2] = {(cuuint64_t)k, (cuuint64_t)rows};
@@ -81,6 +70,7 @@ static mnnb200_status make_tmap_i8(CUtensorMap* m, const void* ptr, int rows, in
     if (r != CUDA_SUCCESS) return fail(MNNB200_CUDA_ERROR, "cuTensorMapEncodeTiled failed: " + std::to_string((int)r));
     return MNNB200_OK;
 }
+}  // namespace mnnb200
 // 4-bit weights [rows][k / 2] bytes: boxes of 64 bytes (one 128-channel K block) x box_rows, unswizzled (the GEMM expands
 // them into the 128B-swizzled int8 tile itself)
 static mnnb200_status make_tmap_w4(CUtensorMap* m, const void* ptr, int rows, int k, int box_rows) {
@@ -1739,8 +1729,6 @@ mnnb200_status mnnb200_matmul_execute(mnnb200_exec* ex, const void* a, const voi
 // Float convolutions and their fp32 neighbours (device fp32 tensors are NCHW-linear): the CPU backend's float path
 // (CPUConvolution / ConvolutionTiledExecutor, CPUConvolutionDepthwise, CPUBinary ADD, CPUScale, CPUSoftmax) on the GPU.
 // =================================================================================================
-static int float_act(const mnnb200_conv_desc* d, int relu6) { return relu6 ? 2 : (d->relu ? 1 : 0); }
-
 struct ConvF32Exec : Tagged<kConvF32, ConvExec> {
     int act = 0, cp8 = 0, taps = 0, kp = 0, ocp = 0, bn = 0;
     DevBuf<float> d_hi, d_lo, d_bias;
@@ -1757,11 +1745,6 @@ struct ScaleF32Exec : Tagged<kScaleF32> {
     size_t plane = 0;
     DevBuf<float> d_scale, d_bias;
 };
-
-static bool conv_desc_valid(const mnnb200_conv_desc* d) {
-    return d->ic > 0 && d->oc > 0 && d->kh > 0 && d->kw > 0 && d->stride_h > 0 && d->stride_w > 0 && d->dilate_h > 0 &&
-           d->dilate_w > 0 && d->pad_h >= 0 && d->pad_w >= 0;
-}
 
 extern "C" {
 mnnb200_status mnnb200_conv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight, const float* bias,

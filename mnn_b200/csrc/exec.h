@@ -3,6 +3,7 @@
 // error reporting of mnnb200_last_error.  A handle made by either library is destroyed by mnnb200_exec_destroy (virtual
 // destructor) and refused by the other library's entry points (its type tag).
 #pragma once
+#include <cuda.h>
 #include <cuda_runtime.h>
 #include <memory>
 #include <string>
@@ -16,6 +17,8 @@
 // Sets the message mnnb200_last_error returns and passes the status through (capi.cu)
 namespace mnnb200 {
 MNNB200_INTERNAL mnnb200_status fail(mnnb200_status s, const std::string& m);
+// row-major int8 matrix [rows][k] -> 2D tensor map with a {128 bytes, box_rows} box, 128B swizzle, zero OOB fill (capi.cu)
+MNNB200_INTERNAL mnnb200_status make_tmap_i8(CUtensorMap* m, const void* ptr, int rows, int k, int box_rows);
 }
 #define CK(call)                                                                                   \
     do {                                                                                           \
@@ -78,7 +81,7 @@ class DevBuf {
 enum ExecType : unsigned {
     kConvInt8 = 1u << 0, kDwConvInt8 = 1u << 1, kLinearW8 = 1u << 2, kWinoInt8 = 1u << 3, kMatMul = 1u << 4,
     kConvGroup = 1u << 5, kScaleInt8 = 1u << 6, kConvF32 = 1u << 7, kDwConvF32 = 1u << 8, kScaleF32 = 1u << 9,
-    kLayerNormF32 = 1u << 10, kRoPEF32 = 1u << 11,
+    kLayerNormF32 = 1u << 10, kRoPEF32 = 1u << 11, kDeconvF32 = 1u << 12, kDwDeconvF32 = 1u << 13,
 };
 struct mnnb200_exec {
     unsigned type = 0;  // the ExecType of the struct new_exec made
@@ -105,4 +108,21 @@ inline std::unique_ptr<T> new_exec(mnnb200_runtime* rt) {
 template <class T>
 inline T* exec_as(mnnb200_exec* ex, unsigned types = T::kTypes) {
     return ex && (ex->type & types) ? static_cast<T*>(ex) : nullptr;
+}
+
+// The convolutions: the descriptor that set_pad edits.
+struct ConvExec : mnnb200_exec {
+    mnnb200_conv_desc d;
+};
+inline bool conv_desc_valid(const mnnb200_conv_desc* d) {
+    return d->ic > 0 && d->oc > 0 && d->kh > 0 && d->kw > 0 && d->stride_h > 0 && d->stride_w > 0 && d->dilate_h > 0 &&
+           d->dilate_w > 0 && d->pad_h >= 0 && d->pad_w >= 0;
+}
+// the activation code of the float convolutions' epilogues: 0 none, 1 ReLU, 2 ReLU6
+inline int float_act(const mnnb200_conv_desc* d, int relu6) { return relu6 ? 2 : (d->relu ? 1 : 0); }
+// a plan query: the first `count` (at most N) of the plan's fields go to `fields`
+template <size_t N>
+inline mnnb200_status copy_fields(const int (&v)[N], int* fields, int count) {
+    for (int i = 0; i < count && i < (int)N; ++i) fields[i] = v[i];
+    return MNNB200_OK;
 }

@@ -38,6 +38,7 @@
 #include "core/OpCommonUtils.hpp"
 #include "core/TensorUtils.hpp"
 
+#include "../../../include/mnn_b200_deconv.h"
 #include "../../../include/mnn_b200_llm.h"
 
 namespace MNN {
@@ -937,6 +938,76 @@ private:
     bool mDepthwise;
     int mIc;
 };
+// Deconvolution (group 1, split-TF32 wgmma over the stride phases) and DeconvolutionDepthwise on float tensors: CPUDeconvolution /
+// CPUDeconvolutionDepthwise with the weights in the op.  The input channel count is the input's (CPUDeconvolution ignores group);
+// dynamic weights (a second input without an output shape) are declined.  A clone is made again from the op with the same input
+// channel count.
+class DeconvF32Exec : public B200Exec {
+public:
+    DeconvF32Exec(Backend* bn, const Op* op, mnnb200_exec* h, bool dw, int ic) : B200Exec(bn), mOp(op), mH(h), mDepthwise(dw), mIc(ic) {}
+    static bool takes(const Op* op, const std::vector<Tensor*>& inputs) {
+        auto conv = op->main_as_Convolution2D();
+        return conv && conv->common() && !inputs.empty() && isF32Nchw(inputs[0]) &&
+               (inputs.size() == 1 || (inputs.size() == 2 && conv->common()->hasOutputShape()));
+    }
+    static Execution* create(B200Backend* bn, const Op* op, int ic) {
+        auto conv = op->main_as_Convolution2D();
+        if (!conv || !conv->common()) return nullptr;
+        auto cm = conv->common();
+        const bool dw = op->type() == OpType_DeconvolutionDepthwise;
+        const int oc = cm->outputCount(), kh = cm->kernelY(), kw = cm->kernelX();
+        if (!dw && cm->group() != 1) return nullptr;
+        if (dw && (ic != oc || (cm->group() != 1 && cm->group() != oc))) return nullptr;
+        std::shared_ptr<ConvolutionCommon::Int8Common> quanCommon;
+        const float* w = nullptr;
+        int wsize = 0;
+        ConvolutionCommon::getConvParameters(&quanCommon, bn, op, &w, &wsize);
+        if (!w || oc <= 0 || kh <= 0 || kw <= 0 || ic <= 0 || (size_t)wsize != (size_t)(dw ? 1 : ic) * oc * kh * kw) return nullptr;
+        mnnb200_conv_desc d;
+        d.ic = ic; d.oc = oc; d.kh = kh; d.kw = kw; d.stride_h = cm->strideY(); d.stride_w = cm->strideX();
+        d.pad_h = 0; d.pad_w = 0; d.dilate_h = cm->dilateY(); d.dilate_w = cm->dilateX();   // pads: set at resize
+        d.group = dw ? oc : 1; d.relu = cm->relu() ? 1 : 0;
+        const float* bias = (conv->bias() && (int)conv->bias()->size() == oc) ? conv->bias()->data() : nullptr;
+        mnnb200_exec* h = nullptr;
+        mnnb200_status st = dw ? mnnb200_dwdeconv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &h)
+                               : mnnb200_deconv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &h);
+        if (st != MNNB200_OK) {
+            if (st != MNNB200_NOT_SUPPORT) MNN_ERROR("mnn_b200 float deconv create: %s\n", mnnb200_last_error());
+            return nullptr;
+        }
+        return new DeconvF32Exec(bn, op, h, dw, ic);
+    }
+    bool onClone(Backend* bn, const Op* op, Execution** dst) override {
+        if (dst == nullptr) return true;
+        *dst = create(static_cast<B200Backend*>(bn), op, mIc);
+        return *dst != nullptr;
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto in = inputs[0], out = outputs[0];
+        if (in->dimensions() != 4 || in->channel() != mIc) {   // the kernels index the input by the weights' channel count
+            MNN_ERROR("mnn_b200 float deconv: input has %d channels, the weights %d\n", in->channel(), mIc);
+            return NOT_SUPPORT;
+        }
+        auto pad = ConvolutionCommon::convolutionTransposePad(in, out, mOp->main_as_Convolution2D()->common());   // (padX, padY)
+        int oh = out->height(), ow = out->width();
+        mnnb200_status st = mnnb200_deconv_f32_set_pad(mH.get(), pad.second, pad.first);
+        if (st == MNNB200_OK)
+            st = mDepthwise ? mnnb200_dwdeconv_f32_resize(mH.get(), in->batch(), in->height(), in->width(), &oh, &ow)
+                            : mnnb200_deconv_f32_resize(mH.get(), in->batch(), in->height(), in->width(), &oh, &ow);
+        return toErr(st, "float deconv resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto x = (const float*)dev(inputs[0]);
+        auto y = (float*)dev(outputs[0]);
+        return toErr(mDepthwise ? mnnb200_dwdeconv_f32_execute(mH.get(), x, y) : mnnb200_deconv_f32_execute(mH.get(), x, y),
+                     "float deconv");
+    }
+private:
+    const Op* mOp;
+    ExecHandle mH;
+    bool mDepthwise;
+    int mIc;
+};
 static bool isF32(const Tensor* t) { return t->getType().code == halide_type_float && t->getType().bytes() == 4; }
 // a full-size operand has the output's bytes: the same linear layout, or both of <= 2 dims (NCHW and NHWC are then the same)
 static bool sameLinear(const Tensor* t, const Tensor* out) {
@@ -1243,6 +1314,10 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
         case OpType_DepthwiseConvInt8:
             if (quantOut || op->type() == OpType_DepthwiseConvInt8) e = ConvInt8Exec::create(this, op);
             else if (inputs.size() == 1 && isF32Nchw(inputs[0])) e = ConvF32Exec::create(this, op);
+            break;
+        case OpType_Deconvolution:
+        case OpType_DeconvolutionDepthwise:
+            if (!quantOut && DeconvF32Exec::takes(op, inputs)) e = DeconvF32Exec::create(this, op, inputs[0]->channel());
             break;
         case OpType_FloatToInt8:   // the cast kernels read/write NCHW-linear fp32 (NHWC-format tensors of <= 2 dims are the same bytes)
             // only the pipeline-inserted casts (quant info on the tensor, Pipeline.cpp:361-395); an op that carries its own
