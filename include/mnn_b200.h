@@ -331,19 +331,29 @@ MNNB200_API mnnb200_status mnnb200_matmul_execute(mnnb200_exec* e, const void* a
  *                execute runs one split-TF32 wgmma implicit GEMM (a_hi*w_hi + a_hi*w_lo + a_lo*w_hi, fp32 accumulate: error near
  *                fp32's).  resize plans the launch for the shape (*oh / *ow as in conv_int8_resize); set_pad sets the begin pads
  *                (ConvolutionCommon::convolutionPad) of a conv_f32 or dwconv_f32 execution, before resize.
+ *      conv_f32_create_grouped: any desc->group >= 1 that divides ic and oc (ConvolutionGroup: group i is a conv over input
+ *                channels [i ic/group, (i+1) ic/group) with weights [oc][ic/group][kh][kw] and bias [oc]).  Returns a conv_f32
+ *                execution (set_pad / resize / execute / plan as above) on the same kernel: each n chunk of the launch covers
+ *                whole consecutive groups, or a 128-wide slice of one group, with block-diagonal weights, and its tile width is
+ *                fixed at create (resize keeps it).  group 1 gives the execution conv_f32_create gives.  NULL runtime,
+ *                descriptor, weights or out, a bad descriptor or group < 1: INVALID_VALUE; a group that does not divide ic or oc:
+ *                NOT_SUPPORT.
  *      dwconv_f32: group == ic == oc, weights [c][kh][kw].
  *      binary_add_f32: y = a + b over count elements (equal shapes, no broadcast).
  *      scale_f32: y[n][c][h][w] = x * scale[c] + bias[c] (bias may be NULL).
  *      softmax_f32: softmax over the middle axis of an [outside][axis][inside] view. */
 MNNB200_API mnnb200_status mnnb200_conv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight,
                                                    const float* bias, int relu6, mnnb200_exec** out);
+MNNB200_API mnnb200_status mnnb200_conv_f32_create_grouped(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight,
+                                                           const float* bias, int relu6, mnnb200_exec** out);
 MNNB200_API mnnb200_status mnnb200_conv_f32_set_pad(mnnb200_exec* e, int pad_h, int pad_w);
 MNNB200_API mnnb200_status mnnb200_conv_f32_resize(mnnb200_exec* e, int n, int ih, int iw, int* oh, int* ow);
 MNNB200_API mnnb200_status mnnb200_conv_f32_execute(mnnb200_exec* e, const float* x_nchw, float* y_nchw);
-/* read-only view of the resized conv_f32 execution's launch, as resize planned it: the first `count` (at most 7) of
+/* read-only view of the resized conv_f32 execution's launch, as resize planned it: the first `count` (at most 9) of
  * {bn (tile width 32 / 64 / 128), n_chunks, m_tiles (128-pixel M tiles), num_kb (32-wide K blocks per tile), stages (K blocks the
- * bn-wide kernel's shared-memory ring holds), cp8 (ic rounded up to 8), taps (kh * kw)} go to fields.  NO_EXECUTION before resize,
- * INVALID_VALUE for any other kind of execution.  Changes nothing. */
+ * bn-wide kernel's shared-memory ring holds), cp8 (an n chunk's input channels rounded up to 8: ic for group 1), taps (kh * kw),
+ * P (whole groups per n chunk; 1 for group 1), Q (n chunks per group; n_chunks for group 1)} go to fields.  NO_EXECUTION before
+ * resize, INVALID_VALUE for any other kind of execution.  Changes nothing. */
 MNNB200_API mnnb200_status mnnb200_conv_f32_plan(mnnb200_exec* e, int* fields, int count);
 MNNB200_API mnnb200_status mnnb200_dwconv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight,
                                                      const float* bias, int relu6, mnnb200_exec** out);

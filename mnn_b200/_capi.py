@@ -105,6 +105,7 @@ SIGNATURES = {
     "mnnb200_matmul_create": (C.c_int, [P] + [C.c_int] * 7 + [C.POINTER(P)]),
     "mnnb200_matmul_execute": (C.c_int, [P, P, P, P, P]),
     "mnnb200_conv_f32_create": (C.c_int, [P, C.POINTER(ConvDesc), P, P, C.c_int, C.POINTER(P)]),
+    "mnnb200_conv_f32_create_grouped": (C.c_int, [P, C.POINTER(ConvDesc), P, P, C.c_int, C.POINTER(P)]),
     "mnnb200_conv_f32_set_pad": (C.c_int, [P, C.c_int, C.c_int]),
     "mnnb200_conv_f32_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int)]),
     "mnnb200_conv_f32_execute": (C.c_int, [P, P, P]),

@@ -433,7 +433,7 @@ class MatMulExecution(Execution):
 
 
 class ConvF32Execution(Execution):
-    """Float Convolution (group 1, split-TF32 wgmma) or ConvolutionDepthwise on NCHW fp32 tensors: the CPU backend's float
+    """Float Convolution (any group, split-TF32 wgmma) or ConvolutionDepthwise on NCHW fp32 tensors: the CPU backend's float
     convolutions.  op.weight fp32 [oc][ic/group][kh][kw], op.bias fp32 [oc] or None; op.conv['relu'] / op.relu6."""
 
     def __init__(self, backend, op: Op, depthwise=False):
@@ -442,9 +442,11 @@ class ConvF32Execution(Execution):
         d = _desc(op.conv)
         w = np.ascontiguousarray(op.weight, np.float32)
         b = None if op.bias is None else np.ascontiguousarray(op.bias, np.float32)
-        f = _capi.lib().mnnb200_dwconv_f32_create if depthwise else _capi.lib().mnnb200_conv_f32_create
-        check(f(backend.runtime._h, C.byref(d), _np_ptr(w), _np_ptr(b), int(op.relu6), C.byref(self._h)),
-              "dwconv_f32_create" if depthwise else "conv_f32_create")
+        L = _capi.lib()
+        f, name = ((L.mnnb200_dwconv_f32_create, "dwconv_f32_create") if depthwise else
+                   (L.mnnb200_conv_f32_create_grouped, "conv_f32_create_grouped") if d.group > 1 else
+                   (L.mnnb200_conv_f32_create, "conv_f32_create"))
+        check(f(backend.runtime._h, C.byref(d), _np_ptr(w), _np_ptr(b), int(op.relu6), C.byref(self._h)), name)
 
     def onResize(self, inputs, outputs):
         n, _, ih, iw = inputs[0].shape
@@ -570,8 +572,10 @@ Backend.addCreator("LinearW8", lambda b, i, o, op: LinearW8Execution(b, op))
 
 
 def _create_conv_f32(b, i, o, op):
-    if op.conv.get("group", 1) != 1:      # grouped float convs are not taken (depthwise has its own op type)
-        return None
+    c, g = op.conv, op.conv.get("group", 1)
+    kh, kw = c.get("kernel", (1, 1))
+    if g < 1 or c["ic"] % g or c["oc"] % g or np.size(op.weight) != c["oc"] * (c["ic"] // g) * kh * kw:
+        return None                       # weights not shaped [oc][ic/group][kh][kw]
     return ConvF32Execution(b, op)
 
 

@@ -1731,6 +1731,8 @@ mnnb200_status mnnb200_matmul_execute(mnnb200_exec* ex, const void* a, const voi
 // =================================================================================================
 struct ConvF32Exec : Tagged<kConvF32, ConvExec> {
     int act = 0, cp8 = 0, taps = 0, kp = 0, ocp = 0, bn = 0;
+    int G = 1, icg = 0, ocg = 0, P = 1, Q = 1;   // groups (ConvF32Params); G > 1: bn and the n chunks are fixed at create
+    int n_chunks = 0;                            // G > 1 only
     DevBuf<float> d_hi, d_lo, d_bias;
     CUtensorMap tmap_hi, tmap_lo;
     ConvF32Params p;
@@ -1746,19 +1748,32 @@ struct ScaleF32Exec : Tagged<kScaleF32> {
     DevBuf<float> d_scale, d_bias;
 };
 
-extern "C" {
-mnnb200_status mnnb200_conv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight, const float* bias,
-                                       int relu6, mnnb200_exec** out) {
-    if (!rt || !desc || !weight || !out) return fail(MNNB200_INVALID_VALUE, "conv_f32_create: NULL argument");
-    if (!conv_desc_valid(desc)) return fail(MNNB200_INVALID_VALUE, "conv_f32_create: bad descriptor");
-    if (desc->group != 1) return fail(MNNB200_NOT_SUPPORT, "conv_f32: group > 1 (depthwise has its own execution)");
+// the one creator of both entry points: desc checked, desc->group >= 1 dividing ic and oc, weights [oc][ic / group][kh][kw].
+// Group 1 keeps choosing its tile width at resize; a grouped layer's width is fixed here, because the packed K layout depends on
+// it: the smallest of 32 / 64 / 128 that holds one whole group (P = bn / ocg groups per n chunk), else 128 with Q = ceil(ocg / 128)
+// chunks per group.
+static mnnb200_status conv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight, const float* bias,
+                                      int relu6, mnnb200_exec** out) {
     auto e = new_exec<ConvF32Exec>(rt);
     e->d = *desc; e->act = float_act(desc, relu6);
     e->taps = desc->kh * desc->kw;
-    e->cp8 = (desc->ic + 7) & ~7;
+    const int G = desc->group, icg = desc->ic / G, ocg = desc->oc / G;
+    e->G = G; e->icg = icg; e->ocg = ocg;
+    ConvF32Groups g{1, icg, ocg, 1, 1, 0};
+    if (G == 1) {
+        e->ocp = (desc->oc + 127) & ~127;      // a whole number of tiles of every width: no weight tile reads past the array
+        g.bn = e->ocp;                         // one chunk: row o is channel o
+    } else {
+        e->bn = ocg <= 32 ? 32 : (ocg <= 64 ? 64 : 128);
+        e->P = ocg <= e->bn ? std::min(e->bn / ocg, G) : 1;
+        e->Q = ocg <= e->bn ? 1 : (ocg + e->bn - 1) / e->bn;
+        e->n_chunks = e->Q == 1 ? (G + e->P - 1) / e->P : G * e->Q;
+        e->ocp = e->n_chunks * e->bn;
+        g = ConvF32Groups{G, icg, ocg, e->P, e->Q, e->bn};
+    }
+    e->cp8 = (e->P * icg + 7) & ~7;
     e->kp = (e->taps * e->cp8 + 31) & ~31;
-    e->ocp = (desc->oc + 127) & ~127;          // a whole number of tiles of every width: no weight tile reads past the array
-    const size_t wn = (size_t)desc->oc * desc->ic * e->taps, packed = (size_t)e->ocp * e->kp;
+    const size_t wn = (size_t)desc->oc * icg * e->taps, packed = (size_t)e->ocp * e->kp;
     std::vector<float> hw(weight, weight + wn), hb(desc->oc, 0.f);
     if (bias) hb.assign(bias, bias + desc->oc);
     DevBuf<float> raw;
@@ -1766,12 +1781,34 @@ mnnb200_status mnnb200_conv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_d
     if ((st = raw.upload(hw, rt->stream)) || (st = e->d_bias.upload(hb, rt->stream)) || (st = e->d_hi.reserve(packed)) ||
         (st = e->d_lo.reserve(packed)))
         return st;
-    cudaError_t ce = launch_pack_conv_w_f32(raw, desc->oc, desc->ic, e->taps, e->cp8, e->kp, e->ocp, e->d_hi, e->d_lo, rt->stream);
+    cudaError_t ce = launch_pack_conv_w_f32(raw, desc->oc, e->taps, e->cp8, e->kp, e->ocp, g, e->d_hi, e->d_lo, rt->stream);
     if (ce == cudaSuccess) ce = cudaStreamSynchronize(rt->stream);
     raw.reset();                                 // the unpacked weights are not needed after the split
     if (ce != cudaSuccess) return fail(MNNB200_CUDA_ERROR, std::string("conv_f32_create: ") + cudaGetErrorString(ce));
+    // a grouped layer's width never changes: its weight maps are made once, here
+    if (G > 1 && ((st = make_tmap_i8(&e->tmap_hi, e->d_hi, e->ocp, e->kp * 4, e->bn)) ||
+                  (st = make_tmap_i8(&e->tmap_lo, e->d_lo, e->ocp, e->kp * 4, e->bn))))
+        return st;
     *out = e.release();
     return MNNB200_OK;
+}
+
+extern "C" {
+mnnb200_status mnnb200_conv_f32_create(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight, const float* bias,
+                                       int relu6, mnnb200_exec** out) {
+    if (!rt || !desc || !weight || !out) return fail(MNNB200_INVALID_VALUE, "conv_f32_create: NULL argument");
+    if (!conv_desc_valid(desc)) return fail(MNNB200_INVALID_VALUE, "conv_f32_create: bad descriptor");
+    if (desc->group != 1) return fail(MNNB200_NOT_SUPPORT, "conv_f32: group > 1 (conv_f32_create_grouped / dwconv_f32_create)");
+    return conv_f32_create(rt, desc, weight, bias, relu6, out);
+}
+
+mnnb200_status mnnb200_conv_f32_create_grouped(mnnb200_runtime* rt, const mnnb200_conv_desc* desc, const float* weight,
+                                               const float* bias, int relu6, mnnb200_exec** out) {
+    if (!rt || !desc || !weight || !out) return fail(MNNB200_INVALID_VALUE, "conv_f32_create_grouped: NULL argument");
+    if (!conv_desc_valid(desc) || desc->group < 1) return fail(MNNB200_INVALID_VALUE, "conv_f32_create_grouped: bad descriptor");
+    if (desc->ic % desc->group || desc->oc % desc->group)
+        return fail(MNNB200_NOT_SUPPORT, "conv_f32_create_grouped: group does not divide ic and oc");
+    return conv_f32_create(rt, desc, weight, bias, relu6, out);
 }
 
 mnnb200_status mnnb200_conv_f32_set_pad(mnnb200_exec* ex, int pad_h, int pad_w) {
@@ -1792,10 +1829,12 @@ mnnb200_status mnnb200_conv_f32_resize(mnnb200_exec* ex, int n, int ih, int iw, 
     if (M > 0x7fffffffLL - 128 || (long long)n * d.ic * ih * iw > 0x7fffffffLL || (long long)n * d.oc * OH * OW > 0x7fffffffLL)
         return fail(MNNB200_NOT_SUPPORT, "conv_f32_resize: tensor too large for 32-bit indexing");
     // the plan, once per shape: tile width from the layer's shape (fill the SMs before widening the tile), then the weight maps
+    // (a grouped layer's width was fixed at create)
     const int sm = e->rt->prop.multiProcessorCount;
     const int m_tiles = (int)((M + 127) / 128);
     int bn = d.oc <= 32 ? 32 : (d.oc <= 64 ? 64 : 128);
     while (bn > 32 && (long long)m_tiles * ((d.oc + bn - 1) / bn) < sm) bn >>= 1;
+    if (e->G > 1) bn = e->bn;
     mnnb200_status st;
     if (bn != e->bn) {
         if ((st = make_tmap_i8(&e->tmap_hi, e->d_hi, e->ocp, e->kp * 4, bn)) ||
@@ -1808,10 +1847,12 @@ mnnb200_status mnnb200_conv_f32_resize(mnnb200_exec* ex, int n, int ih, int iw, 
     p.bias = e->d_bias;
     p.N = n; p.IC = d.ic; p.IH = ih; p.IW = iw; p.OC = d.oc; p.OH = OH; p.OW = OW;
     p.KH = d.kh; p.KW = d.kw; p.sh = d.stride_h; p.sw = d.stride_w; p.ph = d.pad_h; p.pw = d.pad_w; p.dh = d.dilate_h; p.dw = d.dilate_w;
-    p.Cp8 = e->cp8; p.taps = e->taps; p.M = (int)M; p.num_kb = e->kp / 32; p.m_tiles = m_tiles; p.n_chunks = (d.oc + bn - 1) / bn;
+    p.Cp8 = e->cp8; p.taps = e->taps; p.M = (int)M; p.num_kb = e->kp / 32; p.m_tiles = m_tiles;
+    p.n_chunks = e->G > 1 ? e->n_chunks : (d.oc + bn - 1) / bn;
     p.act = e->act;
-    e->cost_bytes = 4.0 * ((double)n * d.ic * ih * iw + (double)M * d.oc + (double)d.oc * d.ic * e->taps);
-    e->cost_macs = (double)M * d.oc * d.ic * e->taps;
+    p.G = e->G; p.icg = e->icg; p.ocg = e->ocg; p.P = e->P; p.Q = e->G > 1 ? e->Q : p.n_chunks;
+    e->cost_bytes = 4.0 * ((double)n * d.ic * ih * iw + (double)M * d.oc + (double)d.oc * e->icg * e->taps);
+    e->cost_macs = (double)M * d.oc * e->icg * e->taps;
     e->resized = true;
     return out.done();
 }
@@ -1832,7 +1873,7 @@ mnnb200_status mnnb200_conv_f32_plan(mnnb200_exec* ex, int* fields, int count) {
     if (!e || !fields || count < 0) return fail(MNNB200_INVALID_VALUE, "conv_f32_plan: bad argument");
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_f32_plan before resize");
     const ConvF32Params& p = e->p;
-    const int v[] = {e->bn, p.n_chunks, p.m_tiles, p.num_kb, conv_f32_stages(e->bn), p.Cp8, p.taps};
+    const int v[] = {e->bn, p.n_chunks, p.m_tiles, p.num_kb, conv_f32_stages(e->bn), p.Cp8, p.taps, p.P, p.Q};
     return copy_fields(v, fields, count);
 }
 

@@ -153,8 +153,11 @@ cudaError_t launch_gemm_f16_wgmma(const void* tmap_a, const void* tmap_b, int ba
                                   int a_batch_rows, int b_batch_rows, int bn, float* c, const float* bias, cudaStream_t stream,
                                   int sm_count);
 
-// fp32 Conv2D (group 1) on split-TF32 wgmma (conv_f32_wgmma.cu): NCHW-linear fp32 in and out.  Weights are packed once into two
-// K-major arrays hi / lo [ocp][kp] (k = tap * cp8 + c, cp8 = ic rounded up to 8, kp = taps * cp8 rounded up to 32), w = hi + lo.
+// fp32 Conv2D (any group) on split-TF32 wgmma (conv_f32_wgmma.cu): NCHW-linear fp32 in and out.  Weights are packed once into two
+// K-major arrays hi / lo [ocp][kp] (k = tap * cp8 + c, cp8 = an n chunk's input channels rounded up to 8, kp = taps * cp8 rounded
+// up to 32), w = hi + lo.  n chunk nc covers the groups from g0 = nc / Q * P, ng = min(P, G - g0) of them, and the output channels
+// from oc0 = g0 * ocg + (nc % Q) * bn, min(bn, ng * ocg - (nc % Q) * bn) of them.  Group 1: G = 1, icg = IC, ocg = OC, P = 1,
+// Q = n_chunks.
 struct ConvF32Params {
     const float* x;       // [N][IC][IH][IW]
     float* y;             // [N][OC][OH][OW]
@@ -165,9 +168,15 @@ struct ConvF32Params {
     int M, num_kb;        // M = N * OH * OW, num_kb = kp / 32
     int m_tiles, n_chunks;
     int act;              // 0 none, 1 ReLU, 2 ReLU6
+    int G, icg, ocg;      // groups, input and output channels per group
+    int P, Q;             // whole groups per n chunk (ocg <= bn), n chunks per group (ocg > bn); one of them is 1
 };
-cudaError_t launch_pack_conv_w_f32(const float* w, int oc, int ic, int taps, int cp8, int kp, int ocp, float* hi, float* lo,
-                                   cudaStream_t s);
+// the packing's view of the n chunks: groups as in ConvF32Params, bn weight rows per chunk
+struct ConvF32Groups {
+    int G, icg, ocg, P, Q, bn;
+};
+cudaError_t launch_pack_conv_w_f32(const float* w, int oc, int taps, int cp8, int kp, int ocp, const ConvF32Groups& g, float* hi,
+                                   float* lo, cudaStream_t s);
 // tmap_hi / tmap_lo: 2D maps over the [ocp][kp * 4 bytes] weight arrays with {128 bytes, bn rows} boxes, 128B swizzle; bn 32 / 64 / 128
 cudaError_t launch_conv_f32_wgmma(const ConvF32Params& p, const void* tmap_hi, const void* tmap_lo, int bn, cudaStream_t s,
                                   int sm_count);

@@ -880,11 +880,15 @@ private:
 static bool isF32Nchw(const Tensor* t) {
     return t->getType().code == halide_type_float && t->getType().bytes() == 4 && linearFormat(t) == MNN_DATA_FORMAT_NCHW;
 }
-// Convolution (group 1, split-TF32 wgmma) and ConvolutionDepthwise (also a Convolution whose group == ic == oc) on float tensors
-class ConvF32Exec : public ClonedFromOp<ConvF32Exec> {
+// Convolution (any group, split-TF32 wgmma) and ConvolutionDepthwise (also a Convolution whose group == ic == oc) on float
+// tensors.  The group follows ConvolutionFloatFactory: common->group(), unless inputCount > 0 differs from the input's channel
+// count `in_c`, when it is in_c / inputCount; group i then convolves input channels [i icg, (i+1) icg) with the weights
+// [oc][icg][kh][kw], icg = wsize / (oc kh kw) = in_c / group.  A clone is made again from the op with the same input channel count.
+class ConvF32Exec : public B200Exec {
 public:
-    ConvF32Exec(Backend* bn, const Op* op, mnnb200_exec* h, bool dw, int ic) : ClonedFromOp(bn), mOp(op), mH(h), mDepthwise(dw), mIc(ic) {}
-    static Execution* create(B200Backend* bn, const Op* op) {
+    ConvF32Exec(Backend* bn, const Op* op, mnnb200_exec* h, bool dw, int ic, int inC)
+        : B200Exec(bn), mOp(op), mH(h), mDepthwise(dw), mIc(ic), mInC(inC) {}
+    static Execution* create(B200Backend* bn, const Op* op, int inC) {
         auto conv = op->main_as_Convolution2D();
         if (!conv || !conv->common()) return nullptr;
         auto cm = conv->common();
@@ -895,23 +899,36 @@ public:
         // plain float weights and IDST-coded ones, decoded as the CPU's float path does
         ConvolutionCommon::getConvParameters(&quanCommon, bn, op, &w, &wsize);
         if (!w || oc <= 0 || kh <= 0 || kw <= 0 || wsize <= 0) return nullptr;
-        const bool dw = op->type() == OpType_ConvolutionDepthwise || (cm->group() > 1 && cm->group() == oc && wsize == oc * kh * kw);
-        if (!dw && cm->group() != 1) return nullptr;          // grouped (1 < group < channels): not on this path
-        const int ic = dw ? oc : wsize / (oc * kh * kw);
-        if (ic <= 0 || (size_t)wsize != (size_t)oc * (dw ? 1 : ic) * kh * kw) return nullptr;
+        const bool dwOp = op->type() == OpType_ConvolutionDepthwise;
+        int group = cm->group(), ic = oc;
+        if (!dwOp && cm->inputCount() > 0 && cm->inputCount() != inC) group = inC / cm->inputCount();
+        const bool dw = dwOp || (group > 1 && group == oc && wsize == oc * kh * kw);
+        if (!dw) {
+            if (group <= 0 || wsize % (oc * kh * kw)) return nullptr;
+            const int icg = wsize / (oc * kh * kw);
+            ic = icg * group;
+            if (icg <= 0 || (group > 1 && ic != inC) || oc % group) return nullptr;
+        }
+        if ((size_t)wsize != (size_t)oc * (dw ? 1 : ic / group) * kh * kw) return nullptr;
         mnnb200_conv_desc d;
         d.ic = ic; d.oc = oc; d.kh = kh; d.kw = kw; d.stride_h = cm->strideY(); d.stride_w = cm->strideX();
         d.pad_h = 0; d.pad_w = 0; d.dilate_h = cm->dilateY(); d.dilate_w = cm->dilateX();   // pads: set at resize
-        d.group = dw ? oc : 1; d.relu = cm->relu() ? 1 : 0;
+        d.group = dw ? oc : group; d.relu = cm->relu() ? 1 : 0;
         const float* bias = (conv->bias() && (int)conv->bias()->size() == oc) ? conv->bias()->data() : nullptr;
         mnnb200_exec* h = nullptr;
-        mnnb200_status st = dw ? mnnb200_dwconv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &h)
-                               : mnnb200_conv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &h);
+        mnnb200_status st = dw          ? mnnb200_dwconv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &h)
+                            : group > 1 ? mnnb200_conv_f32_create_grouped(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &h)
+                                        : mnnb200_conv_f32_create(bn->handle(), &d, w, bias, cm->relu6() ? 1 : 0, &h);
         if (st != MNNB200_OK) {
             if (st != MNNB200_NOT_SUPPORT) MNN_ERROR("mnn_b200 float conv create: %s\n", mnnb200_last_error());
             return nullptr;
         }
-        return new ConvF32Exec(bn, op, h, dw, ic);
+        return new ConvF32Exec(bn, op, h, dw, ic, inC);
+    }
+    bool onClone(Backend* bn, const Op* op, Execution** dst) override {
+        if (dst == nullptr) return true;
+        *dst = create(static_cast<B200Backend*>(bn), op, mInC);
+        return *dst != nullptr;
     }
     ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto in = inputs[0], out = outputs[0];
@@ -936,7 +953,7 @@ private:
     const Op* mOp;
     ExecHandle mH;
     bool mDepthwise;
-    int mIc;
+    int mIc, mInC;
 };
 // Deconvolution (group 1, split-TF32 wgmma over the stride phases) and DeconvolutionDepthwise on float tensors: CPUDeconvolution /
 // CPUDeconvolutionDepthwise with the weights in the op.  The input channel count is the input's (CPUDeconvolution ignores group);
@@ -1303,7 +1320,7 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
             // (ConvolutionFloatFactory.cpp:140-149), which only LinearW8Exec reproduces: such a conv is not taken in fp32
             else if (!quantOut && op->type() == OpType_Convolution && inputs.size() == 1 && isF32Nchw(inputs[0]) &&
                      !(mMemoryLow && op->main_as_Convolution2D() && op->main_as_Convolution2D()->quanParameter()))
-                e = ConvF32Exec::create(this, op);
+                e = ConvF32Exec::create(this, op, inputs[0]->channel());
             break;
         case OpType_MatMul:
             if (!quantOut && inputs.size() >= 2 && op->main_as_MatMul() && inputs[0]->getType().code == halide_type_float &&
@@ -1313,7 +1330,7 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
         case OpType_ConvolutionDepthwise:
         case OpType_DepthwiseConvInt8:
             if (quantOut || op->type() == OpType_DepthwiseConvInt8) e = ConvInt8Exec::create(this, op);
-            else if (inputs.size() == 1 && isF32Nchw(inputs[0])) e = ConvF32Exec::create(this, op);
+            else if (inputs.size() == 1 && isF32Nchw(inputs[0])) e = ConvF32Exec::create(this, op, inputs[0]->channel());
             break;
         case OpType_Deconvolution:
         case OpType_DeconvolutionDepthwise:

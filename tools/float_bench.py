@@ -30,6 +30,7 @@ MODELS = {   # --model: (fixture under oracle/_ref, name in the JSON line)
     "squeezenet_v10": ("squeezenet_v10_f32.mnn", "SqueezeNet v1.0 fp32 (seeded weights)"),
     "squeezenet_v11": ("squeezenet_v11_f32.mnn", "SqueezeNet v1.1 fp32 (seeded weights)"),
     "mbv1": ("mbv1_f32.mnn", "MobileNet-v1 fp32 (seeded weights)"),
+    "resnext50": ("resnext50_f32.mnn", "ResNeXt-50 32x4d fp32 (seeded weights, oracle/refdump_gconv.cpp)"),
 }
 
 
