@@ -139,6 +139,16 @@ DECONV_SIGNATURES = {
 }
 _deconv_lib = None
 
+# libmnn_b200_interp.so (include/mnn_b200_interp.h): the float Interp execution, on the runtime and execution handles above
+INTERP_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_interp.so")
+INTERP_SIGNATURES = {
+    "mnnb200_interp_f32_create": (C.c_int, [P, C.c_int, C.c_float, C.c_float, C.c_float, C.c_float, C.POINTER(P)]),
+    "mnnb200_interp_f32_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mnnb200_interp_f32_execute": (C.c_int, [P, P, P]),
+    "mnnb200_interp_f32_plan": (C.c_int, [P, C.POINTER(C.c_int), C.c_int]),
+}
+_interp_lib = None
+
 # libmnn_b200_llm.so (include/mnn_b200_llm.h): MNN-LLM's LayerNorm / RoPE executions, on the runtime and execution handles above
 LLM_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_llm.so")
 LLM_SIGNATURES = {
@@ -183,6 +193,23 @@ def deconv_lib():
             fn.argtypes = args
         _deconv_lib = L
     return _deconv_lib
+
+
+def interp_lib():
+    """libmnn_b200_interp.so with every INTERP_SIGNATURES symbol resolved (after libmnn_b200.so, whose handles it shares)"""
+    global _interp_lib
+    if _interp_lib is None:
+        lib()
+        if not os.path.exists(INTERP_LIB_PATH):
+            raise MnnB200Error(f"{INTERP_LIB_PATH} is missing: run `python -m mnn_b200.build` (there is no CPU fallback)")
+        L = C.CDLL(INTERP_LIB_PATH)
+        for name, (res, args) in INTERP_SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype = res
+            fn.argtypes = args
+        _interp_lib = L
+    return _interp_lib
+
 
 def lib():
     global _lib

@@ -491,6 +491,31 @@ class DeconvF32Execution(Execution):
         return f(self._h, inputs[0].ptr(), outputs[0].ptr())
 
 
+class InterpF32Execution(Execution):
+    """Float Interp on NCHW fp32 tensors: the CPU backend's CPUInterp as the geometry stage leaves it.  op.extra: resize_type (1
+    nearest, 2 bilinear, 3 cubic, 4 nearest-round), scale (h, w), offset (h, w) -- the lowered op's coordinate transform, src =
+    dst * scale + offset -- and out_hw, the output size."""
+
+    def __init__(self, backend, op: Op):
+        super().__init__(backend)
+        self.op = op
+        e = op.extra
+        (hs, ws), (ho, wo) = e["scale"], e.get("offset", (0.0, 0.0))
+        check(_capi.interp_lib().mnnb200_interp_f32_create(backend.runtime._h, int(e["resize_type"]), ws, hs, wo, ho,
+                                                           C.byref(self._h)), "interp_f32_create")
+
+    def onResize(self, inputs, outputs):
+        n, c, ih, iw = inputs[0].shape
+        oh, ow = self.op.extra["out_hw"]
+        st = _capi.interp_lib().mnnb200_interp_f32_resize(self._h, n * c, ih, iw, oh, ow)
+        if st == 0:
+            outputs[0].shape = (n, c, oh, ow)
+        return st
+
+    def onExecute(self, inputs, outputs):
+        return _capi.interp_lib().mnnb200_interp_f32_execute(self._h, inputs[0].ptr(), outputs[0].ptr())
+
+
 class Backend:
     """CUDABackend's role: creator map, buffer acquisition, host<->device copies with layout + quant casts."""
 
@@ -591,3 +616,4 @@ def _create_deconv_f32(b, i, o, op):
 
 Backend.addCreator("DeconvF32", _create_deconv_f32)
 Backend.addCreator("DwDeconvF32", lambda b, i, o, op: DeconvF32Execution(b, op, depthwise=True))
+Backend.addCreator("InterpF32", lambda b, i, o, op: InterpF32Execution(b, op))

@@ -39,6 +39,7 @@
 #include "core/TensorUtils.hpp"
 
 #include "../../../include/mnn_b200_deconv.h"
+#include "../../../include/mnn_b200_interp.h"
 #include "../../../include/mnn_b200_llm.h"
 
 namespace MNN {
@@ -1303,6 +1304,44 @@ private:
     ExecHandle mH;
 };
 
+// Interp on float tensors (CPUInterp): the op the geometry stage lowers Interp and Resize to, one 4-D input, NCHW-linear (NC4HW4 is
+// stored so here), whose widthScale / heightScale / widthOffset / heightOffset already hold the coordinate transform.  They are
+// read as CPUInterpCreator reads them, with the resize type; resize types outside 1-4 and TensorflowCropAndResize (the geometry
+// leaves its scales unset) are declined, as are int8 tensors.  The planes are batch * channels, the sizes those of onResize.
+class InterpF32Exec : public ClonedFromOp<InterpF32Exec> {
+public:
+    InterpF32Exec(Backend* bn, mnnb200_exec* h) : ClonedFromOp(bn), mH(h) {}
+    static Execution* create(B200Backend* bn, const Op* op) {
+        auto ip = op->main_as_Interp();
+        if (!ip || ip->resizeType() < 1 || ip->resizeType() > 4 || ip->ctm() == CoordinateTransformationMode_TensorflowCropAndResize)
+            return nullptr;
+        mnnb200_exec* h = nullptr;
+        if (mnnb200_interp_f32_create(bn->handle(), ip->resizeType(), ip->widthScale(), ip->heightScale(), ip->widthOffset(),
+                                      ip->heightOffset(), &h) != MNNB200_OK)
+            return nullptr;
+        return new InterpF32Exec(bn, h);
+    }
+    static bool takes(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) {
+        if (inputs.size() != 1 || outputs.size() != 1) return false;
+        auto in = inputs[0], out = outputs[0];
+        return isF32(in) && isF32(out) && !isInt8(in) && !isInt8(out) && in->dimensions() == 4 && out->dimensions() == 4 &&
+               linearFormat(in) == MNN_DATA_FORMAT_NCHW && linearFormat(out) == MNN_DATA_FORMAT_NCHW &&
+               in->batch() == out->batch() && in->channel() == out->channel();
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto in = inputs[0], out = outputs[0];
+        const long long planes = (long long)in->batch() * in->channel();
+        if (!takes(inputs, outputs) || planes > 0x7fffffffLL) return NOT_SUPPORT;
+        return toErr(mnnb200_interp_f32_resize(mH.get(), (int)planes, in->height(), in->width(), out->height(), out->width()),
+                     "Interp fp32 resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        return toErr(mnnb200_interp_f32_execute(mH.get(), (const float*)dev(inputs[0]), (float*)dev(outputs[0])), "Interp fp32");
+    }
+private:
+    ExecHandle mH;
+};
+
 Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs, const MNN::Op* op) {
     Execution* e = nullptr;
     const bool quantOut = !outputs.empty() && TensorUtils::getDescribe(outputs[0])->quantAttr.get() != nullptr &&
@@ -1444,6 +1483,9 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
             break;
         case OpType_RoPE:
             if (!quantOut && RoPEF32Exec::takes(op, inputs, outputs)) e = RoPEF32Exec::create(this, op);
+            break;
+        case OpType_Interp:
+            if (!quantOut && InterpF32Exec::takes(inputs, outputs)) e = InterpF32Exec::create(this, op);
             break;
         default:
             break;

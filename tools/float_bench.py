@@ -31,6 +31,7 @@ MODELS = {   # --model: (fixture under oracle/_ref, name in the JSON line)
     "squeezenet_v11": ("squeezenet_v11_f32.mnn", "SqueezeNet v1.1 fp32 (seeded weights)"),
     "mbv1": ("mbv1_f32.mnn", "MobileNet-v1 fp32 (seeded weights)"),
     "resnext50": ("resnext50_f32.mnn", "ResNeXt-50 32x4d fp32 (seeded weights, oracle/refdump_gconv.cpp)"),
+    "deeplab": ("deeplab_f32.mnn", "DeepLab-v3-style segmentation fp32, 128x128 (seeded weights, oracle/refdump_interp.cpp)"),
 }
 
 
