@@ -462,12 +462,18 @@ __global__ void pool_f32_kernel(const PoolParams p, const float* __restrict__ x,
             r = interior ? sum : __fmul_rn(sum, div);
         } else {
             // pooling_max_pad (CPUPool.hpp:19-51) reads the edge row / column for a tap in the padding, so a window wholly in
-            // the padding (large pads, ceil mode) takes its edge's maximum; the reduction starts at VEC(-16777216)
-            const int ys = min(max(iy0, 0), p.IH - 1), ye = min(max(iy0 + p.KH - 1, 0), p.IH - 1);
-            const int xs = min(max(ix0, 0), p.IW - 1), xe = min(max(ix0 + p.KW - 1, 0), p.IW - 1);
+            // the padding (large pads, ceil mode) takes its edge's maximum; the reduction starts at VEC(-16777216) and takes
+            // each tap as VEC::max(max, tap), maxps: the tap unless the running max is strictly greater (a NaN is replaced by
+            // the next tap, of -0 and +0 the later one stays)
+            // the taps in the CPU's order, an edge tap read again for each padded tap it stands for
             r = -16777216.f;
-            for (int yy = ys; yy <= ye; ++yy)
-                for (int xx = xs; xx <= xe; ++xx) r = fmaxf(r, xp[(size_t)yy * p.IW + xx]);
+            for (int ky = 0; ky < p.KH; ++ky) {
+                const int yy = min(max(iy0 + ky, 0), p.IH - 1);
+                for (int kx = 0; kx < p.KW; ++kx) {
+                    const float v = xp[(size_t)yy * p.IW + min(max(ix0 + kx, 0), p.IW - 1)];
+                    r = r > v ? r : v;
+                }
+            }
         }
         y[i] = r;
     }
@@ -826,17 +832,43 @@ cudaError_t launch_relu_f32(const float* x, float* y, size_t n, float slope, cud
 
 // ---- float Reduction over the middle axis of [outside][axis][inside] (CPUReduction.cpp: sum / mean / max / min / prod).
 //      One thread per (outside, inside) when inside > 1 (coalesced along inside); one warp per row when inside == 1.
-//      op: 0 SUM, 1 MEAN, 2 MAX, 3 MIN, 4 PROD.  fp32 accumulation order differs from the CPU's SIMD order: 1e-3 tolerance op.
+//      op: 0 SUM, 1 MEAN, 2 MAX, 3 MIN, 4 PROD.  SUM / MEAN / PROD: fp32 accumulation in another order than the CPU's SIMD order.
+//      MAX / MIN restate CPUReduction.cpp:297-318 (`float Max = srcInside[0]; ... Max = std::max(Max, srcInside[a * inside])`,
+//      MinReduce alike): the row's first element, then a value replaces it only when strictly greater (smaller), so a row of -inf
+//      gives -inf, a NaN is kept only when it comes first, and of equal values (-0 and +0) the first one stays.
 __device__ __forceinline__ float red_combine(float a, float b, int op) {
-    return op <= 1 ? a + b : (op == 2 ? fmaxf(a, b) : (op == 3 ? fminf(a, b) : a * b));
+    return op <= 1 ? a + b : a * b;
+}
+__device__ __forceinline__ bool red_better(float v, float best, int op) {
+    return op == 2 ? best < v : v < best;
 }
 __global__ void reduce_f32_kernel(const float* __restrict__ x, float* __restrict__ y, int outside, int axis, int inside, int op) {
-    const float init = op <= 1 ? 0.f : (op == 2 ? -3.402823466e38f : (op == 3 ? 3.402823466e38f : 1.f));
+    const float init = op <= 1 ? 0.f : 1.f;
     if (inside == 1) {
         const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
         if (warp >= outside) return;
+        const float* xp = x + (size_t)warp * axis;
+        if (op >= 2 && op <= 3) {
+            // each lane keeps its first best non-NaN value and its index; the lanes' bests merge by value, then by index
+            float best = 0.f;
+            int idx = axis;
+            for (int a = lane; a < axis; a += 32) {
+                const float v = xp[a];
+                if (v == v && (idx == axis || red_better(v, best, op))) { best = v; idx = a; }
+            }
+            for (int o = 16; o > 0; o >>= 1) {
+                const float ov = __shfl_xor_sync(0xffffffffu, best, o);
+                const int oi = __shfl_xor_sync(0xffffffffu, idx, o);
+                if (oi < axis && (idx == axis || red_better(ov, best, op) || (!red_better(best, ov, op) && oi < idx))) {
+                    best = ov;
+                    idx = oi;
+                }
+            }
+            if (lane == 0) y[warp] = (xp[0] != xp[0] || idx == axis) ? xp[0] : best;
+            return;
+        }
         float acc = init;
-        for (int a = lane; a < axis; a += 32) acc = red_combine(acc, x[(size_t)warp * axis + a], op);
+        for (int a = lane; a < axis; a += 32) acc = red_combine(acc, xp[a], op);
         for (int o = 16; o > 0; o >>= 1) acc = red_combine(acc, __shfl_xor_sync(0xffffffffu, acc, o), op);
         if (lane == 0) y[warp] = op == 1 ? acc / (float)axis : acc;
         return;
@@ -844,8 +876,18 @@ __global__ void reduce_f32_kernel(const float* __restrict__ x, float* __restrict
     const size_t total = (size_t)outside * inside;
     for (size_t i = blockIdx.x * (size_t)blockDim.x + threadIdx.x; i < total; i += (size_t)gridDim.x * blockDim.x) {
         const size_t o = i / inside, in = i - o * inside;
-        float acc = init;
-        for (int a = 0; a < axis; ++a) acc = red_combine(acc, x[(o * axis + a) * inside + in], op);
+        const float* xp = x + o * axis * inside + in;
+        float acc;
+        if (op >= 2 && op <= 3) {
+            acc = xp[0];
+            for (int a = 1; a < axis; ++a) {
+                const float v = xp[(size_t)a * inside];
+                if (red_better(v, acc, op)) acc = v;
+            }
+        } else {
+            acc = init;
+            for (int a = 0; a < axis; ++a) acc = red_combine(acc, xp[(size_t)a * inside], op);
+        }
         y[i] = op == 1 ? acc / (float)axis : acc;
     }
 }
@@ -905,15 +947,19 @@ __device__ __forceinline__ float binary_f32_op(float a, float b) {
     if (OP == kBinarySub) return __fsub_rn(a, b);
     if (OP == kBinaryMul) return __fmul_rn(a, b);
     if (OP == kBinaryRealDiv) return __fdiv_rn(a, b);
-    if (OP == kBinaryMinimum) return fminf(a, b);
-    if (OP == kBinaryMaximum) return fmaxf(a, b);
+    // x86 minps / maxps, which the CPU's VecBinaryMin / VecBinaryMax run (BinaryUtils.hpp:335-347, Vec::min / Vec::max):
+    // the second operand unless the first is strictly smaller (greater), so MIN(-0, +0) = +0, MIN(NaN, 1) = 1, MIN(1, NaN) = NaN
+    if (OP == kBinaryMinimum) return a < b ? a : b;
+    if (OP == kBinaryMaximum) return a > b ? a : b;
     const float d = __fsub_rn(a, b);   // kBinarySquaredDifference
     return __fmul_rn(d, d);
 }
 template <int OP>
 __device__ __forceinline__ float binary_f32_one(float a, float b, int relu) {
+    // activationType 1 is CPURelu(0) over the output (CPUBinary.cpp:36-37, MNNReluWithSlopeChannel): x < 0 ? x * 0 : x, so a
+    // negative result becomes -0, -inf becomes NaN and NaN stays NaN
     const float v = binary_f32_op<OP>(a, b);
-    return relu ? fmaxf(v, 0.f) : v;
+    return relu && v < 0.f ? __fmul_rn(v, 0.f) : v;
 }
 template <int OP>
 __global__ void binary_f32_kernel(const float* a, const float* b, float* y, size_t n, int a_one, int b_one, int relu, int vec) {
@@ -964,10 +1010,24 @@ cudaError_t launch_binary_add_f32(const float* a, const float* b, float* y, size
 // ---- fp32 UnaryOp (CPUUnary::selectForFloat, CPUUnary.cpp:353-440).  HARDSWISH, ABS, NEG, SQUARE, SQRT, RSQRT and RECIPROCAL
 //      use the CPU's own formula in round-to-nearest steps; the transcendental ops (the CPU uses its own polynomials) are
 //      accurate to a few ulp: SIGMOID / SILU / GELU through expf in a cancellation-free form, GELU_STANDARD through erfcf.
+// x * sigmoid(t) = x / (1 + e^-t) for t >= 0, x e^t / (1 + e^t) for t < 0: e^-|t| never overflows, so the result keeps its
+// magnitude where 1 / (1 + e^-t) would be 1 / inf (t < -88.7).  Below t = -64 (1 + e^t is then 1) the exponential is taken at
+// t + 32 (exact for |t| < 256, beyond which the result is 0 anyway) and the product scaled by e^-32, so that a subnormal e^t
+// does not lose the digits the product still has.
+__device__ __forceinline__ float times_sigmoid(float x, float t) {
+    if (t >= 0.f) return __fdiv_rn(x, __fadd_rn(1.f, expf(-t)));
+    if (t >= -64.f) {
+        const float e = expf(t);
+        return __fdiv_rn(__fmul_rn(x, e), __fadd_rn(1.f, e));
+    }
+    return __fmul_rn(__fmul_rn(x, expf(__fadd_rn(t, 32.f))), 1.26641655e-14f);   // e^-32
+}
 template <int OP>
 __device__ __forceinline__ float unary_f32_op(float x) {
-    if (OP == kUnaryAbs) return fabsf(x);
-    if (OP == kUnaryNeg) return -x;
+    // ABS is MNNReluWithSlope(x, -1) (CPUUnary.cpp:323-325): (x < 0 ? x * -1 : 0) + (x >= 0 ? x : 0), so |-0| = +0 and
+    // |NaN| = +0; NEG is x * -1 + 0 (CPUUnary.cpp:47-49, MNNScaleAndAddBiasScalar), so -(+0) = +0
+    if (OP == kUnaryAbs) return x < 0.f ? -x : (x >= 0.f ? __fadd_rn(0.f, x) : 0.f);
+    if (OP == kUnaryNeg) return __fadd_rn(-x, 0.f);
     if (OP == kUnarySquare) return __fmul_rn(x, x);
     if (OP == kUnarySqrt) return __fsqrt_rn(x);
     if (OP == kUnaryRsqrt) return __fdiv_rn(1.f, __fsqrt_rn(x));
@@ -975,13 +1035,13 @@ __device__ __forceinline__ float unary_f32_op(float x) {
     if (OP == kUnaryExp) return expf(x);
     if (OP == kUnaryLog) return logf(x);
     if (OP == kUnaryTanh) return tanhf(x);
-    if (OP == kUnarySigmoid) return __fdiv_rn(1.f, __fadd_rn(1.f, expf(-x)));
-    if (OP == kUnarySilu) return __fdiv_rn(x, __fadd_rn(1.f, expf(-x)));
+    if (OP == kUnarySigmoid) return x >= -64.f ? times_sigmoid(1.f, x) : expf(x);   // 1 + e^x is 1 below -64
+    if (OP == kUnarySilu) return times_sigmoid(x, x);
     if (OP == kUnaryHardSwish)   // x86_x64/sse/MathFunctions.cpp:251-259: (x * min(max(x + 3, 0), 6)) / 6
         return __fdiv_rn(__fmul_rn(x, fminf(fmaxf(__fadd_rn(x, 3.f), 0.f), 6.f)), 6.f);
-    if (OP == kUnaryGelu) {      // 0.5 x (1 + tanh(z)) = x / (1 + exp(-2z)), z = 0.79788458 (x + 0.044715 x^3)
+    if (OP == kUnaryGelu) {      // 0.5 x (1 + tanh(z)) = x sigmoid(2z), z = 0.79788458 (x + 0.044715 x^3)
         const float z = 0.79788458f * (x + 0.044715f * x * x * x);
-        return __fdiv_rn(x, __fadd_rn(1.f, expf(-2.f * z)));
+        return times_sigmoid(x, 2.f * z);
     }
     return 0.5f * x * erfcf(-0.70710678f * x);   // kUnaryGeluStandard: 0.5 x (1 + erf(x / sqrt 2))
 }
