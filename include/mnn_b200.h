@@ -322,6 +322,16 @@ MNNB200_API mnnb200_status mnnb200_linear_w8_plan(mnnb200_exec* e, int* fields, 
 MNNB200_API mnnb200_status mnnb200_matmul_create(mnnb200_runtime* rt, int batch, int e, int l, int h, int transpose_a,
                                                  int transpose_b, int inputs_are_f16, mnnb200_exec** out);
 MNNB200_API mnnb200_status mnnb200_matmul_execute(mnnb200_exec* e, const void* a, const void* b, const float* bias, float* c);
+/* ---- The same fp32 MatMul over broadcast batches (ShapeMatMul's rule): c_batch[0..nd) are C's batch dims, a_batch / b_batch
+ *      each operand's, right-aligned to C's and padded with leading 1s by the caller; each a_batch[i] / b_batch[i] is 1 or
+ *      c_batch[i].  A holds prod(a_batch) batches of [e][l] (or [l][e]), B prod(b_batch) of [l][h] (or [h][l]), C prod(c_batch)
+ *      of [e][h]; output batch bt reads the A and B batches its coordinates select.  The table of those batch pairs is built
+ *      and uploaded here, once; with no broadcast dim there is none and the execution is mnnb200_matmul_create's.  nd at most
+ *      8, else INVALID_VALUE.  A 1-D operand is the caller's to squeeze: A of [l] is e = 1, B of [l] is h = 1 with
+ *      transpose_b = 1.  Executed by mnnb200_matmul_execute. */
+MNNB200_API mnnb200_status mnnb200_matmul_create_broadcast(mnnb200_runtime* rt, int nd, const int* c_batch, const int* a_batch,
+                                                           const int* b_batch, int e, int l, int h, int transpose_a,
+                                                           int transpose_b, mnnb200_exec** out);
 
 /* ---- Float convolutions of fp32 models and their fp32 neighbours: the CPU backend's float path (CPUConvolution /
  *      ConvolutionTiledExecutor, CPUConvolutionDepthwise, CPUBinary ADD, CPUScale, CPUSoftmax) on NCHW-linear device fp32 tensors.

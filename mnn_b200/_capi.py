@@ -104,6 +104,8 @@ SIGNATURES = {
     "mnnb200_linear_w8_plan": (C.c_int, [P, C.POINTER(C.c_int), C.c_int]),
     "mnnb200_matmul_create": (C.c_int, [P] + [C.c_int] * 7 + [C.POINTER(P)]),
     "mnnb200_matmul_execute": (C.c_int, [P, P, P, P, P]),
+    "mnnb200_matmul_create_broadcast": (C.c_int, [P, C.c_int, C.POINTER(C.c_int), C.POINTER(C.c_int), C.POINTER(C.c_int)] +
+                                        [C.c_int] * 5 + [C.POINTER(P)]),
     "mnnb200_conv_f32_create": (C.c_int, [P, C.POINTER(ConvDesc), P, P, C.c_int, C.POINTER(P)]),
     "mnnb200_conv_f32_create_grouped": (C.c_int, [P, C.POINTER(ConvDesc), P, P, C.c_int, C.POINTER(P)]),
     "mnnb200_conv_f32_set_pad": (C.c_int, [P, C.c_int, C.c_int]),
@@ -148,6 +150,18 @@ INTERP_SIGNATURES = {
     "mnnb200_interp_f32_plan": (C.c_int, [P, C.POINTER(C.c_int), C.c_int]),
 }
 _interp_lib = None
+
+# libmnn_b200_gather.so (include/mnn_b200_gather.h): the gathers and the int32 / fp32 Cast, on the runtime and execution handles above
+GATHER_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_gather.so")
+GATHER_SIGNATURES = {
+    "mnnb200_gather_create": (C.c_int, [P, C.c_int, C.POINTER(P)]),
+    "mnnb200_gather_resize": (C.c_int, [P, C.POINTER(C.c_int), C.c_int, C.POINTER(C.c_int), C.c_int, C.c_int]),
+    "mnnb200_gather_execute": (C.c_int, [P, P, P, P]),
+    "mnnb200_gather_plan": (C.c_int, [P, C.POINTER(C.c_int), C.c_int]),
+    "mnnb200_cast_i32_f32": (C.c_int, [P, P, P, C.c_longlong]),
+    "mnnb200_cast_f32_i32": (C.c_int, [P, P, P, C.c_longlong]),
+}
+_gather_lib = None
 
 # libmnn_b200_llm.so (include/mnn_b200_llm.h): MNN-LLM's LayerNorm / RoPE executions, on the runtime and execution handles above
 LLM_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_llm.so")
@@ -209,6 +223,22 @@ def interp_lib():
             fn.argtypes = args
         _interp_lib = L
     return _interp_lib
+
+
+def gather_lib():
+    """libmnn_b200_gather.so with every GATHER_SIGNATURES symbol resolved (after libmnn_b200.so, whose handles it shares)"""
+    global _gather_lib
+    if _gather_lib is None:
+        lib()
+        if not os.path.exists(GATHER_LIB_PATH):
+            raise MnnB200Error(f"{GATHER_LIB_PATH} is missing: run `python -m mnn_b200.build` (there is no CPU fallback)")
+        L = C.CDLL(GATHER_LIB_PATH)
+        for name, (res, args) in GATHER_SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype = res
+            fn.argtypes = args
+        _gather_lib = L
+    return _gather_lib
 
 
 def lib():

@@ -516,6 +516,39 @@ class InterpF32Execution(Execution):
         return _capi.interp_lib().mnnb200_interp_f32_execute(self._h, inputs[0].ptr(), outputs[0].ptr())
 
 
+class GatherExecution(Execution):
+    """Gather / GatherV2 / GatherND / GatherElements on 4-byte tensors (fp32 or int32) with int32 indices, shapes as given (any
+    rank): the CPU backend's While loops of GeometryGather.cpp.  op.type: "Gather" (GatherV2 alike), "GatherND" or
+    "GatherElements"; op.extra["axis"]: the Gather / GatherElements axis or GatherND's batch dims (default 0).  The output's
+    shape is set at onResize."""
+
+    MODES = {"Gather": 0, "GatherND": 1, "GatherElements": 2}
+
+    def __init__(self, backend, op: Op):
+        super().__init__(backend)
+        self.op = op
+        self.mode = self.MODES[op.type]
+        check(_capi.gather_lib().mnnb200_gather_create(backend.runtime._h, self.mode, C.byref(self._h)), "gather_create")
+
+    def onResize(self, inputs, outputs):
+        p, i = tuple(inputs[0].shape), tuple(inputs[1].shape) or (1,)
+        axis = int(self.op.extra.get("axis", 0))
+        ints = lambda v: (C.c_int * len(v))(*v)   # noqa: E731
+        st = _capi.gather_lib().mnnb200_gather_resize(self._h, ints(p), len(p), ints(i), len(i), axis)
+        if st == 0:
+            if self.mode == 0:
+                a = axis % len(p)
+                outputs[0].shape = p[:a] + tuple(inputs[1].shape) + p[a + 1:]
+            elif self.mode == 1:
+                outputs[0].shape = i[:-1] + p[axis + i[-1]:]
+            else:
+                outputs[0].shape = i
+        return st
+
+    def onExecute(self, inputs, outputs):
+        return _capi.gather_lib().mnnb200_gather_execute(self._h, inputs[0].ptr(), inputs[1].ptr(), outputs[0].ptr())
+
+
 class Backend:
     """CUDABackend's role: creator map, buffer acquisition, host<->device copies with layout + quant casts."""
 
@@ -617,3 +650,5 @@ def _create_deconv_f32(b, i, o, op):
 Backend.addCreator("DeconvF32", _create_deconv_f32)
 Backend.addCreator("DwDeconvF32", lambda b, i, o, op: DeconvF32Execution(b, op, depthwise=True))
 Backend.addCreator("InterpF32", lambda b, i, o, op: InterpF32Execution(b, op))
+for _t in ("Gather", "GatherND", "GatherElements"):
+    Backend.addCreator(_t, lambda b, i, o, op: GatherExecution(b, op))

@@ -1659,8 +1659,11 @@ mnnb200_status mnnb200_conv_int8_wino_plan(mnnb200_exec* ex, int* fields, int co
 // =================================================================================================
 struct MatMulExec : Tagged<kMatMul> {
     int batch = 0, e = 0, l = 0, h = 0, lp = 0, ta = 0, tb = 0, bn = 0;
+    int a_batches = 0, b_batches = 0;      // each operand's own batches (= batch unless broadcast)
     int tf32 = 0, esize = 2;               // tf32: fp32 operands consumed as tf32 (no conversion pass); else fp16 operands
-    DevBuf<uint8_t> d_a, d_b;              // K-major scratch operands [batch][e][lp], [batch][h][lp] (only when a pack is needed)
+    DevBuf<int> d_map;                     // broadcast: [batch][2] A and B batch of each output batch
+    bool broadcast = false;
+    DevBuf<uint8_t> d_a, d_b;              // K-major scratch operands [a_batches][e][lp], [b_batches][h][lp] (only when a pack is needed)
     CUtensorMap tmap_a, tmap_b;
     const void *tmap_a_ptr = nullptr, *tmap_b_ptr = nullptr;
 };
@@ -1671,6 +1674,7 @@ mnnb200_status mnnb200_matmul_create(mnnb200_runtime* rt, int batch, int e, int 
     if (!rt || !out || batch <= 0 || e <= 0 || l <= 0 || h <= 0) return fail(MNNB200_INVALID_VALUE, "matmul_create: bad argument");
     auto m = new_exec<MatMulExec>(rt);
     m->batch = batch; m->e = e; m->l = l; m->h = h; m->ta = transpose_a; m->tb = transpose_b;
+    m->a_batches = m->b_batches = batch;
     // fp32 operands: tf32 wgmma reads them in place (K-major operands need no pass at all)
     m->tf32 = inputs_are_f16 ? 0 : 1;
     m->esize = m->tf32 ? 4 : 2;
@@ -1679,6 +1683,51 @@ mnnb200_status mnnb200_matmul_create(mnnb200_runtime* rt, int batch, int e, int 
     m->bn = pick_bn(up16(h), batch * ((e + 127) / 128), rt->prop.multiProcessorCount);
     m->cost_bytes = (double)batch * ((double)e * l + (double)l * h + (double)e * h) * 4;
     m->cost_macs = (double)batch * e * l * h;
+    *out = m.release();
+    return MNNB200_OK;
+}
+// C's batch dims c[0..nd) and each operand's (1 or c[i] each, the caller pads the shorter operand with leading 1s): an fp32
+// MatMul of prod(c) output batches with a table of each output batch's A and B batch, made here once; no table when neither
+// operand broadcasts, which is then the execution mnnb200_matmul_create makes
+mnnb200_status mnnb200_matmul_create_broadcast(mnnb200_runtime* rt, int nd, const int* c_batch, const int* a_batch,
+                                               const int* b_batch, int e, int l, int h, int transpose_a, int transpose_b,
+                                               mnnb200_exec** out) {
+    if (!rt || !out || nd < 0 || nd > 8 || (nd > 0 && (!c_batch || !a_batch || !b_batch)) || e <= 0 || l <= 0 || h <= 0)
+        return fail(MNNB200_INVALID_VALUE, "matmul_create_broadcast: bad argument");
+    long long batch = 1, na = 1, nb = 1;
+    bool bc = false;
+    for (int i = 0; i < nd; ++i) {
+        if (c_batch[i] <= 0 || (a_batch[i] != 1 && a_batch[i] != c_batch[i]) || (b_batch[i] != 1 && b_batch[i] != c_batch[i]))
+            return fail(MNNB200_INVALID_VALUE, "matmul_create_broadcast: dim " + std::to_string(i) + " does not broadcast");
+        batch *= c_batch[i]; na *= a_batch[i]; nb *= b_batch[i];
+        bc = bc || a_batch[i] != c_batch[i] || b_batch[i] != c_batch[i];
+    }
+    if (batch > 0x7fffffffLL) return fail(MNNB200_INVALID_VALUE, "matmul_create_broadcast: too many batches");
+    mnnb200_exec* made = nullptr;
+    mnnb200_status st = mnnb200_matmul_create(rt, (int)batch, e, l, h, transpose_a, transpose_b, 0, &made);
+    if (st) return st;
+    std::unique_ptr<MatMulExec> m(static_cast<MatMulExec*>(made));
+    if (bc) {
+        std::vector<int> map((size_t)batch * 2);
+        for (long long bt = 0; bt < batch; ++bt) {
+            long long rest = bt, ia = 0, ib = 0, sa = 1, sb = 1;
+            for (int i = nd - 1; i >= 0; --i) {
+                const long long ci = rest % c_batch[i];
+                rest /= c_batch[i];
+                if (a_batch[i] > 1) ia += ci * sa;
+                if (b_batch[i] > 1) ib += ci * sb;
+                sa *= a_batch[i];
+                sb *= b_batch[i];
+            }
+            map[(size_t)bt * 2] = (int)ia;
+            map[(size_t)bt * 2 + 1] = (int)ib;
+        }
+        if ((st = m->d_map.upload(map, rt->stream))) return st;
+        m->broadcast = true;
+        m->a_batches = (int)na;
+        m->b_batches = (int)nb;
+        m->cost_bytes = ((double)na * e * l + (double)nb * l * h + (double)batch * e * h) * 4;
+    }
     *out = m.release();
     return MNNB200_OK;
 }
@@ -1693,34 +1742,34 @@ mnnb200_status mnnb200_matmul_execute(mnnb200_exec* ex, const void* a, const voi
     const size_t row_bytes = (size_t)m->lp * m->esize;
     // packs an operand of `rows` rows per batch K-major into its scratch and points *dst at it.  The scratch is zeroed when
     // first allocated and has one extra tile of rows: the last tile of the last batch reads past the operand.
-    auto pack = [&](DevBuf<uint8_t>& buf, const void* src, int rows, int trans, const void** dst) -> mnnb200_status {
-        const size_t bytes = ((size_t)m->batch * rows + 256) * row_bytes;
+    auto pack = [&](DevBuf<uint8_t>& buf, const void* src, int batches, int rows, int trans, const void** dst) -> mnnb200_status {
+        const size_t bytes = ((size_t)batches * rows + 256) * row_bytes;
         if (!buf) {
             mnnb200_status st = buf.reserve(bytes);
             if (st) return st;
             CK(cudaMemsetAsync(buf, 0, bytes, m->rt->stream));
         }
         void* d = buf;
-        if (m->tf32) CK(launch_pack_kmajor_f32((const float*)src, (float*)d, m->batch, rows, m->l, m->lp, trans, m->rt->stream));
-        else CK(launch_pack_kmajor_f16(src, d, m->batch, rows, m->l, m->lp, trans, m->rt->stream));
+        if (m->tf32) CK(launch_pack_kmajor_f32((const float*)src, (float*)d, batches, rows, m->l, m->lp, trans, m->rt->stream));
+        else CK(launch_pack_kmajor_f16(src, d, batches, rows, m->l, m->lp, trans, m->rt->stream));
         *dst = d;
         return MNNB200_OK;
     };
     mnnb200_status st;
     const void *pa = a, *pb = b;
-    if (!a_direct && (st = pack(m->d_a, a, m->e, m->ta ? 1 : 0, &pa))) return st;
-    if (!b_direct && (st = pack(m->d_b, b, m->h, m->tb ? 0 : 1, &pb))) return st;
+    if (!a_direct && (st = pack(m->d_a, a, m->a_batches, m->e, m->ta ? 1 : 0, &pa))) return st;
+    if (!b_direct && (st = pack(m->d_b, b, m->b_batches, m->h, m->tb ? 0 : 1, &pb))) return st;
     if (m->tmap_a_ptr != pa) {
-        // direct operands are exactly batch*e rows (TMA zero-fills rows past the end); scratch has a padded tail
-        if ((st = make_tmap_i8(&m->tmap_a, pa, m->batch * m->e + (a_direct ? 0 : 128), (int)row_bytes, 128))) return st;
+        // direct operands are exactly a_batches*e rows (TMA zero-fills rows past the end); scratch has a padded tail
+        if ((st = make_tmap_i8(&m->tmap_a, pa, m->a_batches * m->e + (a_direct ? 0 : 128), (int)row_bytes, 128))) return st;
         m->tmap_a_ptr = pa;
     }
     if (m->tmap_b_ptr != pb) {
-        if ((st = make_tmap_i8(&m->tmap_b, pb, m->batch * m->h + (b_direct ? 0 : 256), (int)row_bytes, m->bn))) return st;
+        if ((st = make_tmap_i8(&m->tmap_b, pb, m->b_batches * m->h + (b_direct ? 0 : 256), (int)row_bytes, m->bn))) return st;
         m->tmap_b_ptr = pb;
     }
     CK(launch_gemm_f16_wgmma(&m->tmap_a, &m->tmap_b, m->batch, m->e, m->h, (int)row_bytes, m->tf32, m->e, m->h, m->bn, c, bias,
-                               m->rt->stream, m->rt->prop.multiProcessorCount));
+                               m->rt->stream, m->rt->prop.multiProcessorCount, m->broadcast ? (const int*)m->d_map : nullptr));
     return MNNB200_OK;
 }
 }  // extern "C"

@@ -27,6 +27,7 @@ struct FParams {
     int M, N, K;           // K in BYTES of one operand row (multiple of 16)
     int bn, n_chunks, m_tiles, batch;
     int a_batch_rows, b_batch_rows;
+    const int* batch_map;  // [batch][2]: the A and B batch of each output batch (broadcast), or nullptr: both are the output's
     float* c;              // [batch][M][N]
     const float* bias;     // [N] or nullptr
     int stages;
@@ -61,7 +62,8 @@ gemm_f16_wgmma_kernel(const __grid_constant__ CUtensorMap tmap_a, const __grid_c
             int stage = 0, phase = 0;
             for (int w = blockIdx.x; w < work_total; w += gridDim.x) {
                 const int nc = w % p.n_chunks, wq = w / p.n_chunks, mt = wq % p.m_tiles, bt = wq / p.m_tiles;
-                const int a_row = bt * p.a_batch_rows + mt * kBM, b_row = bt * p.b_batch_rows + nc * p.bn;
+                const int ab = p.batch_map ? p.batch_map[2 * bt] : bt, bb = p.batch_map ? p.batch_map[2 * bt + 1] : bt;
+                const int a_row = ab * p.a_batch_rows + mt * kBM, b_row = bb * p.b_batch_rows + nc * p.bn;
                 for (int kb = 0; kb < num_kb; ++kb) {
                     mbar_wait(empty_bar(stage), phase ^ 1);
                     mbar_expect_tx(full_bar(stage), (uint32_t)stage_bytes);
@@ -208,11 +210,11 @@ cudaError_t launch_pack_kmajor_f16(const void* src, void* dst, int batch, int ro
 
 cudaError_t launch_gemm_f16_wgmma(const void* tmap_a, const void* tmap_b, int batch, int M, int N, int k_bytes, int tf32,
                                   int a_batch_rows, int b_batch_rows, int bn, float* c, const float* bias, cudaStream_t stream,
-                                  int sm_count) {
+                                  int sm_count, const int* batch_map) {
     if (bn < 16 || bn > kMaxBN || (bn & 15)) return cudaErrorInvalidValue;
     FParams p;
     p.M = M; p.N = N; p.K = k_bytes; p.bn = bn; p.n_chunks = (N + bn - 1) / bn; p.m_tiles = (M + kBM - 1) / kBM; p.batch = batch;
-    p.a_batch_rows = a_batch_rows; p.b_batch_rows = b_batch_rows; p.c = c; p.bias = bias;
+    p.a_batch_rows = a_batch_rows; p.b_batch_rows = b_batch_rows; p.batch_map = batch_map; p.c = c; p.bias = bias;
     const int stage_bytes = kBM * kBK + bn * kBK;
     int st = (227 * 1024 - 256 - 1024) / stage_bytes;
     p.stages = st > kMaxStages ? kMaxStages : st;

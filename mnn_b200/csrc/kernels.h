@@ -148,10 +148,12 @@ GemmI8Launch gemm_i8_2cta_launch(const GemmI8Params& p, int bn, int sm_count);
 // own type (fp16 or fp32)
 cudaError_t launch_pack_kmajor_f16(const void* src, void* dst, int batch, int rows, int k, int kp, int trans, cudaStream_t s);
 cudaError_t launch_pack_kmajor_f32(const float* src, float* dst, int batch, int rows, int k, int kp, int trans, cudaStream_t s);
-// k_bytes = bytes of one K-major operand row; tf32 = 1: operands are fp32 consumed as tf32, else fp16
+// k_bytes = bytes of one K-major operand row; tf32 = 1: operands are fp32 consumed as tf32, else fp16.  Output batch bt reads
+// A's rows from bt * a_batch_rows and B's from bt * b_batch_rows, or, with a batch_map (device, [batch][2]), from
+// batch_map[2 bt] * a_batch_rows and batch_map[2 bt + 1] * b_batch_rows (broadcast batches)
 cudaError_t launch_gemm_f16_wgmma(const void* tmap_a, const void* tmap_b, int batch, int M, int N, int k_bytes, int tf32,
                                   int a_batch_rows, int b_batch_rows, int bn, float* c, const float* bias, cudaStream_t stream,
-                                  int sm_count);
+                                  int sm_count, const int* batch_map = nullptr);
 
 // fp32 Conv2D (any group) on split-TF32 wgmma (conv_f32_wgmma.cu): NCHW-linear fp32 in and out.  Weights are packed once into two
 // K-major arrays hi / lo [ocp][kp] (k = tap * cp8 + c, cp8 = an n chunk's input channels rounded up to 8, kp = taps * cp8 rounded

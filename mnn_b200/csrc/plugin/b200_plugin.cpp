@@ -39,6 +39,7 @@
 #include "core/TensorUtils.hpp"
 
 #include "../../../include/mnn_b200_deconv.h"
+#include "../../../include/mnn_b200_gather.h"
 #include "../../../include/mnn_b200_interp.h"
 #include "../../../include/mnn_b200_llm.h"
 
@@ -683,25 +684,39 @@ private:
     DeviceScratch mX, mY;   // token-major input and output when H*W > 1
 };
 
-// MatMul on float tensors (MatMulExecution.cu's role): C[e,h] = op(A) op(B) (+ bias input)
+// MatMul and BatchMatMul on float tensors (MatMulExecution.cu's role): C = op(A) op(B) (+ bias input), over the batch dims
+// ShapeMatMul broadcasts (right-aligned, a dim of 1 against any) and with its squeeze of a 1-D operand: A of [l] is one row
+// (transposeA ignored), B of [l] one column (transposeB ignored).  Under Compiler_Geometry the geometry stage hands every
+// MatMul / BatchMatMul over unlowered (GeometryBatchMatMul is registered for Compiler_Loop only).
 class MatMulExec : public B200Exec {
 public:
     MatMulExec(Backend* bn, bool ta, bool tb) : B200Exec(bn), mTa(ta), mTb(tb) {}
     ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
         auto a = inputs[0], b = inputs[1];
         const int na = a->dimensions(), nb = b->dimensions();
-        if (na < 2 || nb < 2) return NOT_SUPPORT;
-        int batch = 1;
-        for (int i = 0; i < na - 2; ++i) batch *= a->length(i);
-        int bb = 1;
-        for (int i = 0; i < nb - 2; ++i) bb *= b->length(i);
-        if (bb != batch) return NOT_SUPPORT;
-        const int e = mTa ? a->length(na - 1) : a->length(na - 2), l = mTa ? a->length(na - 2) : a->length(na - 1);
-        const int h = mTb ? b->length(nb - 2) : b->length(nb - 1), l2 = mTb ? b->length(nb - 1) : b->length(nb - 2);
+        if (na < 1 || nb < 1) return NOT_SUPPORT;
+        const bool ta = na > 1 && mTa, tb = nb == 1 || mTb;   // B of [l] is K-major [h = 1][l]
+        const int e = na == 1 ? 1 : (ta ? a->length(na - 1) : a->length(na - 2));
+        const int l = na == 1 ? a->length(0) : (ta ? a->length(na - 2) : a->length(na - 1));
+        const int h = nb == 1 ? 1 : (tb ? b->length(nb - 2) : b->length(nb - 1));
+        const int l2 = nb == 1 ? b->length(0) : (tb ? b->length(nb - 1) : b->length(nb - 2));
         if (l != l2) return COMPUTE_SIZE_ERROR;
+        const int ba = std::max(na - 2, 0), bb = std::max(nb - 2, 0), nd = std::max(ba, bb);
+        if (nd > 8) return NOT_SUPPORT;
+        int cd[8], ad[8], bd[8];
+        size_t batch = 1;
+        for (int i = 0; i < nd; ++i) {
+            const int ia = i - (nd - ba), ib = i - (nd - bb);
+            ad[i] = ia >= 0 ? a->length(ia) : 1;
+            bd[i] = ib >= 0 ? b->length(ib) : 1;
+            if (ad[i] != bd[i] && ad[i] != 1 && bd[i] != 1) return NOT_SUPPORT;
+            cd[i] = ad[i] == 1 ? bd[i] : ad[i];
+            batch *= (size_t)cd[i];
+        }
+        if (batch * (size_t)e * (size_t)h != elemCount(outputs[0])) return NOT_SUPPORT;
         mH.reset();
         mnnb200_exec* m = nullptr;
-        const mnnb200_status st = mnnb200_matmul_create(rt(), batch, e, l, h, mTa, mTb, 0, &m);
+        const mnnb200_status st = mnnb200_matmul_create_broadcast(rt(), nd, cd, ad, bd, e, l, h, ta, tb, &m);
         mH.reset(m);
         return toErr(st, "matmul create");
     }
@@ -1344,6 +1359,96 @@ private:
     ExecHandle mH;
 };
 
+// Gather / GatherV2 / GatherND / GatherElements (the CPU runs them as While loops of GeometryGather.cpp; under Compiler_Geometry
+// they reach the backend unlowered) on tensors of 4-byte elements, fp32 or int32, with int32 indices.  Params and output are
+// linear in their logical dim order: any format but NC4HW4, which only a 4-D tensor may have (it is stored NCHW-linear here).
+// The axis is read as the geometry reads it: Gather from the op's Axis, else its third input, else 0; GatherND's batch dims
+// from the op's Axis; GatherElements' axis from its third input, else 0.  A third input must be a constant (read at resize).
+class GatherExec : public ClonedFromOp<GatherExec> {
+public:
+    GatherExec(Backend* bn, const Op* op, mnnb200_exec* h) : ClonedFromOp(bn), mOp(op), mH(h) {}
+    static int mode(const Op* op) {
+        return op->type() == OpType_GatherND ? 1 : (op->type() == OpType_GatherElements ? 2 : 0);
+    }
+    static Execution* create(B200Backend* bn, const Op* op) {
+        mnnb200_exec* h = nullptr;
+        if (mnnb200_gather_create(bn->handle(), mode(op), &h) != MNNB200_OK) return nullptr;
+        return new GatherExec(bn, op, h);
+    }
+    static bool word(const Tensor* t) {
+        const auto f = TensorUtils::getDescribe(t)->dimensionFormat;
+        return t->getType().bytes() == 4 && !isInt8(t) && (f != MNN_DATA_FORMAT_NC4HW4 || t->dimensions() == 4);
+    }
+    static bool takes(const Op* op, const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) {
+        const size_t most = op->type() == OpType_GatherND ? 2 : 3;
+        if (inputs.size() < 2 || inputs.size() > most || outputs.size() != 1) return false;
+        auto x = inputs[0], idx = inputs[1], y = outputs[0];
+        const bool i32 = idx->getType().code == halide_type_int && idx->getType().bits == 32 && !isInt8(idx);
+        bool ok = i32 && word(x) && word(y) && x->getType() == y->getType() && linearFormat(x) == linearFormat(y) &&
+                  x->dimensions() >= 1;
+        if (inputs.size() == 3) {
+            auto ax = inputs[2];
+            ok = ok && ax->getType().code == halide_type_int && ax->getType().bits == 32 && elemCount(ax) >= 1 &&
+                 (ax->host<int>() != nullptr || TensorUtils::getDescribe(ax)->usage == Tensor::InsideDescribe::CONSTANT);
+        }
+        return ok;
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto x = inputs[0], idx = inputs[1];
+        const int m = mode(mOp);
+        int axis = 0;
+        if (m == 1) {
+            if (mOp->main_as_Axis()) axis = mOp->main_as_Axis()->axis();
+        } else {
+            if (inputs.size() == 3) {
+                auto ax = inputs[2];
+                if (ax->host<int>()) axis = ax->host<int>()[0];
+                else if (mnnb200_memcpy_d2h(rt(), &axis, dev(ax), sizeof(int)) != MNNB200_OK || mnnb200_runtime_sync(rt()) != MNNB200_OK)
+                    return toErr(MNNB200_CUDA_ERROR, "Gather axis read");
+            }
+            if (m == 0 && mOp->main_type() == OpParameter_Axis && mOp->main_as_Axis()) axis = mOp->main_as_Axis()->axis();
+        }
+        std::vector<int> pd(x->dimensions()), id(std::max(idx->dimensions(), 1));
+        for (int i = 0; i < x->dimensions(); ++i) pd[i] = x->length(i);
+        if (m == 0) id = {(int)elemCount(idx)};   // Gather reads the indices flat; a scalar index is one
+        else for (int i = 0; i < idx->dimensions(); ++i) id[i] = idx->length(i);
+        if (m != 0 && idx->dimensions() == 0) id[0] = 1;
+        return toErr(mnnb200_gather_resize(mH.get(), pd.data(), (int)pd.size(), id.data(), (int)id.size(), axis), "gather resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        return toErr(mnnb200_gather_execute(mH.get(), dev(inputs[0]), (const int*)dev(inputs[1]), dev(outputs[0])), "gather");
+    }
+private:
+    const Op* mOp;
+    ExecHandle mH;
+};
+
+// Cast between int32 and fp32 (CPUCast's CastDataType): an attention mask's int32 -> fp32, or fp32 -> int32 (truncation)
+class CastExec : public B200Exec {
+public:
+    CastExec(Backend* bn, bool toFloat) : B200Exec(bn), mToFloat(toFloat) {}
+    static int direction(const Op* op, const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) {
+        auto cp = op->main_as_CastParam();
+        if (!cp || inputs.size() != 1 || outputs.size() != 1 || isInt8(inputs[0]) || isInt8(outputs[0]) ||
+            elemCount(inputs[0]) != elemCount(outputs[0]) || !sameLinear(inputs[0], outputs[0]))
+            return -1;
+        const auto it = inputs[0]->getType(), ot = outputs[0]->getType();
+        const bool iI32 = it.code == halide_type_int && it.bits == 32, iF32 = it.code == halide_type_float && it.bits == 32;
+        const bool oI32 = ot.code == halide_type_int && ot.bits == 32, oF32 = ot.code == halide_type_float && ot.bits == 32;
+        const auto dst = cp->dstT();
+        if (dst == DataType_DT_FLOAT && iI32 && oF32) return 1;
+        if ((dst == DataType_DT_INT32 || dst == DataType_DT_INT64) && iF32 && oI32) return 0;
+        return -1;
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        const long long n = (long long)elemCount(inputs[0]);
+        if (mToFloat) return toErr(mnnb200_cast_i32_f32(rt(), (const int*)dev(inputs[0]), (float*)dev(outputs[0]), n), "Cast i32 -> f32");
+        return toErr(mnnb200_cast_f32_i32(rt(), (const float*)dev(inputs[0]), (int*)dev(outputs[0]), n), "Cast f32 -> i32");
+    }
+private:
+    bool mToFloat;
+};
+
 Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs, const MNN::Op* op) {
     Execution* e = nullptr;
     const bool quantOut = !outputs.empty() && TensorUtils::getDescribe(outputs[0])->quantAttr.get() != nullptr &&
@@ -1368,6 +1473,22 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
                 inputs[0]->getType().bytes() == 4 && linearFormat(inputs[0]) == MNN_DATA_FORMAT_NCHW)
                 e = new MatMulExec(this, op->main_as_MatMul()->transposeA(), op->main_as_MatMul()->transposeB());
             break;
+        case OpType_BatchMatMul:
+            if (!quantOut && inputs.size() == 2 && op->main_as_BatchMatMulParam() && isF32(inputs[0]) && isF32(inputs[1]) &&
+                linearFormat(inputs[0]) == MNN_DATA_FORMAT_NCHW)
+                e = new MatMulExec(this, op->main_as_BatchMatMulParam()->adjX(), op->main_as_BatchMatMulParam()->adjY());
+            break;
+        case OpType_Gather:
+        case OpType_GatherV2:
+        case OpType_GatherND:
+        case OpType_GatherElements:
+            if (!quantOut && GatherExec::takes(op, inputs, outputs)) e = GatherExec::create(this, op);
+            break;
+        case OpType_Cast: {
+            const int dir = quantOut ? -1 : CastExec::direction(op, inputs, outputs);
+            if (dir >= 0) e = new CastExec(this, dir == 1);
+            break;
+        }
         case OpType_ConvolutionDepthwise:
         case OpType_DepthwiseConvInt8:
             if (quantOut || op->type() == OpType_DepthwiseConvInt8) e = ConvInt8Exec::create(this, op);

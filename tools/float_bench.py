@@ -32,7 +32,11 @@ MODELS = {   # --model: (fixture under oracle/_ref, name in the JSON line)
     "mbv1": ("mbv1_f32.mnn", "MobileNet-v1 fp32 (seeded weights)"),
     "resnext50": ("resnext50_f32.mnn", "ResNeXt-50 32x4d fp32 (seeded weights, oracle/refdump_gconv.cpp)"),
     "deeplab": ("deeplab_f32.mnn", "DeepLab-v3-style segmentation fp32, 128x128 (seeded weights, oracle/refdump_interp.cpp)"),
+    "bert": ("bert_f32.mnn", "BERT-style encoder fp32, 4 layers, D 256, S 64, int32 ids and mask (seeded weights, oracle/refdump_gather.cpp)"),
+    "vit": ("vit_f32.mnn", "ViT-style encoder fp32, 4 layers, D 192, 64x64 image (seeded weights, oracle/refdump_gather.cpp)"),
 }
+# models whose inputs refdump's bench does not fill (int32 token ids and masks): timed by oracle/refdump_gather's bench instead
+GATHER_HARNESS = {"bert", "vit"}
 
 
 def shapes_from_cpu_run(model, refdump, env):
@@ -148,11 +152,15 @@ def main():
     res = dict(model=title, batch=a.batch, card=card)
     if a.model == "mbv2":
         res.update(time_convs(shapes_from_cpu_run(model, O.REFDUMP, env), a.batch, a.iters))
+    harness = O.REFDUMP
+    if a.model in GATHER_HARNESS:
+        from oracle import gather_oracle
+        harness = gather_oracle.REFDUMP_GATHER
     penv = dict(env, REFDUMP_BENCH_WINDOWS="5", REFDUMP_PLUGIN=os.path.join(ROOT, "mnn_b200", "libmnn_b200_plugin.so"))
-    p = refdump_bench(O.REFDUMP, model, a.batch, 4, penv, 20)
+    p = refdump_bench(harness, model, a.batch, 4, penv, 20)
     res.update(plugin_e2e_img_per_s=p["img_per_s"], plugin_e2e_ms=p["ms_median_window"], plugin_created=p["plugin_created"],
                plugin_declined=p["plugin_declined"])
-    c = refdump_bench(O.REFDUMP, model, a.batch, a.cpu_threads, dict(env, REFDUMP_BENCH_WINDOWS="1"), 2)
+    c = refdump_bench(harness, model, a.batch, a.cpu_threads, dict(env, REFDUMP_BENCH_WINDOWS="1"), 2)
     res.update(cpu_img_per_s=c["img_per_s"], cpu_threads=a.cpu_threads)
     print(json.dumps(res))
 
