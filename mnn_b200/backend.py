@@ -402,8 +402,11 @@ class LinearW8Execution(Execution):
 
 
 class MatMulExecution(Execution):
-    """MatMul / BatchMatMul on float tensors (MatMulExecution.cu's role): inputs [b, e, l] x [b, l, h] (after the op's
-    transposeA / transposeB), output [b, e, h] fp32.  op.extra: transpose_a, transpose_b."""
+    """MatMul / BatchMatMul on float tensors (MatMulExecution.cu's role): C = op(A) op(B) (+ bias) over the batch dims
+    ShapeMatMul broadcasts (right-aligned, a dim of 1 against any size), with its squeeze of a 1-D operand: A of [l] is one
+    row, B of [l] one column (their transpose flags ignored), and the output drops that dim.  fp32 operands run through
+    mnnb200_matmul_create_broadcast; fp16 operands (the f16 kernel) through mnnb200_matmul_create, without broadcast.
+    op.extra: transpose_a, transpose_b."""
 
     def __init__(self, backend, op: Op):
         super().__init__(backend)
@@ -412,19 +415,39 @@ class MatMulExecution(Execution):
 
     def onResize(self, inputs, outputs):
         a, b = inputs[0], inputs[1]
-        sa, sb = a.shape, b.shape
-        batch = int(np.prod(sa[:-2])) if len(sa) > 2 else 1
-        e, l = (sa[-1], sa[-2]) if self.ta else (sa[-2], sa[-1])
-        h, l2 = (sb[-2], sb[-1]) if self.tb else (sb[-1], sb[-2])
-        if l != l2 or (len(sb) > 2 and int(np.prod(sb[:-2])) != batch):
+        sa, sb = tuple(int(v) for v in a.shape), tuple(int(v) for v in b.shape)
+        if len(sa) < 1 or len(sb) < 1:
+            return NOT_SUPPORT
+        ta, tb = int(len(sa) > 1 and self.ta), int(len(sb) == 1 or self.tb)   # B of [l] is K-major [h = 1][l]
+        e, l = (1, sa[0]) if len(sa) == 1 else (sa[-1], sa[-2]) if ta else (sa[-2], sa[-1])
+        h, l2 = (1, sb[0]) if len(sb) == 1 else (sb[-2], sb[-1]) if tb else (sb[-1], sb[-2])
+        if l != l2:
             return COMPUTE_SIZE_ERROR
+        nd = max(len(sa), len(sb), 2) - 2
+        if nd > 8:
+            return NOT_SUPPORT
+        ad = (1,) * (nd - max(len(sa) - 2, 0)) + sa[:-2]
+        bd = (1,) * (nd - max(len(sb) - 2, 0)) + sb[:-2]
+        if any(x != y and x != 1 and y != 1 for x, y in zip(ad, bd)):
+            return NOT_SUPPORT
+        cd = tuple(y if x == 1 else x for x, y in zip(ad, bd))
+        f16 = a.data is not None and a.data.dtype == torch.float16
+        if f16 and ad != bd:
+            return NOT_SUPPORT
         if self._h:
             _capi.lib().mnnb200_exec_destroy(self._h)
             self._h = C.c_void_p()
-        st = _capi.lib().mnnb200_matmul_create(self.backend.runtime._h, batch, e, l, h, self.ta, self.tb,
-                                               int(a.data is not None and a.data.dtype == torch.float16), C.byref(self._h))
+        L = _capi.lib()
+        if f16:
+            st = L.mnnb200_matmul_create(self.backend.runtime._h, int(np.prod(cd, dtype=np.int64)), e, l, h, ta, tb, 1,
+                                         C.byref(self._h))
+        else:
+            def arr(v):
+                return (C.c_int * max(len(v), 1))(*v)
+            st = L.mnnb200_matmul_create_broadcast(self.backend.runtime._h, nd, arr(cd), arr(ad), arr(bd), e, l, h, ta, tb,
+                                                   C.byref(self._h))
         if st == 0:
-            outputs[0].shape = tuple(sa[:-2]) + (e, h)
+            outputs[0].shape = cd + ((e,) if len(sa) > 1 else ()) + ((h,) if len(sb) > 1 else ()) or (1,)
         return st
 
     def onExecute(self, inputs, outputs):

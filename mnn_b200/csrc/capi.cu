@@ -1660,27 +1660,38 @@ mnnb200_status mnnb200_conv_int8_wino_plan(mnnb200_exec* ex, int* fields, int co
 struct MatMulExec : Tagged<kMatMul> {
     int batch = 0, e = 0, l = 0, h = 0, lp = 0, ta = 0, tb = 0, bn = 0;
     int a_batches = 0, b_batches = 0;      // each operand's own batches (= batch unless broadcast)
-    int tf32 = 0, esize = 2;               // tf32: fp32 operands consumed as tf32 (no conversion pass); else fp16 operands
+    int split = 0, esize = 2;              // split: fp32 operands packed as TF32 hi / lo planes; else fp16 operands
     DevBuf<int> d_map;                     // broadcast: [batch][2] A and B batch of each output batch
     bool broadcast = false;
-    DevBuf<uint8_t> d_a, d_b;              // K-major scratch operands [a_batches][e][lp], [b_batches][h][lp] (only when a pack is needed)
-    CUtensorMap tmap_a, tmap_b;
-    const void *tmap_a_ptr = nullptr, *tmap_b_ptr = nullptr;
+    DevBuf<uint8_t> d_a, d_b;              // K-major scratch operands: per plane [a_batches * e + pad][lp], [b_batches * h + pad][lp]
+    CUtensorMap tmap_a, tmap_b;            // over the scratch, both planes; made with it at the first execute
 };
+// rows past an operand's last batch in each scratch plane: a 128-row tile (A) or an n chunk (B) that starts in the last batch
+// reads up to a tile past it
+constexpr int kMatMulPadA = 128, kMatMulPadB = 256;
 
 extern "C" {
 mnnb200_status mnnb200_matmul_create(mnnb200_runtime* rt, int batch, int e, int l, int h, int transpose_a, int transpose_b,
                                      int inputs_are_f16, mnnb200_exec** out) {
     if (!rt || !out || batch <= 0 || e <= 0 || l <= 0 || h <= 0) return fail(MNNB200_INVALID_VALUE, "matmul_create: bad argument");
+    const int split = inputs_are_f16 ? 0 : 1, esize = split ? 4 : 2, kalign = 16 / esize;
+    const long long lp = ((long long)l + kalign - 1) / kalign * kalign;
+    // the tensor maps' row coordinates (both planes of an operand), the row bytes and the kernel's work index are 32-bit
+    const long long planes = split ? 2 : 1, m_tiles = (e + 127LL) / 128;
+    if (lp * esize > 0x7fffffffLL || planes * ((long long)batch * e + kMatMulPadA) > 0x7fffffffLL ||
+        planes * ((long long)batch * h + kMatMulPadB) > 0x7fffffffLL)
+        return fail(MNNB200_NOT_SUPPORT, "matmul_create: operands beyond the kernel's 32-bit row and byte indices");
+    const int bn = pick_bn(up16(h), (int)std::min(batch * m_tiles, 1LL << 30), rt->prop.multiProcessorCount,
+                           gemm_f16_wgmma_max_bn(split));
+    if ((long long)batch * m_tiles * ((h + bn - 1) / bn) > 0x7fffffffLL)
+        return fail(MNNB200_NOT_SUPPORT, "matmul_create: 2^31 or more work items");
     auto m = new_exec<MatMulExec>(rt);
     m->batch = batch; m->e = e; m->l = l; m->h = h; m->ta = transpose_a; m->tb = transpose_b;
     m->a_batches = m->b_batches = batch;
-    // fp32 operands: tf32 wgmma reads them in place (K-major operands need no pass at all)
-    m->tf32 = inputs_are_f16 ? 0 : 1;
-    m->esize = m->tf32 ? 4 : 2;
-    const int kalign = 16 / m->esize;
-    m->lp = (l + kalign - 1) / kalign * kalign;
-    m->bn = pick_bn(up16(h), batch * ((e + 127) / 128), rt->prop.multiProcessorCount);
+    m->split = split;
+    m->esize = esize;
+    m->lp = (int)lp;
+    m->bn = bn;
     m->cost_bytes = (double)batch * ((double)e * l + (double)l * h + (double)e * h) * 4;
     m->cost_macs = (double)batch * e * l * h;
     *out = m.release();
@@ -1701,8 +1712,9 @@ mnnb200_status mnnb200_matmul_create_broadcast(mnnb200_runtime* rt, int nd, cons
             return fail(MNNB200_INVALID_VALUE, "matmul_create_broadcast: dim " + std::to_string(i) + " does not broadcast");
         batch *= c_batch[i]; na *= a_batch[i]; nb *= b_batch[i];
         bc = bc || a_batch[i] != c_batch[i] || b_batch[i] != c_batch[i];
+        if (batch > 0x7fffffffLL) return fail(MNNB200_INVALID_VALUE, "matmul_create_broadcast: too many batches");
     }
-    if (batch > 0x7fffffffLL) return fail(MNNB200_INVALID_VALUE, "matmul_create_broadcast: too many batches");
+    // the operands have at most batch batches each: mnnb200_matmul_create's limits cover them
     mnnb200_exec* made = nullptr;
     mnnb200_status st = mnnb200_matmul_create(rt, (int)batch, e, l, h, transpose_a, transpose_b, 0, &made);
     if (st) return st;
@@ -1736,40 +1748,33 @@ mnnb200_status mnnb200_matmul_execute(mnnb200_exec* ex, const void* a, const voi
     if (!m) return fail(MNNB200_INVALID_VALUE, "matmul_execute: not a matmul execution");
     // A logical [e][l]: memory [e][l] (ta = 0) or [l][e] (ta = 1).  B logical [l][h]; the kernel wants B^T = [h][l]:
     // memory [l][h] (tb = 0) is the transposed form, memory [h][l] (tb = 1) is already K-major.
-    const bool aligned = m->lp == m->l;
-    const bool a_direct = m->tf32 && !m->ta && aligned && ((uintptr_t)a & 15) == 0;
-    const bool b_direct = m->tf32 && m->tb && aligned && ((uintptr_t)b & 15) == 0;
     const size_t row_bytes = (size_t)m->lp * m->esize;
-    // packs an operand of `rows` rows per batch K-major into its scratch and points *dst at it.  The scratch is zeroed when
-    // first allocated and has one extra tile of rows: the last tile of the last batch reads past the operand.
-    auto pack = [&](DevBuf<uint8_t>& buf, const void* src, int batches, int rows, int trans, const void** dst) -> mnnb200_status {
-        const size_t bytes = ((size_t)batches * rows + 256) * row_bytes;
+    const int planes = m->split ? 2 : 1;
+    const int a_plane = m->a_batches * m->e + kMatMulPadA, b_plane = m->b_batches * m->h + kMatMulPadB;
+    // packs an operand of `rows` rows per batch K-major into its scratch (split: hi plane, then lo plane).  The scratch, and
+    // its tensor map, are made at the first execute; the scratch is zeroed then, so the pad rows read as zeros.
+    auto pack = [&](DevBuf<uint8_t>& buf, CUtensorMap* tmap, const void* src, int batches, int rows, int plane_rows, int trans,
+                    int box_rows) -> mnnb200_status {
         if (!buf) {
+            const size_t bytes = (size_t)planes * plane_rows * row_bytes;
             mnnb200_status st = buf.reserve(bytes);
             if (st) return st;
             CK(cudaMemsetAsync(buf, 0, bytes, m->rt->stream));
+            if ((st = make_tmap_i8(tmap, buf, planes * plane_rows, (int)row_bytes, box_rows))) return st;
         }
         void* d = buf;
-        if (m->tf32) CK(launch_pack_kmajor_f32((const float*)src, (float*)d, batches, rows, m->l, m->lp, trans, m->rt->stream));
+        if (m->split)
+            CK(launch_pack_split_tf32((const float*)src, (float*)d, (size_t)plane_rows * m->lp, batches, rows, m->l, m->lp, trans,
+                                      m->rt->stream));
         else CK(launch_pack_kmajor_f16(src, d, batches, rows, m->l, m->lp, trans, m->rt->stream));
-        *dst = d;
         return MNNB200_OK;
     };
     mnnb200_status st;
-    const void *pa = a, *pb = b;
-    if (!a_direct && (st = pack(m->d_a, a, m->a_batches, m->e, m->ta ? 1 : 0, &pa))) return st;
-    if (!b_direct && (st = pack(m->d_b, b, m->b_batches, m->h, m->tb ? 0 : 1, &pb))) return st;
-    if (m->tmap_a_ptr != pa) {
-        // direct operands are exactly a_batches*e rows (TMA zero-fills rows past the end); scratch has a padded tail
-        if ((st = make_tmap_i8(&m->tmap_a, pa, m->a_batches * m->e + (a_direct ? 0 : 128), (int)row_bytes, 128))) return st;
-        m->tmap_a_ptr = pa;
-    }
-    if (m->tmap_b_ptr != pb) {
-        if ((st = make_tmap_i8(&m->tmap_b, pb, m->b_batches * m->h + (b_direct ? 0 : 256), (int)row_bytes, m->bn))) return st;
-        m->tmap_b_ptr = pb;
-    }
-    CK(launch_gemm_f16_wgmma(&m->tmap_a, &m->tmap_b, m->batch, m->e, m->h, (int)row_bytes, m->tf32, m->e, m->h, m->bn, c, bias,
-                               m->rt->stream, m->rt->prop.multiProcessorCount, m->broadcast ? (const int*)m->d_map : nullptr));
+    if ((st = pack(m->d_a, &m->tmap_a, a, m->a_batches, m->e, a_plane, m->ta ? 1 : 0, 128))) return st;
+    if ((st = pack(m->d_b, &m->tmap_b, b, m->b_batches, m->h, b_plane, m->tb ? 0 : 1, m->bn))) return st;
+    CK(launch_gemm_f16_wgmma(&m->tmap_a, &m->tmap_b, m->batch, m->e, m->h, (int)row_bytes, m->split, m->e, m->h,
+                               m->split ? a_plane : 0, m->split ? b_plane : 0, m->bn, c, bias, m->rt->stream,
+                               m->rt->prop.multiProcessorCount, m->broadcast ? (const int*)m->d_map : nullptr));
     return MNNB200_OK;
 }
 }  // extern "C"

@@ -144,16 +144,23 @@ cudaError_t launch_gemm_i8_2cta(const GemmI8Params& p, const void* tmap_a, const
 // (at most sm_count / 2 pairs); one_tile and resident_b are 0, the pair kernel has neither mode
 GemmI8Launch gemm_i8_2cta_launch(const GemmI8Params& p, int bn, int sm_count);
 
-// float (batched) MatMul on wgmma f16 / tf32 (gemm_f16_wgmma.cu): an operand that is not K-major already is packed first, in its
-// own type (fp16 or fp32)
+// float (batched) MatMul on wgmma (gemm_f16_wgmma.cu).  Both operands are packed K-major first ([batch][rows][kp], zero padded
+// along k; trans = 1: the source is [batch][k][rows]), for any batch and row count: fp16 operands into fp16; fp32 operands
+// split into two TF32 planes, x = hi + lo (split_tf32), the hi plane at dst and the lo plane lo_off floats further.
 cudaError_t launch_pack_kmajor_f16(const void* src, void* dst, int batch, int rows, int k, int kp, int trans, cudaStream_t s);
-cudaError_t launch_pack_kmajor_f32(const float* src, float* dst, int batch, int rows, int k, int kp, int trans, cudaStream_t s);
-// k_bytes = bytes of one K-major operand row; tf32 = 1: operands are fp32 consumed as tf32, else fp16.  Output batch bt reads
-// A's rows from bt * a_batch_rows and B's from bt * b_batch_rows, or, with a batch_map (device, [batch][2]), from
-// batch_map[2 bt] * a_batch_rows and batch_map[2 bt + 1] * b_batch_rows (broadcast batches)
-cudaError_t launch_gemm_f16_wgmma(const void* tmap_a, const void* tmap_b, int batch, int M, int N, int k_bytes, int tf32,
-                                  int a_batch_rows, int b_batch_rows, int bn, float* c, const float* bias, cudaStream_t stream,
-                                  int sm_count, const int* batch_map = nullptr);
+cudaError_t launch_pack_split_tf32(const float* src, float* dst, size_t lo_off, int batch, int rows, int k, int kp, int trans,
+                                   cudaStream_t s);
+// the widest n chunk (bn) the kernel takes: 256 columns for fp16, 128 for the split kernel (whose stage holds four tiles)
+int gemm_f16_wgmma_max_bn(int split);
+// k_bytes = bytes of one K-major operand row; split = 1: the operands are fp32 hi / lo planes and C = a_hi*b_hi + a_hi*b_lo +
+// a_lo*b_hi (fp32 accumulate), the lo plane a_lo_row / b_lo_row rows after the hi plane in each tensor map; split = 0: fp16
+// operands.  Output batch bt reads A's rows from bt * a_batch_rows and B's from bt * b_batch_rows, or, with a batch_map (device,
+// [batch][2]), from batch_map[2 bt] * a_batch_rows and batch_map[2 bt + 1] * b_batch_rows (broadcast batches).  c needs only
+// 4-byte alignment (column pairs are stored as float2 when N is even and c 8-byte aligned).  batch * m_tiles * n_chunks must be
+// below 2^31 (cudaErrorInvalidValue otherwise).
+cudaError_t launch_gemm_f16_wgmma(const void* tmap_a, const void* tmap_b, int batch, int M, int N, int k_bytes, int split,
+                                  int a_batch_rows, int b_batch_rows, int a_lo_row, int b_lo_row, int bn, float* c,
+                                  const float* bias, cudaStream_t stream, int sm_count, const int* batch_map = nullptr);
 
 // fp32 Conv2D (any group) on split-TF32 wgmma (conv_f32_wgmma.cu): NCHW-linear fp32 in and out.  Weights are packed once into two
 // K-major arrays hi / lo [ocp][kp] (k = tap * cp8 + c, cp8 = an n chunk's input channels rounded up to 8, kp = taps * cp8 rounded

@@ -1,5 +1,6 @@
-// split_tf32.cuh -- what the split-TF32 wgmma kernels (conv_f32_wgmma.cu, deconv_f32_wgmma.cu) share: the 128-row tile and its
-// stage layout, the TF32 rounding, the 4-byte cp.async gather of the activation tile and the register-A wgmma m64nNk8 tf32.
+// split_tf32.cuh -- what the split-TF32 wgmma kernels (conv_f32_wgmma.cu, deconv_f32_wgmma.cu, gemm_f16_wgmma.cu) share: the
+// 128-row tile and its stage layout, the TF32 rounding and split, the 4-byte cp.async gather of the activation tile and the
+// register-A wgmma m64nNk8 tf32.
 #pragma once
 #include <cuda.h>
 #include "common.cuh"
@@ -26,6 +27,24 @@ __device__ __forceinline__ uint32_t tf32_rna(float x) {
     uint32_t r;
     asm("cvt.rna.tf32.f32 %0, %1;\n" : "=r"(r) : "f"(x));
     return r;
+}
+// x = hi + lo, both TF32, for a_hi*b_hi + a_hi*b_lo + a_lo*b_hi: hi = tf32_rna(x), lo = tf32_rna(x - hi), |x - hi - lo| <=
+// 2^-22 |x|.  A finite x that rounds past FLT_MAX (|x| >= (2 - 2^-11) 2^127) truncates instead, so both parts stay finite.
+// A non-finite x goes whole into lo, with hi = 0 (tf32_rna(x - hi) would be NaN for an infinity): of the three products only
+// x_lo * partner_hi then sees it, and partner_hi is 0 only when the partner is 0 and has the partner's sign, so Inf * b is what
+// fp32 makes of it for every finite b (Inf * Inf is NaN: each infinity meets the other's hi part, 0).  A NaN keeps its sign
+// with every mantissa bit set: its payload may lie only in the 13 bits TF32 drops, which would read as an infinity.  (The
+// MatMul's operand pack; the convolutions split their own way.)
+__device__ __forceinline__ void split_tf32(float x, float& hi, float& lo) {
+    if (!isfinite(x)) {
+        hi = 0.f;
+        lo = isnan(x) ? __int_as_float(__float_as_int(x) | 0x7fffffff) : x;
+        return;
+    }
+    uint32_t h = tf32_rna(x);
+    if ((h & 0x7f800000u) == 0x7f800000u) h = __float_as_uint(x) & 0xffffe000u;
+    hi = __uint_as_float(h);
+    lo = __uint_as_float(tf32_rna(x - hi));
 }
 __device__ __forceinline__ void cp_async4(uint32_t dst, const void* src, int src_bytes) {
     asm volatile("cp.async.ca.shared.global [%0], [%1], 4, %2;\n" ::"r"(dst), "l"(src), "r"(src_bytes) : "memory");

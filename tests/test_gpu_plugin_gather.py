@@ -4,9 +4,8 @@ reference core runs each recorded op through its Express executor on MNN_FORWARD
 gathers and casts bit for bit, MatMuls within 1e-3.  Every case of matmul_golden.npz, the batched ones included, runs the same
 way.  The BERT- and ViT-style fixtures (oracle/_ref/{bert,vit}_f32.mnn) run through the Interpreter at batch 2 with nothing
 declined: the CPU runs the gathers and the broadcast / batched MatMuls as While loops, which are matched with the plugin's
-commands by name.  Every compute command's fp32 output before the first MatMul is within 1e-3 of the CPU's (max|d| / max|ref|),
-every later one and the session output within MODEL_REL (the TF32 MatMul's error, below), and a graph-replayed forward equals
-the eager one bit for bit."""
+commands by name.  Every compute command's fp32 output and the session output are within 1e-3 of the CPU's (max|d| / max|ref|),
+and a graph-replayed forward equals the eager one bit for bit."""
 import os
 import re
 import tempfile
@@ -102,14 +101,8 @@ def _norm(name):
     return re.sub(r"_raster_\d+$", "", name)
 
 
-# The float MatMul reads fp32 operands as TF32: the tensor cores drop the low 13 mantissa bits of both operands, up to 2^-10 of
-# each, always toward zero.  A product loses up to 2 * 2^-10 of itself, and a sum dominated by products of one sign keeps that
-# bias whole, so the first attention MatMul differs from the CPU's by about 2e-3 of its largest value, and the error grows
-# through the layers (up to 7.5e-3 of a tensor's largest value in these encoders on an H100).  These fixtures therefore do not
-# meet the 1e-3 rule after their first attention MatMul (INTEGRATION.md, known limits).  They are held
-# to 1e-2, which any indexing, layout or broadcast error exceeds by far; the tensors before the first MatMul to 1e-3; and the
-# graph-replayed forward to the eager one bit for bit.
-MODEL_REL = 1e-2
+# every compute command and the session output, MatMuls and all they feed included
+MODEL_REL = 1e-3
 
 
 def _compare_models(d, cpu, gpu, stats, r):
@@ -120,7 +113,7 @@ def _compare_models(d, cpu, gpu, stats, r):
     for f, n, t in cpu:
         if not t.startswith("Raster"):
             cpu_by[_norm(n)] = f
-    compared, worst, before_matmul = 0, {}, True
+    compared, worst = 0, {}
     for f, n, t in gpu:
         if t.startswith("Raster"):
             continue
@@ -132,9 +125,8 @@ def _compare_models(d, cpu, gpu, stats, r):
         a = np.fromfile(os.path.join(d, "cpu", cpu_by[_norm(n)]), np.float32)
         b = np.fromfile(os.path.join(d, "gpu", f), np.float32)
         assert a.shape == b.shape, n
-        before_matmul = before_matmul and t not in ("MatMul", "BatchMatMul")
         err = _rel(b, a)
-        assert err <= (1e-3 if before_matmul else MODEL_REL), f"{n} ({t}) rel err {err}"
+        assert err <= MODEL_REL, f"{n} ({t}) rel err {err}"
         compared += 1
         worst[t] = max(worst.get(t, 0.0), err)
     oc = np.fromfile(os.path.join(d, "cpu", "output.f32"), np.float32)

@@ -1,5 +1,6 @@
 """Float MatMul / BatchMatMul (SURVEY a9): oracle pinned on the reference CPU backend and on a committed fixture; the
-wgmma f16 / tf32 path (-m gpu) within BASELINE's 1e-3 (max|d| / max|ref|)."""
+wgmma f16 / split-TF32 path (-m gpu) within BASELINE's 1e-3 (max|d| / max|ref|) and every element within a model of its
+arithmetic against float64."""
 import os
 
 import numpy as np
@@ -87,13 +88,13 @@ def test_gpu_attention_shapes_vs_oracle(backend, bd, e, l, h, ta, tb):
 # accumulator by aligning all K + 1 terms to the largest exponent and truncating, then truncating the normalised sum to
 # 24 bits.  Each step then errs by at most (K + 2) 2^-23 times the magnitude sum of its terms, which is at most
 # S = sum_k |a_ik| |b_kj|; over ceil(l / K) steps the accumulation error is <= (K + 2) ceil(l / K) 2^-23 S.
-# fp16 operands: products of 11-bit significands are exact in fp32, so that is all.  fp32 operands are read as tf32 (10-bit
-# mantissa, truncated): each operand errs by < 2^-10 relative, a product by < 2^-9 + 2^-20.  The epilogue's bias add
-# rounds once: <= 2^-24 |C + bias|, which 2^-23 (S + |bias|) covers.
+# fp16 operands: products of 11-bit significands are exact in fp32, so that is all.  fp32 operands are split into TF32 parts,
+# a = a_hi + a_lo, and summed as a_hi b_hi + a_hi b_lo + a_lo b_hi (three k8 steps per 8 products): the split misses a by
+# <= 2^-22 |a|, the dropped a_lo b_lo is <= 2^-22 |a||b|, under 2^-20 S in all (tests/test_gpu_matmul_f32.py::tolerance).
+# The epilogue's bias add rounds once: <= 2^-24 |C + bias|, which 2^-23 (S + |bias|) covers.
 def tolerance(a64, b64, l, f16, bias):
     s = np.matmul(np.abs(a64), np.abs(b64))
-    k = 16 if f16 else 8
-    tau = (k + 2) * -(-l // k) * 2.0 ** -23 + (0.0 if f16 else 2.0 ** -9 + 2.0 ** -20)
+    tau = 18 * -(-l // 16) * 2.0 ** -23 if f16 else 2.0 ** -20 + 3 * -(-l // 8) * 10 * 2.0 ** -23
     return tau * s + 2.0 ** -23 * (s + (0.0 if bias is None else np.abs(bias.astype(np.float64))))
 
 
@@ -135,12 +136,11 @@ def test_gpu_matmul_vs_float64(backend, si, ta, tb, f16):
 
 @pytest.mark.gpu
 def test_gpu_matmul_rebinds_and_packs_misaligned(backend):
-    """One execution run three times: on aligned K-major operands (read in place), on other aligned buffers (the cached
-    tensor maps must follow the pointers), and on operands that start one float past a 16-byte boundary (must take the
-    pack path)."""
+    """One execution run three times: on aligned K-major operands, on other aligned buffers (every run must read its own
+    operands), and on operands that start one float past a 16-byte boundary."""
     import torch
     from mnn_b200.backend import Op, Tensor
-    bd, e, l, h = (2,), 150, 64, 72          # ta = 0, tb = 1, l % 4 == 0: both operands can be read in place
+    bd, e, l, h = (2,), 150, 64, 72          # ta = 0, tb = 1, l % 4 == 0: both operands K-major and aligned
     rng = np.random.default_rng(21)
     bias = rng.uniform(-1, 1, h).astype(np.float32)
 
