@@ -305,11 +305,14 @@ MNNB200_API mnnb200_status mnnb200_linear_w8_resize(mnnb200_exec* e, int tokens)
 /* x and y need only be 4-byte aligned. */
 MNNB200_API mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* e, const float* x, float* y);
 /* Read-only view of the launch mnnb200_linear_w8_execute would make for the resized execution at its current variant: the first
- * `count` (at most 11) of {path (0 GEMV, 1 single-CTA wgmma GEMM, 2 CTA-pair GEMM, -1 refused: execute returns NOT_SUPPORT),
+ * `count` (at most 17) of {path (0 GEMV, 1 single-CTA wgmma GEMM, 2 CTA-pair GEMM, -1 refused: execute returns NOT_SUPPORT),
  * bn (columns per work item), n_chunks, m_tiles (128-row tiles; 256-row pair tiles for the CTA pair), items (work items), grid
  * (persistent CTAs), one_tile (every CTA owns exactly one item), resident_b (the weights stay in shared memory), stages
- * (operand ring), num_kb (128-byte K blocks per item), smem (dynamic shared memory bytes)} go to fields.  For the GEMV and a
- * refusal every field but path is 0; the CTA pair has neither one_tile nor resident_b.  NO_EXECUTION before resize,
+ * (operand ring), num_kb (128-byte K blocks per item), smem (dynamic shared memory bytes), then the GEMV's gemv_t (token rows
+ * of the instantiation: 1, 2, 4 or 8), gemv_r (output rows per warp), gemv_grid (blocks of 8 warps), gemv_passes (trips of
+ * each warp over the output rows: ceil(oc / (gemv_grid * 8 * gemv_r))), gemv_smem (dynamic shared memory bytes), gemv_w4 (1:
+ * the 4-bit weight branch runs)} go to fields.  For the GEMV the first eleven fields but path are 0, for the GEMMs the last
+ * six, for a refusal every field but path; the CTA pair has neither one_tile nor resident_b.  NO_EXECUTION before resize,
  * INVALID_VALUE for any other kind of execution.  Changes nothing. */
 MNNB200_API mnnb200_status mnnb200_linear_w8_plan(mnnb200_exec* e, int* fields, int count);
 

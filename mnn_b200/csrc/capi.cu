@@ -1165,6 +1165,16 @@ static LinearPath linear_path(const LinearW8Exec* e, const char** why) {
     if (e->variant == 3 || (e->variant == 0 && e->bn2)) return LinearPath::Pair;
     return LinearPath::Gemm;
 }
+// the GEMV's parameters for the resized execution reading x and writing y (nullptr for a plan query)
+static GemvW8Params linear_gemv_params(const LinearW8Exec* e, const float* x, float* y) {
+    GemvW8Params g;
+    memset(&g, 0, sizeof(g));
+    g.x = x; g.w = e->d_w; g.y = y; g.alpha = e->d_alpha; g.bias = e->has_bias ? static_cast<const float*>(e->d_bias) : nullptr;
+    g.wsumf = e->d_wsumf; g.wzero = e->has_zero ? static_cast<const float*>(e->d_wzero) : nullptr; g.wsum128 = e->d_wsum128;
+    g.tokens = e->tokens; g.ic = e->ic; g.oc = e->oc; g.ocp = e->ocp; g.icp = e->icp; g.ldy = e->oc; g.relu = e->relu; g.relu6 = e->relu6;
+    g.bs = e->bs; g.balpha = e->d_balpha; g.bwzero = e->d_bwzero; g.w4 = e->w4;
+    return g;
+}
 // the tensor-core GEMMs' parameters for the resized execution writing y (nullptr for a plan query, which launches nothing)
 static GemmI8Params linear_gemm_params(const LinearW8Exec* e, float* y) {
     GemmI8Params g;
@@ -1358,12 +1368,7 @@ mnnb200_status mnnb200_linear_w8_execute(mnnb200_exec* ex, const float* x, float
     const LinearPath path = linear_path(e, &why);
     if (path == LinearPath::Refused) return fail(MNNB200_NOT_SUPPORT, why);
     if (path == LinearPath::Gemv) {
-        GemvW8Params g;
-        g.x = x; g.w = e->d_w; g.y = y; g.alpha = e->d_alpha; g.bias = e->has_bias ? static_cast<float*>(e->d_bias) : nullptr; g.wsumf = e->d_wsumf;
-        g.wzero = e->has_zero ? static_cast<float*>(e->d_wzero) : nullptr; g.wsum128 = e->d_wsum128;
-        g.tokens = e->tokens; g.ic = e->ic; g.oc = e->oc; g.ocp = e->ocp; g.icp = e->icp; g.ldy = e->oc; g.relu = e->relu; g.relu6 = e->relu6;
-        g.bs = e->bs; g.balpha = e->d_balpha; g.bwzero = e->d_bwzero; g.w4 = e->w4;
-        CK(launch_linear_w8_gemv(g, e->rt->stream, e->rt->prop.multiProcessorCount));
+        CK(launch_linear_w8_gemv(linear_gemv_params(e, x, y), e->rt->stream, e->rt->prop.multiProcessorCount));
         return MNNB200_OK;
     }
     CK(launch_dynamic_quant(x, e->tokens, e->ic, e->icp, e->d_xq, e->d_dq, e->d_srcsum, e->rt->stream, e->bs, e->d_xsb));
@@ -1388,7 +1393,11 @@ mnnb200_status mnnb200_linear_w8_plan(mnnb200_exec* ex, int* fields, int count) 
     memset(&l, 0, sizeof(l));
     if (path == LinearPath::Gemm) { bn = e->bn; l = gemm_i8_wgmma_launch(linear_gemm_params(e, nullptr), bn, sm); }
     if (path == LinearPath::Pair) { bn = e->bn2; l = gemm_i8_2cta_launch(linear_gemm_params(e, nullptr), bn, sm); }
-    const int v[] = {(int)path, bn, l.n_chunks, l.m_tiles, l.items, l.grid, l.one_tile, l.resident_b, l.stages, l.num_kb, l.smem};
+    GemvW8Launch g;
+    memset(&g, 0, sizeof(g));
+    if (path == LinearPath::Gemv) g = linear_w8_gemv_launch(linear_gemv_params(e, nullptr, nullptr), sm);
+    const int v[] = {(int)path, bn, l.n_chunks, l.m_tiles, l.items, l.grid, l.one_tile, l.resident_b, l.stages, l.num_kb, l.smem,
+                     g.t, g.r, g.grid, g.passes, g.smem, g.w4};
     return copy_fields(v, fields, count);
 }
 }  // extern "C"

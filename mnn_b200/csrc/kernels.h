@@ -314,6 +314,13 @@ struct GemvW8Params {
     int w4;
 };
 bool linear_w8_gemv_supported(int tokens, int icp, int bs = 0, int w4 = 0);
+// The launch launch_linear_w8_gemv makes for p on sm_count SMs (x and y are not read): the tokens template t (1, 2, 4, 8), rows
+// per warp r, grid (blocks of 8 warps), passes over the output rows (ceil(oc / (grid * 8 * r))), dynamic shared-memory bytes,
+// and whether the 4-bit branch runs
+struct GemvW8Launch {
+    int t, r, grid, passes, smem, w4;
+};
+GemvW8Launch linear_w8_gemv_launch(const GemvW8Params& p, int sm_count);
 cudaError_t launch_linear_w8_gemv(const GemvW8Params& p, cudaStream_t s, int sm_count);
 
 // dynamic per-token quantisation (MNNAbsMax + MNNQuantScale + MNNDynamicQuant fused); bs > 0 also writes

@@ -19,6 +19,7 @@
 #include "common.cuh"
 #include "kernels.h"
 
+#include <algorithm>
 #include <type_traits>
 
 namespace mnnb200 {
@@ -447,22 +448,17 @@ __global__ void __launch_bounds__(256, 2) linear_w8_gemv_kernel(GemvW8Params p) 
 }
 
 template <int T, int R, int U>
-cudaError_t launch_t(const GemvW8Params& p, cudaStream_t stream, int sms) {
-    // blocked: + the per-block input sums [T][ic / bs] and each warp's block parts
-    const size_t smem = (size_t)T * p.icp + (p.bs ? ((size_t)T * (p.ic / p.bs) + 8 * (T * R + R) * (16 << p.w4)) * sizeof(float) : 0);
-    if (smem > 40 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(linear_w8_gemv_kernel<T, R, U>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+cudaError_t launch_t(const GemvW8Params& p, const GemvW8Launch& l, cudaStream_t stream) {
+    if (l.smem > 40 * 1024) {
+        cudaError_t e = cudaFuncSetAttribute(linear_w8_gemv_kernel<T, R, U>, cudaFuncAttributeMaxDynamicSharedMemorySize, l.smem);
         if (e != cudaSuccess) return e;
     }
-    const int rows_per_block = 8 * R;
-    int blocks = (p.oc + rows_per_block - 1) / rows_per_block;
-    blocks = blocks < sms * 8 ? blocks : sms * 8;
     ++g_launch_count;
     cudaLaunchConfig_t cfg;
     memset(&cfg, 0, sizeof(cfg));
-    cfg.gridDim = dim3((unsigned)blocks);
+    cfg.gridDim = dim3((unsigned)l.grid);
     cfg.blockDim = dim3(256);
-    cfg.dynamicSmemBytes = smem;
+    cfg.dynamicSmemBytes = l.smem;
     cfg.stream = stream;
     cudaLaunchAttribute attr[1];
     attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
@@ -472,15 +468,14 @@ cudaError_t launch_t(const GemvW8Params& p, cudaStream_t stream, int sms) {
     return cudaLaunchKernelEx(&cfg, linear_w8_gemv_kernel<T, R, U>, p);
 }
 
-// rows per warp: as many as keep >= ~2 blocks per SM (the small layers are latency-bound: more blocks = more loads in flight).
-// Four rows only for <= 2 tokens, decided at compile time so that <4, 4, 4> and <8, 4, 4> are not instantiated at all.
+// the instantiation linear_w8_gemv_launch picked; <4, 4, 4> and <8, 4, 4> are not instantiated at all
 template <int T>
-cudaError_t launch_r(const GemvW8Params& p, cudaStream_t stream, int sms) {
+cudaError_t launch_r(const GemvW8Params& p, const GemvW8Launch& l, cudaStream_t stream) {
     if constexpr (T <= 2) {
-        if (p.oc >= sms * 2 * 8 * 4 && !p.w4) return launch_t<T, 4, 4>(p, stream, sms);
+        if (l.r == 4) return launch_t<T, 4, 4>(p, l, stream);
     }
-    if (p.oc >= sms * 2 * 8 * 2) return launch_t<T, 2, 4>(p, stream, sms);
-    return launch_t<T, 1, 4>(p, stream, sms);
+    if (l.r == 2) return launch_t<T, 2, 4>(p, l, stream);
+    return launch_t<T, 1, 4>(p, l, stream);
 }
 
 }  // namespace
@@ -491,11 +486,32 @@ bool linear_w8_gemv_supported(int tokens, int icp, int bs, int w4) {
     return tokens >= 1 && tokens <= 8 && (size_t)8 * icp + extra <= 200 * 1024;
 }
 
+GemvW8Launch linear_w8_gemv_launch(const GemvW8Params& p, int sms) {
+    GemvW8Launch l;
+    // 4-bit layers run one token on the two-token instantiation (the one-token kernel carries no 4-bit branch: stream_rows)
+    l.t = p.tokens <= 1 && !p.w4 ? 1 : p.tokens <= 2 ? 2 : p.tokens <= 4 ? 4 : 8;
+    // rows per warp: as many as keep >= ~2 blocks per SM (the small layers are latency-bound: more blocks = more loads in
+    // flight).  Four rows only for <= 2 tokens and 8-bit weights
+    l.r = l.t <= 2 && !p.w4 && p.oc >= sms * 2 * 8 * 4 ? 4 : p.oc >= sms * 2 * 8 * 2 ? 2 : 1;
+    const int rows_per_block = 8 * l.r;
+    l.grid = std::min((p.oc + rows_per_block - 1) / rows_per_block, sms * 8);
+    l.passes = (p.oc + l.grid * rows_per_block - 1) / (l.grid * rows_per_block);
+    // blocked: + the per-block input sums [T][ic / bs] and each warp's block parts
+    const size_t smem = (size_t)l.t * p.icp +
+                        (p.bs ? ((size_t)l.t * (p.ic / p.bs) + 8 * (l.t * l.r + l.r) * (16 << p.w4)) * sizeof(float) : 0);
+    l.smem = (int)smem;
+    l.w4 = l.t > 1 && l.r < 4 ? p.w4 : 0;      // the kernel's own rule
+    return l;
+}
+
 cudaError_t launch_linear_w8_gemv(const GemvW8Params& p, cudaStream_t stream, int sms) {
-    if (p.tokens <= 1 && !p.w4) return launch_r<1>(p, stream, sms);
-    if (p.tokens <= 2) return launch_r<2>(p, stream, sms);
-    if (p.tokens <= 4) return launch_r<4>(p, stream, sms);
-    return launch_r<8>(p, stream, sms);
+    const GemvW8Launch l = linear_w8_gemv_launch(p, sms);
+    switch (l.t) {
+        case 1: return launch_r<1>(p, l, stream);
+        case 2: return launch_r<2>(p, l, stream);
+        case 4: return launch_r<4>(p, l, stream);
+        default: return launch_r<8>(p, l, stream);
+    }
 }
 
 }  // namespace mnnb200

@@ -292,14 +292,14 @@ def linear_oracle(x, w, alpha, wzero, bias, bits=8, relu=False, relu6=False):
     return O.linear_w8_dynamic(x, w, alpha, wzero, bias, relu=relu, relu6=relu6)
 
 
-def create_linear(backend, ic, oc, w, alpha, wzero=None, bias=None, bits=8, blocks=None):
+def create_linear(backend, ic, oc, w, alpha, wzero=None, bias=None, bits=8, blocks=None, relu=0, relu6=0):
     """(status, handle) of the C entry of the weight form: mnnb200_linear_w8_create, or the blocked entry of `bits` with
-    `blocks` (default alpha's)"""
+    `blocks` (default alpha's); relu / relu6 the layer's fused activation"""
     from mnn_b200 import _capi
     lib = _capi.lib()
     h = C.c_void_p()
     ptr = lambda a: None if a is None else a.ctypes.data_as(C.c_void_p)
-    args = (ptr(w), ptr(alpha), ptr(wzero), ptr(bias), 0, 0, C.byref(h))
+    args = (ptr(w), ptr(alpha), ptr(wzero), ptr(bias), int(relu), int(relu6), C.byref(h))
     if bits == 8 and alpha.ndim == 1:
         return lib.mnnb200_linear_w8_create(backend.runtime._h, ic, oc, *args), h
     fn = lib.mnnb200_linear_w4_create_blocked if bits == 4 else lib.mnnb200_linear_w8_create_blocked
