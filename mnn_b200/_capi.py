@@ -163,6 +163,17 @@ GATHER_SIGNATURES = {
 }
 _gather_lib = None
 
+# libmnn_b200_scatter.so (include/mnn_b200_scatter.h): ScatterNd and ScatterElements, on the runtime and execution handles above
+SCATTER_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_scatter.so")
+_IP = C.POINTER(C.c_int)
+SCATTER_SIGNATURES = {
+    "mnnb200_scatter_create": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.POINTER(P)]),
+    "mnnb200_scatter_resize": (C.c_int, [P, _IP, C.c_int, _IP, C.c_int, _IP, C.c_int, C.c_int, C.c_int]),
+    "mnnb200_scatter_execute": (C.c_int, [P, P, P, P, P]),
+    "mnnb200_scatter_plan": (C.c_int, [P, _IP, C.c_int]),
+}
+_scatter_lib = None
+
 # libmnn_b200_llm.so (include/mnn_b200_llm.h): MNN-LLM's LayerNorm / RoPE executions, on the runtime and execution handles above
 LLM_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_llm.so")
 LLM_SIGNATURES = {
@@ -239,6 +250,22 @@ def gather_lib():
             fn.argtypes = args
         _gather_lib = L
     return _gather_lib
+
+
+def scatter_lib():
+    """libmnn_b200_scatter.so with every SCATTER_SIGNATURES symbol resolved (after libmnn_b200.so, whose handles it shares)"""
+    global _scatter_lib
+    if _scatter_lib is None:
+        lib()
+        if not os.path.exists(SCATTER_LIB_PATH):
+            raise MnnB200Error(f"{SCATTER_LIB_PATH} is missing: run `python -m mnn_b200.build` (there is no CPU fallback)")
+        L = C.CDLL(SCATTER_LIB_PATH)
+        for name, (res, args) in SCATTER_SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype = res
+            fn.argtypes = args
+        _scatter_lib = L
+    return _scatter_lib
 
 
 def lib():

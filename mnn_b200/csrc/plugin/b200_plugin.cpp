@@ -40,6 +40,7 @@
 
 #include "../../../include/mnn_b200_deconv.h"
 #include "../../../include/mnn_b200_gather.h"
+#include "../../../include/mnn_b200_scatter.h"
 #include "../../../include/mnn_b200_interp.h"
 #include "../../../include/mnn_b200_llm.h"
 
@@ -1423,6 +1424,78 @@ private:
     ExecHandle mH;
 };
 
+// ScatterNd(indices, updates, shape[, data]) / ScatterElements(data, indices, updates[, axis]) (GeometryScatter.cpp registers
+// their lowering for Compiler_Loop only, so under Compiler_Geometry they reach the backend unlowered) on tensors of 4-byte
+// elements, fp32, or int32 without a reduction, with int32 indices; data, updates and output linear in their logical dim order
+// as GatherExec's.  The reduction is read as the geometry reads it: the op's BinaryOp opType (ScatterNd: none without one);
+// ADD, SUB and MUL are taken, other codes declined.  The ScatterElements axis is a constant fourth input (read at resize), else
+// 0.  A 3-input ScatterNd has no data (the output starts zero-filled), so the handle is made at resize, for the inputs given.
+class ScatterExec : public ClonedFromOp<ScatterExec> {
+public:
+    ScatterExec(Backend* bn, const Op* op) : ClonedFromOp(bn), mOp(op) {}
+    static Execution* create(B200Backend* bn, const Op* op) { return new ScatterExec(bn, op); }
+    static bool elements(const Op* op) { return op->type() == OpType_ScatterElements; }
+    static int reduction(const Op* op) { return op->main_as_BinaryOp() ? (int)op->main_as_BinaryOp()->opType() : -1; }
+    static Tensor* data(const Op* op, const std::vector<Tensor*>& inputs) {
+        return elements(op) ? inputs[0] : (inputs.size() == 4 ? inputs[3] : nullptr);
+    }
+    static bool takes(const Op* op, const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) {
+        if (inputs.size() < 3 || inputs.size() > 4 || outputs.size() != 1) return false;
+        if (elements(op) && !op->main_as_BinaryOp()) return false;
+        const int red = reduction(op);
+        auto idx = inputs[elements(op) ? 1 : 0], upd = inputs[elements(op) ? 2 : 1], y = outputs[0], x = data(op, inputs);
+        const bool i32 = idx->getType().code == halide_type_int && idx->getType().bits == 32 && !isInt8(idx);
+        bool ok = red <= 2 && i32 && GatherExec::word(upd) && GatherExec::word(y) && upd->getType() == y->getType() &&
+                  linearFormat(upd) == linearFormat(y) && y->dimensions() >= 1 && idx->dimensions() >= 1;
+        if (red >= 0) ok = ok && y->getType().code == halide_type_float;
+        if (x) ok = ok && GatherExec::word(x) && x->getType() == y->getType() && linearFormat(x) == linearFormat(y) &&
+                    elemCount(x) == elemCount(y);
+        if (elements(op) && inputs.size() == 4) {
+            auto ax = inputs[3];
+            ok = ok && ax->getType().code == halide_type_int && ax->getType().bits == 32 && elemCount(ax) >= 1 &&
+                 (ax->host<int>() != nullptr || TensorUtils::getDescribe(ax)->usage == Tensor::InsideDescribe::CONSTANT);
+        }
+        return ok;
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        if (!takes(mOp, inputs, outputs)) return NOT_SUPPORT;
+        const bool withData = data(mOp, inputs) != nullptr;
+        if (!mH || withData != mWithData) {
+            mnnb200_exec* h = nullptr;
+            const mnnb200_status st = mnnb200_scatter_create(rt(), elements(mOp) ? 1 : 0, reduction(mOp), withData ? 1 : 0, &h);
+            if (st != MNNB200_OK) return toErr(st, "scatter create");
+            mH.reset(h);
+            mWithData = withData;
+        }
+        int axis = 0;
+        if (elements(mOp) && inputs.size() == 4) {
+            auto ax = inputs[3];
+            if (ax->host<int>()) axis = ax->host<int>()[0];
+            else if (mnnb200_memcpy_d2h(rt(), &axis, dev(ax), sizeof(int)) != MNNB200_OK || mnnb200_runtime_sync(rt()) != MNNB200_OK)
+                return toErr(MNNB200_CUDA_ERROR, "ScatterElements axis read");
+        }
+        auto dims = [](const Tensor* t) {
+            std::vector<int> d(t->dimensions());
+            for (int i = 0; i < t->dimensions(); ++i) d[i] = t->length(i);
+            return d;
+        };
+        auto idx = inputs[elements(mOp) ? 1 : 0], upd = inputs[elements(mOp) ? 2 : 1], y = outputs[0];
+        const std::vector<int> od = dims(y), id = dims(idx), ud = dims(upd);
+        return toErr(mnnb200_scatter_resize(mH.get(), od.data(), (int)od.size(), id.data(), (int)id.size(), ud.data(), (int)ud.size(),
+                                            axis, y->getType().code == halide_type_int ? 1 : 0),
+                     "scatter resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto x = data(mOp, inputs);
+        auto idx = inputs[elements(mOp) ? 1 : 0], upd = inputs[elements(mOp) ? 2 : 1];
+        return toErr(mnnb200_scatter_execute(mH.get(), x ? dev(x) : nullptr, (const int*)dev(idx), dev(upd), dev(outputs[0])), "scatter");
+    }
+private:
+    const Op* mOp;
+    ExecHandle mH;
+    bool mWithData = false;
+};
+
 // Cast between int32 and fp32 (CPUCast's CastDataType): an attention mask's int32 -> fp32, or fp32 -> int32 (truncation)
 class CastExec : public B200Exec {
 public:
@@ -1483,6 +1556,10 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
         case OpType_GatherND:
         case OpType_GatherElements:
             if (!quantOut && GatherExec::takes(op, inputs, outputs)) e = GatherExec::create(this, op);
+            break;
+        case OpType_ScatterNd:
+        case OpType_ScatterElements:
+            if (!quantOut && ScatterExec::takes(op, inputs, outputs)) e = ScatterExec::create(this, op);
             break;
         case OpType_Cast: {
             const int dir = quantOut ? -1 : CastExec::direction(op, inputs, outputs);

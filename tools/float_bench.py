@@ -34,9 +34,13 @@ MODELS = {   # --model: (fixture under oracle/_ref, name in the JSON line)
     "deeplab": ("deeplab_f32.mnn", "DeepLab-v3-style segmentation fp32, 128x128 (seeded weights, oracle/refdump_interp.cpp)"),
     "bert": ("bert_f32.mnn", "BERT-style encoder fp32, 4 layers, D 256, S 64, int32 ids and mask (seeded weights, oracle/refdump_gather.cpp)"),
     "vit": ("vit_f32.mnn", "ViT-style encoder fp32, 4 layers, D 192, 64x64 image (seeded weights, oracle/refdump_gather.cpp)"),
+    "pillars": ("pillars_f32.mnn", "PointPillars-style BEV net fp32, 2,048 pillars into 64x48, batch 1 (seeded weights, oracle/refdump_scatter.cpp)"),
+    "gnn": ("gnn_f32.mnn", "GraphSAGE-mean-style net fp32, 512 nodes, 4,096 skewed edges, batch 1 (seeded weights, oracle/refdump_scatter.cpp)"),
 }
 # models whose inputs refdump's bench does not fill (int32 token ids and masks): timed by oracle/refdump_gather's bench instead
 GATHER_HARNESS = {"bert", "vit"}
+# models with int32 pillar cells or edge lists, built for batch 1: timed at batch 1 by oracle/refdump_scatter's bench
+SCATTER_HARNESS = {"pillars", "gnn"}
 
 
 def shapes_from_cpu_run(model, refdump, env):
@@ -149,6 +153,8 @@ def main():
     env.pop("REFDUMP_PLUGIN", None)
     card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
                           text=True, check=True).stdout.strip().splitlines()[0]
+    if a.model in SCATTER_HARNESS:
+        a.batch = 1
     res = dict(model=title, batch=a.batch, card=card)
     if a.model == "mbv2":
         res.update(time_convs(shapes_from_cpu_run(model, O.REFDUMP, env), a.batch, a.iters))
@@ -156,6 +162,9 @@ def main():
     if a.model in GATHER_HARNESS:
         from oracle import gather_oracle
         harness = gather_oracle.REFDUMP_GATHER
+    if a.model in SCATTER_HARNESS:
+        from oracle import scatter_oracle
+        harness = scatter_oracle.REFDUMP_SCATTER
     penv = dict(env, REFDUMP_BENCH_WINDOWS="5", REFDUMP_PLUGIN=os.path.join(ROOT, "mnn_b200", "libmnn_b200_plugin.so"))
     p = refdump_bench(harness, model, a.batch, 4, penv, 20)
     res.update(plugin_e2e_img_per_s=p["img_per_s"], plugin_e2e_ms=p["ms_median_window"], plugin_created=p["plugin_created"],
