@@ -174,6 +174,16 @@ SCATTER_SIGNATURES = {
 }
 _scatter_lib = None
 
+# libmnn_b200_rnn.so (include/mnn_b200_rnn.h): LSTM and RNN, on the runtime and execution handles above
+RNN_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_rnn.so")
+RNN_SIGNATURES = {
+    "mnnb200_rnn_create": (C.c_int, [P, C.c_int, C.POINTER(P)]),
+    "mnnb200_rnn_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mnnb200_rnn_execute": (C.c_int, [P, P, P, P, P, P, P, P, P, P]),
+    "mnnb200_rnn_plan": (C.c_int, [P, _IP, C.c_int]),
+}
+_rnn_lib = None
+
 # libmnn_b200_llm.so (include/mnn_b200_llm.h): MNN-LLM's LayerNorm / RoPE executions, on the runtime and execution handles above
 LLM_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_llm.so")
 LLM_SIGNATURES = {
@@ -266,6 +276,22 @@ def scatter_lib():
             fn.argtypes = args
         _scatter_lib = L
     return _scatter_lib
+
+
+def rnn_lib():
+    """libmnn_b200_rnn.so with every RNN_SIGNATURES symbol resolved (after libmnn_b200.so, whose handles it shares)"""
+    global _rnn_lib
+    if _rnn_lib is None:
+        lib()
+        if not os.path.exists(RNN_LIB_PATH):
+            raise MnnB200Error(f"{RNN_LIB_PATH} is missing: run `python -m mnn_b200.build` (there is no CPU fallback)")
+        L = C.CDLL(RNN_LIB_PATH)
+        for name, (res, args) in RNN_SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype = res
+            fn.argtypes = args
+        _rnn_lib = L
+    return _rnn_lib
 
 
 def lib():

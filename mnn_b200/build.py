@@ -1,7 +1,8 @@
 """Builds libmnn_b200.so (CUDA kernels + C ABI), libmnn_b200_llm.so (the MNN-LLM LayerNorm / RoPE ops, include/mnn_b200_llm.h)
 libmnn_b200_deconv.so (the float Deconvolution, include/mnn_b200_deconv.h), libmnn_b200_interp.so (the float Interp,
 include/mnn_b200_interp.h), libmnn_b200_gather.so (the gathers and the int32 / fp32 Cast, include/mnn_b200_gather.h) and
-libmnn_b200_scatter.so (ScatterNd and ScatterElements, include/mnn_b200_scatter.h), the last five linked against libmnn_b200.so,
+libmnn_b200_scatter.so (ScatterNd and ScatterElements, include/mnn_b200_scatter.h) and libmnn_b200_rnn.so (LSTM and RNN,
+include/mnn_b200_rnn.h), the last six linked against libmnn_b200.so,
 in-tree for sm_90a (H100) with nvcc.  No torch involvement."""
 import os
 import subprocess
@@ -15,12 +16,14 @@ DECONV_LIB = os.path.join(HERE, "libmnn_b200_deconv.so")
 INTERP_LIB = os.path.join(HERE, "libmnn_b200_interp.so")
 GATHER_LIB = os.path.join(HERE, "libmnn_b200_gather.so")
 SCATTER_LIB = os.path.join(HERE, "libmnn_b200_scatter.so")
+RNN_LIB = os.path.join(HERE, "libmnn_b200_rnn.so")
 SOURCES = ["capi.cu", "conv_int8_mma.cu", "elementwise.cu", "gemm_i8_wgmma.cu", "winograd_int8.cu", "gemm_f16_wgmma.cu", "conv_int8_stem.cu", "conv_group_wgmma.cu", "linear_w8_gemv.cu", "conv_f32_wgmma.cu"]
 LLM_SOURCES = ["llm_ops.cu", "llm_capi.cu"]
 DECONV_SOURCES = ["deconv_f32_wgmma.cu", "deconv_capi.cu"]
 INTERP_SOURCES = ["interp_f32.cu", "interp_capi.cu"]
 GATHER_SOURCES = ["gather.cu", "gather_capi.cu"]
 SCATTER_SOURCES = ["scatter.cu", "scatter_capi.cu"]
+RNN_SOURCES = ["rnn.cu", "rnn_capi.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-ffp-contract=off,-fvisibility=hidden", "--expt-relaxed-constexpr"]
@@ -48,7 +51,7 @@ def _compile(srcs, nvcc, verbose):
 
 
 def build(force=False, verbose=False):
-    """the six libraries; returns the path of libmnn_b200.so"""
+    """the seven libraries; returns the path of libmnn_b200.so"""
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
     llm_srcs = [os.path.join(CSRC, s) for s in LLM_SOURCES]
     inc = os.path.join(HERE, "..", "include")
@@ -63,6 +66,8 @@ def build(force=False, verbose=False):
     gather_deps = deps + gather_srcs + [os.path.join(inc, "mnn_b200_gather.h")]
     scatter_srcs = [os.path.join(CSRC, s) for s in SCATTER_SOURCES]
     scatter_deps = deps + scatter_srcs + [os.path.join(inc, "mnn_b200_scatter.h")]
+    rnn_srcs = [os.path.join(CSRC, s) for s in RNN_SOURCES]
+    rnn_deps = deps + rnn_srcs + [os.path.join(inc, "mnn_b200_rnn.h")]
     fresh = lambda lib, ds: os.path.exists(lib) and all(os.path.getmtime(lib) > os.path.getmtime(d) for d in ds)
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     if force or not fresh(LIB, deps):
@@ -81,6 +86,9 @@ def build(force=False, verbose=False):
                               ["-L" + HERE, "-lmnn_b200", "-Xlinker", "-rpath,$ORIGIN", "-lcudart"])
     if force or not fresh(SCATTER_LIB, scatter_deps + [LIB]):
         subprocess.check_call([nvcc, "-shared", "-o", SCATTER_LIB] + _compile(scatter_srcs, nvcc, verbose) + ARCH +
+                              ["-L" + HERE, "-lmnn_b200", "-Xlinker", "-rpath,$ORIGIN", "-lcudart"])
+    if force or not fresh(RNN_LIB, rnn_deps + [LIB]):
+        subprocess.check_call([nvcc, "-shared", "-o", RNN_LIB] + _compile(rnn_srcs, nvcc, verbose) + ARCH +
                               ["-L" + HERE, "-lmnn_b200", "-Xlinker", "-rpath,$ORIGIN", "-lcudart"])
     return LIB
 

@@ -1,6 +1,7 @@
 // elementwise.cu -- HBM-bound neighbours of the int8 GEMM path: boundary casts (fused with the
 // NCHW <-> NHWC16 layout change), depthwise int8 conv, per-token dynamic activation quantisation.
 // All are bandwidth kernels: 16-byte vector accesses on the NHWC16 side, one 16-channel group per thread.
+#include "activations.cuh"
 #include "common.cuh"
 #include "kernels.h"
 
@@ -1009,19 +1010,8 @@ cudaError_t launch_binary_add_f32(const float* a, const float* b, float* y, size
 
 // ---- fp32 UnaryOp (CPUUnary::selectForFloat, CPUUnary.cpp:353-440).  HARDSWISH, ABS, NEG, SQUARE, SQRT, RSQRT and RECIPROCAL
 //      use the CPU's own formula in round-to-nearest steps; the transcendental ops (the CPU uses its own polynomials) are
-//      accurate to a few ulp: SIGMOID / SILU / GELU through expf in a cancellation-free form, GELU_STANDARD through erfcf.
-// x * sigmoid(t) = x / (1 + e^-t) for t >= 0, x e^t / (1 + e^t) for t < 0: e^-|t| never overflows, so the result keeps its
-// magnitude where 1 / (1 + e^-t) would be 1 / inf (t < -88.7).  Below t = -64 (1 + e^t is then 1) the exponential is taken at
-// t + 32 (exact for |t| < 256, beyond which the result is 0 anyway) and the product scaled by e^-32, so that a subnormal e^t
-// does not lose the digits the product still has.
-__device__ __forceinline__ float times_sigmoid(float x, float t) {
-    if (t >= 0.f) return __fdiv_rn(x, __fadd_rn(1.f, expf(-t)));
-    if (t >= -64.f) {
-        const float e = expf(t);
-        return __fdiv_rn(__fmul_rn(x, e), __fadd_rn(1.f, e));
-    }
-    return __fmul_rn(__fmul_rn(x, expf(__fadd_rn(t, 32.f))), 1.26641655e-14f);   // e^-32
-}
+//      accurate to a few ulp: SIGMOID / SILU / GELU through expf in a cancellation-free form (times_sigmoid, activations.cuh),
+//      GELU_STANDARD through erfcf.
 template <int OP>
 __device__ __forceinline__ float unary_f32_op(float x) {
     // ABS is MNNReluWithSlope(x, -1) (CPUUnary.cpp:323-325): (x < 0 ? x * -1 : 0) + (x >= 0 ? x : 0), so |-0| = +0 and
@@ -1034,8 +1024,8 @@ __device__ __forceinline__ float unary_f32_op(float x) {
     if (OP == kUnaryReciprocal) return __fdiv_rn(1.f, x);
     if (OP == kUnaryExp) return expf(x);
     if (OP == kUnaryLog) return logf(x);
-    if (OP == kUnaryTanh) return tanhf(x);
-    if (OP == kUnarySigmoid) return x >= -64.f ? times_sigmoid(1.f, x) : expf(x);   // 1 + e^x is 1 below -64
+    if (OP == kUnaryTanh) return tanh_f32(x);
+    if (OP == kUnarySigmoid) return sigmoid_f32(x);
     if (OP == kUnarySilu) return times_sigmoid(x, x);
     if (OP == kUnaryHardSwish)   // x86_x64/sse/MathFunctions.cpp:251-259: (x * min(max(x + 3, 0), 6)) / 6
         return __fdiv_rn(__fmul_rn(x, fminf(fmaxf(__fadd_rn(x, 3.f), 0.f), 6.f)), 6.f);

@@ -41,6 +41,7 @@
 #include "../../../include/mnn_b200_deconv.h"
 #include "../../../include/mnn_b200_gather.h"
 #include "../../../include/mnn_b200_scatter.h"
+#include "../../../include/mnn_b200_rnn.h"
 #include "../../../include/mnn_b200_interp.h"
 #include "../../../include/mnn_b200_llm.h"
 
@@ -1496,6 +1497,64 @@ private:
     bool mWithData = false;
 };
 
+// ONNX LSTM / RNN (OpType_LSTM / OpType_RNN with X, W, R, B[, h0[, c0]]; GeometryLSTM.cpp registers their lowering for
+// Compiler_Loop only, so under Compiler_Geometry they reach the backend unlowered) on fp32 tensors in a linear layout: X [T, B, I],
+// W [D, G*H, I], R [D, G*H, H], B of D*G*H elements, h0 / c0 [D, B, H], outputs Y [T, D, B, H], Y_h (and for LSTM Y_c)
+// [D, B, H], with H = the op's outputCount and G = 4 (LSTM) or 1 (RNN).  Declined: the Caffe single-input LSTM (one input, one
+// output), an RNN with a cell input, int8 / fp16 / NC4HW4 tensors and inconsistent shapes.
+class RnnExec : public ClonedFromOp<RnnExec> {
+public:
+    RnnExec(Backend* bn, const Op* op, mnnb200_exec* h) : ClonedFromOp(bn), mOp(op), mH(h) {}
+    static Execution* create(B200Backend* bn, const Op* op) {
+        mnnb200_exec* h = nullptr;
+        if (mnnb200_rnn_create(bn->handle(), op->type() == OpType_RNN ? 1 : 0, &h) != MNNB200_OK) return nullptr;
+        return new RnnExec(bn, op, h);
+    }
+    static bool f32Linear(const Tensor* t) {
+        return isF32(t) && !isInt8(t) && TensorUtils::getDescribe(t)->dimensionFormat != MNN_DATA_FORMAT_NC4HW4;
+    }
+    static bool shaped(const Tensor* t, std::initializer_list<int> d) {
+        if (t->dimensions() != (int)d.size()) return false;
+        int i = 0;
+        for (int v : d) if (t->length(i++) != v) return false;
+        return true;
+    }
+    static bool takes(const Op* op, const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) {
+        const bool lstm = op->type() == OpType_LSTM;
+        if (!op->main_as_LSTM() || inputs.size() < 4 || inputs.size() > (lstm ? 6u : 5u) || outputs.size() != (lstm ? 3u : 2u))
+            return false;
+        for (auto t : inputs) if (!f32Linear(t)) return false;
+        for (auto t : outputs) if (!f32Linear(t)) return false;
+        auto x = inputs[0], w = inputs[1], r = inputs[2];
+        if (x->dimensions() != 3 || w->dimensions() != 3) return false;
+        const int T = x->length(0), B = x->length(1), I = x->length(2), D = w->length(0), H = op->main_as_LSTM()->outputCount();
+        const int G = lstm ? 4 : 1;
+        if (T < 1 || B < 1 || I < 1 || H < 1 || (D != 1 && D != 2)) return false;
+        bool ok = shaped(w, {D, G * H, I}) && shaped(r, {D, G * H, H}) && elemCount(inputs[3]) == (size_t)D * G * H &&
+                  shaped(outputs[0], {T, D, B, H});
+        for (size_t k = 4; k < inputs.size(); ++k) ok = ok && shaped(inputs[k], {D, B, H});
+        for (size_t k = 1; k < outputs.size(); ++k) ok = ok && shaped(outputs[k], {D, B, H});
+        return ok;
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        if (!takes(mOp, inputs, outputs)) return NOT_SUPPORT;
+        auto x = inputs[0];
+        return toErr(mnnb200_rnn_resize(mH.get(), x->length(0), x->length(1), x->length(2), mOp->main_as_LSTM()->outputCount(),
+                                        inputs[1]->length(0), inputs.size() >= 5 ? 1 : 0, inputs.size() >= 6 ? 1 : 0),
+                     "rnn resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto f = [](const Tensor* t) { return (float*)dev(t); };
+        return toErr(mnnb200_rnn_execute(mH.get(), f(inputs[0]), f(inputs[1]), f(inputs[2]), f(inputs[3]),
+                                         inputs.size() >= 5 ? f(inputs[4]) : nullptr, inputs.size() >= 6 ? f(inputs[5]) : nullptr,
+                                         f(outputs[0]), f(outputs[1]), outputs.size() >= 3 ? f(outputs[2]) : nullptr),
+                     "rnn");
+    }
+private:
+    const Op* mOp;
+    ExecHandle mH;
+};
+
 // Cast between int32 and fp32 (CPUCast's CastDataType): an attention mask's int32 -> fp32, or fp32 -> int32 (truncation)
 class CastExec : public B200Exec {
 public:
@@ -1560,6 +1619,10 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
         case OpType_ScatterNd:
         case OpType_ScatterElements:
             if (!quantOut && ScatterExec::takes(op, inputs, outputs)) e = ScatterExec::create(this, op);
+            break;
+        case OpType_LSTM:
+        case OpType_RNN:
+            if (!quantOut && RnnExec::takes(op, inputs, outputs)) e = RnnExec::create(this, op);
             break;
         case OpType_Cast: {
             const int dir = quantOut ? -1 : CastExec::direction(op, inputs, outputs);

@@ -36,11 +36,15 @@ MODELS = {   # --model: (fixture under oracle/_ref, name in the JSON line)
     "vit": ("vit_f32.mnn", "ViT-style encoder fp32, 4 layers, D 192, 64x64 image (seeded weights, oracle/refdump_gather.cpp)"),
     "pillars": ("pillars_f32.mnn", "PointPillars-style BEV net fp32, 2,048 pillars into 64x48, batch 1 (seeded weights, oracle/refdump_scatter.cpp)"),
     "gnn": ("gnn_f32.mnn", "GraphSAGE-mean-style net fp32, 512 nodes, 4,096 skewed edges, batch 1 (seeded weights, oracle/refdump_scatter.cpp)"),
+    "crnn": ("crnn_f32.mnn", "CRNN-style text recogniser fp32, 32x128 grey, 2 BiLSTM H 256 (seeded weights, oracle/refdump_rnn.cpp)"),
+    "kws": ("kws_f32.mnn", "streaming keyword-spotter chunk fp32, 16 frames, LSTM H 128 + RNN H 64 with states (seeded weights, oracle/refdump_rnn.cpp)"),
 }
 # models whose inputs refdump's bench does not fill (int32 token ids and masks): timed by oracle/refdump_gather's bench instead
 GATHER_HARNESS = {"bert", "vit"}
 # models with int32 pillar cells or edge lists, built for batch 1: timed at batch 1 by oracle/refdump_scatter's bench
 SCATTER_HARNESS = {"pillars", "gnn"}
+# models with sequence and state inputs (batch on dim 1): timed by oracle/refdump_rnn's bench
+RNN_HARNESS = {"crnn", "kws"}
 
 
 def shapes_from_cpu_run(model, refdump, env):
@@ -165,6 +169,9 @@ def main():
     if a.model in SCATTER_HARNESS:
         from oracle import scatter_oracle
         harness = scatter_oracle.REFDUMP_SCATTER
+    if a.model in RNN_HARNESS:
+        from oracle import rnn_oracle
+        harness = rnn_oracle.REFDUMP_RNN
     penv = dict(env, REFDUMP_BENCH_WINDOWS="5", REFDUMP_PLUGIN=os.path.join(ROOT, "mnn_b200", "libmnn_b200_plugin.so"))
     p = refdump_bench(harness, model, a.batch, 4, penv, 20)
     res.update(plugin_e2e_img_per_s=p["img_per_s"], plugin_e2e_ms=p["ms_median_window"], plugin_created=p["plugin_created"],
