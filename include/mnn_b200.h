@@ -169,7 +169,9 @@ MNNB200_API mnnb200_status mnnb200_reduce_f32(mnnb200_runtime* rt, const float* 
  *      bind:   after every member's resize; xs[i] / ys[i] = member i's NHWC16 input / output (must not alias another
  *              member's output: members are NOT ordered against each other).  NOT_SUPPORT if the conv-group kernel does
  *              not take a member (mnnb200_conv_int8_group_plan says which).
- *      execute: enqueue the one launch on the runtime's stream.  NO_EXECUTION until bound, and again once a member has been
+ *      execute: enqueue the group's launches on the runtime's stream: one per kernel that runs a member (the shallow
+ *              kernel for 1x1 convs of one K block up to 96 columns wide, then the conv-group kernel for the rest; the last
+ *              field of mnnb200_conv_int8_group_plan says which).  NO_EXECUTION until bound, and again once a member has been
  *              resized since the last bind: bind again first. */
 MNNB200_API mnnb200_status mnnb200_conv_group_create(mnnb200_runtime* rt, mnnb200_exec* const* members, int count,
                                                      mnnb200_exec** out);
@@ -177,9 +179,10 @@ MNNB200_API mnnb200_status mnnb200_conv_group_bind(mnnb200_exec* group, const in
 MNNB200_API mnnb200_status mnnb200_conv_group_execute(mnnb200_exec* group);
 /* 1 if auto execute runs the (resized) conv on the conv-group kernel; such a conv can be a member of a conv group */
 MNNB200_API int mnnb200_conv_int8_groupable(mnnb200_exec* e);
-/* read-only view of the resized conv's layer on the conv-group kernel, as resize planned it: the first `count` (at most 10) of
+/* read-only view of the resized conv's layer on the conv-group kernel, as resize planned it: the first `count` (at most 11) of
  * {mode (0 = 1x1 GEMM, 1 = implicit GEMM), cb (bytes of K per TMA chunk: 128 / 64 / 32 / 16), bn (tile width), n_chunks, m_tiles,
- * num_kb (K blocks per tile), K, R (row boxes per M tile), TWp (pixels per row box), BH (output rows per box)} go to fields.
+ * num_kb (K blocks per tile), K, R (row boxes per M tile), TWp (pixels per row box), BH (output rows per box), kernel (0 = the
+ * conv-group kernel, 1 = the shallow kernel: mode 0, one K block, bn <= 96)} go to fields.
  * NO_EXECUTION before resize, NOT_SUPPORT if the conv-group kernel does not take the conv.  Changes nothing. */
 MNNB200_API mnnb200_status mnnb200_conv_int8_group_plan(mnnb200_exec* e, int* fields, int count);
 /* the schedule bind builds for a list of `layers` (<= 64) members with m_tiles[l] M tiles and n_chunks[l] n chunks (both from

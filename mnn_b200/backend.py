@@ -210,6 +210,15 @@ class ConvGroupExecution(Execution):
     def onExecute(self, inputs=None, outputs=None):
         return _capi.lib().mnnb200_conv_group_execute(self._h)
 
+    def launches(self) -> int:
+        """kernel launches per execute: one per kernel that runs a member (the last field of mnnb200_conv_int8_group_plan)"""
+        kernels = set()
+        for m in self.members:
+            f = (C.c_int * 11)()
+            check(_capi.lib().mnnb200_conv_int8_group_plan(m._h, f, 11), "conv_int8_group_plan")
+            kernels.add(f[10])
+        return len(kernels)
+
 
 def encode_winograd_attr(units):
     """WinogradInt8Attr::encode (source/core/WinogradInt8Attr.hpp:45-63): units = [(kyStart, kxStart, kernelY, kernelX,

@@ -2,8 +2,8 @@
 libmnn_b200_deconv.so (the float Deconvolution, include/mnn_b200_deconv.h), libmnn_b200_interp.so (the float Interp,
 include/mnn_b200_interp.h), libmnn_b200_gather.so (the gathers and the int32 / fp32 Cast, include/mnn_b200_gather.h) and
 libmnn_b200_scatter.so (ScatterNd and ScatterElements, include/mnn_b200_scatter.h) and libmnn_b200_rnn.so (LSTM and RNN,
-include/mnn_b200_rnn.h), the last six linked against libmnn_b200.so,
-in-tree for sm_90a (H100) with nvcc.  No torch involvement."""
+include/mnn_b200_rnn.h), the last six linked against libmnn_b200.so, and libmnn_b200_shallow.so (the shallow conv-group
+kernel, which libmnn_b200.so launches and links against), in-tree for sm_90a (H100) with nvcc.  No torch involvement."""
 import os
 import subprocess
 import sys
@@ -17,6 +17,7 @@ INTERP_LIB = os.path.join(HERE, "libmnn_b200_interp.so")
 GATHER_LIB = os.path.join(HERE, "libmnn_b200_gather.so")
 SCATTER_LIB = os.path.join(HERE, "libmnn_b200_scatter.so")
 RNN_LIB = os.path.join(HERE, "libmnn_b200_rnn.so")
+SHALLOW_LIB = os.path.join(HERE, "libmnn_b200_shallow.so")
 SOURCES = ["capi.cu", "conv_int8_mma.cu", "elementwise.cu", "gemm_i8_wgmma.cu", "winograd_int8.cu", "gemm_f16_wgmma.cu", "conv_int8_stem.cu", "conv_group_wgmma.cu", "linear_w8_gemv.cu", "conv_f32_wgmma.cu"]
 LLM_SOURCES = ["llm_ops.cu", "llm_capi.cu"]
 DECONV_SOURCES = ["deconv_f32_wgmma.cu", "deconv_capi.cu"]
@@ -24,11 +25,13 @@ INTERP_SOURCES = ["interp_f32.cu", "interp_capi.cu"]
 GATHER_SOURCES = ["gather.cu", "gather_capi.cu"]
 SCATTER_SOURCES = ["scatter.cu", "scatter_capi.cu"]
 RNN_SOURCES = ["rnn.cu", "rnn_capi.cu"]
+# the shallow conv-group kernel, launched by libmnn_b200.so, which links against it
+SHALLOW_SOURCES = ["conv_group_shallow_wgmma.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ARCH + ["-lineinfo", "-O3", "-std=c++17",
               "-Xcompiler", "-fPIC,-ffp-contract=off,-fvisibility=hidden", "--expt-relaxed-constexpr"]
 # every float operation in that file is an explicit intrinsic / PTX instruction: no implicit contraction wanted anywhere in it
-PER_FILE_FLAGS = {"conv_group_wgmma.cu": ["--fmad=false"], "interp_f32.cu": ["--fmad=false"]}
+PER_FILE_FLAGS = {"conv_group_wgmma.cu": ["--fmad=false"], "conv_group_shallow_wgmma.cu": ["--fmad=false"], "interp_f32.cu": ["--fmad=false"]}
 
 
 def _compile(srcs, nvcc, verbose):
@@ -51,7 +54,7 @@ def _compile(srcs, nvcc, verbose):
 
 
 def build(force=False, verbose=False):
-    """the seven libraries; returns the path of libmnn_b200.so"""
+    """the eight libraries; returns the path of libmnn_b200.so"""
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
     llm_srcs = [os.path.join(CSRC, s) for s in LLM_SOURCES]
     inc = os.path.join(HERE, "..", "include")
@@ -70,8 +73,13 @@ def build(force=False, verbose=False):
     rnn_deps = deps + rnn_srcs + [os.path.join(inc, "mnn_b200_rnn.h")]
     fresh = lambda lib, ds: os.path.exists(lib) and all(os.path.getmtime(lib) > os.path.getmtime(d) for d in ds)
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    if force or not fresh(LIB, deps):
-        subprocess.check_call([nvcc, "-shared", "-o", LIB] + _compile(srcs, nvcc, verbose) + ARCH + ["-lcudart"])
+    shallow_srcs = [os.path.join(CSRC, s) for s in SHALLOW_SOURCES]
+    shallow_deps = shallow_srcs + [os.path.join(CSRC, f) for f in os.listdir(CSRC) if f.endswith((".h", ".cuh"))]
+    if force or not fresh(SHALLOW_LIB, shallow_deps):
+        subprocess.check_call([nvcc, "-shared", "-o", SHALLOW_LIB] + _compile(shallow_srcs, nvcc, verbose) + ARCH + ["-lcudart"])
+    if force or not fresh(LIB, deps + [SHALLOW_LIB]):
+        subprocess.check_call([nvcc, "-shared", "-o", LIB] + _compile(srcs, nvcc, verbose) + ARCH +
+                              ["-L" + HERE, "-lmnn_b200_shallow", "-Xlinker", "-rpath,$ORIGIN", "-lcudart"])
     if force or not fresh(LLM_LIB, llm_deps + [LIB]):
         subprocess.check_call([nvcc, "-shared", "-o", LLM_LIB] + _compile(llm_srcs, nvcc, verbose) + ARCH +
                               ["-L" + HERE, "-lmnn_b200", "-Xlinker", "-rpath,$ORIGIN", "-lcudart"])

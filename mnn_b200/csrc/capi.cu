@@ -141,6 +141,7 @@ struct ConvPlan {
     bool gemm = false;    // 1x1, stride 1, no pad: mode 0 on the conv-group kernel
     bool stem = false;    // <= 4 input channels: the dp4a stem kernel
     bool group = false;   // the conv-group kernel takes it: q / g / tmap_b hold the layer and the schedule word can address it
+    bool shallow = false; // group only: a 1x1 layer of one K block the shallow kernel takes (conv_group_shallow_wgmma.cu)
     GroupLayerParams q;   // y = nullptr
     GroupConvGeom g;      // mode 1 only; hcls / wcls / corr point into the execution's d_border
     CUtensorMap tmap_b;   // weights, boxes of q.cb bytes x q.bn rows
@@ -234,15 +235,19 @@ static mnnb200_status conv_create_common(const mnnb200_conv_desc* desc, const in
     return MNNB200_OK;
 }
 
-// ---- conv group: one persistent launch over a list of convolutions (conv_group_wgmma.cu) ----------------------------
-struct GroupState {
-    std::vector<ConvInt8Exec*> members;
-    std::vector<unsigned> built_resizes;    // each member's resize count at the last successful build; empty: not built
+// ---- conv group: persistent launches over a list of convolutions (conv_group_wgmma.cu, conv_group_shallow_wgmma.cu) ---
+// One persistent launch over the members one kernel takes.
+struct GroupLaunch {
     std::unique_ptr<GroupMapsParam> h_maps; // host: passed by value as the kernel's __grid_constant__ parameter
     DevBuf<GroupLayerParams> d_params;
     DevBuf<GroupConvGeom> d_geom;
     DevBuf<uint32_t> d_sched;               // grow-only
-    int n_layers = 0, sched_stride = 0, grid = 0;
+    int n_layers = 0, sched_stride = 0, grid = 0;   // n_layers 0: no member runs on this kernel
+};
+struct GroupState {
+    std::vector<ConvInt8Exec*> members;
+    std::vector<unsigned> built_resizes;    // each member's resize count at the last successful build; empty: not built
+    GroupLaunch shallow, wide;              // the members plan.shallow sends to the shallow kernel, and the others
     // Built, and no member resized since: a resize rebuilds the epilogue and border tables the layer table points at (and
     // may free them) and changes the layer's geometry.
     bool current() const {
@@ -385,6 +390,7 @@ static mnnb200_status conv_plan(ConvInt8Exec* e, int zin, const std::vector<floa
         }
     }
     plan.group = true;
+    plan.shallow = q.mode == 0 && q.num_kb == 1 && q.bn <= kGroupShallowMaxBN;
     return MNNB200_OK;
 }
 
@@ -444,67 +450,86 @@ static std::vector<uint32_t> group_schedule(const int* m_tiles, const int* n_chu
     return sched;
 }
 
-// Binds the members' plans to their activations: the A tensor maps, the y pointers and the schedule.
+// Binds the members' plans to their activations: the A tensor maps, the y pointers and the schedule, for each kernel over the
+// members it takes.  The shallow kernel's warpgroups load 64-row halves of the M tiles.
 static mnnb200_status group_build(GroupState& gs, mnnb200_runtime* rt, const int8_t* const* xs, int8_t* const* ys,
                                   double* cost_bytes, double* cost_macs) {
-    const int L = (int)gs.members.size();
     gs.built_resizes.clear();
     CK(cudaSetDevice(rt->device));
-    if (!gs.h_maps) gs.h_maps = std::make_unique<GroupMapsParam>();
-    mnnb200_status st;
-    if ((st = gs.d_params.reserve(kGroupMaxLayers)) || (st = gs.d_geom.reserve(kGroupMaxLayers))) return st;
-    static_assert(sizeof(CUtensorMap) == sizeof(CUtensorMap_st_opaque), "tensor map size");
-    std::vector<GroupLayerParams> prm(L);
-    std::vector<GroupConvGeom> geo(L);
-    std::vector<int> m_tiles(L), n_chunks(L);
     if (cost_bytes) *cost_bytes = 0;
     if (cost_macs) *cost_macs = 0;
-    for (int l = 0; l < L; ++l) {
-        const ConvInt8Exec* e = gs.members[l];
+    for (const ConvInt8Exec* e : gs.members)
         if (!e->resized || !e->plan.group) return fail(MNNB200_NOT_SUPPORT, "conv group: a member is not a resized conv the wgmma group kernel takes");
-        const ConvParams& p = e->p;
-        const GroupLayerParams& q = e->plan.q;
-        if ((uintptr_t)ys[l] % 8) return fail(MNNB200_INVALID_VALUE, "conv group: an output is not 8-byte aligned");
-        prm[l] = q;
-        prm[l].y = ys[l];
-        geo[l] = e->plan.g;
-        CUtensorMap* ta = reinterpret_cast<CUtensorMap*>(&gs.h_maps->a[l]);
-        CUtensorMap* ta1 = reinterpret_cast<CUtensorMap*>(&gs.h_maps->a1[l]);
-        memcpy(&gs.h_maps->b[l], &e->plan.tmap_b, sizeof(CUtensorMap));
-        if (q.mode == 0) {
-            cuuint64_t dims[2] = {(cuuint64_t)e->Cp, (cuuint64_t)p.M};
-            cuuint64_t strides[1] = {(cuuint64_t)e->Cp};
-            cuuint32_t box[2] = {(cuuint32_t)q.cb, 128u};
-            if ((st = make_tmap_u8(ta, xs[l], 2, dims, strides, box))) return st;
-        } else {
-            // A: one 4D {C, W', H, N} view of the NHWC16 input per column parity (W' = every sw-th column)
-            for (int par = 0; par < p.sw; ++par) {
-                cuuint64_t dims[4] = {(cuuint64_t)e->Cp, (cuuint64_t)((p.IW - par + p.sw - 1) / p.sw), (cuuint64_t)p.IH, (cuuint64_t)p.N};
-                cuuint64_t strides[3] = {(cuuint64_t)p.sw * e->Cp, (cuuint64_t)p.IW * e->Cp, (cuuint64_t)p.IH * p.IW * e->Cp};
-                cuuint32_t box[4] = {(cuuint32_t)q.cb, (cuuint32_t)q.TWp, (cuuint32_t)e->plan.g.BH, 1u};
-                if ((st = make_tmap_u8(par ? ta1 : ta, xs[l] + (size_t)par * e->Cp, 4, dims, strides, box))) return st;
+    static_assert(sizeof(CUtensorMap) == sizeof(CUtensorMap_st_opaque), "tensor map size");
+    for (const bool shallow : {true, false}) {
+        GroupLaunch& gl = shallow ? gs.shallow : gs.wide;
+        std::vector<int> idx;
+        for (int l = 0; l < (int)gs.members.size(); ++l)
+            if (gs.members[l]->plan.shallow == shallow) idx.push_back(l);
+        const int L = (int)idx.size();
+        gl.n_layers = 0;
+        if (L == 0) continue;
+        if (!gl.h_maps) gl.h_maps = std::make_unique<GroupMapsParam>();
+        mnnb200_status st;
+        if ((st = gl.d_params.reserve(kGroupMaxLayers)) || (st = gl.d_geom.reserve(kGroupMaxLayers))) return st;
+        std::vector<GroupLayerParams> prm(L);
+        std::vector<GroupConvGeom> geo(L);
+        std::vector<int> m_tiles(L), n_chunks(L);
+        for (int l = 0; l < L; ++l) {
+            const ConvInt8Exec* e = gs.members[idx[l]];
+            const ConvParams& p = e->p;
+            const GroupLayerParams& q = e->plan.q;
+            if ((uintptr_t)ys[idx[l]] % 8) return fail(MNNB200_INVALID_VALUE, "conv group: an output is not 8-byte aligned");
+            prm[l] = q;
+            prm[l].y = ys[idx[l]];
+            geo[l] = e->plan.g;
+            CUtensorMap* ta = reinterpret_cast<CUtensorMap*>(&gl.h_maps->a[l]);
+            CUtensorMap* ta1 = reinterpret_cast<CUtensorMap*>(&gl.h_maps->a1[l]);
+            memcpy(&gl.h_maps->b[l], &e->plan.tmap_b, sizeof(CUtensorMap));
+            if (q.mode == 0) {
+                cuuint64_t dims[2] = {(cuuint64_t)e->Cp, (cuuint64_t)p.M};
+                cuuint64_t strides[1] = {(cuuint64_t)e->Cp};
+                cuuint32_t box[2] = {(cuuint32_t)q.cb, shallow ? 64u : 128u};
+                if ((st = make_tmap_u8(ta, xs[idx[l]], 2, dims, strides, box))) return st;
+            } else {
+                // A: one 4D {C, W', H, N} view of the NHWC16 input per column parity (W' = every sw-th column)
+                for (int par = 0; par < p.sw; ++par) {
+                    cuuint64_t dims[4] = {(cuuint64_t)e->Cp, (cuuint64_t)((p.IW - par + p.sw - 1) / p.sw), (cuuint64_t)p.IH, (cuuint64_t)p.N};
+                    cuuint64_t strides[3] = {(cuuint64_t)p.sw * e->Cp, (cuuint64_t)p.IW * e->Cp, (cuuint64_t)p.IH * p.IW * e->Cp};
+                    cuuint32_t box[4] = {(cuuint32_t)q.cb, (cuuint32_t)q.TWp, (cuuint32_t)e->plan.g.BH, 1u};
+                    if ((st = make_tmap_u8(par ? ta1 : ta, xs[idx[l]] + (size_t)par * e->Cp, 4, dims, strides, box))) return st;
+                }
             }
+            if (p.sw == 1) *ta1 = *ta;
+            if (cost_bytes) *cost_bytes += e->cost_bytes;
+            if (cost_macs) *cost_macs += e->cost_macs;
+            m_tiles[l] = q.m_tiles;
+            n_chunks[l] = q.n_chunks;
         }
-        if (p.sw == 1) *ta1 = *ta;
-        if (cost_bytes) *cost_bytes += e->cost_bytes;
-        if (cost_macs) *cost_macs += e->cost_macs;
-        m_tiles[l] = q.m_tiles;
-        n_chunks[l] = q.n_chunks;
+        int grid = 0, stride = 0;
+        const std::vector<uint32_t> sched = group_schedule(m_tiles.data(), n_chunks.data(), L, rt->prop.multiProcessorCount, &grid, &stride);
+        if ((st = gl.d_sched.reserve(sched.size()))) return st;
+        CK(cudaMemcpy(gl.d_params, prm.data(), sizeof(GroupLayerParams) * L, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(gl.d_geom, geo.data(), sizeof(GroupConvGeom) * L, cudaMemcpyHostToDevice));
+        CK(cudaMemcpy(gl.d_sched, sched.data(), sched.size() * 4, cudaMemcpyHostToDevice));
+        gl.sched_stride = stride;
+        gl.grid = grid;
+        gl.n_layers = L;
     }
-    int grid = 0, stride = 0;
-    const std::vector<uint32_t> sched = group_schedule(m_tiles.data(), n_chunks.data(), L, rt->prop.multiProcessorCount, &grid, &stride);
-    if ((st = gs.d_sched.reserve(sched.size()))) return st;
-    CK(cudaMemcpy(gs.d_params, prm.data(), sizeof(GroupLayerParams) * L, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(gs.d_geom, geo.data(), sizeof(GroupConvGeom) * L, cudaMemcpyHostToDevice));
-    CK(cudaMemcpy(gs.d_sched, sched.data(), sched.size() * 4, cudaMemcpyHostToDevice));
-    gs.sched_stride = stride;
-    gs.grid = grid;
-    gs.n_layers = L;
     for (const ConvInt8Exec* e : gs.members) gs.built_resizes.push_back(e->resizes);
     return MNNB200_OK;
 }
+// The shallow kernel first, then the conv-group kernel over the other members.  The two write different outputs and read
+// nothing the other writes, so the second launch is programmatic: its CTAs take each SM as soon as the first's CTA there ends.
 static mnnb200_status group_launch(const GroupState& gs, cudaStream_t stream) {
-    CK(launch_conv_group(gs.h_maps.get(), gs.d_params, gs.d_geom, gs.n_layers, gs.d_sched, gs.sched_stride, gs.grid, stream));
+    const GroupLaunch& s = gs.shallow;
+    const GroupLaunch& w = gs.wide;
+    if (s.n_layers) {
+        ++g_launch_count;
+        CK(launch_conv_group_shallow(s.h_maps.get(), s.d_params, s.n_layers, s.d_sched, s.sched_stride, s.grid, stream));
+    }
+    if (w.n_layers)
+        CK(launch_conv_group(w.h_maps.get(), w.d_params, w.d_geom, w.n_layers, w.d_sched, w.sched_stride, w.grid, s.n_layers > 0, stream));
     return MNNB200_OK;
 }
 
@@ -973,7 +998,8 @@ mnnb200_status mnnb200_conv_int8_group_plan(mnnb200_exec* ex, int* fields, int c
     if (!e->resized) return fail(MNNB200_NO_EXECUTION, "conv_int8_group_plan before resize");
     if (!e->plan.group) return fail(MNNB200_NOT_SUPPORT, "conv_int8_group_plan: the conv-group kernel does not take this conv");
     const GroupLayerParams& q = e->plan.q;
-    const int v[] = {q.mode, q.cb, q.bn, q.n_chunks, q.m_tiles, q.num_kb, q.K, q.R, q.TWp, e->plan.g.BH};
+    // the last field: the kernel that runs the layer in a group, 0 the conv-group kernel, 1 the shallow kernel
+    const int v[] = {q.mode, q.cb, q.bn, q.n_chunks, q.m_tiles, q.num_kb, q.K, q.R, q.TWp, e->plan.g.BH, e->plan.shallow ? 1 : 0};
     return copy_fields(v, fields, count);
 }
 mnnb200_status mnnb200_conv_group_schedule(const int* m_tiles, const int* n_chunks, int layers, int sm_count, uint32_t* items,

@@ -29,8 +29,8 @@
 //              (layer, n chunk), the next one copied in with cp.async while the current item runs
 #include <cuda.h>
 #include <cstdlib>
-#include <type_traits>
 #include "common.cuh"
+#include "conv_group_epilogue.cuh"
 #include "hopper_common.cuh"
 #include "host_util.h"
 #include "kernels.h"
@@ -73,34 +73,6 @@ constexpr int kCgThreads = kConsumerThreads + 128;
 constexpr int kProducerRegs = 88, kConsumerRegs = 208;
 static_assert(kProducerRegs + 2 * kConsumerRegs <= 512, "conv group kernel: register split does not fit");
 
-// requant_cpu_exact (common.cuh) WITHOUT its clamp, which the epilogue applies to the rounded integers (see consume_run's
-// column run for why that is exact).  The +-0.5 is copysign(0.5, f) = (f & sign) | 0.5 in one LOP3 with 0.5 in a register:
-// written as an and and an or of two immediates, ptxas emits two LOP3s.
-__device__ __forceinline__ int round_half_away(float f) {
-    uint32_t h;
-    asm("lop3.b32 %0, %1, 0x80000000, 0x3f000000, 0xEA;" : "=r"(h) : "r"(__float_as_uint(f)));   // 0xEA: (a & b) | c
-    return __float2int_rz(__fadd_rn(f, __uint_as_float(h)));
-}
-__device__ __forceinline__ int requant_round(int acc_u, float wscale, float scale_x, float bias_float) {
-    float f = __fmul_rn(__int2float_rn(acc_u), wscale);
-    f = __fmul_rn(f, scale_x);
-    return round_half_away(__fadd_rn(f, bias_float));
-}
-// the same sequence for accumulators with |acc_u| < 2^22: float(acc_u) = as_float(0x4B400000 + acc_u) - 1.5 * 2^23 is exact (the
-// integer lands in the mantissa of a float in [2^23, 2^24)): one IADD + one FADD instead of an I2F on the conversion unit
-// (the conv-group kernel's accumulators start at 0x4B400000 + 128 sum w, so acc_m here is already 0x4B400000 + acc_u)
-__device__ __forceinline__ int requant_round_small(int acc_m, float wscale, float scale_x, float bias_float) {
-    float f = __fmul_rn(__fsub_rn(__int_as_float(acc_m), 12582912.0f), wscale);
-    f = __fmul_rn(f, scale_x);
-    return round_half_away(__fadd_rn(f, bias_float));
-}
-// two int32 -> one s16 pair, each saturated to [-32768, 32767] (one I2IP): lo in bits 0-15, hi in bits 16-31
-__device__ __forceinline__ uint32_t pack_sat_s16x2(int lo, int hi) {
-    uint32_t d;
-    asm("cvt.pack.sat.s16.s32 %0, %1, %2;" : "=r"(d) : "r"(hi), "r"(lo));
-    return d;
-}
-
 // work item = `cnt` consecutive M tiles of one (layer, n chunk), encoded as kernels.h describes.
 // The producer pays its per-item bookkeeping (schedule word, layer parameters, descriptors) once per item.
 __device__ __forceinline__ void decode_item(uint32_t w, int& layer, int& nc, int& mt, int& cnt) {
@@ -108,17 +80,6 @@ __device__ __forceinline__ void decode_item(uint32_t w, int& layer, int& nc, int
     nc = (int)((w >> kGroupItemChunkShift) & kGroupItemChunkMask);
     cnt = (int)((w >> kGroupItemCountShift) & kGroupItemCountMask) + 1;
     mt = (int)(w & kGroupItemTileMask);
-}
-
-// A global store the compiler does not treat as a memory write (no "memory" clobber): nothing in the kernel reads the output
-// back, and the compiler may then keep shared-memory values in registers and issue later loads across it.  Predicated on
-// j < lim inside the instruction, so a run of such stores over a column loop stays one straight run of code.
-__device__ __forceinline__ void st_global_v2_if(int8_t* p, uint32_t lo, uint32_t hi, int j, int lim) {
-    asm volatile("{\n .reg .pred q;\n setp.lt.s32 q, %3, %4;\n @q st.global.v2.b32 [%0], {%1, %2};\n}\n" ::"l"(p), "r"(lo), "r"(hi),
-                 "r"(j), "r"(lim));
-}
-__device__ __forceinline__ void st_global_b32_if(int8_t* p, uint32_t v, int j, int lim) {
-    asm volatile("{\n .reg .pred q;\n setp.lt.s32 q, %2, %3;\n @q st.global.b32 [%0], %1;\n}\n" ::"l"(p), "r"(v), "r"(j), "r"(lim));
 }
 
 // Has the phase of parity `parity` of barrier `bar` completed, in EVERY thread of this consumer warpgroup?  test_wait does not
@@ -204,13 +165,12 @@ __device__ __forceinline__ void consume_run(const GroupLayerParams& lp, const Gr
     // registers next to BN / 2 accumulators do not fit.
     constexpr bool kRegConsts = BN <= kConstRegsMaxBN;
     float2 ws[kRegConsts ? BN / 8 : 1], bs[kRegConsts ? BN / 8 : 1];
-    auto load_consts = [&](int j, float2& w, float2& b) {
-        w = *reinterpret_cast<const float2*>(wscale + 8 * j + 2 * q4);
-        b = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4);
-    };
     if constexpr (kRegConsts) {
 #pragma unroll
-        for (int j = 0; j < BN / 8; ++j) load_consts(j, ws[j], bs[j]);
+        for (int j = 0; j < BN / 8; ++j) {
+            ws[j] = *reinterpret_cast<const float2*>(wscale + 8 * j + 2 * q4);
+            bs[j] = *reinterpret_cast<const float2*>(bias + 8 * j + 2 * q4);
+        }
     }
     // |sum (x + 128) w| <= 128 * 255 * 128 < 2^22.  Broadcast like cb: the epilogue branches on it and on mode while the next
     // tile's wgmmas run, and a branch ptxas cannot prove uniform there makes it serialise the wgmmas
@@ -368,64 +328,14 @@ __device__ __forceinline__ void consume_run(const GroupLayerParams& lp, const Gr
             }
             corr = __any_sync(0xffffffffu, corr);
         }
-        // Then one straight run over every column group of both rows, the BN-wide tile whole: columns past the chunk's valid
-        // ones read zero constants, only their stores are predicated off (a thread's run of channels is valid or not as a
-        // whole: valid columns come in multiples of 16).  With no control flow inside, ptxas overlaps the requant chains.  The
-        // requant path and the border correction are chosen once per run.
-        auto columns = [&](auto small, auto with_corr) {
-            // 4 rounded outputs -> their 4 clamped bytes, q[0] in byte 0 (see clamp above)
-            auto clamp4 = [&](const int* q) -> uint32_t {
-                const uint32_t p0 = __vmaxs2(__vmins2(pack_sat_s16x2(q[0], q[1]), max2), min2);
-                const uint32_t p1 = __vmaxs2(__vmins2(pack_sat_s16x2(q[2], q[3]), max2), min2);
-                return __byte_perm(p0, p1, 0x6420);
-            };
-#pragma unroll
-            for (int G = 0; G < (BN + 31) / 32; ++G) {
-                constexpr int kFull = 4;
-                const int S = BN - 32 * G >= 32 ? kFull : 2;      // column pairs of the thread per row in this group
-                const int ch = 32 * G + 2 * S * q4;              // its first channel
-                float2 wg[kFull], bg[kFull];         // the group's constants serve both rows
-#pragma unroll
-                for (int s = 0; s < S; ++s) {
-                    if constexpr (kRegConsts) { wg[s] = ws[4 * G + s]; bg[s] = bs[4 * G + s]; }
-                    else load_consts(4 * G + s, wg[s], bg[s]);
-                }
-#pragma unroll
-                for (int h = 0; h < 2; ++h) {
-                    int q[2 * kFull];
-#pragma unroll
-                    for (int s = 0; s < S; ++s) {
-                        const int j = 4 * G + s;
-                        int a0 = acc[j * 4 + 2 * h], a1 = acc[j * 4 + 2 * h + 1];
-                        if constexpr (decltype(with_corr)::value) {
-                            const int2 k = __ldg(reinterpret_cast<const int2*>(corrp[h] + 8 * j + 2 * q4));
-                            a0 += k.x;
-                            a1 += k.y;
-                        }
-                        if constexpr (decltype(small)::value) {   // |acc_u| < 2^22: int -> float on the FP32 pipe (exact)
-                            q[2 * s] = requant_round_small(a0, wg[s].x, scale_x, bg[s].x);
-                            q[2 * s + 1] = requant_round_small(a1, wg[s].y, scale_x, bg[s].y);
-                        } else {
-                            q[2 * s] = requant_round(a0, wg[s].x, scale_x, bg[s].x);
-                            q[2 * s + 1] = requant_round(a1, wg[s].y, scale_x, bg[s].y);
-                        }
-                    }
-                    const uint32_t lo = clamp4(q) & mlo[G];
-                    if (S == kFull) {
-                        const uint32_t hi = clamp4(q + 4) & mhi[G];
-                        st_global_v2_if(yrow[h] + ch, lo, hi, ch, lim[h]);
-                    } else {
-                        st_global_b32_if(yrow[h] + ch, lo, ch, lim[h]);
-                    }
-                }
-            }
-        };
+        // Then one straight run over every column group of both rows (group_column_run); the requant path and the border
+        // correction are chosen once per run.
         if (corr) {
-            if (small_acc) columns(std::true_type{}, std::true_type{});
-            else columns(std::false_type{}, std::true_type{});
+            if (small_acc) group_column_run<BN, kRegConsts, true, true>(acc, ws, bs, wscale, bias, q4, scale_x, min2, max2, mlo, mhi, yrow, lim, corrp);
+            else group_column_run<BN, kRegConsts, false, true>(acc, ws, bs, wscale, bias, q4, scale_x, min2, max2, mlo, mhi, yrow, lim, corrp);
         } else {
-            if (small_acc) columns(std::true_type{}, std::false_type{});
-            else columns(std::false_type{}, std::false_type{});
+            if (small_acc) group_column_run<BN, kRegConsts, true, false>(acc, ws, bs, wscale, bias, q4, scale_x, min2, max2, mlo, mhi, yrow, lim, corrp);
+            else group_column_run<BN, kRegConsts, false, false>(acc, ws, bs, wscale, bias, q4, scale_x, min2, max2, mlo, mhi, yrow, lim, corrp);
         }
         if constexpr (kTwoSets) {
             // the next tile starts in acc: the preset, + its first K block if that was issued (into nxt, which is written by
@@ -707,17 +617,29 @@ conv_group_wgmma_kernel(const __grid_constant__ GroupMapsParam mp, const GroupLa
             }
         }
     }
+    // launched programmatically after the shallow kernel (group_launch, capi.cu): this grid ends only after that one has, so
+    // the launches after it on the stream see both grids' outputs (a no-op in a launch without a programmatic predecessor)
+    asm volatile("griddepcontrol.wait;\n" ::: "memory");
 }
 
 }  // namespace
 
 cudaError_t launch_conv_group(const GroupMapsParam* maps_host, const GroupLayerParams* params, const GroupConvGeom* geom, int n_layers,
-                              const uint32_t* sched, int sched_stride, int grid, cudaStream_t stream) {
+                              const uint32_t* sched, int sched_stride, int grid, bool programmatic, cudaStream_t stream) {
     cudaError_t e = ensure_max_dynamic_smem((const void*)conv_group_wgmma_kernel, 227 * 1024);
     if (e != cudaSuccess) return e;
     ++g_launch_count;
-    conv_group_wgmma_kernel<<<grid, kCgThreads, kSmemTotal + 1024, stream>>>(*maps_host, params, geom, n_layers, sched, sched_stride);
-    return cudaGetLastError();
+    cudaLaunchConfig_t cfg = {};
+    cfg.gridDim = dim3(grid);
+    cfg.blockDim = dim3(kCgThreads);
+    cfg.dynamicSmemBytes = kSmemTotal + 1024;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr[1];
+    attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+    attr[0].val.programmaticStreamSerializationAllowed = 1;
+    cfg.attrs = attr;
+    cfg.numAttrs = programmatic ? 1 : 0;
+    return cudaLaunchKernelEx(&cfg, conv_group_wgmma_kernel, *maps_host, params, geom, n_layers, sched, sched_stride);
 }
 
 }  // namespace mnnb200

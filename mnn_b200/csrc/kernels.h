@@ -132,8 +132,15 @@ struct GroupConvGeom {               // mode 1 only; stays in global memory (rea
 constexpr int kGroupItemLayerShift = 26, kGroupItemChunkShift = 20, kGroupItemCountShift = 14;
 constexpr uint32_t kGroupItemChunkMask = 0x3fu, kGroupItemCountMask = 0x3fu, kGroupItemTileMask = 0x3fffu;
 constexpr int kGroupMaxNChunks = 63, kGroupMaxMTiles = 16383;
+// The shallow conv-group kernel (conv_group_shallow_wgmma.cu, libmnn_b200_shallow.so) takes the mode-0 layers of one K block
+// whose tile width is at most kGroupShallowMaxBN: the widths its 112-register consumers hold without spills (ptxas -v).
+constexpr int kGroupShallowMaxBN = 96;
+__attribute__((visibility("default"))) cudaError_t launch_conv_group_shallow(const GroupMapsParam* maps_host,
+                                                                            const GroupLayerParams* params, int n_layers,
+                                                                            const uint32_t* sched, int sched_stride, int grid,
+                                                                            cudaStream_t stream);
 cudaError_t launch_conv_group(const GroupMapsParam* maps_host, const GroupLayerParams* params, const GroupConvGeom* geom, int n_layers,
-                              const uint32_t* sched, int sched_stride, int grid, cudaStream_t stream);
+                              const uint32_t* sched, int sched_stride, int grid, bool programmatic, cudaStream_t stream);
 
 // CTA-pair variant (2-CTA cluster, 256 x bn per pair, B halves multicast to both CTAs) for the tensor-bound linear layers;
 // fp32 dynamic-quant epilogue only.  tmap_b must have a box of bn/2 rows (each CTA of the pair loads half of the B tile);

@@ -89,7 +89,7 @@ class ConvPathSession:
                 self.singles = [l for l in self.layers if id(l[1]) not in ids]
         self.stream.synchronize()
         self.graph: Optional[torch.cuda.CUDAGraph] = None
-        self.launches_per_step = len(self.singles) + (1 if self.group is not None else 0)
+        self.launches_per_step = len(self.singles) + (self.group.launches() if self.group is not None else 0)
 
     def enqueue(self):
         for node, ex, x, y in self.singles:

@@ -1,9 +1,12 @@
 """Cost of one work item of the persistent conv-group launch (conv_group_wgmma.cu), per CTA: single-layer groups of a 1x1 int8
 conv at M = 32 x 112 x 112 rows (about 24 items of 128 rows per CTA on a 132-SM part), swept over the tile width (OC at
 K = 16) and over K (at OC = 32), plus the shallow 1x1 shapes of MobileNet-v2's first blocks.  Each configuration is one group launch captured in a CUDA graph and replayed back to back;
-the time is the median of several windows.  Cycles use the SM clock read while the replays run.  Next to each: the
+the time is the median of several windows.  "kernel" is the launch the plan chose for the layer: the conv-group kernel
+(128-row items on two consumer warpgroups) or, for one-K-block layers up to 96 wide, the shallow kernel (the same 128-row items
+split into 64-row halves over four consumer warpgroups).  Cycles use the SM clock read while the replays run.  Next to each: the
 algorithmic bytes (input + output activations, weights) and the time they take at the data-sheet HBM bandwidth.
 Usage (on the GPU): python tools/group_item_costs.py > item_costs.json"""
+import ctypes as C
 import json
 import os
 import subprocess
@@ -13,6 +16,7 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 import numpy as np  # noqa: E402
 import torch  # noqa: E402
 
+from mnn_b200 import _capi  # noqa: E402
 from mnn_b200.backend import ConvGroupExecution, Op, QuantAttr, Runtime, Tensor  # noqa: E402
 
 PEAK_GBS = 3350.0     # H100 SXM data-sheet HBM3 bandwidth
@@ -70,6 +74,8 @@ def measure(backend, stream, k, oc, steps=100, reps=7):
         clocks.append(float(smi("clocks.sm")))           # read while the window's replays are still running
         stream.synchronize()
         times.append(ev0.elapsed_time(ev1) * 1e3 / steps)
+    f = (C.c_int * 11)()
+    assert _capi.lib().mnnb200_conv_int8_group_plan(ex._h, f, 11) == 0
     us = sorted(times)[len(times) // 2]
     mhz = sorted(clocks)[len(clocks) // 2]
     M = N * H * W
@@ -77,7 +83,7 @@ def measure(backend, stream, k, oc, steps=100, reps=7):
     grid = min(items, backend.runtime.sm_count)
     per_cta = items / grid
     alg = M * up16(k) + M * up16(oc) + up16(oc) * up16(k)
-    return {"K": k, "OC": oc, "us": round(us, 2), "items": items, "items_per_cta": round(per_cta, 2),
+    return {"K": k, "OC": oc, "kernel": ("conv_group", "shallow")[f[10]], "us": round(us, 2), "items": items, "items_per_cta": round(per_cta, 2),
             "us_per_item": round(us / per_cta, 3), "cycles_per_item": round(us / per_cta * mhz),
             "sm_mhz": mhz, "alg_MB": round(alg / 1e6, 2), "hbm_us": round(alg / PEAK_GBS / 1e3, 2),
             "share_of_hbm": round(alg / PEAK_GBS / 1e3 / us, 3)}

@@ -1,8 +1,9 @@
 """Marginal cost of every layer INSIDE the persistent conv-group launch (MobileNet-v2 int8 conv path, batch 32): the step is
 timed with the group of all layers and then with a group of every layer but one, bound to the same tensors; the difference is
 what that layer costs in situ (cache state, co-scheduling with the other layers), next to its algorithmic bytes and the HBM
-time those bytes would take.  "alone" splits the step: the launches outside the group (stem, strided convs) and the group
-launch, each captured in a CUDA graph of its own and replayed back to back.  Usage (on the GPU): python tools/group_layer_costs.py > layer_costs.json"""
+time those bytes would take.  "alone" splits the step: the launches outside the group (stem, strided convs) and the group's
+launches, each captured in a CUDA graph of its own and replayed back to back; group_launches_ms splits the group into its
+shallow-kernel and conv-group-kernel launches (torch.profiler).  Usage (on the GPU): python tools/group_layer_costs.py > layer_costs.json"""
 import json
 import os
 import sys
@@ -67,7 +68,26 @@ def split(sess):
         assert sess.group.onExecute() == 0
 
     return {"step_ms": time_alone(sess, lambda: (singles(), group())), "singles_ms": time_alone(sess, singles),
-            "group_ms": time_alone(sess, group)}
+            "group_ms": time_alone(sess, group), "group_launches_ms": per_launch(sess, group)}
+
+
+def per_launch(sess, enqueue, steps=50):
+    """the group's launches (the shallow kernel, then the conv-group kernel) timed one by one under torch.profiler: mean device
+    ms per step of each kernel"""
+    from torch.profiler import ProfilerActivity, profile
+    for _ in range(5):
+        enqueue()
+    sess.stream.synchronize()
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        for _ in range(steps):
+            enqueue()
+        sess.stream.synchronize()
+    out = {}
+    for ev in prof.key_averages():
+        for name in ("conv_group_shallow_wgmma_kernel", "conv_group_wgmma_kernel"):
+            if name in ev.key:
+                out[name] = round(ev.device_time_total / 1e3 / steps, 4)
+    return out
 
 
 def main():
