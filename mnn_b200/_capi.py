@@ -184,6 +184,16 @@ RNN_SIGNATURES = {
 }
 _rnn_lib = None
 
+# libmnn_b200_grid_sample.so (include/mnn_b200_grid_sample.h): the float GridSample execution, on the runtime and execution handles above
+GRID_SAMPLE_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_grid_sample.so")
+GRID_SAMPLE_SIGNATURES = {
+    "mnnb200_grid_sample_f32_create": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.POINTER(P)]),
+    "mnnb200_grid_sample_f32_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int, _IP, _IP]),
+    "mnnb200_grid_sample_f32_execute": (C.c_int, [P, P, P, P]),
+    "mnnb200_grid_sample_f32_plan": (C.c_int, [P, _IP, C.c_int]),
+}
+_grid_sample_lib = None
+
 # libmnn_b200_llm.so (include/mnn_b200_llm.h): MNN-LLM's LayerNorm / RoPE executions, on the runtime and execution handles above
 LLM_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_llm.so")
 LLM_SIGNATURES = {
@@ -292,6 +302,22 @@ def rnn_lib():
             fn.argtypes = args
         _rnn_lib = L
     return _rnn_lib
+
+
+def grid_sample_lib():
+    """libmnn_b200_grid_sample.so with every GRID_SAMPLE_SIGNATURES symbol resolved (after libmnn_b200.so, whose handles it shares)"""
+    global _grid_sample_lib
+    if _grid_sample_lib is None:
+        lib()
+        if not os.path.exists(GRID_SAMPLE_LIB_PATH):
+            raise MnnB200Error(f"{GRID_SAMPLE_LIB_PATH} is missing: run `python -m mnn_b200.build` (there is no CPU fallback)")
+        L = C.CDLL(GRID_SAMPLE_LIB_PATH)
+        for name, (res, args) in GRID_SAMPLE_SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype = res
+            fn.argtypes = args
+        _grid_sample_lib = L
+    return _grid_sample_lib
 
 
 def lib():

@@ -548,6 +548,33 @@ class InterpF32Execution(Execution):
         return _capi.interp_lib().mnnb200_interp_f32_execute(self._h, inputs[0].ptr(), outputs[0].ptr())
 
 
+class GridSampleF32Execution(Execution):
+    """Float GridSample on NCHW fp32 tensors: the CPU backend's CPUGridSample.  inputs: x [n, c, (id,) ih, iw] and grid [n,
+    (od,) oh, ow, rank - 2]; the output [n, c, (od,) oh, ow].  op.extra: mode (0 bilinear, 1 nearest), padding (0 zeros, 1
+    border, 2 reflection, which samples as border) and align_corners."""
+
+    def __init__(self, backend, op: Op):
+        super().__init__(backend)
+        e = op.extra
+        check(_capi.grid_sample_lib().mnnb200_grid_sample_f32_create(backend.runtime._h, int(e.get("mode", 0)),
+                                                                     int(e.get("padding", 0)), int(bool(e.get("align_corners"))),
+                                                                     C.byref(self._h)), "grid_sample_f32_create")
+
+    def onResize(self, inputs, outputs):
+        x, g = inputs[0].shape, inputs[1].shape
+        rank = len(x)
+        if len(g) != rank or g[0] != x[0] or g[-1] != rank - 2:
+            return NOT_SUPPORT
+        ind, outd = (C.c_int * (rank - 2))(*x[2:]), (C.c_int * (rank - 2))(*g[1:-1])
+        st = _capi.grid_sample_lib().mnnb200_grid_sample_f32_resize(self._h, rank, x[0], x[1], ind, outd)
+        if st == 0:
+            outputs[0].shape = (x[0], x[1]) + tuple(g[1:-1])
+        return st
+
+    def onExecute(self, inputs, outputs):
+        return _capi.grid_sample_lib().mnnb200_grid_sample_f32_execute(self._h, inputs[0].ptr(), inputs[1].ptr(), outputs[0].ptr())
+
+
 class GatherExecution(Execution):
     """Gather / GatherV2 / GatherND / GatherElements on 4-byte tensors (fp32 or int32) with int32 indices, shapes as given (any
     rank): the CPU backend's While loops of GeometryGather.cpp.  op.type: "Gather" (GatherV2 alike), "GatherND" or
@@ -682,5 +709,6 @@ def _create_deconv_f32(b, i, o, op):
 Backend.addCreator("DeconvF32", _create_deconv_f32)
 Backend.addCreator("DwDeconvF32", lambda b, i, o, op: DeconvF32Execution(b, op, depthwise=True))
 Backend.addCreator("InterpF32", lambda b, i, o, op: InterpF32Execution(b, op))
+Backend.addCreator("GridSampleF32", lambda b, i, o, op: GridSampleF32Execution(b, op))
 for _t in ("Gather", "GatherND", "GatherElements"):
     Backend.addCreator(_t, lambda b, i, o, op: GatherExecution(b, op))

@@ -43,6 +43,7 @@
 #include "../../../include/mnn_b200_scatter.h"
 #include "../../../include/mnn_b200_rnn.h"
 #include "../../../include/mnn_b200_interp.h"
+#include "../../../include/mnn_b200_grid_sample.h"
 #include "../../../include/mnn_b200_llm.h"
 
 namespace MNN {
@@ -1361,6 +1362,61 @@ private:
     ExecHandle mH;
 };
 
+// GridSample on float tensors (CPUGridSample): x [N, C, (D,) H, W] NCHW-linear (NC4HW4 is stored so here), grid [N, (oD,) oH, oW,
+// rank - 2] in a linear format (an NC4HW4 grid is declined: the CPU reads the grid linearly), y [N, C, (oD,) oH, oW].  The op's
+// mode, paddingMode and alignCorners are read as CPUGridSampleCreator reads them; REFLECTION samples as CLAMP there and here.
+// Declined: the backward form (and its third input), other input / output counts, non-fp32 or int8 tensors, ranks other than 4
+// and 5, a batch mismatch, a grid whose last dim is not rank - 2, and any index past 31 bits (resize refuses those).
+class GridSampleF32Exec : public ClonedFromOp<GridSampleF32Exec> {
+public:
+    GridSampleF32Exec(Backend* bn, const Op* op, mnnb200_exec* h) : ClonedFromOp(bn), mOp(op), mH(h) {}
+    static Execution* create(B200Backend* bn, const Op* op) {
+        auto gp = op->main_as_GridSample();
+        if (!gp || gp->backward()) return nullptr;
+        mnnb200_exec* h = nullptr;
+        if (mnnb200_grid_sample_f32_create(bn->handle(), (int)gp->mode(), (int)gp->paddingMode(), gp->alignCorners() ? 1 : 0, &h) !=
+            MNNB200_OK)
+            return nullptr;
+        return new GridSampleF32Exec(bn, op, h);
+    }
+    static bool takes(const Op* op, const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) {
+        auto gp = op->main_as_GridSample();
+        if (!gp || gp->backward() || inputs.size() != 2 || outputs.size() != 1) return false;
+        auto x = inputs[0], g = inputs[1], y = outputs[0];
+        for (auto t : {x, g, y})
+            if (!isF32(t) || isInt8(t)) return false;
+        const int rank = x->dimensions();
+        if ((rank != 4 && rank != 5) || g->dimensions() != rank || y->dimensions() != rank) return false;
+        if (linearFormat(x) != MNN_DATA_FORMAT_NCHW || linearFormat(y) != MNN_DATA_FORMAT_NCHW ||
+            TensorUtils::getDescribe(g)->dimensionFormat == MNN_DATA_FORMAT_NC4HW4)
+            return false;
+        if (g->length(0) != x->length(0) || g->length(rank - 1) != rank - 2) return false;
+        if (y->length(0) != x->length(0) || y->length(1) != x->length(1)) return false;
+        for (int i = 2; i < rank; ++i)
+            if (y->length(i) != g->length(i - 1)) return false;
+        return true;
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        if (!takes(mOp, inputs, outputs)) return NOT_SUPPORT;
+        auto x = inputs[0], g = inputs[1];
+        const int rank = x->dimensions();
+        int ind[3] = {0, 0, 0}, outd[3] = {0, 0, 0};
+        for (int i = 2; i < rank; ++i) {
+            ind[i - 2] = x->length(i);
+            outd[i - 2] = g->length(i - 1);
+        }
+        return toErr(mnnb200_grid_sample_f32_resize(mH.get(), rank, x->length(0), x->length(1), ind, outd), "GridSample fp32 resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        return toErr(mnnb200_grid_sample_f32_execute(mH.get(), (const float*)dev(inputs[0]), (const float*)dev(inputs[1]),
+                                                     (float*)dev(outputs[0])),
+                     "GridSample fp32");
+    }
+private:
+    const Op* mOp;
+    ExecHandle mH;
+};
+
 // Gather / GatherV2 / GatherND / GatherElements (the CPU runs them as While loops of GeometryGather.cpp; under Compiler_Geometry
 // they reach the backend unlowered) on tensors of 4-byte elements, fp32 or int32, with int32 indices.  Params and output are
 // linear in their logical dim order: any format but NC4HW4, which only a 4-D tensor may have (it is stored NCHW-linear here).
@@ -1752,6 +1808,9 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
             break;
         case OpType_Interp:
             if (!quantOut && InterpF32Exec::takes(inputs, outputs)) e = InterpF32Exec::create(this, op);
+            break;
+        case OpType_GridSample:
+            if (!quantOut && GridSampleF32Exec::takes(op, inputs, outputs)) e = GridSampleF32Exec::create(this, op);
             break;
         default:
             break;

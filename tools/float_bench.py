@@ -38,6 +38,8 @@ MODELS = {   # --model: (fixture under oracle/_ref, name in the JSON line)
     "gnn": ("gnn_f32.mnn", "GraphSAGE-mean-style net fp32, 512 nodes, 4,096 skewed edges, batch 1 (seeded weights, oracle/refdump_scatter.cpp)"),
     "crnn": ("crnn_f32.mnn", "CRNN-style text recogniser fp32, 32x128 grey, 2 BiLSTM H 256 (seeded weights, oracle/refdump_rnn.cpp)"),
     "kws": ("kws_f32.mnn", "streaming keyword-spotter chunk fp32, 16 frames, LSTM H 128 + RNN H 64 with states (seeded weights, oracle/refdump_rnn.cpp)"),
+    "flow": ("flow_f32.mnn", "two-frame flow-warp net fp32, 6x64x64, bilinear GridSample at 16x16 (seeded weights, oracle/refdump_grid_sample.cpp)"),
+    "lut": ("lut_f32.mnn", "image-adaptive 3D-LUT enhancer fp32, 3x64x64, trilinear GridSample into 33^3 (seeded weights, oracle/refdump_grid_sample.cpp)"),
 }
 # models whose inputs refdump's bench does not fill (int32 token ids and masks): timed by oracle/refdump_gather's bench instead
 GATHER_HARNESS = {"bert", "vit"}
