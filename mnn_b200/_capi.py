@@ -194,6 +194,17 @@ GRID_SAMPLE_SIGNATURES = {
 }
 _grid_sample_lib = None
 
+# libmnn_b200_gru.so (include/mnn_b200_gru.h): the GRU execution, on the runtime and execution handles above.  execute's
+# params is a host array of 5 * D device pointers
+GRU_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_gru.so")
+GRU_SIGNATURES = {
+    "mnnb200_gru_create": (C.c_int, [P, C.c_int, C.POINTER(P)]),
+    "mnnb200_gru_resize": (C.c_int, [P, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int]),
+    "mnnb200_gru_execute": (C.c_int, [P, P, C.POINTER(P), P, P, P]),
+    "mnnb200_gru_plan": (C.c_int, [P, _IP, C.c_int]),
+}
+_gru_lib = None
+
 # libmnn_b200_llm.so (include/mnn_b200_llm.h): MNN-LLM's LayerNorm / RoPE executions, on the runtime and execution handles above
 LLM_LIB_PATH = os.path.join(os.path.dirname(LIB_PATH), "libmnn_b200_llm.so")
 LLM_SIGNATURES = {
@@ -318,6 +329,22 @@ def grid_sample_lib():
             fn.argtypes = args
         _grid_sample_lib = L
     return _grid_sample_lib
+
+
+def gru_lib():
+    """libmnn_b200_gru.so with every GRU_SIGNATURES symbol resolved (after libmnn_b200.so, whose handles it shares)"""
+    global _gru_lib
+    if _gru_lib is None:
+        lib()
+        if not os.path.exists(GRU_LIB_PATH):
+            raise MnnB200Error(f"{GRU_LIB_PATH} is missing: run `python -m mnn_b200.build` (there is no CPU fallback)")
+        L = C.CDLL(GRU_LIB_PATH)
+        for name, (res, args) in GRU_SIGNATURES.items():
+            fn = getattr(L, name)
+            fn.restype = res
+            fn.argtypes = args
+        _gru_lib = L
+    return _gru_lib
 
 
 def lib():

@@ -2,8 +2,8 @@
 libmnn_b200_deconv.so (the float Deconvolution, include/mnn_b200_deconv.h), libmnn_b200_interp.so (the float Interp,
 include/mnn_b200_interp.h), libmnn_b200_gather.so (the gathers and the int32 / fp32 Cast, include/mnn_b200_gather.h) and
 libmnn_b200_scatter.so (ScatterNd and ScatterElements, include/mnn_b200_scatter.h), libmnn_b200_rnn.so (LSTM and RNN,
-include/mnn_b200_rnn.h) and libmnn_b200_grid_sample.so (the float GridSample, include/mnn_b200_grid_sample.h), the last seven
-linked against libmnn_b200.so, and libmnn_b200_shallow.so (the shallow conv-group
+include/mnn_b200_rnn.h), libmnn_b200_grid_sample.so (the float GridSample, include/mnn_b200_grid_sample.h) and
+libmnn_b200_gru.so (GRU, include/mnn_b200_gru.h), the last eight linked against libmnn_b200.so, and libmnn_b200_shallow.so (the shallow conv-group
 kernel, which libmnn_b200.so launches and links against), in-tree for sm_90a (H100) with nvcc.  No torch involvement."""
 import os
 import subprocess
@@ -19,6 +19,7 @@ GATHER_LIB = os.path.join(HERE, "libmnn_b200_gather.so")
 SCATTER_LIB = os.path.join(HERE, "libmnn_b200_scatter.so")
 RNN_LIB = os.path.join(HERE, "libmnn_b200_rnn.so")
 GRID_SAMPLE_LIB = os.path.join(HERE, "libmnn_b200_grid_sample.so")
+GRU_LIB = os.path.join(HERE, "libmnn_b200_gru.so")
 SHALLOW_LIB = os.path.join(HERE, "libmnn_b200_shallow.so")
 SOURCES = ["capi.cu", "conv_int8_mma.cu", "elementwise.cu", "gemm_i8_wgmma.cu", "winograd_int8.cu", "gemm_f16_wgmma.cu", "conv_int8_stem.cu", "conv_group_wgmma.cu", "linear_w8_gemv.cu", "conv_f32_wgmma.cu"]
 LLM_SOURCES = ["llm_ops.cu", "llm_capi.cu"]
@@ -28,6 +29,7 @@ GATHER_SOURCES = ["gather.cu", "gather_capi.cu"]
 SCATTER_SOURCES = ["scatter.cu", "scatter_capi.cu"]
 RNN_SOURCES = ["rnn.cu", "rnn_capi.cu"]
 GRID_SAMPLE_SOURCES = ["grid_sample_f32.cu", "grid_sample_capi.cu"]
+GRU_SOURCES = ["gru.cu", "gru_capi.cu"]
 # the shallow conv-group kernel, launched by libmnn_b200.so, which links against it
 SHALLOW_SOURCES = ["conv_group_shallow_wgmma.cu"]
 ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
@@ -58,7 +60,7 @@ def _compile(srcs, nvcc, verbose):
 
 
 def build(force=False, verbose=False):
-    """the nine libraries; returns the path of libmnn_b200.so"""
+    """the ten libraries; returns the path of libmnn_b200.so"""
     srcs = [os.path.join(CSRC, s) for s in SOURCES if os.path.exists(os.path.join(CSRC, s))]
     llm_srcs = [os.path.join(CSRC, s) for s in LLM_SOURCES]
     inc = os.path.join(HERE, "..", "include")
@@ -77,6 +79,8 @@ def build(force=False, verbose=False):
     rnn_deps = deps + rnn_srcs + [os.path.join(inc, "mnn_b200_rnn.h")]
     gs_srcs = [os.path.join(CSRC, s) for s in GRID_SAMPLE_SOURCES]
     gs_deps = deps + gs_srcs + [os.path.join(inc, "mnn_b200_grid_sample.h")]
+    gru_srcs = [os.path.join(CSRC, s) for s in GRU_SOURCES]
+    gru_deps = deps + gru_srcs + [os.path.join(inc, "mnn_b200_gru.h")]
     fresh = lambda lib, ds: os.path.exists(lib) and all(os.path.getmtime(lib) > os.path.getmtime(d) for d in ds)
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
     shallow_srcs = [os.path.join(CSRC, s) for s in SHALLOW_SOURCES]
@@ -106,6 +110,9 @@ def build(force=False, verbose=False):
                               ["-L" + HERE, "-lmnn_b200", "-Xlinker", "-rpath,$ORIGIN", "-lcudart"])
     if force or not fresh(GRID_SAMPLE_LIB, gs_deps + [LIB]):
         subprocess.check_call([nvcc, "-shared", "-o", GRID_SAMPLE_LIB] + _compile(gs_srcs, nvcc, verbose) + ARCH +
+                              ["-L" + HERE, "-lmnn_b200", "-Xlinker", "-rpath,$ORIGIN", "-lcudart"])
+    if force or not fresh(GRU_LIB, gru_deps + [LIB]):
+        subprocess.check_call([nvcc, "-shared", "-o", GRU_LIB] + _compile(gru_srcs, nvcc, verbose) + ARCH +
                               ["-L" + HERE, "-lmnn_b200", "-Xlinker", "-rpath,$ORIGIN", "-lcudart"])
     return LIB
 

@@ -83,7 +83,7 @@ enum ExecType : unsigned {
     kConvGroup = 1u << 5, kScaleInt8 = 1u << 6, kConvF32 = 1u << 7, kDwConvF32 = 1u << 8, kScaleF32 = 1u << 9,
     kLayerNormF32 = 1u << 10, kRoPEF32 = 1u << 11, kDeconvF32 = 1u << 12, kDwDeconvF32 = 1u << 13,
     kInterpF32 = 1u << 14, kGather = 1u << 15, kScatter = 1u << 16, kRnn = 1u << 17,
-    kGridSampleF32 = 1u << 18,
+    kGridSampleF32 = 1u << 18, kGru = 1u << 19,
 };
 struct mnnb200_exec {
     unsigned type = 0;  // the ExecType of the struct new_exec made

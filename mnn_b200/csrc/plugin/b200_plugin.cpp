@@ -42,6 +42,7 @@
 #include "../../../include/mnn_b200_gather.h"
 #include "../../../include/mnn_b200_scatter.h"
 #include "../../../include/mnn_b200_rnn.h"
+#include "../../../include/mnn_b200_gru.h"
 #include "../../../include/mnn_b200_interp.h"
 #include "../../../include/mnn_b200_grid_sample.h"
 #include "../../../include/mnn_b200_llm.h"
@@ -1611,6 +1612,75 @@ private:
     ExecHandle mH;
 };
 
+// GRU (OpType_RNNSequenceGRU, as the ONNX converter writes it: X, then per direction gateWeight [I + H, 2H], gateBias (2H),
+// candidateWeight [I + H, H], candidateBias (H), recurrentBias (3H), then an optional h0 [D, B, H]) on fp32 tensors in a linear
+// layout, H = the RNNParam's numUnits and D = 2 when isBidirectionalRNN.  Outputs: with keepAllOutputs Y [T, D, B, H] and
+// optionally Y_h [D, B, H], else Y_h only.  Y_h is ONNX's (each direction's last h), where the CPU's backward half, with both
+// outputs, is its scratch.  Declined: the legacy form with the weights in the parameter's Blobs, int8 / fp16 / NC4HW4 tensors
+// and inconsistent shapes.
+class GruExec : public ClonedFromOp<GruExec> {
+public:
+    GruExec(Backend* bn, const Op* op, mnnb200_exec* h) : ClonedFromOp(bn), mOp(op), mH(h) {}
+    static Execution* create(B200Backend* bn, const Op* op) {
+        auto p = op->main_as_RNNParam();
+        mnnb200_exec* h = nullptr;
+        if (!p || mnnb200_gru_create(bn->handle(), p->linearBeforeReset() ? 1 : 0, &h) != MNNB200_OK) return nullptr;
+        return new GruExec(bn, op, h);
+    }
+    static int directions(const Op* op) { return op->main_as_RNNParam()->isBidirectionalRNN() ? 2 : 1; }
+    static bool takes(const Op* op, const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) {
+        auto p = op->main_as_RNNParam();
+        if (!p) return false;
+        const int D = directions(op), H = p->numUnits();
+        const size_t n = 1 + 5 * (size_t)D;
+        const bool keep = p->keepAllOutputs();
+        if ((inputs.size() != n && inputs.size() != n + 1) || outputs.empty() || outputs.size() > (keep ? 2u : 1u)) return false;
+        for (auto t : inputs) if (!RnnExec::f32Linear(t)) return false;
+        for (auto t : outputs) if (!RnnExec::f32Linear(t)) return false;
+        auto x = inputs[0];
+        if (x->dimensions() != 3) return false;
+        const int T = x->length(0), B = x->length(1), I = x->length(2);
+        if (T < 1 || B < 1 || I < 1 || H < 1) return false;
+        bool ok = true;
+        for (int d = 0; d < D; ++d) {
+            auto w = inputs.begin() + 1 + 5 * d;
+            ok = ok && RnnExec::shaped(w[0], {I + H, 2 * H}) && elemCount(w[1]) == 2 * (size_t)H &&
+                 RnnExec::shaped(w[2], {I + H, H}) && elemCount(w[3]) == (size_t)H && elemCount(w[4]) == 3 * (size_t)H;
+        }
+        if (inputs.size() == n + 1) ok = ok && RnnExec::shaped(inputs[n], {D, B, H});
+        if (keep) {
+            ok = ok && RnnExec::shaped(outputs[0], {T, D, B, H});
+            if (outputs.size() > 1) ok = ok && RnnExec::shaped(outputs[1], {D, B, H});
+        } else {
+            ok = ok && RnnExec::shaped(outputs[0], {D, B, H});
+        }
+        return ok;
+    }
+    ErrorCode onResize(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        if (!takes(mOp, inputs, outputs)) return NOT_SUPPORT;
+        auto x = inputs[0];
+        const int D = directions(mOp);
+        return toErr(mnnb200_gru_resize(mH.get(), x->length(0), x->length(1), x->length(2), mOp->main_as_RNNParam()->numUnits(), D,
+                                        inputs.size() > 1 + 5 * (size_t)D ? 1 : 0),
+                     "gru resize");
+    }
+    ErrorCode launch(const std::vector<Tensor*>& inputs, const std::vector<Tensor*>& outputs) override {
+        auto f = [](const Tensor* t) { return (float*)dev(t); };
+        const int D = directions(mOp);
+        const float* params[10];
+        for (int k = 0; k < 5 * D; ++k) params[k] = f(inputs[1 + k]);
+        const bool keep = mOp->main_as_RNNParam()->keepAllOutputs();
+        float* y = keep ? f(outputs[0]) : nullptr;
+        float* yh = keep ? (outputs.size() > 1 ? f(outputs[1]) : nullptr) : f(outputs[0]);
+        return toErr(mnnb200_gru_execute(mH.get(), f(inputs[0]), params, inputs.size() > 1 + 5 * (size_t)D ? f(inputs.back()) : nullptr,
+                                         y, yh),
+                     "gru");
+    }
+private:
+    const Op* mOp;
+    ExecHandle mH;
+};
+
 // Cast between int32 and fp32 (CPUCast's CastDataType): an attention mask's int32 -> fp32, or fp32 -> int32 (truncation)
 class CastExec : public B200Exec {
 public:
@@ -1679,6 +1749,9 @@ Execution* B200Backend::onCreate(const std::vector<Tensor*>& inputs, const std::
         case OpType_LSTM:
         case OpType_RNN:
             if (!quantOut && RnnExec::takes(op, inputs, outputs)) e = RnnExec::create(this, op);
+            break;
+        case OpType_RNNSequenceGRU:
+            if (!quantOut && GruExec::takes(op, inputs, outputs)) e = GruExec::create(this, op);
             break;
         case OpType_Cast: {
             const int dir = quantOut ? -1 : CastExec::direction(op, inputs, outputs);

@@ -23,7 +23,7 @@ def build():
     inc = ["include", "source", "schema/current", "3rd_party/flatbuffers/include", "3rd_party"]
     cmd = ["g++", "-std=gnu++11", "-O2", "-fPIC", "-shared", "-fno-rtti", "-fno-exceptions", "-fvisibility=hidden", "-w",
            "-DMNN_USE_SSE", "-o", OUT, src] + ["-I" + os.path.join(REF, i) for i in inc] + \
-          ["-L" + PKG, "-lmnn_b200", "-lmnn_b200_llm", "-lmnn_b200_deconv", "-lmnn_b200_interp", "-lmnn_b200_gather", "-lmnn_b200_scatter", "-lmnn_b200_rnn", "-lmnn_b200_grid_sample", "-Wl,-rpath,$ORIGIN"]
+          ["-L" + PKG, "-lmnn_b200", "-lmnn_b200_llm", "-lmnn_b200_deconv", "-lmnn_b200_interp", "-lmnn_b200_gather", "-lmnn_b200_scatter", "-lmnn_b200_rnn", "-lmnn_b200_grid_sample", "-lmnn_b200_gru", "-Wl,-rpath,$ORIGIN"]
     subprocess.check_call(cmd)
     print("[build_plugin] wrote", OUT)
     return OUT

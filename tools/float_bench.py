@@ -40,6 +40,8 @@ MODELS = {   # --model: (fixture under oracle/_ref, name in the JSON line)
     "kws": ("kws_f32.mnn", "streaming keyword-spotter chunk fp32, 16 frames, LSTM H 128 + RNN H 64 with states (seeded weights, oracle/refdump_rnn.cpp)"),
     "flow": ("flow_f32.mnn", "two-frame flow-warp net fp32, 6x64x64, bilinear GridSample at 16x16 (seeded weights, oracle/refdump_grid_sample.cpp)"),
     "lut": ("lut_f32.mnn", "image-adaptive 3D-LUT enhancer fp32, 3x64x64, trilinear GridSample into 33^3 (seeded weights, oracle/refdump_grid_sample.cpp)"),
+    "denoise": ("denoise_f32.mnn", "RNNoise-style streaming denoiser chunk fp32, 16 frames of 42 features, GRUs H 24 / 48 / 96 with states (seeded weights, oracle/refdump_gru.cpp)"),
+    "tagger": ("tagger_f32.mnn", "BiGRU sequence tagger fp32, 64 int32 tokens, embedding 8000x128, 2 BiGRU H 256 (seeded weights, oracle/refdump_gru.cpp)"),
 }
 # models whose inputs refdump's bench does not fill (int32 token ids and masks): timed by oracle/refdump_gather's bench instead
 GATHER_HARNESS = {"bert", "vit"}
@@ -47,6 +49,8 @@ GATHER_HARNESS = {"bert", "vit"}
 SCATTER_HARNESS = {"pillars", "gnn"}
 # models with sequence and state inputs (batch on dim 1): timed by oracle/refdump_rnn's bench
 RNN_HARNESS = {"crnn", "kws"}
+# GRU models with sequence, state or int32 token-id inputs (batch on dim 1): timed by oracle/refdump_gru's bench
+GRU_HARNESS = {"denoise", "tagger"}
 
 
 def shapes_from_cpu_run(model, refdump, env):
@@ -174,6 +178,9 @@ def main():
     if a.model in RNN_HARNESS:
         from oracle import rnn_oracle
         harness = rnn_oracle.REFDUMP_RNN
+    if a.model in GRU_HARNESS:
+        from oracle import gru_oracle
+        harness = gru_oracle.REFDUMP_GRU
     penv = dict(env, REFDUMP_BENCH_WINDOWS="5", REFDUMP_PLUGIN=os.path.join(ROOT, "mnn_b200", "libmnn_b200_plugin.so"))
     p = refdump_bench(harness, model, a.batch, 4, penv, 20)
     res.update(plugin_e2e_img_per_s=p["img_per_s"], plugin_e2e_ms=p["ms_median_window"], plugin_created=p["plugin_created"],
